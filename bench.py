@@ -1,20 +1,24 @@
 #!/usr/bin/env python3
-"""bench.py — headline benchmark of the B200 validation hot path.
+"""bench.py — headline benchmark of the H100 validation hot path.
 
 Workload (BASELINE.json configs[1]): batch-verify 1 Mi standalone BIP-340 Schnorr (pubkey, msg, sig)
 triples per GPU; ~98 % valid, ~1 % single-bit corruptions, ~1 % adversarial encodings
 (rusty_kaspa_b200/workload.py).  One "step" = one pass of the verify kernel over the rank's batch,
 followed (N > 1) by the NCCL all-gather of the per-shard validity bitmaps.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--n ITEMS]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--n ITEMS] [--dump-outputs DIR]
 
 N > 1 is launched by torchrun, one rank per GPU; shards are independent (weak scaling: every rank
 verifies its own 1 Mi triples), the only collective is the bitmap all-gather.
 
 Timing rules followed: W >= 3 warm-ups; L2 flushed (256 MiB write) before every timed step and the
-inputs (128 MiB) exceed the 126 MB L2 anyway; CUDA events on the stream the kernels are launched
+inputs (128 MiB) exceed the 50 MB L2 anyway; CUDA events on the stream the kernels are launched
 on, per step, summed; max over ranks; barrier + synchronize on both sides; clocks sampled with
 nvidia-smi during the timed region.
+
+--dump-outputs DIR writes what the timed path returned in its last timed step (rank 0): the verdict of
+every triple and the validity bitmap, as float32 .npy files.  The inputs are seeded, so two builds run
+with the same arguments can be compared output for output.
 
 --impl reference times the CPU path instead: the reference's own implementation cannot be built
 here (no Rust toolchain, libsecp256k1 not vendored; DESIGN.md), so this arm runs the C restatement
@@ -79,8 +83,7 @@ def cpu_quota():
 
 def host_threads():
     """Threads for the CPU arm: all CPUs this process may run on, but no more than twice the container's CPU quota
-    (cgroup cpu.max).  On the GPU boxes (128 logical CPUs, quota 16) 32 threads give 111 k verifies/s while 128 threads
-    spend their time being throttled (87 k/s) — tools/cpu_threads.py."""
+    (cgroup cpu.max): threads beyond the quota spend their time being throttled (tools/cpu_threads.py measures the rate per thread count)."""
     try:
         n = len(os.sched_getaffinity(0))
     except Exception:
@@ -95,12 +98,11 @@ def host_threads():
 
 
 class ClockSampler:
-    """SM clock / power / throttle reasons of ONE GPU during the timed region (B200_PROFILING.md's clocks line).
+    """SM clock / power / throttle reasons of ONE GPU during the timed region.
 
     Sampled in-process through NVML (nvidia_ml_py), attached to this rank's GPU only and initialised in prepare() BEFORE the warm-up: spawning
     `nvidia-smi -lms` per rank at the start of the timed region - the round-1 form - makes eight NVML initialisations enumerate every GPU of
-    the node while the steps run, which stalled rank 0's GPU by ~12 ms per step and WAS the N=8 scaling cliff (measured: 197.8 -> 277.3 M
-    verifies/s at N=8 with nothing else changed, profiles/r02_scaling_n8.md).  nvidia-smi remains the fallback when NVML cannot be loaded;
+    the node while the steps run, which stalled rank 0's GPU for milliseconds per step and made N=8 scale badly.  nvidia-smi remains the fallback when NVML cannot be loaded;
     it is then started in prepare() as well and only rows that fall inside the timed region are kept."""
     Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
@@ -211,12 +213,8 @@ class ClockSampler:
                 "power_w_max": max(power) if power else None, "samples": len(sm), "reasons": sorted(reasons), "sampler": self.how}
 
 
-def measured_peak_hbm():
-    try:
-        with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
-            return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
-    except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md)"
+# HBM3 bandwidth of the H100 SXM (NVIDIA data sheet); the roofline fractions are relative to it
+HBM_PEAK_GBS, HBM_PEAK_SOURCE = 3350.0, "H100 SXM data sheet (HBM3)"
 
 
 # ------------------------------------------------------------------------------------------------
@@ -251,22 +249,6 @@ def run_reference(args, rank, world):
                                        f"4x64 limbs), {threads} pthreads with static chunks on {logical} logical CPUs under a cgroup quota of {quota} CPUs"},
             "e2e": {"value": value, "unit": UNIT, "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0}}
     emit_json_line(line)
-
-
-# Issue cycles per Schnorr verify per SM sub-partition for the shipping kernel's instruction stream (DESIGN.md §4):
-# 1.355e5 IMAD.WIDE x 4.3 cycles + 2.772e5 other instructions x 1 cycle, per warp of 32 verifies (ncu: 412.7 k thread instructions per verify
-# in the final round-2 build, profiles/r02_schnorr_verify_ncu_summary.json - the multiply count is that of the unchanged field arithmetic,
-# profiles/r01_schnorr_verify_ncu_summary.json; per-instruction costs, profiles/r01_pipe_microbench.txt).
-ISSUE_CYCLES_PER_WARP_VERIFY = 1.355e5 * 4.3 + 2.772e5 * 1.0
-SCHEDULERS = 148 * 4
-
-
-def integer_issue_roofline(n_items, kernel_ms, clocks):
-    mhz = (clocks or {}).get("sm_mhz") or 1965.0
-    peak = SCHEDULERS * mhz * 1e6 * 32.0 / ISSUE_CYCLES_PER_WARP_VERIFY
-    achieved = n_items / (kernel_ms * 1e-3)
-    return {"bound": "integer issue (IMAD.WIDE 4.3 cyc, other 1 cyc per warp instruction per scheduler, measured)", "achieved": achieved,
-            "peak": peak, "unit": "verifies/s", "frac": achieved / peak, "sm_mhz": mhz}
 
 
 def measure_tx_validation(ctx, dev, n_txs, steps, mix=(1.0, 0.0, 0.0, 0.0), label="config 3"):
@@ -528,11 +510,11 @@ def measure_ecdsa(ctx, dev, stream, n, steps):
     return {"what": "kgv_ecdsa_verify, device-resident", "n": n, "verifies_per_s": n / s, "ms_per_call": s * 1e3, "generation_s": round(gen_s, 1)}
 
 
-def measure_utxo_table(ctx, dev, stream, peak_gbs):
+def measure_utxo_table(ctx, dev, stream, peak_gbs, steps):
     """K5: the GPU UTXO table on its own: 4 Mi entries in a 16 Mi-slot (2 GiB) table; every timed call looks up a DIFFERENT random
     permutation of all 4 Mi entries (occupied slots = 512 MiB, four times L2), keys and results device-resident; then erase / re-insert of 1 Mi
-    entries per call (kgv_utxo_apply_diff, device arrays).  Algorithmic bytes per lookup (SURVEY §8d): 36 B key + one 128 B slot = 164 B
-    (+ 33 B of results written).  The probe itself reads only the first 64 bytes of a slot (two LDG.256), so DRAM moves LESS than that."""
+    entries per call (kgv_utxo_apply_diff, device arrays); `steps` timed calls of each.  Algorithmic bytes per lookup (SURVEY §8d): 36 B key + one 128 B slot = 164 B
+    (+ 33 B of results written).  The probe itself reads only the first 64 bytes of a slot (four 128-bit loads), so DRAM moves LESS than that."""
     import torch
     from rusty_kaspa_b200 import GpuUtxoSet
     from rusty_kaspa_b200.txbatch import ENTRY_DTYPE
@@ -551,21 +533,19 @@ def measure_utxo_table(ctx, dev, stream, peak_gbs):
     ctx.synchronize()
     ins_s = time.perf_counter() - t0
     assert us.count() == n_ent
-    reps = 4
     dkeys = torch.from_numpy(keys).to(dev)
-    dks = [dkeys[torch.randperm(n_ent, device=dev)].contiguous() for _ in range(reps + 1)]
     de = torch.empty(n * ENTRY_DTYPE.itemsize, dtype=torch.uint8, device=dev)
     df = torch.empty(n, dtype=torch.uint8, device=dev)
     call = lambda dk: ctx._check(ctx._lib.kgv_utxo_lookup(ctx._h, us._h, dk.data_ptr(), n, de.data_ptr(), None, 0, df.data_ptr()))
-    call(dks[reps]); stream.synchronize()
+    call(dkeys[torch.randperm(n_ent, device=dev)].contiguous()); stream.synchronize()
     assert int(df.sum().item()) == n
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record(stream)
-    for r in range(reps):
-        call(dks[r])
-    e1.record(stream)
-    stream.synchronize()
-    s = e0.elapsed_time(e1) * 1e-3 / reps
+    s = 0.0
+    for _ in range(steps):
+        dk = dkeys[torch.randperm(n_ent, device=dev)].contiguous()  # a new order every call, shuffled outside the timed events
+        e0.record(stream); call(dk); e1.record(stream)
+        stream.synchronize()
+        s += e0.elapsed_time(e1) * 1e-3 / steps
     # erase + re-insert 1 Mi entries per call, device arrays
     m = 1 << 20
     sel = torch.randperm(n_ent, device=dev)[:m]
@@ -579,9 +559,9 @@ def measure_utxo_table(ctx, dev, stream, peak_gbs):
     erase(); insert(); stream.synchronize()
     ev = [torch.cuda.Event(enable_timing=True) for _ in range(3)]
     t_er = t_in = 0.0
-    for _ in range(3):
+    for _ in range(steps):
         ev[0].record(stream); erase(); ev[1].record(stream); insert(); ev[2].record(stream); stream.synchronize()
-        t_er += ev[0].elapsed_time(ev[1]) * 1e-3 / 3; t_in += ev[1].elapsed_time(ev[2]) * 1e-3 / 3
+        t_er += ev[0].elapsed_time(ev[1]) * 1e-3 / steps; t_in += ev[1].elapsed_time(ev[2]) * 1e-3 / steps
     assert int(drs.sum().item()) == m and us.count() == n_ent
     us.close()
     gbs = n * 164 / s * 1e-9
@@ -597,9 +577,9 @@ def measure_utxo_table(ctx, dev, stream, peak_gbs):
                                 "frac": m * (36 + 32 + 34 + 128) / t_in * 1e-9 / peak_gbs if peak_gbs else None, "bytes_per_op": 230}}
 
 
-def measure_small_batches(ctx):
+def measure_small_batches(ctx, steps):
     """Mempool-shaped use (SURVEY §8f-3): latency of ONE kgv_validate_txs call on small host-resident batches
-    (upload + populate + context rules + scripts + verdict download), median of 20 calls."""
+    (upload + populate + context rules + scripts + verdict download), median of `steps` calls after 3 untimed ones."""
     from rusty_kaspa_b200 import GpuUtxoSet, Params, TransactionValidator, simgen
     from rusty_kaspa_b200.txbatch import build_batch
     fkeys, fentries, txs = simgen.funded_window(256, n_keys=64, n_nonces=64)
@@ -610,13 +590,15 @@ def measure_small_batches(ctx):
     out = {}
     for n in (1, 16, 256):
         b = build_batch(txs[:n])
+        for _ in range(3):
+            tv.validate_transactions_in_parallel(us, b, 10)
         ts = []
-        for _ in range(23):
+        for _ in range(steps):
             t0 = time.perf_counter()
             res = tv.validate_transactions_in_parallel(us, b, 10)
             ts.append(time.perf_counter() - t0)
         assert (res["status"] == 0).all()
-        out[str(n)] = round(sorted(ts[3:])[10] * 1e3, 3)
+        out[str(n)] = round(float(np.median(ts)) * 1e3, 3)
     us.close()
     return {"what": "median wall-clock ms of one kgv_validate_txs call, host arrays in, verdicts out", "ms_by_batch_size": out}
 
@@ -716,6 +698,16 @@ def measure_dag_replay_sharded(ctx, dev, comm, rank, world, n_blocks, tpb, windo
             "generation_s": round(gen_s, 1), "replicas_identical": True}
 
 
+def dump_outputs(out_dir, status, bitmap):
+    """What the timed path returned in its last step: one verdict per triple (0 invalid, 1 valid, 2/3 parse errors) and the validity
+    bitmap (one byte per 8 triples; N > 1: every rank's bitmap, in rank order), as float32 arrays.  The status is capped at 8 Mi values
+    (32 MiB) and the bitmap at 4 Mi (16 MiB): a longer array is written as every k-th value, k the smallest stride that fits, so that the
+    two files stay under 64 MB together for any --n and --gpus."""
+    os.makedirs(out_dir, exist_ok=True)
+    for name, a, cap in (("status", status, 8 << 20), ("bitmap", bitmap, 4 << 20)):
+        np.save(os.path.join(out_dir, name + ".npy"), a[::max(1, -(-len(a) // cap))].astype(np.float32))
+
+
 def run_ours(args, rank, world, local_rank):
     import torch
     import torch.distributed as dist
@@ -812,6 +804,8 @@ def run_ours(args, rank, world, local_rank):
         total_ms = float(sum(step_ms))
         # correctness guard inside the bench: verdict counts must match the generator's ground truth
         st = dst.cpu().numpy()
+        if args.dump_outputs and rank == 0:
+            dump_outputs(args.dump_outputs, st, (gathered if world > 1 else dbm).cpu().numpy())
         assert int((st == 1).sum()) == expected_valid, "GPU verdicts disagree with the generator's ground truth"
         assert not (st[kind != 0] == 1).any()
         mine = np.zeros(nbm, dtype=np.uint8)
@@ -829,7 +823,7 @@ def run_ours(args, rank, world, local_rank):
         hpk, hmsg, hsig = (torch.from_numpy(a).pin_memory() for a in (pk, msg, sig))
         hst = torch.empty(n, dtype=torch.uint8).pin_memory()
         hall = torch.empty(nbm * world, dtype=torch.uint8).pin_memory() if world > 1 else None
-        e2e_steps = max(2, min(args.steps, 5))
+        e2e_steps = args.steps
 
         def e2e_step():
             if world == 1:  # kgv_schnorr_verify with host pointers: chunked H2D overlapped with the verification, D2H of the verdicts
@@ -880,14 +874,8 @@ def run_ours(args, rank, world, local_rank):
     value = n * world * args.steps / (total_ms * 1e-3)
     e2e_value = n * world * e2e_steps / e2e_s
     kern_ms_avg = kern_total_ms / args.steps
-    peak, peak_src = measured_peak_hbm()
+    peak, peak_src = HBM_PEAK_GBS, HBM_PEAK_SOURCE
     achieved = ALG_BYTES_PER_VERIFY * n / (kern_ms_avg * 1e-3) / 1e9
-    traffic = None
-    try:
-        with open(os.path.join(ROOT, "profiles", "r02_schnorr_verify_ncu_summary.json")) as f:  # one `ncu --set full` capture at the bench size (1 Mi triples per launch)
-            traffic = int(json.load(f).get("dram_bytes_per_launch"))
-    except Exception:
-        pass
 
     # ---- CPU baseline beside it: the oracle port on the host cores, bounded sample (rank 0, N=1 only)
     cpu = None
@@ -913,10 +901,10 @@ def run_ours(args, rank, world, local_rank):
                                       mix=(0.0, 0.5, 0.25, 0.25), label="config 4", seed=0x4B475634)
     if world == 1 and args.tx_window > 0:
         with torch.cuda.stream(stream):
-            txv = measure_tx_validation(ctx, dev, args.tx_window, max(2, min(args.steps, 5)))
-            ecd = measure_ecdsa(ctx, dev, stream, min(n, 1 << 19), 3)
-            small = measure_small_batches(ctx)
-            utx = measure_utxo_table(ctx, dev, stream, peak)
+            txv = measure_tx_validation(ctx, dev, args.tx_window, args.steps)
+            ecd = measure_ecdsa(ctx, dev, stream, min(n, 1 << 19), args.steps)
+            small = measure_small_batches(ctx, args.steps)
+            utx = measure_utxo_table(ctx, dev, stream, peak, args.steps)
 
     line = {"metric": METRIC, "value": value, "unit": UNIT, "n_gpus": world, "steps": args.steps, "warmup": max(args.warmup, 3),
             "ms_per_step": total_ms / args.steps, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
@@ -927,10 +915,9 @@ def run_ours(args, rank, world, local_rank):
                                                               "nccl": "kgv_shard_allgather: ncclAllGather called from libkgv", "torch": "torch.distributed all_gather_into_tensor"}[args.collective],
                        "items_per_gpu_per_step": n, "input_bytes_per_gpu": 128 * n, "l2": "256 MiB flush write before every timed step; inputs 128 MiB > L2",
                        "parallelism": f"{world} independent shard(s), one process per GPU", "generation_s": round(gen_s, 1)},
-            "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak, "traffic": traffic,
+            "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
                          "peak_source": peak_src, "kernel": "k_schnorr_verify", "kernel_ms": kern_ms_avg,
-                         "note": "integer-issue bound by construction: 129 algorithmic bytes per verify vs 4.1e5 integer instructions; the binding roofline is integer_issue",
-                         "integer_issue": integer_issue_roofline(n, kern_ms_avg, merge_clocks(cl_all))},
+                         "note": "129 algorithmic bytes per verify against some 4e5 integer instructions: the kernel is bound by integer issue, not by HBM"},
             "cpu_baseline": cpu,
             "e2e": {"value": e2e_value, "unit": UNIT, "h2d_bytes_per_step": 128 * n * world, "d2h_bytes_per_step": (n if world == 1 else nbm * world) * world,
                     "steps": e2e_steps,
@@ -967,7 +954,8 @@ def emit_json_line(line):
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
-    ap.add_argument("--steps", type=int, default=10)
+    ap.add_argument("--steps", type=int, default=10, help="timed steps of the headline loop and of every repeated secondary measurement "
+                    "(the DAG-replay legs time one pass over their chain, sized by --replay-blocks)")
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--n", type=int, default=N_DEFAULT, help="triples per GPU per step")
@@ -977,7 +965,10 @@ def main():
     ap.add_argument("--replay-blocks", type=int, default=10000, help="blocks of the DAG-replay leg (BASELINE configs[2]: 10k blocks; 0 = skip)")
     ap.add_argument("--replay-window", type=int, default=1024, help="blocks per kgv_replay_window call")
     ap.add_argument("--tx-window", type=int, default=32768, help="transactions in the secondary txs-validated/s measurement (0 = skip)")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the verdicts and the bitmap of the last timed step to DIR/*.npy (float32)")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     _quiet_stdout()
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))

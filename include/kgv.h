@@ -1,5 +1,5 @@
 /*
- * kgv.h — C ABI of the B200 transaction-validation library (libkgv.so).
+ * kgv.h — C ABI of the H100 transaction-validation library (libkgv.so).
  *
  * "kgv" = Kaspa GPU Validator.  This is the drop-in boundary for the hot path named by
  * BASELINE.json: batched secp256k1 Schnorr/ECDSA verification, sighash / tx-id hashing, the

@@ -1,9 +1,9 @@
-// kgv_arith.cuh — 256-bit limb primitives and secp256k1 field arithmetic for sm_100a.
+// kgv_arith.cuh — 256-bit limb primitives and secp256k1 field arithmetic for sm_90a.
 //
 // One number per thread, 8 x 32-bit little-endian limbs held in registers.  Products are
 // built from IMAD.WIDE.U32(.X) carry chains (mad.lo.cc / madc.hi.cc pairs, which ptxas fuses
-// into one IMAD.WIDE.U32.X each); measured on B200 (tools/microbench/pipes.cu, femul.cu): an
-// IMAD.WIDE costs ~4.3 cycles per warp instruction per SM sub-partition, IADD3 ~1.
+// into one IMAD.WIDE.U32.X each); tools/microbench/pipes.cu and femul.cu measure what an IMAD.WIDE
+// and an IADD3 cost per warp instruction per SM sub-partition.
 //
 // Replaces, for the GPU path, the field arithmetic of the C libsecp256k1 that the reference
 // reaches through crypto/txscript/src/lib.rs:593 / :628 (`sig.verify`).
@@ -649,8 +649,8 @@ KGV_HD void fe_sqr_inl(fe& r, const fe& a) {
 
 // r = a^(2^n).  KGV_SQRN_CALL=1 makes a whole run of squarings ONE call (the squaring inlined into the loop of a non-inlined function: the
 // exponentiation chains - square root of lift_x, the shared inversion, ~510 squarings per verification - then pay the by-value call ABI once per
-// run instead of once per squaring).  Measured on B200: fewer instructions but SLOWER for the field (34.95 vs 36.11 M verifies/s: a second copy of
-// the squaring in the hot code), faster for the scalar inversion of ECDSA (32.0 vs 31.4 M/s) - so it is on for scalars only (KGV_SC_SQRN_CALL).
+// run instead of once per squaring).  Measured when the kernels were tuned on the previous target GPU (not re-measured on H100): fewer instructions but
+// slower for the field (a second copy of the squaring in the hot code), faster for the scalar inversion of ECDSA - so it is on for scalars only (KGV_SC_SQRN_CALL).
 #ifndef KGV_SQRN_CALL
 #define KGV_SQRN_CALL 0
 #endif

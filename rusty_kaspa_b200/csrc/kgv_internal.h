@@ -70,7 +70,7 @@ struct kgv_ctx {
   struct kgv_comm* shard_comm = nullptr;  // kgv_set_sharding: signature checks of the validation calls are split over its ranks
   std::vector<uint8_t*> parked;  // outgrown per-call buffers, released when the caller synchronises / destroys the context (kgv_reserve)
   uint64_t launches = 0;
-  int resident_blocks = 148 * KGV_BLOCKS_PER_SM;  // verification kernels: blocks that fit the device at once (persistent grid)
+  int resident_blocks = 132 * KGV_BLOCKS_PER_SM;  // verification kernels: blocks that fit the device at once (persistent grid)
   std::recursive_mutex mu;  // recursive: the host-VM resolution inside a validation call re-enters the ABI (kgv_sighash, kgv_*_verify)
   std::string err;
 };

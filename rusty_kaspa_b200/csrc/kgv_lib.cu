@@ -1,6 +1,6 @@
 // kgv_lib.cu — kernels and C ABI of libkgv.so (see include/kgv.h).
 //
-// Hand-written CUDA for sm_100a.  No CPU fallback: every entry point needs a CUDA device.
+// Hand-written CUDA for sm_90a (H100).  No CPU fallback: every entry point needs a CUDA device.
 #include "../../include/kgv.h"
 #include "kgv_internal.h"
 #include "kgv_verify.cuh"
@@ -24,15 +24,17 @@ struct SmemTab {
   __device__ __forceinline__ uint32_t get(int e, int w) const { return base[(e * 16 + w) * KGV_BLOCK]; }
 };
 
-// 256-bit read-only load (LDG.E.256 on sm_100a)
+// 256-bit read-only load: sm_90 has no 256-bit LDG, so two 128-bit loads of the same 32-byte sector, issued back to back
 __device__ __forceinline__ void ldg256(uint32_t* w, const void* p) {
-  asm volatile("ld.global.nc.v8.u32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
+  asm volatile("ld.global.nc.v4.u32 {%0,%1,%2,%3}, [%8];\n\t"
+               "ld.global.nc.v4.u32 {%4,%5,%6,%7}, [%8+16];"
                : "=r"(w[0]), "=r"(w[1]), "=r"(w[2]), "=r"(w[3]), "=r"(w[4]), "=r"(w[5]), "=r"(w[6]), "=r"(w[7])
                : "l"(p));
 }
 // streaming variant for the signature triples (read once)
 __device__ __forceinline__ void ldg256_stream(uint32_t* w, const void* p) {
-  asm volatile("ld.global.nc.L1::no_allocate.v8.u32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
+  asm volatile("ld.global.nc.L1::no_allocate.v4.u32 {%0,%1,%2,%3}, [%8];\n\t"
+               "ld.global.nc.L1::no_allocate.v4.u32 {%4,%5,%6,%7}, [%8+16];"
                : "=r"(w[0]), "=r"(w[1]), "=r"(w[2]), "=r"(w[3]), "=r"(w[4]), "=r"(w[5]), "=r"(w[6]), "=r"(w[7])
                : "l"(p));
 }
@@ -360,7 +362,7 @@ extern "C" int kgv_create(int device, uint32_t flags, kgv_ctx** out) {
     int per_sm = 0, sms = 0;
     CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_schnorr_verify<true, false>, KGV_BLOCK, smem));
     CK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device));
-    ctx->resident_blocks = per_sm * sms > 0 ? per_sm * sms : 148 * KGV_BLOCKS_PER_SM;
+    ctx->resident_blocks = per_sm * sms > 0 ? per_sm * sms : 132 * KGV_BLOCKS_PER_SM;  // 132 SMs: H100 SXM
     CK(cudaStreamSynchronize(ctx->stream));
     return KGV_OK;
   };

@@ -7,7 +7,7 @@
 // (:262-309), and every accepted transaction is folded into the diff (UtxoDiff::add_transaction, utxo_diff.rs:233-247)
 // before the next block is looked at.  simpa prints the rate of exactly this loop (simpa/src/main.rs:454-460).
 //
-// A 10-BPS block carries a few hundred signatures - three orders of magnitude too few for a B200 - but signatures are
+// A 10-BPS block carries a few hundred signatures - three orders of magnitude too few for an H100 - but signatures are
 // context free given the spent output (SURVEY.md §0-6: the sighash reads only the entry's script_public_key and amount,
 // sighash.rs:252-255, and both are fixed by the outpoint).  So the window is processed in two device-resident passes:
 //
@@ -159,7 +159,7 @@ __device__ __forceinline__ void prefetch_range(const void* p, size_t bytes, uint
 }
 
 // The walk is a chain of dependent memory accesses per block (record -> key -> slot -> entry -> verdict -> slot update).  Left in global
-// memory every link costs an L2 round trip (~0.3 us on a two-die B200) or a DRAM miss (~1 us): ~40 links = 17-20 us per block (measured).
+// memory every link costs an L2 round trip or a DRAM miss, and ~40 dependent links per block add up to many microseconds per block.
 // So each block is STAGED in shared memory first: all 1024 threads copy its transaction / input / output records, tx ids, script verdicts
 // and index maps with independent 8-byte loads (one memory latency for everything), then the output scripts the inserts will store; the
 // three phases then run out of shared memory and touch global memory only for the table itself (probe, claim, store) and for the results.

@@ -31,8 +31,8 @@ namespace kgv {
 #define KGV_A2_LIMBS {0x9D44CFD8u, 0x57C1108Du, 0xA8E2F3F6u, 0x14CA50F7u, 1u}
 
 #ifndef KGV_PAIRED_MUL
-#define KGV_PAIRED_MUL 0   // 1: issue independent field products of the group law in pairs (fe_mul2). Measured SLOWER on B200
-                           // (28.8 vs 33.7 M verifies/s: argument moves + spills outweigh the extra ILP), kept for reference.
+#define KGV_PAIRED_MUL 0   // 1: issue independent field products of the group law in pairs (fe_mul2). Measured slower when the kernels
+                           // were tuned on the previous target GPU (argument moves + spills outweigh the extra ILP); not re-measured on H100.
 #endif
 
 struct gej {

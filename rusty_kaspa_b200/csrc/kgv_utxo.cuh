@@ -2,12 +2,12 @@
 // entry = one L2 line = four 32-byte DRAM sectors.  Plays the role of DbUtxoSetStore / UtxoCollection behind UtxoView::get
 // (consensus/src/model/stores/utxo_set.rs:143-152, consensus/core/src/utxo/utxo_collection.rs:28-32).
 //
-// Memory traffic is the whole cost of this stage, so every access is a 256-bit vector access:
+// Memory traffic is the whole cost of this stage, so every slot access is a 128-bit vector access:
 //   key      36 bytes at a 4-byte aligned address: nine 32-bit loads (a warp's keys are 1 152 contiguous bytes)
-//   probe    the first 64 bytes of a slot (state, outpoint, amount, DAA score, meta, 4 script bytes) with two LDG.256
+//   probe    the first 64 bytes of a slot (state, outpoint, amount, DAA score, meta, 4 script bytes) with four LDG.128
 //            issued back to back: ONE memory round trip per probe, and everything the UTXO-context rules need;
 //            the remaining 64 script bytes are read by whoever hashes / parses the script (pointer into the slot)
-//   insert   four STG.256 + one release store of the state word
+//   insert   eight STG.128 + one release store of the state word
 // Slot loads are L2-coherent (ld.global.cg: the table is written by other SMs of the same launch), never L1 cached
 // (random 128-byte accesses have no L1 reuse).
 #pragma once
@@ -58,14 +58,17 @@ static inline TableView view_of(const kgv_utxo_table* t) { return TableView{t->s
 
 namespace kgv {
 
+// 32 bytes as two 128-bit accesses issued back to back (sm_90 has no 256-bit LDG / STG)
 __device__ __forceinline__ void ld256_cg(uint32_t* w, const void* p) {
-  asm volatile("ld.global.cg.v8.u32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
+  asm volatile("ld.global.cg.v4.u32 {%0,%1,%2,%3}, [%8];\n\t"
+               "ld.global.cg.v4.u32 {%4,%5,%6,%7}, [%8+16];"
                : "=r"(w[0]), "=r"(w[1]), "=r"(w[2]), "=r"(w[3]), "=r"(w[4]), "=r"(w[5]), "=r"(w[6]), "=r"(w[7])
                : "l"(p)
                : "memory");
 }
 __device__ __forceinline__ void st256(void* p, const uint32_t* w) {
-  asm volatile("st.global.v8.u32 [%8], {%0,%1,%2,%3,%4,%5,%6,%7};" ::"r"(w[0]), "r"(w[1]), "r"(w[2]), "r"(w[3]), "r"(w[4]), "r"(w[5]), "r"(w[6]),
+  asm volatile("st.global.v4.u32 [%8], {%0,%1,%2,%3};\n\t"
+               "st.global.v4.u32 [%8+16], {%4,%5,%6,%7};" ::"r"(w[0]), "r"(w[1]), "r"(w[2]), "r"(w[3]), "r"(w[4]), "r"(w[5]), "r"(w[6]),
                "r"(w[7]), "l"(p)
                : "memory");
 }

@@ -65,7 +65,7 @@ __global__ void k_utxo_lookup(TableView t, const uint8_t* __restrict__ keys, siz
   load_key(k, keys + 36 * i);
   SlotHead h;
   UtxoSlot* s = table_find(t, k, h);
-  // the 32-byte entry record is written with one 256-bit store
+  // the 32-byte entry record is written with two 128-bit stores
   uint32_t e[8] = {0, 0, 0, 0, 0, 0, 0, 0};
   e[4] = (uint32_t)(i * stride);  // script_off
   if (s) {

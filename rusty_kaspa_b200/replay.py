@@ -5,7 +5,7 @@ Two schedules with identical results:
 
   blockwise   for every (merged) block in order: validate_transactions_in_parallel(Full) against the UTXO
               table, then UtxoDiff::add_transaction for the accepted ones.  This is the reference's order; a
-              10-BPS block carries <= ~300 signatures, far too few to fill a B200.
+              10-BPS block carries <= ~300 signatures, far too few to fill an H100.
 
   windowed    ONE library call per window of blocks (kgv_replay_window, include/kgv.h): every script of the window
               is checked in one large batch (signatures are context free given the spent output, SURVEY §0-6; outputs

@@ -11,7 +11,7 @@ sys.path.insert(0, os.path.join(ROOT, "oracle"))
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with `-m gpu`)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on an H100 with `-m gpu`)")
 
 
 def _build_if_missing(target, cmd, cwd):

@@ -1,10 +1,11 @@
 import sys, os, time, ctypes
-sys.path.insert(0, "/root/repo")
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
 import numpy as np
 from rusty_kaspa_b200 import workload as W
 pk, msg, sig, kind = W.schnorr_triples(1 << 14, seed=5, n_keys=4096, n_nonces=4096)
 pk, msg, sig, kind = W.tile_triples(pk, msg, sig, kind, 1 << 17)
-O = ctypes.CDLL("/root/repo/oracle/libkaspa_oracle.so"); O.ok_secp_init()
+O = ctypes.CDLL(os.path.join(ROOT, "oracle", "libkaspa_oracle.so")); O.ok_secp_init()
 vp = lambda a: a.ctypes.data_as(ctypes.c_void_p)
 out = np.zeros(len(kind), dtype=np.uint8)
 print("cpu_count", os.cpu_count(), "cpu.max", open("/sys/fs/cgroup/cpu.max").read().strip() if os.path.exists("/sys/fs/cgroup/cpu.max") else "?")

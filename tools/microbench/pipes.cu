@@ -1,4 +1,4 @@
-// Integer / FP64 pipe throughput probe for sm_100a (B200).
+// Integer / FP64 pipe throughput probe (build with the -gencode flags of __graft_entry__.py).
 // Measures per-SM lane-ops/clk for the instruction mixes a 256-bit modular
 // multiply is made of, so DESIGN.md's IMAD roofline is a measured number.
 #include <cstdio>

@@ -1,4 +1,4 @@
-// Reproducer (nvcc 12.9, sm_100a) for the miscompile first seen as "results are wrong when the multiplications are inlined"
+// Reproducer (nvcc 12.9, found when building for sm_100a) for the miscompile first seen as "results are wrong when the multiplications are inlined"
 // (DESIGN.md §6).  Root cause: two local arrays that are live at the same time get the SAME stack offset.
 // Here: `uint32_t r[96]` (written by u3072_canonical, read in the loop after the hasher is initialised) and the
 // 14-byte key string inside the inlined keyed-BLAKE2b init (KEY_ARRAY=1).  The kernel then outputs the ASCII key
@@ -7,8 +7,8 @@
 // It does not depend on ptxas (-Xptxas -O0 fails too), on the number of inlined multiplier call sites (SITES=1 fails),
 // or on how the block multiplier is called; it disappears when the multiplier is a __noinline__ function (different
 // stack layout) or when the key array is removed (KEY_ARRAY=0, the shipped form: key given as two 64-bit words).
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -std=c++17 -DKEY_ARRAY=1 -o bad  stack_coloring_overlap.cu
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -std=c++17 -DKEY_ARRAY=0 -o good stack_coloring_overlap.cu
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -DKEY_ARRAY=1 -o repro_bad  stack_coloring_overlap.cu
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -DKEY_ARRAY=0 -o repro_good stack_coloring_overlap.cu
 #include <cstdio>
 #include <cstdint>
 #include <cuda_runtime.h>
