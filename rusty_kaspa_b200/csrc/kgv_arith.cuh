@@ -312,6 +312,48 @@ KGV_HD void fe_set_u32(fe& r, uint32_t x) { fe_set_zero(r); r.v[0] = x; }
 // r += k * (2^32 + 977) for k in {0,1}; returns carry out
 KGV_HD uint32_t fe_add_kC(fe& r, uint32_t k) { return add8_small3(r.v, 977u * k, k, 0u); }
 
+// r[3..7] += 1 / r[3..7] -= 1; returns the carry / borrow out.  The rare tails of add_low2_rare, sub_low2_rare and
+// fe_fold: one straight carry chain, so the untaken path stays short in the hot code.
+KGV_HD uint32_t inc_hi5(uint32_t* r) {
+  uint32_t c;
+#if defined(__CUDACC__)
+  asm("add.cc.u32 %0, %0, 1;\n\t"
+      "addc.cc.u32 %1, %1, 0;\n\t"
+      "addc.cc.u32 %2, %2, 0;\n\t"
+      "addc.cc.u32 %3, %3, 0;\n\t"
+      "addc.cc.u32 %4, %4, 0;\n\t"
+      "addc.u32 %5, 0, 0;"
+      : "+r"(r[3]), "+r"(r[4]), "+r"(r[5]), "+r"(r[6]), "+r"(r[7]), "=r"(c));
+#else
+  uint64_t t = 1;
+  for (int i = 3; i < 8; i++) { t += r[i]; r[i] = (uint32_t)t; t >>= 32; }
+  c = (uint32_t)t;
+#endif
+  return c;
+}
+KGV_HD uint32_t dec_hi5(uint32_t* r) {
+  uint32_t bo;
+#if defined(__CUDACC__)
+  asm("sub.cc.u32 %0, %0, 1;\n\t"
+      "subc.cc.u32 %1, %1, 0;\n\t"
+      "subc.cc.u32 %2, %2, 0;\n\t"
+      "subc.cc.u32 %3, %3, 0;\n\t"
+      "subc.cc.u32 %4, %4, 0;\n\t"
+      "subc.u32 %5, 0, 0;"
+      : "+r"(r[3]), "+r"(r[4]), "+r"(r[5]), "+r"(r[6]), "+r"(r[7]), "=r"(bo));
+  bo &= 1u;
+#else
+  uint64_t br = 1;
+  for (int i = 3; i < 8; i++) {
+    uint64_t t = (uint64_t)r[i] - br;
+    r[i] = (uint32_t)t;
+    br = (t >> 32) & 1;
+  }
+  bo = (uint32_t)br;
+#endif
+  return bo;
+}
+
 // r += (a1:a0) where the carry almost never leaves limb 2: three-limb chain, the (probability 2^-32)
 // propagation through the upper limbs sits on a separate, normally untaken path.  Returns the carry out.
 KGV_HD uint32_t add_low2_rare(uint32_t* r, uint32_t a0, uint32_t a1) {
@@ -329,15 +371,7 @@ KGV_HD uint32_t add_low2_rare(uint32_t* r, uint32_t a0, uint32_t a1) {
   t += (uint64_t)r[2]; r[2] = (uint32_t)t; t >>= 32;
   c = (uint32_t)t;
 #endif
-  if (c) {
-    c = 0;
-#pragma unroll
-    for (int i = 3; i < 8; i++) {
-      r[i] += 1u;
-      if (r[i] != 0) break;
-      if (i == 7) c = 1;
-    }
-  }
+  if (c) c = inc_hi5(r);
   return c;
 }
 // r -= (a1:a0), same structure; returns the borrow out
@@ -357,16 +391,7 @@ KGV_HD uint32_t sub_low2_rare(uint32_t* r, uint32_t a0, uint32_t a1) {
   t = (uint64_t)r[2] - br; r[2] = (uint32_t)t; br = (t >> 32) & 1;
   bo = (uint32_t)br;
 #endif
-  if (bo) {
-    bo = 0;
-#pragma unroll
-    for (int i = 3; i < 8; i++) {
-      uint32_t old = r[i];
-      r[i] = old - 1u;
-      if (old != 0) break;
-      if (i == 7) bo = 1;
-    }
-  }
+  if (bo) bo = dec_hi5(r);
   return bo;
 }
 
@@ -389,6 +414,135 @@ KGV_HD void fe_neg(fe& r, const fe& a) {
 }
 
 KGV_HD void fe_dbl(fe& r, const fe& a) { fe_add(r, a, a); }
+
+// Wide accumulator for the additions around the group-law products: a 256-bit value plus a small signed multiple
+// of 2^256 (|top| < 2^20, two's complement).  A whole sum such as 2((X+B)^2 - A - C) is one carry chain per operand
+// into `top` and ONE fold (fe_fold) at the end, instead of a fold after every fe_add / fe_sub.
+struct fex {
+  uint32_t v[8];
+  uint32_t top;
+};
+KGV_HD void fex_set(fex& r, const fe& a) {
+#pragma unroll
+  for (int i = 0; i < 8; i++) r.v[i] = a.v[i];
+  r.top = 0;
+}
+// r += b
+KGV_HD void fex_add(fex& r, const fe& b) {
+#if defined(__CUDACC__)
+  asm("add.cc.u32 %0, %0, %9;\n\t"
+      "addc.cc.u32 %1, %1, %10;\n\t"
+      "addc.cc.u32 %2, %2, %11;\n\t"
+      "addc.cc.u32 %3, %3, %12;\n\t"
+      "addc.cc.u32 %4, %4, %13;\n\t"
+      "addc.cc.u32 %5, %5, %14;\n\t"
+      "addc.cc.u32 %6, %6, %15;\n\t"
+      "addc.cc.u32 %7, %7, %16;\n\t"
+      "addc.u32 %8, %8, 0;"
+      : "+r"(r.v[0]), "+r"(r.v[1]), "+r"(r.v[2]), "+r"(r.v[3]), "+r"(r.v[4]), "+r"(r.v[5]), "+r"(r.v[6]), "+r"(r.v[7]), "+r"(r.top)
+      : "r"(b.v[0]), "r"(b.v[1]), "r"(b.v[2]), "r"(b.v[3]), "r"(b.v[4]), "r"(b.v[5]), "r"(b.v[6]), "r"(b.v[7]));
+#else
+  uint64_t c = 0;
+  for (int i = 0; i < 8; i++) { c += (uint64_t)r.v[i] + b.v[i]; r.v[i] = (uint32_t)c; c >>= 32; }
+  r.top += (uint32_t)c;
+#endif
+}
+// r -= b
+KGV_HD void fex_sub(fex& r, const fe& b) {
+#if defined(__CUDACC__)
+  asm("sub.cc.u32 %0, %0, %9;\n\t"
+      "subc.cc.u32 %1, %1, %10;\n\t"
+      "subc.cc.u32 %2, %2, %11;\n\t"
+      "subc.cc.u32 %3, %3, %12;\n\t"
+      "subc.cc.u32 %4, %4, %13;\n\t"
+      "subc.cc.u32 %5, %5, %14;\n\t"
+      "subc.cc.u32 %6, %6, %15;\n\t"
+      "subc.cc.u32 %7, %7, %16;\n\t"
+      "subc.u32 %8, %8, 0;"
+      : "+r"(r.v[0]), "+r"(r.v[1]), "+r"(r.v[2]), "+r"(r.v[3]), "+r"(r.v[4]), "+r"(r.v[5]), "+r"(r.v[6]), "+r"(r.v[7]), "+r"(r.top)
+      : "r"(b.v[0]), "r"(b.v[1]), "r"(b.v[2]), "r"(b.v[3]), "r"(b.v[4]), "r"(b.v[5]), "r"(b.v[6]), "r"(b.v[7]));
+#else
+  uint64_t br = 0;
+  for (int i = 0; i < 8; i++) {
+    uint64_t t = (uint64_t)r.v[i] - b.v[i] - br;
+    r.v[i] = (uint32_t)t;
+    br = (t >> 32) & 1;
+  }
+  r.top -= (uint32_t)br;
+#endif
+}
+// r -= b, both wide
+KGV_HD void fex_sub_x(fex& r, const fex& b) {
+#if defined(__CUDACC__)
+  asm("sub.cc.u32 %0, %0, %9;\n\t"
+      "subc.cc.u32 %1, %1, %10;\n\t"
+      "subc.cc.u32 %2, %2, %11;\n\t"
+      "subc.cc.u32 %3, %3, %12;\n\t"
+      "subc.cc.u32 %4, %4, %13;\n\t"
+      "subc.cc.u32 %5, %5, %14;\n\t"
+      "subc.cc.u32 %6, %6, %15;\n\t"
+      "subc.cc.u32 %7, %7, %16;\n\t"
+      "subc.u32 %8, %8, %17;"
+      : "+r"(r.v[0]), "+r"(r.v[1]), "+r"(r.v[2]), "+r"(r.v[3]), "+r"(r.v[4]), "+r"(r.v[5]), "+r"(r.v[6]), "+r"(r.v[7]), "+r"(r.top)
+      : "r"(b.v[0]), "r"(b.v[1]), "r"(b.v[2]), "r"(b.v[3]), "r"(b.v[4]), "r"(b.v[5]), "r"(b.v[6]), "r"(b.v[7]), "r"(b.top));
+#else
+  uint64_t br = 0;
+  for (int i = 0; i < 8; i++) {
+    uint64_t t = (uint64_t)r.v[i] - b.v[i] - br;
+    r.v[i] = (uint32_t)t;
+    br = (t >> 32) & 1;
+  }
+  r.top = r.top - b.top - (uint32_t)br;
+#endif
+}
+// r <<= k, 1 <= k <= 3
+KGV_HD void fex_shl(fex& r, int k) {
+#if defined(__CUDACC__)
+  r.top = __funnelshift_l(r.v[7], r.top, k);
+#pragma unroll
+  for (int i = 7; i > 0; i--) r.v[i] = __funnelshift_l(r.v[i - 1], r.v[i], k);
+#else
+  r.top = (r.top << k) | (r.v[7] >> (32 - k));
+  for (int i = 7; i > 0; i--) r.v[i] = (r.v[i] << k) | (r.v[i - 1] >> (32 - k));
+#endif
+  r.v[0] <<= k;
+}
+// r = a mod p, weakly reduced: a.v + top * 2^256 == a.v + top * (2^32 + 977).  top * (2^32 + 977) is a signed 96-bit
+// addend (a0, a1, a2 sign-extended); after a three-limb chain the carry into limb 3 is -1, 0 or +1, and it is nonzero
+// with probability ~2^-32 per unit of |top|: that propagation (and the wrap past 2^256 it may cause) sits on an
+// untaken branch, like add_low2_rare.
+KGV_HD void fe_fold(fe& r, const fex& a) {
+  const int32_t top = (int32_t)a.top;
+  const int32_t s = top * 977;
+  const int32_t h = top + (s >> 31);  // top*C = (uint32)s + h * 2^32
+  const uint32_t a0 = (uint32_t)s, a1 = (uint32_t)h, a2 = (uint32_t)(h >> 31);
+#pragma unroll
+  for (int i = 0; i < 8; i++) r.v[i] = a.v[i];
+  uint32_t c;
+#if defined(__CUDACC__)
+  asm("add.cc.u32 %0, %0, %4;\n\t"
+      "addc.cc.u32 %1, %1, %5;\n\t"
+      "addc.cc.u32 %2, %2, %6;\n\t"
+      "addc.u32 %3, 0, 0;"
+      : "+r"(r.v[0]), "+r"(r.v[1]), "+r"(r.v[2]), "=r"(c)
+      : "r"(a0), "r"(a1), "r"(a2));
+#else
+  {
+    uint64_t t = (uint64_t)r.v[0] + a0; r.v[0] = (uint32_t)t; t >>= 32;
+    t += (uint64_t)r.v[1] + a1; r.v[1] = (uint32_t)t; t >>= 32;
+    t += (uint64_t)r.v[2] + a2; r.v[2] = (uint32_t)t; t >>= 32;
+    c = (uint32_t)t;
+  }
+#endif
+  const uint32_t net = c + a2;  // carry into limb 3 (a2 = 0xFFFFFFFF stands for -1): 0, 1 or 0xFFFFFFFF
+  if (net != 0) {  // past 2^256 the rest is tiny (+1) or within 2^40 of 2^256 (-1): +-C cannot wrap again
+    if (net == 1u) {
+      if (inc_hi5(r.v)) (void)add8_small3(r.v, 977u, 1u, 0u);
+    } else if (dec_hi5(r.v)) {
+      (void)sub8_small2(r.v, 977u, 1u);
+    }
+  }
+}
 
 // canonical representative in [0, p)
 KGV_HD void fe_normalize(fe& r) {
@@ -589,63 +743,6 @@ KGV_HD void fe_sqr(fe& r, const fe& a) {
   fe_reduce_wide(r, t);
 }
 #endif
-
-// Paired products: two INDEPENDENT field multiplications / squarings in one call.  The two carry-chain
-// streams have no data dependence, so ptxas interleaves them and the fixed-latency stalls of one stream are
-// filled by the other (the kernel runs only 3 warps per scheduler; ILP has to come from inside the warp).
-struct fe2 { fe a, b; };
-#if defined(__CUDACC__) && KGV_NOINLINE_MUL
-static __device__ __noinline__ fe2 fe_mul2_call(fe a1, fe b1, fe a2, fe b2) {
-  fe2 r;
-  uint32_t t1[16], t2[16];
-  mul_wide(t1, a1.v, b1.v);
-  mul_wide(t2, a2.v, b2.v);
-  fe_reduce_wide(r.a, t1);
-  fe_reduce_wide(r.b, t2);
-  return r;
-}
-static __device__ __noinline__ fe2 fe_sqr2_call(fe a1, fe a2) {
-  fe2 r;
-  uint32_t t1[16], t2[16];
-  sqr_wide(t1, a1.v);
-  sqr_wide(t2, a2.v);
-  fe_reduce_wide(r.a, t1);
-  fe_reduce_wide(r.b, t2);
-  return r;
-}
-static __device__ __noinline__ fe2 fe_mulsqr_call(fe a1, fe b1, fe a2) {
-  fe2 r;
-  uint32_t t1[16], t2[16];
-  mul_wide(t1, a1.v, b1.v);
-  sqr_wide(t2, a2.v);
-  fe_reduce_wide(r.a, t1);
-  fe_reduce_wide(r.b, t2);
-  return r;
-}
-// r1 = a1*b1, r2 = a2*b2
-KGV_HD void fe_mul2(fe& r1, const fe& a1, const fe& b1, fe& r2, const fe& a2, const fe& b2) { fe2 r = fe_mul2_call(a1, b1, a2, b2); r1 = r.a; r2 = r.b; }
-// r1 = a1^2, r2 = a2^2
-KGV_HD void fe_sqr2(fe& r1, const fe& a1, fe& r2, const fe& a2) { fe2 r = fe_sqr2_call(a1, a2); r1 = r.a; r2 = r.b; }
-// r1 = a1*b1, r2 = a2^2
-KGV_HD void fe_mulsqr(fe& r1, const fe& a1, const fe& b1, fe& r2, const fe& a2) { fe2 r = fe_mulsqr_call(a1, b1, a2); r1 = r.a; r2 = r.b; }
-#else
-KGV_HD void fe_mul2(fe& r1, const fe& a1, const fe& b1, fe& r2, const fe& a2, const fe& b2) { fe x, y; fe_mul(x, a1, b1); fe_mul(y, a2, b2); r1 = x; r2 = y; }
-KGV_HD void fe_sqr2(fe& r1, const fe& a1, fe& r2, const fe& a2) { fe x, y; fe_sqr(x, a1); fe_sqr(y, a2); r1 = x; r2 = y; }
-KGV_HD void fe_mulsqr(fe& r1, const fe& a1, const fe& b1, fe& r2, const fe& a2) { fe x, y; fe_mul(x, a1, b1); fe_sqr(y, a2); r1 = x; r2 = y; }
-#endif
-
-// always-inlined forms: used INSIDE the (non-inlined) point operations when KGV_INLINE_MUL_IN_POINT is set, so that no
-// by-value call ABI (16-24 register moves per product) sits between the products of one group-law formula
-KGV_HD void fe_mul_inl(fe& r, const fe& a, const fe& b) {
-  uint32_t t[16];
-  mul_wide(t, a.v, b.v);
-  fe_reduce_wide(r, t);
-}
-KGV_HD void fe_sqr_inl(fe& r, const fe& a) {
-  uint32_t t[16];
-  sqr_wide(t, a.v);
-  fe_reduce_wide(r, t);
-}
 
 // r = a^(2^n).  KGV_SQRN_CALL=1 makes a whole run of squarings ONE call (the squaring inlined into the loop of a non-inlined function: the
 // exponentiation chains - square root of lift_x, the shared inversion, ~510 squarings per verification - then pay the by-value call ABI once per

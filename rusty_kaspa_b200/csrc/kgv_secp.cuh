@@ -30,11 +30,6 @@ namespace kgv {
 #define KGV_MB1_LIMBS {0x0ABFE4C3u, 0x6F547FA9u, 0x010E8828u, 0xE4437ED6u, 0u}
 #define KGV_A2_LIMBS {0x9D44CFD8u, 0x57C1108Du, 0xA8E2F3F6u, 0x14CA50F7u, 1u}
 
-#ifndef KGV_PAIRED_MUL
-#define KGV_PAIRED_MUL 0   // 1: issue independent field products of the group law in pairs (fe_mul2). Measured slower when the kernels
-                           // were tuned on the previous target GPU (argument moves + spills outweigh the extra ILP); not re-measured on H100.
-#endif
-
 struct gej {
   fe x, y, z;
   bool inf;
@@ -393,167 +388,118 @@ KGV_HD void recoded_digit(const uint32_t* h, int i, uint32_t& idx, bool& neg) {
 // group law, Jacobian coordinates on y^2 = x^3 + b (a = 0; b never appears in the formulas,
 // so the same code runs on the isomorphic curves used for the per-thread tables)
 // ------------------------------------------------------------------------------------------
-#ifndef KGV_INLINE_MUL_IN_POINT
-#define KGV_INLINE_MUL_IN_POINT 0  // 1: the field products inside gej_double / gej_add_ge are inlined into those (non-inlined) functions
-#endif
-#if defined(__CUDACC__) && KGV_INLINE_MUL_IN_POINT
-#define FE_PMUL fe_mul_inl
-#define FE_PSQR fe_sqr_inl
-#else
-#define FE_PMUL fe_mul
-#define FE_PSQR fe_sqr
-#endif
+// r = 2r for a finite r (callers test r.inf).  Each sum between the products is one wide accumulator (fex) with a
+// single fold (fe_fold) at the end.
 KGV_HD void gej_double_body(gej& r) {
-  if (r.inf) return;
-  fe A, B, C, D, E, F, t, yz;
-#if KGV_PAIRED_MUL
-  fe_sqr2(A, r.x, B, r.y);       // A = X^2, B = Y^2
+  fe A, B, C, D, E, t;
+  fex w, c8;
+  fe_sqr(A, r.x);
+  fe_sqr(B, r.y);
+  fe_sqr(C, B);
   fe_add(t, r.x, B);
-  fe_sqr2(C, B, t, t);           // C = Y^4, t = (X+B)^2
-  fe_sub(t, t, A);
-  fe_sub(t, t, C);
-  fe_dbl(D, t);                  // D = 4 X Y^2
-  fe_mul3(E, A);                 // E = 3 X^2
-  fe_mulsqr(yz, r.y, r.z, F, E); // Y*Z, E^2
-  fe_dbl(r.z, yz);               // Z3 = 2 Y Z
-  fe_sub(t, F, D);
-  fe_sub(r.x, t, D);             // X3 = E^2 - 2D
+  fe_sqr(t, t);
+  fex_set(w, t); fex_sub(w, A); fex_sub(w, C); fex_shl(w, 1);
+  fe_fold(D, w);                        // D = 2((X+B)^2 - A - C) = 4 X Y^2
+  fex_set(w, A); fex_shl(w, 1); fex_add(w, A);
+  fe_fold(E, w);                        // E = 3 X^2
+  fe_mul(t, r.y, r.z);
+  fex_set(w, t); fex_shl(w, 1);
+  fe_fold(r.z, w);                      // Z3 = 2 Y Z
+  fe_sqr(t, E);
+  fex_set(w, t); fex_sub(w, D); fex_sub(w, D);
+  fe_fold(r.x, w);                      // X3 = E^2 - 2D
   fe_sub(t, D, r.x);
-  FE_PMUL(t, E, t);
-  fe_mul8(C, C);
-  fe_sub(r.y, t, C);             // Y3 = E (D - X3) - 8 Y^4
-#else
-  FE_PSQR(A, r.x);
-  FE_PSQR(B, r.y);
-  FE_PSQR(C, B);
-  fe_add(t, r.x, B);
-  FE_PSQR(t, t);
-  fe_sub(t, t, A);
-  fe_sub(t, t, C);
-  fe_dbl(D, t);        // D = 2((X+B)^2 - A - C) = 4 X Y^2
-  fe_mul3(E, A);       // E = 3 X^2
-  FE_PMUL(r.z, r.y, r.z);
-  fe_dbl(r.z, r.z);    // Z3 = 2 Y Z
-  FE_PSQR(t, E);
-  fe_sub(t, t, D);
-  fe_sub(r.x, t, D);   // X3 = E^2 - 2D
-  fe_sub(t, D, r.x);
-  FE_PMUL(t, E, t);
-  fe_mul8(C, C);
-  fe_sub(r.y, t, C);   // Y3 = E (D - X3) - 8 Y^4
-  (void)F; (void)yz;
-#endif
+  fe_mul(t, E, t);
+  fex_set(c8, C); fex_shl(c8, 3);
+  fex_set(w, t); fex_sub_x(w, c8);
+  fe_fold(r.y, w);                      // Y3 = E (D - X3) - 8 Y^4
 }
 
-#ifndef KGV_NOINLINE_POINT
-#define KGV_NOINLINE_POINT 1
-#endif
-#if defined(__CUDACC__) && KGV_NOINLINE_POINT
-static __device__ __noinline__ gej gej_double_call(gej r) { gej_double_body(r); return r; }
-KGV_HD void gej_double(gej& r) { r = gej_double_call(r); }
-#else
-KGV_HD void gej_double(gej& r) { gej_double_body(r); }
-#endif
-
-// r += (bx,by) with the addend affine and never the point at infinity.  Handles r = inf,
-// r == addend (doubling) and r == -addend (result infinity).  If hout != nullptr it receives
-// the factor by which Z was multiplied (H), used by the table builder.
-KGV_HD void gej_add_ge_body(gej& r, const fe& bx, const fe& by, fe* hout) {
+// r += (bx,by) with the addend affine and never the point at infinity.  Handles r = inf and r == -addend (result
+// infinity); for r == addend it leaves r as it is and returns true: the caller doubles r.  If hout != nullptr it
+// receives the factor by which Z was multiplied (H), used by the table builder.
+KGV_HD bool gej_add_ge_body(gej& r, const fe& bx, const fe& by, fe* hout) {
   if (r.inf) {
     r.x = bx;
     r.y = by;
     fe_set_u32(r.z, 1);
     r.inf = false;
     if (hout) fe_set_u32(*hout, 1);
-    return;
+    return false;
   }
   fe z1z1, u2, s2, h, rr, t;
-  FE_PSQR(z1z1, r.z);
-#if KGV_PAIRED_MUL
-  fe_mul2(u2, bx, z1z1, t, r.z, z1z1);
-#else
-  FE_PMUL(u2, bx, z1z1);
-  FE_PMUL(t, r.z, z1z1);
-#endif
-  FE_PMUL(s2, by, t);
+  fe_sqr(z1z1, r.z);
+  fe_mul(u2, bx, z1z1);
+  fe_mul(t, r.z, z1z1);
+  fe_mul(s2, by, t);
   fe_sub(h, u2, r.x);
   fe_sub(rr, s2, r.y);
   if (fe_is_zero(h)) {
+    if (fe_is_zero(rr)) return true;
     if (hout) fe_set_u32(*hout, 1);
-    if (fe_is_zero(rr)) {
-#if KGV_INLINE_MUL_IN_POINT
-      gej_double(r);                 // rare path: through the (non-inlined) doubling, not a second inlined copy of five products
-#else
-      gej_double_body(r);            // inlined: a CALL here would make gej_add_ge_call a non-leaf function (return-address / register saves
-                                     // on EVERY addition: +1.6 % instructions, -2.5 % throughput, measured in round 2)
-#endif
-      if (hout) fe_dbl(*hout, r.y);  // not used by the table builder (cannot happen there)
-    } else {
-      r.inf = true;
-    }
-    return;
+    r.inf = true;
+    return false;
   }
   if (hout) *hout = h;
   fe hh, hhh, v;
-#if KGV_PAIRED_MUL
-  fe y1h3;
-  fe_mulsqr(r.z, r.z, h, hh, h);          // Z3 = Z1*H, HH = H^2
-  fe_mul2(hhh, hh, h, v, r.x, hh);        // H^3, V = X1*HH
-  fe_mulsqr(y1h3, r.y, hhh, t, rr);       // Y1*H^3, R^2
-  fe_sub(t, t, hhh);
-  fe_sub(t, t, v);
-  fe_sub(r.x, t, v);                      // X3 = R^2 - H^3 - 2V
+  fex w;
+  fe_sqr(hh, h);
+  fe_mul(hhh, hh, h);
+  fe_mul(v, r.x, hh);
+  fe_mul(r.z, r.z, h);
+  fe_sqr(t, rr);
+  fex_set(w, t); fex_sub(w, hhh); fex_sub(w, v); fex_sub(w, v);
+  fe_fold(r.x, w);        // X3 = R^2 - H^3 - 2V
   fe_sub(t, v, r.x);
-  FE_PMUL(t, rr, t);
-  fe_sub(r.y, t, y1h3);                   // Y3 = R (V - X3) - Y1 H^3
-#else
-  FE_PSQR(hh, h);
-  FE_PMUL(hhh, hh, h);
-  FE_PMUL(v, r.x, hh);
-  FE_PMUL(r.z, r.z, h);
-  FE_PSQR(t, rr);
-  fe_sub(t, t, hhh);
-  fe_sub(t, t, v);
-  fe_sub(r.x, t, v);      // X3 = R^2 - H^3 - 2V
-  fe_sub(t, v, r.x);
-  FE_PMUL(t, rr, t);
-  FE_PMUL(hhh, r.y, hhh);
+  fe_mul(t, rr, t);
+  fe_mul(hhh, r.y, hhh);
   fe_sub(r.y, t, hhh);    // Y3 = R (V - X3) - Y1 H^3
-#endif
+  return false;
 }
 
-// KGV_ADD_ONE_BLOCK (default): ONE copy of the mixed addition in the kernel.  The table builder needs the addition's H value and used to get
-// it from an INLINED body - seven unrolled copies, ~160 KB of straight-line code that every signature streamed through once, evicting the
-// ladder's hot code from the instruction cache (DESIGN.md §4 K1).  Now the one non-inlined function always returns H as well (8 more
-// registers by value, ignored by the ladder).
-#ifndef KGV_ADD_ONE_BLOCK
-#define KGV_ADD_ONE_BLOCK 1
+// On the device the whole group law is ONE non-inlined function taking and returning the point by value:
+//  * n > 0: r = 2^n r - the ladder's four doublings per window cross the call ABI once, with r in registers;
+//  * n == 0: r += (bx,by), also returning H (the table builder needs it; it used to take it from an INLINED body:
+//    seven unrolled copies, ~160 KB of straight-line code that evicted the ladder's hot code, DESIGN.md §4 K1).
+//    The rare r == addend case falls through into the same doubling loop: no second copy of the doubling, no call.
+// The point at infinity is tested by the caller of a doubling, once per call, not inside the doubling.
+#ifndef KGV_NOINLINE_POINT
+#define KGV_NOINLINE_POINT 1
 #endif
-#if defined(__CUDACC__) && KGV_NOINLINE_POINT && KGV_ADD_ONE_BLOCK
+#if defined(__CUDACC__) && KGV_NOINLINE_POINT
 struct gej_h { gej r; fe h; };
-static __device__ __noinline__ gej_h gej_add_ge_call(gej r, fe bx, fe by) { gej_h o; gej_add_ge_body(r, bx, by, &o.h); o.r = r; return o; }
+static __device__ __noinline__ gej_h gej_point_call(gej r, fe bx, fe by, int n) {
+  gej_h o;
+  if (n == 0 && gej_add_ge_body(r, bx, by, &o.h)) {
+    fe_dbl(o.h, r.y);  // Z3 = 2 Y1 Z1 (cannot happen in the table builder)
+    n = 1;
+  }
+#pragma unroll 1
+  for (int i = 0; i < n; i++) gej_double_body(r);
+  o.r = r;
+  return o;
+}
+KGV_HD void gej_double_n(gej& r, int n) {
+  if (!r.inf) r = gej_point_call(r, r.x, r.y, n).r;  // (bx, by unused)
+}
 KGV_HD void gej_add_ge(gej& r, const fe& bx, const fe& by, fe* hout = nullptr) {
-  gej_h o = gej_add_ge_call(r, bx, by);
+  gej_h o = gej_point_call(r, bx, by, 0);
   r = o.r;
   if (hout) *hout = o.h;
 }
-#elif defined(__CUDACC__) && KGV_NOINLINE_POINT
-static __device__ __noinline__ gej gej_add_ge_call(gej r, fe bx, fe by) { gej_add_ge_body(r, bx, by, nullptr); return r; }
-#if KGV_INLINE_MUL_IN_POINT
-struct gej_h { gej r; fe h; };
-static __device__ __noinline__ gej_h gej_add_ge_h_call(gej r, fe bx, fe by) { gej_h o; gej_add_ge_body(r, bx, by, &o.h); o.r = r; return o; }
-#endif
-KGV_HD void gej_add_ge(gej& r, const fe& bx, const fe& by, fe* hout = nullptr) {
-#if KGV_INLINE_MUL_IN_POINT
-  if (hout) { gej_h o = gej_add_ge_h_call(r, bx, by); r = o.r; *hout = o.h; }
 #else
-  if (hout) gej_add_ge_body(r, bx, by, hout);
-#endif
-  else r = gej_add_ge_call(r, bx, by);
+KGV_HD void gej_double_n(gej& r, int n) {
+  if (r.inf) return;
+  for (int i = 0; i < n; i++) gej_double_body(r);
 }
-#else
-KGV_HD void gej_add_ge(gej& r, const fe& bx, const fe& by, fe* hout = nullptr) { gej_add_ge_body(r, bx, by, hout); }
+KGV_HD void gej_add_ge(gej& r, const fe& bx, const fe& by, fe* hout = nullptr) {
+  if (gej_add_ge_body(r, bx, by, hout)) {
+    if (hout) fe_dbl(*hout, r.y);
+    gej_double_n(r, 1);
+  }
+}
 #endif
+KGV_HD void gej_double(gej& r) { gej_double_n(r, 1); }
 
 // y^2 = x^3 + 7: solve for y with the requested parity.  false if x is not on the curve.
 // x must be canonical (< p).
@@ -650,9 +596,7 @@ KGV_HD void ecmult_double(gej& R, fe& zs, const fe& px, const fe& py, const uint
   R.inf = true;
   fe_set_zero(R.x); fe_set_zero(R.y); fe_set_zero(R.z);
   for (int i = 32; i >= 0; i--) {
-    if (i != 32) {
-      gej_double(R); gej_double(R); gej_double(R); gej_double(R);
-    }
+    if (i != 32) gej_double_n(R, 4);
     uint32_t idx; bool dn;
     fe ex, ey;
     // k1 digit on P
