@@ -256,6 +256,40 @@ int kgv_utxo_view_create(kgv_ctx* ctx, kgv_utxo_table* base, uint64_t capacity_s
 int kgv_utxo_view_commit(kgv_ctx* ctx, kgv_utxo_table* view);
 int kgv_utxo_view_discard(kgv_ctx* ctx, kgv_utxo_table* view);
 
+/* Table maintenance.  An erase leaves a tombstone and a probe for an absent key ends only at an EMPTY slot, so a table that churns for long
+ * slows down every lookup that misses and every insert until it is rebuilt; long scripts are appended to the overflow arena and their bytes
+ * are only reclaimed by a rebuild.  All three calls work on plain tables and on view layers (a layer alone, never the layers below it). */
+typedef struct {
+  uint64_t capacity_slots;
+  uint64_t live;              /* entries (in a view layer: also its removal markers) */
+  uint64_t tombstones;
+  uint64_t empty;             /* EMPTY slots */
+  uint64_t overflow_used;     /* bytes appended to the long-script arena (8-byte padded) */
+  uint64_t overflow_cap;
+  uint64_t overflow_live;     /* of those, the bytes the live entries' scripts occupy (= overflow_used right after a rehash) */
+  uint64_t insert_failures;   /* entries lost to a full table or arena since the table was created (never reset) */
+  uint64_t rehashes;          /* times this handle was rebuilt */
+  uint64_t max_displacement;  /* over the entries: (slot - home slot) mod capacity */
+  uint64_t sum_displacement;
+  uint64_t longest_run;       /* longest circular run of non-EMPTY slots: the probes of the worst lookup that misses */
+} kgv_utxo_table_stats; /* 96 bytes */
+/* One pass over the slots; synchronises the context's stream. */
+int kgv_utxo_stats(kgv_ctx* ctx, kgv_utxo_table* t, kgv_utxo_table_stats* out);
+/* Rebuild out of place into capacity_slots (0: the current capacity; else rounded up to a power of two, so the table can grow or shrink):
+ * tombstones are dropped and the long-script arena is compacted; entries, count and digest stay as they are, insert_failures too.
+ * A capacity below live + 1 gives KGV_ERR_ARG, a failed allocation KGV_ERR_NOMEM; either leaves the table untouched.  The old and the new
+ * arrays exist side by side during the call; the old ones are released at the next kgv_synchronize (or when an allocation needs the memory).
+ * View layers above the table keep working.  A rehash ends the window kgv_replay_muhash refers to (call that first). */
+int kgv_utxo_rehash(kgv_ctx* ctx, kgv_utxo_table* t, uint64_t capacity_slots);
+/* Growth policy, off (0) by default.  With 1..900 every call that writes to `t` (kgv_utxo_apply_diff, kgv_utxo_import_chunk,
+ * kgv_utxo_apply_accepted, kgv_replay_window, and kgv_utxo_view_commit for the base) first makes room: when its entries would pass
+ * max_load_permille of the capacity the table grows to the smallest power of two that keeps them at half that load; when entries plus
+ * tombstones would, or the arena cannot take the call's long scripts, it is rehashed at its size.  It never shrinks.  The check keeps an
+ * upper bound of the occupied slots on the host and reads the device counters (one synchronisation) only when that bound reaches the
+ * threshold.  The byte bound of a batch call assumes its scripts are disjoint ranges of its byte arena.  A failed growth makes the
+ * writing call return KGV_ERR_NOMEM before it writes anything. */
+int kgv_utxo_set_max_load(kgv_ctx* ctx, kgv_utxo_table* t, uint32_t max_load_permille);
+
 /* validate_transactions_in_parallel (utxo_validation.rs:262-278) against the table: populate every input
  * by table lookup (:319-327), then as kgv_validate_populated.  batch->entries is ignored.
  * Unlike kgv_validate_populated this call never reports KGV_TX_NEEDS_HOST_VM: transactions with non-standard scripts are

@@ -364,6 +364,10 @@ class UtxoSet {
     c_.check(kgv_utxo_apply_accepted(c_.get(), h_, &v, accept.data(), pov_daa_score));
   }
   uint64_t count() { uint64_t n = 0; c_.check(kgv_utxo_count(c_.get(), h_, &n)); return n; }
+  // maintenance: the table's state, an out-of-place rebuild (capacity 0 = same size), the opt-in growth policy (permille, 0 = off)
+  kgv_utxo_table_stats stats() { kgv_utxo_table_stats s{}; c_.check(kgv_utxo_stats(c_.get(), h_, &s)); return s; }
+  void rehash(uint64_t capacity_slots = 0) { c_.check(kgv_utxo_rehash(c_.get(), h_, capacity_slots)); }
+  void set_max_load(uint32_t max_load_permille) { c_.check(kgv_utxo_set_max_load(c_.get(), h_, max_load_permille)); }
   // DbUtxoSetStore::iterator (consensus/src/model/stores/utxo_set.rs:114-129): every live entry, in the table's (arbitrary) order
   std::vector<std::pair<TransactionOutpoint, UtxoEntry>> iterator() {
     size_t n = 0, nb = 0;

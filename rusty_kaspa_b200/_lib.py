@@ -36,6 +36,9 @@ SYMBOLS = [
     ("kgv_utxo_view_create", _c.c_int, [_c.c_void_p, _c.c_void_p, _c.c_uint64, _c.POINTER(_c.c_void_p)]),
     ("kgv_utxo_view_commit", _c.c_int, [_c.c_void_p, _c.c_void_p]),
     ("kgv_utxo_view_discard", _c.c_int, [_c.c_void_p, _c.c_void_p]),
+    ("kgv_utxo_stats", _c.c_int, [_c.c_void_p, _c.c_void_p, _c.c_void_p]),
+    ("kgv_utxo_rehash", _c.c_int, [_c.c_void_p, _c.c_void_p, _c.c_uint64]),
+    ("kgv_utxo_set_max_load", _c.c_int, [_c.c_void_p, _c.c_void_p, _c.c_uint32]),
     ("kgv_utxo_lookup", _c.c_int, [_c.c_void_p, _c.c_void_p, _u8p, _c.c_size_t, _u8p, _u8p, _c.c_uint32, _u8p]),
     ("kgv_utxo_apply_diff", _c.c_int, [_c.c_void_p, _c.c_void_p, _u8p, _c.c_size_t, _u8p, _u8p, _u8p, _u8p, _c.c_size_t, _c.c_size_t, _u8p]),
     ("kgv_utxo_count", _c.c_int, [_c.c_void_p, _c.c_void_p, _c.POINTER(_c.c_uint64)]),

@@ -76,6 +76,8 @@ struct kgv_ctx {
 };
 
 int kgv_ptr_is_device(const void* p);
+// cudaMalloc; under memory pressure the parked buffers are given back (after synchronising the context's streams) and the allocation retried
+int kgv_malloc(kgv_ctx* ctx, void** p, size_t bytes);
 int kgv_reserve(kgv_ctx* ctx, uint8_t** buf, size_t* cap, size_t need);
 
 // ---- transaction batches on the device (kgv_hash.cu) ----
@@ -110,6 +112,10 @@ int kgv_mu_canonicalize(kgv_ctx* ctx, uint32_t* vals, size_t pitch_words, size_t
 
 // ---- shared pieces of the validation path (kgv_validate.cu) ----
 struct kgv_utxo_table;
+// Growth policy of a table (kgv_utxo_set_max_load, kgv_utxo_maint.cu): called by every table writer before it writes.  m bounds the slots the
+// call can newly occupy, b the long-script bytes it can append.  Returns at once when the policy is off; otherwise it may rehash the table
+// (KGV_ERR_NOMEM when that fails: the caller returns before writing anything).
+int utxo_reserve(kgv_ctx* ctx, kgv_utxo_table* t, uint64_t m, uint64_t b);
 
 // ---- multi-GPU exchange used by the sharded script phase (kgv_comm.cu) ----
 // Every rank contributes `per` bytes at buf + rank * per (device memory, n_ranks * per bytes in all); on return (stream order)

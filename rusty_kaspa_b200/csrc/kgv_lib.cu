@@ -309,21 +309,27 @@ int kgv_ptr_is_device(const void* p) {
 // peer-exchange wait kernels of kgv_comm.cu); cudaMallocAsync was tried and blocks in the same situation (measured).  Outgrown buffers are
 // parked and released by kgv_synchronize / kgv_destroy, i.e. at points where the caller has declared the context idle.  Growth is
 // geometric (x1.25), so the parked memory stays below ~4x the live buffer.
-int kgv_reserve(kgv_ctx* ctx, uint8_t** buf, size_t* cap, size_t need) {
-  if (*cap >= need) return KGV_OK;
-  if (*buf) { ctx->parked.push_back(*buf); *buf = nullptr; *cap = 0; }
-  size_t want = need + need / 4 + 4096;
-  cudaError_t e = cudaMalloc((void**)buf, want);
+int kgv_malloc(kgv_ctx* ctx, void** p, size_t bytes) {
+  cudaError_t e = cudaMalloc(p, bytes);
   if (e != cudaSuccess) {
     // memory pressure: now it is worth a device synchronisation to give the parked buffers back and try again
     (void)cudaGetLastError();
     cudaStreamSynchronize(ctx->stream);
     cudaStreamSynchronize(ctx->aux_stream);
-    for (uint8_t* p : ctx->parked) cudaFree(p);
+    for (uint8_t* q : ctx->parked) cudaFree(q);
     ctx->parked.clear();
-    e = cudaMalloc((void**)buf, want);
+    e = cudaMalloc(p, bytes);
   }
-  if (e != cudaSuccess) { ctx->err = std::string("cudaMalloc failed: ") + cudaGetErrorString(e); (void)cudaGetLastError(); *buf = nullptr; return KGV_ERR_NOMEM; }
+  if (e != cudaSuccess) { ctx->err = std::string("cudaMalloc failed: ") + cudaGetErrorString(e); (void)cudaGetLastError(); *p = nullptr; return KGV_ERR_NOMEM; }
+  return KGV_OK;
+}
+
+int kgv_reserve(kgv_ctx* ctx, uint8_t** buf, size_t* cap, size_t need) {
+  if (*cap >= need) return KGV_OK;
+  if (*buf) { ctx->parked.push_back(*buf); *buf = nullptr; *cap = 0; }
+  size_t want = need + need / 4 + 4096;
+  int rc = kgv_malloc(ctx, (void**)buf, want);
+  if (rc) return rc;
   *cap = want;
   return KGV_OK;
 }

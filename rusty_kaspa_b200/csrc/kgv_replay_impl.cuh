@@ -856,8 +856,10 @@ extern "C" int kgv_replay_window(kgv_ctx* ctx, kgv_utxo_table* table, const kgv_
     if (at != batch->n_txs) { ctx->err = "replay blocks do not cover the batch"; return KGV_ERR_ARG; }
   }
   CK(cudaSetDevice(ctx->device));
+  int rc = utxo_reserve(ctx, table, batch->n_outputs + (table->base ? batch->n_inputs : 0), batch->n_bytes + 8 * (uint64_t)batch->n_outputs);
+  if (rc) return rc;
   kgv_dev_batch d;
-  int rc = kgv_batch_to_device(ctx, batch, &d, false);
+  rc = kgv_batch_to_device(ctx, batch, &d, false);
   if (rc) return rc;
   const size_t nt = d.n_txs, ni = d.n_inputs, no = d.n_outputs;
   uint64_t wm_cap = 1024;

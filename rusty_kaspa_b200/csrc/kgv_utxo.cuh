@@ -37,13 +37,18 @@ static_assert(sizeof(UtxoSlot) == 128, "slot must be one 128-byte line");
 struct kgv_utxo_table {
   UtxoSlot* slots = nullptr;
   uint64_t mask = 0;             // capacity - 1
-  uint8_t* overflow = nullptr;   // long scripts (append-only: offsets stay valid for the life of the table)
+  uint8_t* overflow = nullptr;   // long scripts (append-only between rehashes: offsets stay valid until kgv_utxo_rehash compacts the arena)
   uint64_t overflow_cap = 0;
   unsigned long long* counters = nullptr;  // [0] live entries, [1] tombstones, [2] overflow bytes used, [3] insert failures, [8..15] digest scratch
   // Composed views (consensus/core/src/utxo/utxo_view.rs:22-35: ComposedUtxoView = base view + UtxoDiff, nesting arbitrarily): a table with
   // base != nullptr is a DIFF LAYER over `base`; lookups probe it first and fall through, writes go to it and never touch what lies below.
   kgv_utxo_table* base = nullptr;
   struct TableView* d_view = nullptr;  // this table's TableView in device memory (what an upper layer's `below` points to)
+  // maintenance (kgv_utxo_maint.cu)
+  uint64_t rehashes = 0;
+  uint32_t max_load = 0;         // growth policy in permille of the capacity, 0 = off
+  uint64_t occ_bound = 0;        // with the policy on: upper bounds of the non-EMPTY slots and of counters[2] (exact at the last read + every
+  uint64_t arena_bound = 0;      // write's reservation since), so that most writes need no counter read
 };
 
 struct TableView {

@@ -529,12 +529,20 @@ __global__ void k_view_commit_adds(TableView top, TableView below) {
 static int view_clear(kgv_ctx* ctx, kgv_utxo_table* v) {
   CK(cudaMemsetAsync(v->slots, 0, (v->mask + 1) * sizeof(UtxoSlot), ctx->stream));
   CK(cudaMemsetAsync(v->counters, 0, 16 * sizeof(unsigned long long), ctx->stream));
+  v->occ_bound = v->arena_bound = 0;
   return KGV_OK;
 }
 extern "C" int kgv_utxo_view_commit(kgv_ctx* ctx, kgv_utxo_table* view) {
   if (!ctx || !view || !view->base) return KGV_ERR_ARG;
   std::lock_guard<std::recursive_mutex> g(ctx->mu);
   CK(cudaSetDevice(ctx->device));
+  if (view->base->max_load) {  // the base takes at most the layer's entries and its long scripts
+    unsigned long long c[3];
+    CK(cudaMemcpyAsync(c, view->counters, sizeof c, cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+    int rc = utxo_reserve(ctx, view->base, c[0], c[2]);
+    if (rc) return rc;
+  }
   TableView top = view_of(view), below = view_of(view->base);
   k_view_commit_removes<<<nblk(view->mask + 1, 128), 128, 0, ctx->stream>>>(top, below);
   CK(cudaGetLastError());
@@ -605,6 +613,10 @@ extern "C" int kgv_utxo_apply_diff(kgv_ctx* ctx, kgv_utxo_table* t, const uint8_
   CK(cudaSetDevice(ctx->device));
   const void* probe = n_rem ? (const void*)rem_keys36 : (const void*)add_keys36;
   if (!probe) return KGV_OK;
+  {  // a view layer records a removal marker for an entry that lives below
+    int rc = utxo_reserve(ctx, t, n_add + (t->base ? n_rem : 0), n_add_bytes + 8 * (uint64_t)n_add);
+    if (rc) return rc;
+  }
   bool dev = kgv_ptr_is_device(probe);
   size_t o_rk = 0, o_ak = al256(n_rem * 36), o_ae = al256(o_ak + n_add * 36), o_ab = al256(o_ae + n_add * sizeof(kgv_utxo_entry));
   size_t o_rs = 0, o_as = al256(n_rem);
@@ -1078,8 +1090,10 @@ extern "C" int kgv_utxo_apply_accepted(kgv_ctx* ctx, kgv_utxo_table* t, const kg
   if (!batch || (batch->n_txs && !accept)) { ctx->err = "null argument"; return KGV_ERR_ARG; }
   if (batch->n_txs == 0) return KGV_OK;
   CK(cudaSetDevice(ctx->device));
+  int rc = utxo_reserve(ctx, t, batch->n_outputs + (t->base ? batch->n_inputs : 0), batch->n_bytes + 8 * (uint64_t)batch->n_outputs);
+  if (rc) return rc;
   kgv_dev_batch d;
-  int rc = kgv_batch_to_device(ctx, batch, &d, false);
+  rc = kgv_batch_to_device(ctx, batch, &d, false);
   if (rc) return rc;
   size_t nt = d.n_txs, ni = d.n_inputs, no = d.n_outputs;
   size_t o_itx = 0, o_otx = al256(ni * 4), o_ids = al256(o_otx + no * 4), o_acc = al256(o_ids + nt * 32);

@@ -49,10 +49,13 @@ class DagReplayer:
     selected parent of each mergeset with ACCEPT_COINBASE | SKIP_SCRIPTS and gives all merged blocks the chain block's
     pov_daa_score (tests/test_gpu_replay.py replays the reference's simpa fixtures that way)."""
 
-    def __init__(self, ctx, params, capacity_slots=1 << 20):
+    def __init__(self, ctx, params, capacity_slots=1 << 20, max_load=None):
+        """max_load: growth policy of the UTXO table in permille (GpuUtxoSet.set_max_load); None keeps the table at capacity_slots"""
         self.ctx = ctx
         self.tv = TransactionValidator(ctx, params)
         self.us = GpuUtxoSet(ctx, capacity_slots)
+        if max_load is not None:
+            self.us.set_max_load(max_load)
         self.last_stats = None
 
     def close(self):

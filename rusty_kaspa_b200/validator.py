@@ -64,6 +64,15 @@ def script_execute(batch, tx, input_index, verdict=None):
     return int(err.value)
 
 
+class UtxoTableStats(ctypes.Structure):
+    """kgv_utxo_table_stats"""
+    _fields_ = [(n, ctypes.c_uint64) for n in ("capacity_slots", "live", "tombstones", "empty", "overflow_used", "overflow_cap", "overflow_live",
+                                               "insert_failures", "rehashes", "max_displacement", "sum_displacement", "longest_run")]
+
+
+assert ctypes.sizeof(UtxoTableStats) == 96
+
+
 class GpuUtxoSet:
     """GPU-resident UTXO set (kgv_utxo_table)."""
 
@@ -134,6 +143,21 @@ class GpuUtxoSet:
         out = (ctypes.c_uint8 * 32)()
         self.ctx._check(self._lib.kgv_utxo_digest(self.ctx._h, self._h, ctypes.addressof(out)))
         return bytes(out)
+
+    # ---- maintenance: churn leaves tombstones and dead arena bytes behind; a rehash drops them
+    def stats(self):
+        """kgv_utxo_stats: counters and one pass over the slots (of this layer alone for a view), as a dict"""
+        s = UtxoTableStats()
+        self.ctx._check(self._lib.kgv_utxo_stats(self.ctx._h, self._h, ctypes.byref(s)))
+        return {n: int(getattr(s, n)) for n, _ in UtxoTableStats._fields_}
+
+    def rehash(self, capacity=0):
+        """kgv_utxo_rehash: rebuild into `capacity` slots (0: the current size; rounded up to a power of two)"""
+        self.ctx._check(self._lib.kgv_utxo_rehash(self.ctx._h, self._h, int(capacity)))
+
+    def set_max_load(self, permille):
+        """kgv_utxo_set_max_load: 0 = off (the default), 1..900 = grow / rehash before a write would pass that load"""
+        self.ctx._check(self._lib.kgv_utxo_set_max_load(self.ctx._h, self._h, int(permille)))
 
     def export(self):
         """DbUtxoSetStore::iterator (utxo_set.rs:114-129): every live entry. Returns (keys36 (n, 36), entries (n,) ENTRY_DTYPE, arena bytes)."""
