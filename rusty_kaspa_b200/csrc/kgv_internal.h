@@ -56,6 +56,8 @@ struct kgv_ctx {
   size_t d_work_cap = 0;
   uint8_t* d_replay = nullptr;  // kgv_replay_window: window-wide state (tx ids, window map, script verdicts, accept mask)
   size_t d_replay_cap = 0;
+  uint8_t* d_keys[2] = {};      // per-launch key cache of the verify launches (table, item slots, key records): [0] Schnorr, [1] ECDSA
+  size_t d_keys_cap[2] = {};
   uint8_t* d_mu = nullptr;      // MuHash element arrays, product-tree levels and wide-product scratch rows
   size_t d_mu_cap = 0;
   // state of the last kgv_replay_window call, kept for kgv_replay_muhash (cleared by any call that stages another batch)

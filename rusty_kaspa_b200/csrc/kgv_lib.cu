@@ -83,6 +83,112 @@ __global__ void __launch_bounds__(128) k_build_gtab(uint32_t* __restrict__ gtab)
   for (int i = 0; i < 8; i++) { out[i] = x.v[i]; out[8 + i] = y.v[i]; }
 }
 
+// ---- per-launch key cache: the key part of a verification done once per distinct public key of a verify launch ----
+// Records per launch at most (2^17 x 560 B = 73 MB).
+#define KGV_KEY_RECORDS_MAX (1u << 17)
+// A launch uses records when its keys are used twice on average (at most n/2 distinct keys) and fit the cap; then EVERY key has one.  A
+// warp pays for the inline key path of any of its lanes, so records for the repeated keys alone leave singleton lanes costing whole
+// warps; a batch of mostly distinct keys makes no records at all and pays only the dedup pass.
+__device__ __forceinline__ bool key_records_on(uint32_t n_rec, size_t n) { return n_rec <= KGV_KEY_RECORDS_MAX && 2 * (size_t)n_rec <= n; }
+
+// Slot of the open-addressed key table: key = fingerprint << 32 | (representative item + 1), 0 = empty; rec = the key's record + 1.
+struct KeySlot {
+  unsigned long long key;
+  uint32_t rec, unused_;
+};
+struct KeyCacheView {
+  const KeySlot* table;
+  const uint32_t* item_slot;  // item -> table slot (only the items the launch verifies are set)
+  const uint32_t* recs;       // records, KGV_KR_WORDS words each
+  const uint32_t* n_rec;      // distinct keys of the launch; nullptr: no key cache
+  // the record of item i, or nullptr (the launch makes no records)
+  __device__ __forceinline__ const uint32_t* rec_of(size_t i, size_t n) const {
+    if (!n_rec || !key_records_on(*n_rec, n)) return nullptr;
+    return recs + (size_t)(table[item_slot[i]].rec - 1) * KGV_KR_WORDS;
+  }
+};
+
+// the key of item i: 8 big-endian words of x (+ the tag byte as word 8 for ECDSA; 33-byte stride, never word aligned)
+template <bool ALIGNED, bool ECDSA>
+__device__ __forceinline__ void key_words(uint32_t* w, const uint8_t* pk, size_t i) {
+  if (ECDSA) {
+    const uint8_t* kp = pk + 33 * i;
+    w[8] = kp[0];
+    load_be32<false>(w, kp + 1);
+  } else {
+    load_be32<ALIGNED>(w, pk + 32 * i);
+  }
+}
+__device__ __forceinline__ uint64_t key_hash(const uint32_t* w, int nw) {
+  uint64_t h = 0x9E3779B97F4A7C15ull;
+  for (int k = 0; k < nw; k++) {
+    h = (h ^ w[k]) * 0xFF51AFD7ED558CCDull;
+    h ^= h >> 32;
+  }
+  h ^= h >> 33; h *= 0xC4CEB9FE1A85EC53ull; h ^= h >> 33;
+  return h;
+}
+
+// One thread per item: find or claim the key's slot; a claimed slot gets the next record index.  Whichever item's atomicCAS claims the
+// slot becomes its representative: the record depends on the key bytes alone.  Once the launch has more keys than key_records_on allows,
+// the remaining items stop (the verify kernels then take the inline key path for every item).
+template <bool ALIGNED, bool ECDSA>
+__global__ void __launch_bounds__(256) k_key_dedup(const uint8_t* __restrict__ pk, size_t n_arg, const uint32_t* __restrict__ index,
+                                                   const uint32_t* __restrict__ n_dev, KeySlot* __restrict__ table, uint32_t mask,
+                                                   uint32_t* __restrict__ item_slot, uint32_t* __restrict__ rec_rep, uint32_t* n_rec) {
+  const size_t n = n_dev ? (size_t)*n_dev : n_arg;
+  const size_t t = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= n || !key_records_on(*(volatile uint32_t*)n_rec, n)) return;
+  const size_t i = index ? index[t] : t;
+  const int nw = ECDSA ? 9 : 8;
+  uint32_t w[9];
+  key_words<ALIGNED, ECDSA>(w, pk, i);
+  const uint64_t h = key_hash(w, nw);
+  const unsigned long long mine = (h & 0xFFFFFFFF00000000ull) | (uint64_t)(i + 1);
+  uint32_t s = (uint32_t)h & mask;
+  bool won = false;
+  for (;;) {
+    unsigned long long cur = atomicCAS(&table[s].key, 0ull, mine);
+    if (cur == 0) { won = true; break; }
+    if ((cur >> 32) == (mine >> 32)) {
+      uint32_t v[9];
+      key_words<ALIGNED, ECDSA>(v, pk, (uint32_t)cur - 1);
+      bool eq = true;
+      for (int k = 0; k < nw; k++) eq = eq && v[k] == w[k];
+      if (eq) break;
+    }
+    s = (s + 1) & mask;
+  }
+  // one counter update per warp for the slots its lanes claimed
+  const uint32_t act = __activemask(), ball = __ballot_sync(act, won);
+  const int lane = threadIdx.x & 31, leader = __ffs(act) - 1;
+  uint32_t base = 0;
+  if (lane == leader && ball) base = atomicAdd(n_rec, (uint32_t)__popc(ball));
+  base = __shfl_sync(act, base, leader);
+  if (won) {
+    const uint32_t r = base + __popc(ball & ((1u << lane) - 1));
+    if (key_records_on(r + 1, n)) {  // (r < the host's bound of the rec_rep / record arrays)
+      rec_rep[r] = (uint32_t)i;
+      table[s].rec = r + 1;
+    }
+  }
+  item_slot[i] = s;
+}
+
+// One thread per record: the key's verdict, and for a good key its odd-multiples table and zs (key_rec_build).  The verify kernels'
+// occupancy (168 registers): unbounded, ptxas takes 255 and two blocks per SM.
+template <bool ECDSA>
+__global__ void __launch_bounds__(KGV_BLOCK, KGV_BLOCKS_PER_SM) k_key_prepare(const uint8_t* __restrict__ pk, size_t n_arg, const uint32_t* __restrict__ n_dev,
+                                                                              const uint32_t* __restrict__ rec_rep, const uint32_t* __restrict__ n_rec,
+                                                                              uint32_t* __restrict__ recs) {
+  const size_t n = n_dev ? (size_t)*n_dev : n_arg;
+  const uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
+  if (r >= *n_rec || !key_records_on(*n_rec, n)) return;
+  uint32_t w[9];
+  key_words<false, ECDSA>(w, pk, rec_rep[r]);
+  key_rec_build(recs + (size_t)r * KGV_KR_WORDS, ECDSA ? w[8] : 2u, w);
+}
+
 // Each thread verifies KGV_ITEMS consecutive-stride items (i = tid + j * total_threads: coalesced) and shares
 // ONE modular inversion among them (Montgomery's trick): the field inversion of BIP-340's final affine
 // conversion, resp. the scalar inversion s^-1 of ECDSA, drops from 1 to 1/KGV_ITEMS per signature with no
@@ -90,7 +196,8 @@ __global__ void __launch_bounds__(128) k_build_gtab(uint32_t* __restrict__ gtab)
 template <bool ALIGNED, bool INDEXED>
 __global__ void __launch_bounds__(KGV_BLOCK, KGV_BLOCKS_PER_SM)
 k_schnorr_verify(const uint8_t* __restrict__ pk, const uint8_t* __restrict__ msg, const uint8_t* __restrict__ sig, size_t n_arg,
-                 uint8_t* __restrict__ status, const uint32_t* __restrict__ gtab, const uint32_t* __restrict__ index, const uint32_t* __restrict__ n_dev) {
+                 uint8_t* __restrict__ status, const uint32_t* __restrict__ gtab, const uint32_t* __restrict__ index, const uint32_t* __restrict__ n_dev,
+                 KeyCacheView kc) {
   // INDEXED: verify only the listed items (the signature-cache misses), their count read on the device.  A separate instantiation: the two
   // extra pointers live across the whole kernel cost the plain form 3 % (register pressure at the 168-register cap, measured).
   extern __shared__ uint32_t smem[];
@@ -119,7 +226,7 @@ k_schnorr_verify(const uint8_t* __restrict__ pk, const uint8_t* __restrict__ msg
     load_be32<ALIGNED>(sw, sig + 64 * i);
     load_be32<ALIGNED>(sw + 8, sig + 64 * i + 32);
     fe x, y, zt, rx;
-    uint8_t s1 = schnorr_phase1(x, y, zt, rx, pkw, mw, sw, tab, gtab, GLoadDev());
+    uint8_t s1 = schnorr_phase1(x, y, zt, rx, pkw, mw, sw, tab, gtab, GLoadDev(), kc.rec_of(i, n));
     st[j] = s1;
     if (s1 == KGV_ST_PENDING) {
       X[j] = x; Y[j] = y; ZT[j] = zt; RX[j] = rx;
@@ -153,7 +260,8 @@ struct sc_words { uint32_t v[8]; };
 template <bool ALIGNED, bool INDEXED>
 __global__ void __launch_bounds__(KGV_BLOCK, KGV_BLOCKS_PER_SM)
 k_ecdsa_verify(const uint8_t* __restrict__ pk, const uint8_t* __restrict__ msg, const uint8_t* __restrict__ sig, size_t n_arg,
-               uint8_t* __restrict__ status, const uint32_t* __restrict__ gtab, const uint32_t* __restrict__ index, const uint32_t* __restrict__ n_dev) {
+               uint8_t* __restrict__ status, const uint32_t* __restrict__ gtab, const uint32_t* __restrict__ index, const uint32_t* __restrict__ n_dev,
+               KeyCacheView kc) {
   extern __shared__ uint32_t smem[];
   const size_t n = (INDEXED && n_dev) ? (size_t)*n_dev : n_arg;
   const size_t total = (size_t)gridDim.x * KGV_BLOCK;
@@ -161,6 +269,7 @@ k_ecdsa_verify(const uint8_t* __restrict__ pk, const uint8_t* __restrict__ msg, 
   SmemTab tab{smem + threadIdx.x};
   fe QX[KGV_ITEMS], QY[KGV_ITEMS];
   sc_words R_[KGV_ITEMS], S_[KGV_ITEMS], M_[KGV_ITEMS], pre[KGV_ITEMS];
+  const uint32_t* KR[KGV_ITEMS];
   uint8_t st[KGV_ITEMS];
 #pragma unroll 1
   for (size_t base = 0; base < n; base += total * KGV_ITEMS) {
@@ -181,10 +290,11 @@ k_ecdsa_verify(const uint8_t* __restrict__ pk, const uint8_t* __restrict__ msg, 
     load_be32<ALIGNED>(sw + 8, sig + 64 * i + 32);
     fe qx, qy;
     uint32_t r[8], s[8], m[8];
-    uint8_t s1 = ecdsa_phase1(qx, qy, r, s, m, tag, pkw, mw, sw);
+    const uint32_t* krec = kc.rec_of(i, n);
+    uint8_t s1 = ecdsa_phase1(qx, qy, r, s, m, tag, pkw, mw, sw, krec);
     st[j] = s1;
     if (s1 == KGV_ST_PENDING) {
-      QX[j] = qx; QY[j] = qy;
+      QX[j] = qx; QY[j] = qy; KR[j] = krec;
 #pragma unroll
       for (int w = 0; w < 8; w++) { R_[j].v[w] = r[w]; S_[j].v[w] = s[w]; M_[j].v[w] = m[w]; pre[j].v[w] = acc[w]; }
       sc_mul(acc, acc, s);
@@ -200,7 +310,7 @@ k_ecdsa_verify(const uint8_t* __restrict__ pk, const uint8_t* __restrict__ msg, 
       uint32_t sn[8];
       sc_mul(sn, inv, pre[j].v);
       sc_mul(inv, inv, S_[j].v);
-      st[j] = ecdsa_phase2(QX[j], QY[j], R_[j].v, sn, M_[j].v, tab, gtab, GLoadDev());
+      st[j] = ecdsa_phase2(QX[j], QY[j], R_[j].v, sn, M_[j].v, tab, gtab, GLoadDev(), KR[j]);
     }
   }
 #pragma unroll 1
@@ -389,7 +499,7 @@ extern "C" void kgv_destroy(kgv_ctx* ctx) {
   if (ctx->copy_stream) cudaStreamSynchronize(ctx->copy_stream);
   cudaStreamSynchronize(ctx->stream);
   if (ctx->gtab) cudaFree(ctx->gtab);
-  for (uint8_t* b : {ctx->d_in, ctx->d_out, ctx->d_batch, ctx->prefetch[0].buf, ctx->prefetch[1].buf, ctx->d_scratch, ctx->d_mu, ctx->d_work, ctx->d_replay})
+  for (uint8_t* b : {ctx->d_in, ctx->d_out, ctx->d_batch, ctx->prefetch[0].buf, ctx->prefetch[1].buf, ctx->d_scratch, ctx->d_mu, ctx->d_work, ctx->d_replay, ctx->d_keys[0], ctx->d_keys[1]})
     if (b) cudaFree(b);
   for (uint8_t* b : ctx->parked) cudaFree(b);
   for (cudaEvent_t e : ctx->ev_chunk) if (e) cudaEventDestroy(e);
@@ -438,9 +548,44 @@ extern "C" uint64_t kgv_launch_count(const kgv_ctx* ctx) { return ctx ? ctx->lau
 // ---------------------------------------------------------------------------------------------
 // signature verification entry points
 // ---------------------------------------------------------------------------------------------
+// Enqueues the per-launch key cache of a verify launch on st: table cleared, k_key_dedup, k_key_prepare.  Sized from the host's n (an
+// upper bound of *n_dev when given); the scratch belongs to the item kind (Schnorr and ECDSA launches of one validation call run
+// side by side on two streams) and lives until the next launch of that kind, which the stream order puts after this one.
+static int key_cache_launch(kgv_ctx* ctx, const uint8_t* dpk, size_t n, bool ecdsa, bool aligned, cudaStream_t st, const uint32_t* index,
+                            const uint32_t* n_dev, KeyCacheView* kc) {
+  uint32_t slots = 64;
+  while (slots < 2 * n) slots <<= 1;                       // load factor <= 1/2
+  const uint32_t cap = (uint32_t)(n / 2 < KGV_KEY_RECORDS_MAX ? n / 2 : KGV_KEY_RECORDS_MAX);  // key_records_on's bound
+  const size_t o_tab = 256, o_item = o_tab + (size_t)slots * sizeof(KeySlot);
+  const size_t o_rep = (o_item + n * 4 + 255) & ~(size_t)255, o_rec = (o_rep + (size_t)cap * 4 + 255) & ~(size_t)255;
+  int rc = kgv_reserve(ctx, &ctx->d_keys[ecdsa], &ctx->d_keys_cap[ecdsa], o_rec + (size_t)cap * KGV_KR_WORDS * 4);
+  if (rc) return rc;
+  uint8_t* K = ctx->d_keys[ecdsa];
+  uint32_t* n_rec = (uint32_t*)K;
+  KeySlot* table = (KeySlot*)(K + o_tab);
+  uint32_t *item_slot = (uint32_t*)(K + o_item), *rec_rep = (uint32_t*)(K + o_rep), *recs = (uint32_t*)(K + o_rec);
+  CK(cudaMemsetAsync(K, 0, o_item, st));
+  const unsigned gd = (unsigned)((n + 255) / 256);
+  if (ecdsa) k_key_dedup<false, true><<<gd, 256, 0, st>>>(dpk, n, index, n_dev, table, slots - 1, item_slot, rec_rep, n_rec);
+  else if (aligned) k_key_dedup<true, false><<<gd, 256, 0, st>>>(dpk, n, index, n_dev, table, slots - 1, item_slot, rec_rep, n_rec);
+  else k_key_dedup<false, false><<<gd, 256, 0, st>>>(dpk, n, index, n_dev, table, slots - 1, item_slot, rec_rep, n_rec);
+  CK(cudaGetLastError());
+  ctx->launches++;
+  if (cap) {
+    const unsigned gp = (cap + KGV_BLOCK - 1) / KGV_BLOCK;
+    if (ecdsa) k_key_prepare<true><<<gp, KGV_BLOCK, 0, st>>>(dpk, n, n_dev, rec_rep, n_rec, recs);
+    else k_key_prepare<false><<<gp, KGV_BLOCK, 0, st>>>(dpk, n, n_dev, rec_rep, n_rec, recs);
+    CK(cudaGetLastError());
+    ctx->launches++;
+  }
+  *kc = KeyCacheView{table, item_slot, recs, n_rec};
+  return KGV_OK;
+}
+
 int kgv_launch_verify(kgv_ctx* ctx, const uint8_t* dpk, const uint8_t* dmsg, const uint8_t* dsig, size_t n, uint8_t* dst, bool ecdsa,
                       cudaStream_t on, bool use_on, const uint32_t* index, const uint32_t* n_dev) {
   if (n == 0) return KGV_OK;
+  if (n >= 0x7FFFFFFFu) return fail_arg(ctx, "verify launch of 2^31 or more items");
   cudaStream_t st = use_on ? on : ctx->stream;
   const int smem = KGV_BLOCK * 128 * (int)sizeof(uint32_t);
   // one resident wave, persistent; items are strided by the grid size, so a batch smaller than the wave still
@@ -448,21 +593,28 @@ int kgv_launch_verify(kgv_ctx* ctx, const uint8_t* dpk, const uint8_t* dmsg, con
   size_t want = (n + KGV_BLOCK - 1) / KGV_BLOCK;
   unsigned blocks = (unsigned)(want < (size_t)ctx->resident_blocks ? want : (size_t)ctx->resident_blocks);
   bool aligned = (((uintptr_t)dmsg | (uintptr_t)dsig | (ecdsa ? 0 : (uintptr_t)dpk)) & 31) == 0;
+  // The key cache pays off when threads verify several items: in a launch of at most one item per thread the preparation's latency
+  // comes on top of a verify that shortens by the same latency (small batches measured 10 % slower with it).
+  KeyCacheView kc{};
+  if (n > (size_t)ctx->resident_blocks * KGV_BLOCK) {
+    int rc = key_cache_launch(ctx, dpk, n, ecdsa, aligned, st, index, n_dev, &kc);
+    if (rc) return rc;
+  }
   if (ecdsa) {
     if (index) {
-      if (aligned) k_ecdsa_verify<true, true><<<blocks, KGV_BLOCK, smem, st>>>(dpk, dmsg, dsig, n, dst, ctx->gtab, index, n_dev);
-      else k_ecdsa_verify<false, true><<<blocks, KGV_BLOCK, smem, st>>>(dpk, dmsg, dsig, n, dst, ctx->gtab, index, n_dev);
+      if (aligned) k_ecdsa_verify<true, true><<<blocks, KGV_BLOCK, smem, st>>>(dpk, dmsg, dsig, n, dst, ctx->gtab, index, n_dev, kc);
+      else k_ecdsa_verify<false, true><<<blocks, KGV_BLOCK, smem, st>>>(dpk, dmsg, dsig, n, dst, ctx->gtab, index, n_dev, kc);
     } else {
-      if (aligned) k_ecdsa_verify<true, false><<<blocks, KGV_BLOCK, smem, st>>>(dpk, dmsg, dsig, n, dst, ctx->gtab, nullptr, nullptr);
-      else k_ecdsa_verify<false, false><<<blocks, KGV_BLOCK, smem, st>>>(dpk, dmsg, dsig, n, dst, ctx->gtab, nullptr, nullptr);
+      if (aligned) k_ecdsa_verify<true, false><<<blocks, KGV_BLOCK, smem, st>>>(dpk, dmsg, dsig, n, dst, ctx->gtab, nullptr, nullptr, kc);
+      else k_ecdsa_verify<false, false><<<blocks, KGV_BLOCK, smem, st>>>(dpk, dmsg, dsig, n, dst, ctx->gtab, nullptr, nullptr, kc);
     }
   } else {
     if (index) {
-      if (aligned) k_schnorr_verify<true, true><<<blocks, KGV_BLOCK, smem, st>>>(dpk, dmsg, dsig, n, dst, ctx->gtab, index, n_dev);
-      else k_schnorr_verify<false, true><<<blocks, KGV_BLOCK, smem, st>>>(dpk, dmsg, dsig, n, dst, ctx->gtab, index, n_dev);
+      if (aligned) k_schnorr_verify<true, true><<<blocks, KGV_BLOCK, smem, st>>>(dpk, dmsg, dsig, n, dst, ctx->gtab, index, n_dev, kc);
+      else k_schnorr_verify<false, true><<<blocks, KGV_BLOCK, smem, st>>>(dpk, dmsg, dsig, n, dst, ctx->gtab, index, n_dev, kc);
     } else {
-      if (aligned) k_schnorr_verify<true, false><<<blocks, KGV_BLOCK, smem, st>>>(dpk, dmsg, dsig, n, dst, ctx->gtab, nullptr, nullptr);
-      else k_schnorr_verify<false, false><<<blocks, KGV_BLOCK, smem, st>>>(dpk, dmsg, dsig, n, dst, ctx->gtab, nullptr, nullptr);
+      if (aligned) k_schnorr_verify<true, false><<<blocks, KGV_BLOCK, smem, st>>>(dpk, dmsg, dsig, n, dst, ctx->gtab, nullptr, nullptr, kc);
+      else k_schnorr_verify<false, false><<<blocks, KGV_BLOCK, smem, st>>>(dpk, dmsg, dsig, n, dst, ctx->gtab, nullptr, nullptr, kc);
     }
   }
   CK(cudaGetLastError());

@@ -573,11 +573,12 @@ KGV_HD void build_odd_table(Tab& tab, fe& zs, const fe& px, const fe& py) {
 // ------------------------------------------------------------------------------------------
 // R = kP * P + kG * G     (result on the isomorphic curve; true Z = R.z * zs)
 // ------------------------------------------------------------------------------------------
+// tab, zs: P's odd-multiples table and its Z scale, as build_odd_table leaves them (built by the caller, or copied from a key record).
 // gtab: [2][65536][16] u32 — affine (x limbs, y limbs) of v*G and v*2^128*G; entry 0 unused.
 // GLoad is a functor  void operator()(fe& x, fe& y, const uint32_t* entry)  (vectorised loads on device).
 template <class Tab, class GLoad, class Trace = NoTrace>
-KGV_HD void ecmult_double(gej& R, fe& zs, const fe& px, const fe& py, const uint32_t* kP, const uint32_t* kG, Tab& tab,
-                          const uint32_t* gtab, GLoad gload, Trace trace = Trace()) {
+KGV_HD void ecmult_double(gej& R, const fe& zs, const uint32_t* kP, const uint32_t* kG, Tab& tab, const uint32_t* gtab, GLoad gload,
+                          Trace trace = Trace()) {
   const fe beta = {KGV_BETA_LIMBS};
   uint32_t m1[5], m2[5], h1[5], h2[5];
   bool neg1, neg2, fix1, fix2;
@@ -586,7 +587,6 @@ KGV_HD void ecmult_double(gej& R, fe& zs, const fe& px, const fe& py, const uint
   recode_signed_odd(h2, fix2, m2);
   trace(10, m1, 5); trace(11, m2, 5);
   { uint32_t f[4] = {neg1, neg2, fix1, fix2}; trace(12, f, 4); }
-  build_odd_table(tab, zs, px, py);
   trace(13, zs.v, 8);
   { uint32_t e0[16]; for (int w = 0; w < 16; w++) e0[w] = tab.get(7, w); trace(14, e0, 16); }
   fe zs2, zs3;

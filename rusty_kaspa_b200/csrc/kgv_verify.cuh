@@ -21,18 +21,82 @@ KGV_HD bool fe_words_lt_p(const uint32_t* v) {
 
 #define KGV_ST_PENDING 0xFFu  // phase 1 passed: the verdict needs the (batched) inversion of zt
 
+// y^2 = x^3 + 7 for a key given as its tag (2: even y, 3: odd y; a BIP-340 x-only key is tag 2) and the 8 big-endian words of x.
+// false: the key does not parse (bad tag, x >= p, or x not on the curve).
+KGV_HD bool key_lift(fe& x, fe& y, uint32_t tag, const uint32_t* pkw) {
+  if (tag != 2u && tag != 3u) return false;
+  limbs_from_be_words(x.v, pkw);
+  if (!fe_words_lt_p(x.v)) return false;
+  return ge_lift_x(y, x, tag == 3u);
+}
+
+// Key record: the part of a verification that depends on the public key alone, prepared once per distinct key of a verify launch
+// (k_key_prepare) and copied into the thread's table by every signature under that key.  Words, 16-byte aligned, read with 128-bit loads:
+//   [0, 128)   the odd-multiples table {1,3,..,15}*P, entry-major (entry e, word w at 16e + w: x limbs, then y limbs), as build_odd_table leaves it
+//   [128, 136) zs, the table's Z scale
+//   136        the key's verdict: KGV_ST_VALID (the key parses) or KGV_ST_PK_PARSE; the rest of the record is unset then
+#define KGV_KR_ZS 128
+#define KGV_KR_STATUS 136
+#define KGV_KR_WORDS 140  // 560 bytes
+
+// Tab accessor over a key record in global memory (the preparation kernel builds the table in place)
+struct RecTab {
+  uint32_t* rec;
+  KGV_HD void put(int e, int w, uint32_t v) { rec[e * 16 + w] = v; }
+  KGV_HD uint32_t get(int e, int w) const { return rec[e * 16 + w]; }
+};
+// 128-bit read-only load (the records are written by an earlier kernel of the same stream)
+KGV_HD void ldg128(uint32_t* w, const uint32_t* p) {
+#ifdef __CUDA_ARCH__
+  asm volatile("ld.global.nc.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(w[0]), "=r"(w[1]), "=r"(w[2]), "=r"(w[3]) : "l"(p));
+#else
+  for (int i = 0; i < 4; i++) w[i] = p[i];
+#endif
+}
+// table and zs of a prepared key (its verdict is KGV_ST_VALID)
+template <class Tab>
+KGV_HD void key_rec_load(Tab& tab, fe& zs, const uint32_t* rec) {
+#pragma unroll 1
+  for (int e = 0; e < 8; e++) {
+    uint32_t w[16];
+#pragma unroll
+    for (int q = 0; q < 4; q++) ldg128(w + 4 * q, rec + 16 * e + 4 * q);
+#pragma unroll
+    for (int q = 0; q < 16; q++) tab.put(e, q, w[q]);
+  }
+  ldg128(zs.v, rec + KGV_KR_ZS);
+  ldg128(zs.v + 4, rec + KGV_KR_ZS + 4);
+}
+// fills a key record (tag as for key_lift)
+KGV_HD void key_rec_build(uint32_t* rec, uint32_t tag, const uint32_t* pkw) {
+  fe x, y, zs;
+  uint8_t st = KGV_ST_PK_PARSE;
+  if (key_lift(x, y, tag, pkw)) {
+    RecTab tab{rec};
+    build_odd_table(tab, zs, x, y);
+#pragma unroll
+    for (int w = 0; w < 8; w++) rec[KGV_KR_ZS + w] = zs.v[w];
+    st = KGV_ST_VALID;
+  }
+  rec[KGV_KR_STATUS] = st;
+}
+
 // BIP-340 verification, phase 1: everything up to the projective result R = s*G - e*P.
-// pkw/mw: 8 big-endian words, sigw: 16 big-endian words (r || s).
+// pkw/mw: 8 big-endian words, sigw: 16 big-endian words (r || s).  krec: the key's record, or nullptr (the key part is computed here).
 // Returns a final verdict, or KGV_ST_PENDING with (X, Y, zt = true Z, rx) filled in.
 template <class Tab, class GLoad, class Trace = NoTrace>
 KGV_HD uint8_t schnorr_phase1(fe& X, fe& Y, fe& zt, fe& rx, const uint32_t* pkw, const uint32_t* mw, const uint32_t* sigw, Tab& tab,
-                              const uint32_t* gtab, GLoad gload, Trace trace = Trace()) {
+                              const uint32_t* gtab, GLoad gload, const uint32_t* krec, Trace trace = Trace()) {
   fe px, py;
-  limbs_from_be_words(px.v, pkw);
-  if (!fe_words_lt_p(px.v)) return KGV_ST_PK_PARSE;      // x >= p
-  trace(1, px.v, 8);
-  if (!ge_lift_x(py, px, false)) return KGV_ST_PK_PARSE;  // not on the curve
-  trace(2, py.v, 8);
+  if (krec) {
+    if (krec[KGV_KR_STATUS] != KGV_ST_VALID) return KGV_ST_PK_PARSE;
+  } else {
+    limbs_from_be_words(px.v, pkw);
+    if (!fe_words_lt_p(px.v)) return KGV_ST_PK_PARSE;      // x >= p
+    trace(1, px.v, 8);
+    if (!ge_lift_x(py, px, false)) return KGV_ST_PK_PARSE;  // not on the curve
+    trace(2, py.v, 8);
+  }
   limbs_from_be_words(rx.v, sigw);
   if (!fe_words_lt_p(rx.v)) return KGV_ST_INVALID;        // r >= p
   uint32_t s[8], e[8], k[8], ew[8];
@@ -46,7 +110,9 @@ KGV_HD uint8_t schnorr_phase1(fe& X, fe& Y, fe& zt, fe& rx, const uint32_t* pkw,
   trace(3, e, 8); trace(4, k, 8); trace(5, s, 8);
   gej R;
   fe zs;
-  ecmult_double(R, zs, px, py, k, s, tab, gtab, gload, trace);
+  if (krec) key_rec_load(tab, zs, krec);
+  else build_odd_table(tab, zs, px, py);
+  ecmult_double(R, zs, k, s, tab, gtab, gload, trace);
   { uint32_t f[1] = {R.inf}; trace(18, f, 1); }
   if (R.inf) return KGV_ST_INVALID;
   trace(19, R.x.v, 8); trace(20, R.y.v, 8); trace(21, R.z.v, 8);
@@ -75,23 +141,24 @@ KGV_HD uint8_t schnorr_phase2(const fe& X, const fe& Y, const fe& zi, const fe& 
 // single-signature form (audit kernel, host unit tests)
 template <class Tab, class GLoad, class Trace = NoTrace>
 KGV_HD uint8_t schnorr_verify_core(const uint32_t* pkw, const uint32_t* mw, const uint32_t* sigw, Tab& tab, const uint32_t* gtab,
-                                   GLoad gload, Trace trace = Trace()) {
+                                   GLoad gload, Trace trace = Trace(), const uint32_t* krec = nullptr) {
   fe X, Y, zt, rx, zi;
-  uint8_t st = schnorr_phase1(X, Y, zt, rx, pkw, mw, sigw, tab, gtab, gload, trace);
+  uint8_t st = schnorr_phase1(X, Y, zt, rx, pkw, mw, sigw, tab, gtab, gload, krec, trace);
   if (st != KGV_ST_PENDING) return st;
   fe_inv(zi, zt);
   return schnorr_phase2(X, Y, zi, rx, trace);
 }
 
 // ECDSA verification with libsecp256k1 semantics, phase 1: parsing and range checks.
-// pkw: 8 big-endian words of x, tag = first key byte.  Returns a final verdict or KGV_ST_PENDING with
-// the key (qx,qy), r, s (to be inverted, possibly batched) and the reduced message m.
+// pkw: 8 big-endian words of x, tag = first key byte, krec: the key's record or nullptr.  Returns a final verdict or KGV_ST_PENDING with
+// the key (qx,qy; unset with a record), r, s (to be inverted, possibly batched) and the reduced message m.
 KGV_HD uint8_t ecdsa_phase1(fe& qx, fe& qy, uint32_t* r, uint32_t* s, uint32_t* m, uint32_t tag, const uint32_t* pkw, const uint32_t* mw,
-                            const uint32_t* sigw) {
-  if (tag != 2u && tag != 3u) return KGV_ST_PK_PARSE;
-  limbs_from_be_words(qx.v, pkw);
-  if (!fe_words_lt_p(qx.v)) return KGV_ST_PK_PARSE;
-  if (!ge_lift_x(qy, qx, tag == 3u)) return KGV_ST_PK_PARSE;
+                            const uint32_t* sigw, const uint32_t* krec) {
+  if (krec) {
+    if (krec[KGV_KR_STATUS] != KGV_ST_VALID) return KGV_ST_PK_PARSE;
+  } else if (!key_lift(qx, qy, tag, pkw)) {
+    return KGV_ST_PK_PARSE;
+  }
   limbs_from_be_words(r, sigw);
   limbs_from_be_words(s, sigw + 8);
   if (sc_ge_n(r) || sc_ge_n(s)) return KGV_ST_SIG_PARSE;  // from_compact rejects overflow
@@ -104,13 +171,15 @@ KGV_HD uint8_t ecdsa_phase1(fe& qx, fe& qy, uint32_t* r, uint32_t* s, uint32_t* 
 // phase 2: sn = s^-1 mod n.  R = (m/s)*G + (r/s)*Q, valid iff x(R) mod n == r.
 template <class Tab, class GLoad>
 KGV_HD uint8_t ecdsa_phase2(const fe& qx, const fe& qy, const uint32_t* r, const uint32_t* sn, const uint32_t* m, Tab& tab, const uint32_t* gtab,
-                            GLoad gload) {
+                            GLoad gload, const uint32_t* krec) {
   uint32_t u1[8], u2[8];
   sc_mul(u1, sn, m);
   sc_mul(u2, sn, r);
   gej R;
   fe zs;
-  ecmult_double(R, zs, qx, qy, u2, u1, tab, gtab, gload);
+  if (krec) key_rec_load(tab, zs, krec);
+  else build_odd_table(tab, zs, qx, qy);
+  ecmult_double(R, zs, u2, u1, tab, gtab, gload);
   if (R.inf) return KGV_ST_INVALID;
   // x(R) mod n == r  <=>  X == r*Zt^2  or  (r + n < p and X == (r+n)*Zt^2)
   fe zt, zt2, t, rf;
@@ -131,13 +200,13 @@ KGV_HD uint8_t ecdsa_phase2(const fe& qx, const fe& qy, const uint32_t* r, const
 }
 template <class Tab, class GLoad>
 KGV_HD uint8_t ecdsa_verify_core(uint32_t tag, const uint32_t* pkw, const uint32_t* mw, const uint32_t* sigw, Tab& tab,
-                                 const uint32_t* gtab, GLoad gload) {
+                                 const uint32_t* gtab, GLoad gload, const uint32_t* krec = nullptr) {
   fe qx, qy;
   uint32_t r[8], s[8], m[8], sn[8];
-  uint8_t st = ecdsa_phase1(qx, qy, r, s, m, tag, pkw, mw, sigw);
+  uint8_t st = ecdsa_phase1(qx, qy, r, s, m, tag, pkw, mw, sigw, krec);
   if (st != KGV_ST_PENDING) return st;
   sc_inv(sn, s);
-  return ecdsa_phase2(qx, qy, r, sn, m, tab, gtab, gload);
+  return ecdsa_phase2(qx, qy, r, sn, m, tab, gtab, gload, krec);
 }
 
 // One entry of the generator tables: v * B for v in [1, 65535], B affine; result affine.
