@@ -401,6 +401,28 @@ int kgv_replay_window(kgv_ctx* ctx, kgv_utxo_table* t, const kgv_tx_batch* batch
  * found at each block's position).  Must directly follow that kgv_replay_window call (no other batch call in between).
  * With kgv_muhash_prefix_combine and kgv_muhash_finalize_batch this yields every chain block's utxo_commitment of a window (:188-192). */
 int kgv_replay_muhash(kgv_ctx* ctx, const uint32_t* group_first_block, size_t n_groups, uint8_t* values768);
+/* The UtxoDiff of every group of blocks of the LAST kgv_replay_window call (ctx.mergeset_diff of calculate_utxo_state, utxo_validation.rs:119,148:
+ * what commit_utxo_state stores per chain block and what reorgs read back).  Groups tile the window as in kgv_replay_muhash (group_first_block:
+ * a HOST array).  Group g's diff is UtxoDiff::add_transaction (utxo_diff.rs:224-260) of every transaction the window accepted in its blocks, in
+ * block order then transaction order (accepted coinbases included, VERIFY_ONLY blocks contribute nothing), with each spent entry as it was found
+ * at its block's position.  So an output created and spent inside one group is in neither list, and one created in group g and spent in a later
+ * group g' is in g's add (block_daa_score = the accepting block's) and in g''s remove.
+ *   removals:  rem_keys36[first_remove .. +n_remove) and rem_entries, in window input order
+ *   additions: add_keys36[first_add .. +n_add) and add_entries, in window output order
+ * Every entry's script_off points into `bytes` (group after group, each group's removal scripts before its addition scripts).
+ * Forward for group g is kgv_utxo_apply_diff(rem = its removal keys, add = its additions); rollback is kgv_utxo_apply_diff(rem = its addition keys,
+ * add = its removal keys and entries) - on a plain table or on a view layer.
+ * Output arrays (ranges included) are all host or all device memory; device entry arrays must be 8-byte aligned.  With rem_keys36 == NULL only
+ * the sizes (*n_rem_out, *n_add_out, *bytes_out) and `ranges` (may be NULL) are returned; arrays smaller than that give KGV_ERR_NOMEM with the
+ * sizes and ranges still set.  Valid under the same conditions as kgv_replay_muhash: either may come first and either may be repeated.  Without a
+ * current window, with groups that do not tile it, or after a window replayed with KGV_REPLAY_WALK=table: KGV_ERR_ARG. */
+typedef struct {
+  uint64_t first_remove, n_remove;  /* rows of rem_keys36 / rem_entries that belong to the group */
+  uint64_t first_add, n_add;        /* rows of add_keys36 / add_entries */
+} kgv_diff_range; /* 32 bytes */
+int kgv_replay_diffs(kgv_ctx* ctx, const uint32_t* group_first_block, size_t n_groups, kgv_diff_range* ranges, uint8_t* rem_keys36,
+                     kgv_utxo_entry* rem_entries, uint8_t* add_keys36, kgv_utxo_entry* add_entries, uint8_t* bytes, size_t max_rem, size_t max_add,
+                     size_t bytes_cap, size_t* n_rem_out, size_t* n_add_out, size_t* bytes_out);
 /* Overlap of the next window's upload with the current window's compute (IBD: the caller knows the blocks ahead).  A HOST batch is checked and
  * copied to the device on a side stream into a second staging buffer; the next kgv_replay_window / kgv_validate_txs / kgv_tx_ids ... call that is
  * handed exactly this batch (the same arrays and sizes) takes that buffer over instead of uploading.  The arrays must stay unchanged - and be

@@ -472,6 +472,34 @@ class TransactionValidator {
     c_.check(kgv_replay_window(c_.get(), utxo_view.get(), &v, blocks.data(), blocks.size(), &p_, res.data(), accept ? accept->data() : nullptr, stats));
     return res;
   }
+  // ctx.mergeset_diff (utxo_validation.rs:119,148) of every group of blocks of the window replay_window just processed: group g = blocks
+  // [group_first[g], group_first[g+1]) (kgv_replay_diffs)
+  std::vector<UtxoDiff> replay_diffs(const std::vector<uint32_t>& group_first) {
+    if (group_first.size() < 2) return {};
+    const size_t n_groups = group_first.size() - 1;
+    std::vector<kgv_diff_range> ranges(n_groups);
+    size_t nr = 0, na = 0, nb = 0;
+    c_.check(kgv_replay_diffs(c_.get(), group_first.data(), n_groups, ranges.data(), nullptr, nullptr, nullptr, nullptr, nullptr, 0, 0, 0, &nr, &na, &nb));
+    std::vector<uint8_t> rk(36 * nr + 4), ak(36 * na + 4), bytes(nb + 8);
+    std::vector<kgv_utxo_entry> re(nr + 1), ae(na + 1);
+    c_.check(kgv_replay_diffs(c_.get(), group_first.data(), n_groups, ranges.data(), rk.data(), re.data(), ak.data(), ae.data(), bytes.data(), nr, na, nb, &nr, &na,
+                              &nb));
+    auto put = [&](UtxoCollection& c, const uint8_t* k, const kgv_utxo_entry& r) {
+      TransactionOutpoint o;
+      std::memcpy(o.transaction_id.data(), k, 32);
+      for (int b = 0; b < 4; b++) o.index |= (uint32_t)k[32 + b] << (8 * b);
+      UtxoEntry e;
+      e.amount = r.amount; e.block_daa_score = r.block_daa_score; e.is_coinbase = r.is_coinbase != 0; e.script_public_key.version = r.spk_version;
+      e.script_public_key.script.assign(bytes.begin() + r.script_off, bytes.begin() + r.script_off + r.script_len);
+      c[o] = e;
+    };
+    std::vector<UtxoDiff> out(n_groups);
+    for (size_t g = 0; g < n_groups; g++) {
+      for (uint64_t i = ranges[g].first_remove; i < ranges[g].first_remove + ranges[g].n_remove; i++) put(out[g].remove, rk.data() + 36 * i, re[i]);
+      for (uint64_t i = ranges[g].first_add; i < ranges[g].first_add + ranges[g].n_add; i++) put(out[g].add, ak.data() + 36 * i, ae[i]);
+    }
+    return out;
+  }
   // the NEXT window's range checks and upload under the current window's compute (kgv_batch_prefetch): call it with window i+1, then
   // replay_window with window i; `next` must stay alive and unchanged until it is replayed
   void prefetch(const TxBatch& next) {

@@ -60,13 +60,15 @@ struct kgv_ctx {
   size_t d_keys_cap[2] = {};
   uint8_t* d_mu = nullptr;      // MuHash element arrays, product-tree levels and wide-product scratch rows
   size_t d_mu_cap = 0;
-  // state of the last kgv_replay_window call, kept for kgv_replay_muhash (cleared by any call that stages another batch)
+  // state of the last kgv_replay_window call, kept for kgv_replay_muhash / kgv_replay_diffs (cleared by any call that stages another batch)
   struct {
     bool valid = false;
+    bool resolving = false;  // the resolving walk ran (source records, tx info and accepting DAA scores below are valid)
     kgv_dev_batch_fwd* unused_ = nullptr;
     const void *txs = nullptr, *inputs = nullptr, *outputs = nullptr, *bytes = nullptr;
     size_t nt = 0, ni = 0, no = 0, n_blocks = 0;
     size_t o_ids = 0, o_itx = 0, o_otx = 0, o_ent = 0, o_acc = 0, o_txb = 0, o_rng = 0;  // offsets into d_replay
+    size_t o_src = 0, o_inf = 0, o_apv = 0;  // resolving walk only
   } last_replay;
   struct kgv_sigcache* sigcache = nullptr;  // kgv_set_sigcache: verdicts of the validation calls are looked up / remembered here
   struct kgv_comm* shard_comm = nullptr;  // kgv_set_sharding: signature checks of the validation calls are split over its ranks

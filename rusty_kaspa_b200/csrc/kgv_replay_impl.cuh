@@ -1107,6 +1107,8 @@ extern "C" int kgv_replay_window(kgv_ctx* ctx, kgv_utxo_table* table, const kgv_
   ctx->last_replay.nt = nt; ctx->last_replay.ni = ni; ctx->last_replay.no = no; ctx->last_replay.n_blocks = n_blocks;
   ctx->last_replay.o_ids = o_ids; ctx->last_replay.o_itx = o_itx; ctx->last_replay.o_otx = o_otx; ctx->last_replay.o_ent = o_ent; ctx->last_replay.o_acc = o_acc;
   ctx->last_replay.o_txb = o_txb; ctx->last_replay.o_rng = o_rng;
+  ctx->last_replay.resolving = !legacy_walk;
+  ctx->last_replay.o_src = o_src; ctx->last_replay.o_inf = o_inf; ctx->last_replay.o_apv = o_apv;
   if (stats) {
     stats->n_accepted = n_acc; stats->n_sig_checks = n_items; stats->n_host_vm = n_vm;
     CK(cudaEventElapsedTime(&stats->pre_check_ms, ctx->ev_time[0], ctx->ev_time[1]));
@@ -1221,5 +1223,271 @@ extern "C" int kgv_replay_muhash(kgv_ctx* ctx, const uint32_t* group_first_block
   const bool dev = kgv_ptr_is_device(values768);
   CK(cudaMemcpyAsync(values768, vals, n_groups * 768, dev ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, st));
   if (!dev) CK(cudaStreamSynchronize(st));
+  return KGV_OK;
+}
+
+// ---------------------------------------------------------------------------------------------
+// kgv_replay_diffs: the UtxoDiff of every group of blocks of the last kgv_replay_window call - ctx.mergeset_diff of calculate_utxo_state
+// (utxo_validation.rs:119,148), i.e. UtxoDiff::add_transaction (utxo_diff.rs:224-260) over the group's accepted transactions in order.  No table
+// access: everything comes from the state the resolving walk leaves behind (source records, representative / accepted instance, accepting DAA
+// score, the spent entries dent holds with their scripts captured).
+//   removal   an input of an accepted transaction, unless it spends an output whose creator was accepted in the SAME group (the pair cancels)
+//   addition  an output of the accepted instance of a transaction, unless an accepted transaction of the same group spends it
+// Removals come in window input order and additions in window output order, so every group is a contiguous range of each list and the result does
+// not depend on scheduling.  Script bytes are laid out group after group, each as [its removals' scripts][its additions' scripts].
+// ---------------------------------------------------------------------------------------------
+struct DiffArgs {
+  const kgv_tx* txs;
+  const kgv_input* inputs;
+  const kgv_output* outputs;
+  const uint8_t* bytes;
+  const DevEntry* dent;            // spent entry of every input as found at its block's position (window state)
+  const uint64_t* ids;
+  const uint32_t *itx, *otx, *txb;
+  const ReplayRange* ranges;
+  const uint8_t* accept;
+  const ReplaySrc* src;
+  const ReplayTxInfo* info;
+  const unsigned long long* acc_pov;
+  uint32_t nt, ni, no, n_blocks;
+  uint32_t* acc_inst;              // per representative: the instance that was accepted
+  uint32_t* bgrp;                  // per block: its group
+  uint32_t* spg;                   // per window output (representative numbering): group of its accepted spender, ~0 if none
+  uint32_t *gi, *go;               // per group (n_groups + 1): first input / first output
+  uint32_t *rflag, *rlen;          // per input: removal?  its script length if so
+  uint32_t *aflag, *alen;          // per output: addition?  its script length if so
+  unsigned long long *rs, *rb, *as, *ab;  // exclusive scans of the four arrays above (n + 1 entries: the last one is the total)
+};
+
+// a transaction id is accepted at most once in a window (a second instance finds its inputs spent) unless one block carries it twice:
+// the smallest accepted instance then stands for it
+__global__ void k_diff_acc_inst(DiffArgs a) {
+  uint32_t ti = blockIdx.x * blockDim.x + threadIdx.x;
+  if (ti < a.nt && a.accept[ti]) atomicMin(&a.acc_inst[a.info[ti].rep], ti);
+}
+__global__ void k_diff_groups(DiffArgs a, const uint32_t* __restrict__ gf, uint32_t n_groups) {
+  uint32_t g = blockIdx.x * blockDim.x + threadIdx.x;
+  if (g > n_groups) return;
+  const uint32_t b0 = gf[g];
+  const uint32_t t = b0 < a.n_blocks ? a.ranges[b0].t0 : a.nt;  // (an empty block's range still starts at its first_tx)
+  a.gi[g] = t < a.nt ? a.txs[t].first_input : a.ni;
+  a.go[g] = t < a.nt ? a.txs[t].first_output : a.no;
+  if (g < n_groups)
+    for (uint32_t b = b0; b < gf[g + 1]; b++) a.bgrp[b] = g;
+}
+// at most one accepted transaction spends a window output (the walk's spent flag)
+__global__ void k_diff_spender_group(DiffArgs a) {
+  size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= a.ni) return;
+  const uint32_t ti = a.itx[i];
+  if (!a.accept[ti]) return;
+  const ReplaySrc r = a.src[i];
+  if (rs_kind(r) == RS_WINDOW) a.spg[r.flag & RS_FLAG_MASK] = a.bgrp[a.txb[ti]];
+}
+__global__ void k_diff_classify(DiffArgs a) {
+  size_t g = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (g < a.ni) {
+    const uint32_t ti = a.itx[g];
+    uint32_t f = 0;
+    if (a.accept[ti]) {  // an accepted input always has a source (the walk found it)
+      const ReplaySrc r = a.src[g];
+      f = !(rs_kind(r) == RS_WINDOW && a.bgrp[a.txb[a.acc_inst[r.src_tx]]] == a.bgrp[a.txb[ti]]);
+    }
+    a.rflag[g] = f;
+    a.rlen[g] = f ? a.dent[g].script_len : 0;
+    return;
+  }
+  g -= a.ni;
+  if (g >= a.no) return;
+  const uint32_t ti = a.otx[g];
+  uint32_t f = 0;
+  if (a.accept[ti]) {
+    const uint32_t r = a.info[ti].rep;
+    if (a.acc_inst[r] == ti) f = a.spg[a.txs[r].first_output + ((uint32_t)g - a.txs[ti].first_output)] != a.bgrp[a.txb[ti]];
+  }
+  a.aflag[g] = f;
+  a.alen[g] = f ? a.outputs[g].script_len : 0;
+}
+// the four exclusive scans, one block each, as k_exclusive_scan2 (64-bit sums: the byte totals are checked against the 32-bit script_off)
+__global__ void __launch_bounds__(1024) k_diff_scan4(DiffArgs a, unsigned long long* __restrict__ totals) {
+  const uint32_t* in = blockIdx.x == 0 ? a.rflag : blockIdx.x == 1 ? a.rlen : blockIdx.x == 2 ? a.aflag : a.alen;
+  unsigned long long* out = blockIdx.x == 0 ? a.rs : blockIdx.x == 1 ? a.rb : blockIdx.x == 2 ? a.as : a.ab;
+  const size_t n = blockIdx.x < 2 ? a.ni : a.no;
+  __shared__ unsigned long long part[1024];
+  const size_t per = (n + 1023) / 1024;
+  const size_t lo = (size_t)threadIdx.x * per;
+  const size_t hi = lo + per < n ? lo + per : n;
+  unsigned long long s = 0;
+  for (size_t i = lo; i < hi; i++) s += in[i];
+  part[threadIdx.x] = s;
+  __syncthreads();
+  for (int off = 1; off < 1024; off <<= 1) {
+    unsigned long long t = threadIdx.x >= off ? part[threadIdx.x - off] : 0;
+    __syncthreads();
+    part[threadIdx.x] += t;
+    __syncthreads();
+  }
+  unsigned long long run = part[threadIdx.x] - s;
+  for (size_t i = lo; i < hi; i++) {
+    const uint32_t v = in[i];
+    out[i] = run;
+    run += v;
+  }
+  if (threadIdx.x == 1023) { out[n] = part[1023]; totals[blockIdx.x] = part[1023]; }
+}
+__global__ void k_diff_ranges(DiffArgs a, uint32_t n_groups, kgv_diff_range* __restrict__ out) {
+  uint32_t g = blockIdx.x * blockDim.x + threadIdx.x;
+  if (g >= n_groups) return;
+  const uint32_t i0 = a.gi[g], i1 = a.gi[g + 1], o0 = a.go[g], o1 = a.go[g + 1];
+  kgv_diff_range r;
+  r.first_remove = a.rs[i0]; r.n_remove = a.rs[i1] - a.rs[i0];
+  r.first_add = a.as[o0]; r.n_add = a.as[o1] - a.as[o0];
+  out[g] = r;
+}
+__device__ __forceinline__ void store_key36(uint8_t* p, const uint32_t* k) {
+  if ((((uintptr_t)p) & 3) == 0) {
+#pragma unroll
+    for (int w = 0; w < 9; w++) ((uint32_t*)p)[w] = k[w];
+  } else {
+#pragma unroll
+    for (int w = 0; w < 9; w++) { p[4 * w] = (uint8_t)k[w]; p[4 * w + 1] = (uint8_t)(k[w] >> 8); p[4 * w + 2] = (uint8_t)(k[w] >> 16); p[4 * w + 3] = (uint8_t)(k[w] >> 24); }
+  }
+}
+__global__ void k_diff_gather(DiffArgs a, uint8_t* __restrict__ rem_keys, kgv_utxo_entry* __restrict__ rem_entries, uint8_t* __restrict__ add_keys,
+                              kgv_utxo_entry* __restrict__ add_entries, uint8_t* __restrict__ bytes) {
+  size_t g = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  uint32_t k[9];
+  kgv_utxo_entry e;
+  e.pad_[0] = e.pad_[1] = e.pad_[2] = e.pad_[3] = e.pad_[4] = 0;
+  const uint8_t* scr;
+  uint8_t* dst;
+  if (g < a.ni) {
+    if (!a.rflag[g]) return;
+    const uint32_t grp = a.bgrp[a.txb[a.itx[g]]];
+    const size_t j = a.rs[g];
+    const unsigned long long off = a.rb[g] + a.ab[a.go[grp]];
+    input_key(k, a.inputs[g]);
+    store_key36(rem_keys + 36 * j, k);
+    const DevEntry d = a.dent[g];
+    e.amount = d.amount; e.block_daa_score = d.block_daa_score; e.script_off = (uint32_t)off; e.script_len = d.script_len; e.spk_version = d.spk_version;
+    e.is_coinbase = d.is_coinbase;
+    rem_entries[j] = e;
+    scr = d.script; dst = bytes + off;
+  } else {
+    g -= a.ni;
+    if (g >= a.no || !a.aflag[g]) return;
+    const uint32_t ti = a.otx[g];
+    const uint32_t grp = a.bgrp[a.txb[ti]];
+    const size_t j = a.as[g];
+    const unsigned long long off = a.rb[a.gi[grp + 1]] + a.ab[g];
+#pragma unroll
+    for (int w = 0; w < 4; w++) { const uint64_t q = a.ids[4 * (size_t)ti + w]; k[2 * w] = (uint32_t)q; k[2 * w + 1] = (uint32_t)(q >> 32); }
+    k[8] = (uint32_t)g - a.txs[ti].first_output;
+    store_key36(add_keys + 36 * j, k);
+    const kgv_output& o = a.outputs[g];
+    const ReplayTxInfo inf = a.info[ti];
+    // the entry k_replay_finish_outputs stores and k_muhash_replay_elements hashes: the accepting block's DAA score, coinbase by position or subnetwork
+    e.amount = o.value; e.block_daa_score = a.acc_pov[inf.rep]; e.script_off = (uint32_t)off; e.script_len = o.script_len; e.spk_version = o.spk_version;
+    e.is_coinbase = (inf.bits & 1) ? 1 : 0;
+    add_entries[j] = e;
+    scr = a.bytes + o.script_off; dst = bytes + off;
+  }
+  for (uint32_t b = 0; b < e.script_len; b++) dst[b] = scr[b];
+}
+
+extern "C" int kgv_replay_diffs(kgv_ctx* ctx, const uint32_t* group_first_block, size_t n_groups, kgv_diff_range* ranges, uint8_t* rem_keys36,
+                                kgv_utxo_entry* rem_entries, uint8_t* add_keys36, kgv_utxo_entry* add_entries, uint8_t* bytes, size_t max_rem, size_t max_add,
+                                size_t bytes_cap, size_t* n_rem_out, size_t* n_add_out, size_t* bytes_out) {
+  if (!ctx) return KGV_ERR_ARG;
+  std::lock_guard<std::recursive_mutex> g(ctx->mu);
+  if (!group_first_block || n_groups == 0) { ctx->err = "kgv_replay_diffs: no groups"; return KGV_ERR_ARG; }
+  if (!ctx->last_replay.valid) { ctx->err = "kgv_replay_diffs refers to the last kgv_replay_window call, and none is current (another batch was staged or the table rehashed since)"; return KGV_ERR_ARG; }
+  const auto& L = ctx->last_replay;
+  if (!L.resolving) { ctx->err = "kgv_replay_diffs needs the resolving walk: the table-walking form (KGV_REPLAY_WALK=table) keeps no source records"; return KGV_ERR_ARG; }
+  if (kgv_ptr_is_device(group_first_block)) { ctx->err = "group offsets must be a host array"; return KGV_ERR_ARG; }
+  if (group_first_block[0] != 0 || group_first_block[n_groups] != L.n_blocks) { ctx->err = "groups must tile the blocks of the window"; return KGV_ERR_ARG; }
+  for (size_t i = 0; i < n_groups; i++) if (group_first_block[i] > group_first_block[i + 1]) { ctx->err = "group offsets not monotone"; return KGV_ERR_ARG; }
+  const bool counting = !rem_keys36;
+  bool dev = ranges ? kgv_ptr_is_device(ranges) != 0 : false;
+  if (!counting) {
+    if (!rem_entries || !add_keys36 || !add_entries || (bytes_cap && !bytes)) { ctx->err = "null buffer"; return KGV_ERR_ARG; }
+    dev = kgv_ptr_is_device(rem_keys36) != 0;
+    for (const void* p : {(const void*)rem_entries, (const void*)add_keys36, (const void*)add_entries, (const void*)bytes, (const void*)ranges})
+      if (p && (kgv_ptr_is_device(p) != 0) != dev) { ctx->err = "all output arrays of one call must be host pointers or all device pointers"; return KGV_ERR_ARG; }
+    if (dev && (((uintptr_t)rem_entries | (uintptr_t)add_entries) & 7)) { ctx->err = "entry arrays must be 8-byte aligned"; return KGV_ERR_ARG; }
+  }
+  CK(cudaSetDevice(ctx->device));
+  cudaStream_t st = ctx->stream;
+  uint8_t* R = ctx->d_replay;
+  const size_t nt = L.nt, ni = L.ni, no = L.no;
+  // scratch (d_work is free between validation calls)
+  size_t o_ai = 0, o_bg = al256(nt * 4), o_sp = al256(o_bg + L.n_blocks * 4), o_gf = al256(o_sp + no * 4), o_gi = al256(o_gf + (n_groups + 1) * 4),
+         o_go = al256(o_gi + (n_groups + 1) * 4), o_rf = al256(o_go + (n_groups + 1) * 4), o_rl = al256(o_rf + ni * 4), o_af = al256(o_rl + ni * 4),
+         o_al = al256(o_af + no * 4), o_rs = al256(o_al + no * 4), o_rb = al256(o_rs + (ni + 1) * 8), o_as = al256(o_rb + (ni + 1) * 8),
+         o_ab = al256(o_as + (no + 1) * 8), o_rg = al256(o_ab + (no + 1) * 8), o_tot = al256(o_rg + n_groups * sizeof(kgv_diff_range));
+  int rc = kgv_reserve(ctx, &ctx->d_work, &ctx->d_work_cap, o_tot + 64);
+  if (rc) return rc;
+  uint8_t* Wk = ctx->d_work;
+  DiffArgs a;
+  a.txs = (const kgv_tx*)L.txs; a.inputs = (const kgv_input*)L.inputs; a.outputs = (const kgv_output*)L.outputs; a.bytes = (const uint8_t*)L.bytes;
+  a.dent = (const DevEntry*)(R + L.o_ent); a.ids = (const uint64_t*)(R + L.o_ids);
+  a.itx = (const uint32_t*)(R + L.o_itx); a.otx = (const uint32_t*)(R + L.o_otx); a.txb = (const uint32_t*)(R + L.o_txb);
+  a.ranges = (const ReplayRange*)(R + L.o_rng); a.accept = R + L.o_acc; a.src = (const ReplaySrc*)(R + L.o_src); a.info = (const ReplayTxInfo*)(R + L.o_inf);
+  a.acc_pov = (const unsigned long long*)(R + L.o_apv);
+  a.nt = (uint32_t)nt; a.ni = (uint32_t)ni; a.no = (uint32_t)no; a.n_blocks = (uint32_t)L.n_blocks;
+  a.acc_inst = (uint32_t*)(Wk + o_ai); a.bgrp = (uint32_t*)(Wk + o_bg); a.spg = (uint32_t*)(Wk + o_sp); a.gi = (uint32_t*)(Wk + o_gi); a.go = (uint32_t*)(Wk + o_go);
+  a.rflag = (uint32_t*)(Wk + o_rf); a.rlen = (uint32_t*)(Wk + o_rl); a.aflag = (uint32_t*)(Wk + o_af); a.alen = (uint32_t*)(Wk + o_al);
+  a.rs = (unsigned long long*)(Wk + o_rs); a.rb = (unsigned long long*)(Wk + o_rb); a.as = (unsigned long long*)(Wk + o_as); a.ab = (unsigned long long*)(Wk + o_ab);
+  kgv_diff_range* drg = (kgv_diff_range*)(Wk + o_rg);
+  unsigned long long* dtot = (unsigned long long*)(Wk + o_tot);
+  CK(cudaMemcpyAsync(Wk + o_gf, group_first_block, (n_groups + 1) * 4, cudaMemcpyHostToDevice, st));
+  CK(cudaMemsetAsync(a.acc_inst, 0xFF, nt * 4, st));
+  if (no) CK(cudaMemsetAsync(a.spg, 0xFF, no * 4, st));
+  k_diff_acc_inst<<<nblk(nt, 256), 256, 0, st>>>(a);
+  CK(cudaGetLastError());
+  k_diff_groups<<<nblk(n_groups + 1, 128), 128, 0, st>>>(a, (const uint32_t*)(Wk + o_gf), (uint32_t)n_groups);
+  CK(cudaGetLastError());
+  if (ni) { k_diff_spender_group<<<nblk(ni, 256), 256, 0, st>>>(a); CK(cudaGetLastError()); }
+  if (ni + no) { k_diff_classify<<<nblk(ni + no, 256), 256, 0, st>>>(a); CK(cudaGetLastError()); }
+  k_diff_scan4<<<4, 1024, 0, st>>>(a, dtot);
+  CK(cudaGetLastError());
+  k_diff_ranges<<<nblk(n_groups, 128), 128, 0, st>>>(a, (uint32_t)n_groups, drg);
+  CK(cudaGetLastError());
+  ctx->launches += 6 + (ni ? 1 : 0) + (ni + no ? 1 : 0);
+  unsigned long long tot[4];
+  CK(cudaMemcpyAsync(tot, dtot, sizeof tot, cudaMemcpyDeviceToHost, st));
+  if (ranges) CK(cudaMemcpyAsync(ranges, drg, n_groups * sizeof(kgv_diff_range), dev ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  const size_t n_rem = (size_t)tot[0], n_add = (size_t)tot[2], n_bytes = (size_t)(tot[1] + tot[3]);
+  if (n_rem_out) *n_rem_out = n_rem;
+  if (n_add_out) *n_add_out = n_add;
+  if (bytes_out) *bytes_out = n_bytes;
+  if (n_bytes > 0xFFFFFFFFull) { ctx->err = "kgv_replay_diffs: the script bytes of the diffs exceed the 32-bit script_off"; return KGV_ERR_LIMIT; }
+  if (counting) return KGV_OK;
+  if (n_rem > max_rem || n_add > max_add || n_bytes > bytes_cap) { ctx->err = "kgv_replay_diffs: the caller's arrays are too small (sizes returned)"; return KGV_ERR_NOMEM; }
+  if (ni + no == 0) return KGV_OK;
+  uint8_t *rk = rem_keys36, *ak = add_keys36, *db = bytes;
+  kgv_utxo_entry *re = rem_entries, *ae = add_entries;
+  size_t s_re = al256(n_rem * 36), s_ak = al256(s_re + n_rem * sizeof(kgv_utxo_entry)), s_ae = al256(s_ak + n_add * 36), s_b = al256(s_ae + n_add * sizeof(kgv_utxo_entry));
+  if (!dev) {
+    rc = kgv_reserve(ctx, &ctx->d_out, &ctx->d_out_cap, s_b + n_bytes + 16);
+    if (rc) return rc;
+    rk = ctx->d_out; re = (kgv_utxo_entry*)(ctx->d_out + s_re); ak = ctx->d_out + s_ak; ae = (kgv_utxo_entry*)(ctx->d_out + s_ae); db = ctx->d_out + s_b;
+  }
+  k_diff_gather<<<nblk(ni + no, 128), 128, 0, st>>>(a, rk, re, ak, ae, db);
+  CK(cudaGetLastError());
+  ctx->launches++;
+  if (!dev) {
+    if (n_rem) {
+      CK(cudaMemcpyAsync(rem_keys36, rk, n_rem * 36, cudaMemcpyDeviceToHost, st));
+      CK(cudaMemcpyAsync(rem_entries, re, n_rem * sizeof(kgv_utxo_entry), cudaMemcpyDeviceToHost, st));
+    }
+    if (n_add) {
+      CK(cudaMemcpyAsync(add_keys36, ak, n_add * 36, cudaMemcpyDeviceToHost, st));
+      CK(cudaMemcpyAsync(add_entries, ae, n_add * sizeof(kgv_utxo_entry), cudaMemcpyDeviceToHost, st));
+    }
+    if (n_bytes) CK(cudaMemcpyAsync(bytes, db, n_bytes, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+  }
   return KGV_OK;
 }

@@ -18,7 +18,7 @@ import ctypes
 
 import numpy as np
 
-from .txbatch import TxBatch, build_batch
+from .txbatch import ENTRY_DTYPE, TxBatch, build_batch
 from .validator import FLAGS_FULL, RESULT_DTYPE, TX_OK, TX_SKIPPED_COINBASE, GpuUtxoSet, TransactionValidator
 from .verifier import _c_batch
 
@@ -39,6 +39,50 @@ def replay_blocks_array(ranges):
     for i, (f, n, pov, fl) in enumerate(ranges):
         a[i] = (f, n, pov, fl, 0)
     return a
+
+
+class ReplayDiffs:
+    """What kgv_replay_diffs returns: per group g (ranges[g] = first_remove, n_remove, first_add, n_add) its removals (outpoint keys and the
+    entries they had) and additions, in window order; every entry's script_off points into `bytes`."""
+
+    def __init__(self, ranges, rem_keys36, rem_entries, add_keys36, add_entries, arena):
+        self.ranges, self.rem_keys36, self.rem_entries, self.add_keys36, self.add_entries, self.bytes = ranges, rem_keys36, rem_entries, add_keys36, add_entries, arena
+
+    def __len__(self):
+        return len(self.ranges)
+
+    def group(self, g):
+        """(rem_keys36, rem_entries, add_keys36, add_entries) of group g (views into the whole arrays)"""
+        fr, nr, fa, na = (int(x) for x in self.ranges[g])
+        return self.rem_keys36[fr:fr + nr], self.rem_entries[fr:fr + nr], self.add_keys36[fa:fa + na], self.add_entries[fa:fa + na]
+
+    def utxo_diff(self, g):
+        """group g as a utxo_diff.UtxoDiff (outpoint (txid, index) -> entry dict)"""
+        from .utxo_diff import UtxoDiff
+
+        def coll(keys, ents):
+            out = {}
+            for k, e in zip(keys, ents):
+                off, n = int(e["script_off"]), int(e["script_len"])
+                out[(k[:32].tobytes(), int.from_bytes(k[32:].tobytes(), "little"))] = {
+                    "amount": int(e["amount"]), "spk_version": int(e["spk_version"]), "script": self.bytes[off:off + n].tobytes(),
+                    "block_daa_score": int(e["block_daa_score"]), "is_coinbase": bool(e["is_coinbase"])}
+            return out
+        rk, re, ak, ae = self.group(g)
+        return UtxoDiff(add=coll(ak, ae), remove=coll(rk, re))
+
+    def apply(self, utxo_set, g, reverse=False):
+        """write group g's diff into a GpuUtxoSet or view (kgv_utxo_apply_diff); reverse=True undoes it (UtxoDiff::as_reversed, processor.rs:395-397).
+        Returns (rem_status, add_status): 1 = was present / inserted."""
+        rk, re, ak, ae = self.group(g)
+        if reverse:
+            rk, (ak, ae) = ak, (rk, re)
+        ae = ae.copy()
+        lo = int(ae["script_off"].min()) if len(ae) else 0
+        hi = int((ae["script_off"].astype(np.int64) + ae["script_len"]).max()) if len(ae) else 0
+        ae["script_off"] -= lo  # the group's scripts are one contiguous range of the arena: hand over only that
+        return utxo_set.apply_diff(rem_keys36=rk if len(rk) else None, add_keys36=ak if len(ak) else None, add_entries=ae if len(ae) else None,
+                                   add_bytes=np.concatenate([self.bytes[lo:hi], np.zeros(8, np.uint8)]))
 
 
 class DagReplayer:
@@ -113,6 +157,24 @@ class DagReplayer:
         if len(gf) > 1:
             self.ctx._check(self.ctx._lib.kgv_replay_muhash(self.ctx._h, gf.ctypes.data, len(gf) - 1, out.ctypes.data))
         return out
+
+    def replay_diffs(self, group_first_block):
+        """kgv_replay_diffs for the window just replayed: the UtxoDiff of every group of blocks (ctx.mergeset_diff, utxo_validation.rs:119,148)"""
+        gf = np.ascontiguousarray(group_first_block, dtype=np.uint32)
+        n_groups = len(gf) - 1
+        lib, h = self.ctx._lib, self.ctx._h
+        ranges = np.zeros((max(n_groups, 1), 4), dtype=np.uint64)
+        nr, na, nb = ctypes.c_size_t(), ctypes.c_size_t(), ctypes.c_size_t()
+        self.ctx._check(lib.kgv_replay_diffs(h, gf.ctypes.data, n_groups, ranges.ctypes.data, None, None, None, None, None, 0, 0, 0,
+                                             ctypes.byref(nr), ctypes.byref(na), ctypes.byref(nb)))
+        rk = np.zeros((max(nr.value, 1), 36), dtype=np.uint8)
+        re = np.zeros(max(nr.value, 1), dtype=ENTRY_DTYPE)
+        ak = np.zeros((max(na.value, 1), 36), dtype=np.uint8)
+        ae = np.zeros(max(na.value, 1), dtype=ENTRY_DTYPE)
+        by = np.zeros(max(nb.value, 8), dtype=np.uint8)
+        self.ctx._check(lib.kgv_replay_diffs(h, gf.ctypes.data, n_groups, ranges.ctypes.data, rk.ctypes.data, re.ctypes.data, ak.ctypes.data, ae.ctypes.data,
+                                             by.ctypes.data, nr.value, na.value, nb.value, ctypes.byref(nr), ctypes.byref(na), ctypes.byref(nb)))
+        return ReplayDiffs(ranges[:n_groups], rk[:nr.value], re[:nr.value], ak[:na.value], ae[:na.value], by[:nb.value])
 
     def replay_windowed(self, blocks):
         """blocks: list of (txs, pov[, flags]) forming ONE window. Returns per-block RESULT arrays (same values as blockwise)."""
