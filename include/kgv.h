@@ -387,7 +387,8 @@ typedef struct {
   uint64_t n_sig_checks; /* candidate (signature, key) pairs verified in the pre-check */
   uint64_t n_host_vm;    /* transactions decided by the host script engine */
   float pre_check_ms;    /* device time of the batched script pre-check (tx ids, window map, populate, sighash, verify, resolve) */
-  float in_order_ms;     /* device time of the in-order pass */
+  float in_order_ms;     /* device time from the end of the pre-check to the end of the finishing passes (slot map, static rules, walk,
+                            verdicts, table updates, results) */
 } kgv_replay_stats;
 /* results: n_txs records (host or device memory): the UTXO-context verdict when the context rules fail, else the script
  * verdict (KGV_TX_SKIPPED_COINBASE for coinbases).  accept (may be NULL): n_txs bytes, 1 = folded into the table.
@@ -415,7 +416,7 @@ int kgv_replay_muhash(kgv_ctx* ctx, const uint32_t* group_first_block, size_t n_
  * Output arrays (ranges included) are all host or all device memory; device entry arrays must be 8-byte aligned.  With rem_keys36 == NULL only
  * the sizes (*n_rem_out, *n_add_out, *bytes_out) and `ranges` (may be NULL) are returned; arrays smaller than that give KGV_ERR_NOMEM with the
  * sizes and ranges still set.  Valid under the same conditions as kgv_replay_muhash: either may come first and either may be repeated.  Without a
- * current window, with groups that do not tile it, or after a window replayed with KGV_REPLAY_WALK=table: KGV_ERR_ARG. */
+ * current window or with groups that do not tile it: KGV_ERR_ARG. */
 typedef struct {
   uint64_t first_remove, n_remove;  /* rows of rem_keys36 / rem_entries that belong to the group */
   uint64_t first_add, n_add;        /* rows of add_keys36 / add_entries */

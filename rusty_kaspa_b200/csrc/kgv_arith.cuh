@@ -631,10 +631,7 @@ KGV_HD void fe_reduce_wide(fe& r, const uint32_t* t) {
 // operands by value: ptxas keeps everything in registers across the call (no stack traffic), and
 // the kernels shrink from ~1.4 MB of straight-line SASS to a few tens of KB that stay in the
 // instruction cache.  The host unit-test build simply inlines them.
-#ifndef KGV_NOINLINE_MUL
-#define KGV_NOINLINE_MUL 1
-#endif
-#if defined(__CUDACC__) && KGV_NOINLINE_MUL
+#if defined(__CUDACC__)
 static __device__ __noinline__ fe fe_mul_call(fe a, fe b) {
   fe r;
   uint32_t t[16];
@@ -727,7 +724,7 @@ KGV_HD void sqr_wide(uint32_t* t, const uint32_t* a) {
   for (int i = 0; i < 16; i++) t[i] = x[i];
 }
 
-#if defined(__CUDACC__) && KGV_NOINLINE_MUL
+#if defined(__CUDACC__)
 static __device__ __noinline__ fe fe_sqr_call(fe a) {
   fe r;
   uint32_t t[16];
@@ -744,33 +741,15 @@ KGV_HD void fe_sqr(fe& r, const fe& a) {
 }
 #endif
 
-// r = a^(2^n).  KGV_SQRN_CALL=1 makes a whole run of squarings ONE call (the squaring inlined into the loop of a non-inlined function: the
-// exponentiation chains - square root of lift_x, the shared inversion, ~510 squarings per verification - then pay the by-value call ABI once per
-// run instead of once per squaring).  Measured when the kernels were tuned on the previous target GPU (not re-measured on H100): fewer instructions but
-// slower for the field (a second copy of the squaring in the hot code), faster for the scalar inversion of ECDSA - so it is on for scalars only (KGV_SC_SQRN_CALL).
-#ifndef KGV_SQRN_CALL
-#define KGV_SQRN_CALL 0
-#endif
-#ifndef KGV_SC_SQRN_CALL
-#define KGV_SC_SQRN_CALL 1
-#endif
-#if defined(__CUDACC__) && KGV_NOINLINE_MUL && KGV_SQRN_CALL
-static __device__ __noinline__ fe fe_sqr_n_call(fe a, int n) {
-#pragma unroll 1
-  for (int i = 0; i < n; i++) {
-    uint32_t t[16];
-    sqr_wide(t, a.v);
-    fe_reduce_wide(a, t);
-  }
-  return a;
-}
-KGV_HD void fe_sqr_n(fe& r, const fe& a, int n) { r = fe_sqr_n_call(a, n); }
-#else
+// r = a^(2^n), one fe_sqr call per squaring.  Making a whole run of squarings ONE call instead (the squaring inlined into the loop of a
+// non-inlined function, so the exponentiation chains - square root of lift_x, the shared inversion, ~510 squarings per verification - pay the
+// by-value call ABI once per run) was measured when the kernels were tuned on the previous target GPU (not re-measured on H100): fewer
+// instructions but slower for the field (a second copy of the squaring in the hot code).  The scalar side does use it (sc_pow2k_mul_call,
+// kgv_secp.cuh), where it made the scalar inversion of ECDSA faster.
 KGV_HD void fe_sqr_n(fe& r, const fe& a, int n) {
   r = a;
   for (int i = 0; i < n; i++) fe_sqr(r, r);
 }
-#endif
 
 // small multiples
 KGV_HD void fe_mul3(fe& r, const fe& a) { fe t; fe_add(t, a, a); fe_add(r, t, a); }

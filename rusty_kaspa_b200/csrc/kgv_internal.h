@@ -18,7 +18,6 @@
 #define KGV_ITEMS 4           // signatures per thread sharing one modular inversion (see k_schnorr_verify)
 #endif
 
-struct kgv_dev_batch_fwd;
 struct kgv_ctx {
   int device = 0;
   cudaStream_t own_stream = nullptr;
@@ -63,12 +62,10 @@ struct kgv_ctx {
   // state of the last kgv_replay_window call, kept for kgv_replay_muhash / kgv_replay_diffs (cleared by any call that stages another batch)
   struct {
     bool valid = false;
-    bool resolving = false;  // the resolving walk ran (source records, tx info and accepting DAA scores below are valid)
-    kgv_dev_batch_fwd* unused_ = nullptr;
     const void *txs = nullptr, *inputs = nullptr, *outputs = nullptr, *bytes = nullptr;
     size_t nt = 0, ni = 0, no = 0, n_blocks = 0;
     size_t o_ids = 0, o_itx = 0, o_otx = 0, o_ent = 0, o_acc = 0, o_txb = 0, o_rng = 0;  // offsets into d_replay
-    size_t o_src = 0, o_inf = 0, o_apv = 0;  // resolving walk only
+    size_t o_src = 0, o_inf = 0, o_apv = 0;
   } last_replay;
   struct kgv_sigcache* sigcache = nullptr;  // kgv_set_sigcache: verdicts of the validation calls are looked up / remembered here
   struct kgv_comm* shard_comm = nullptr;  // kgv_set_sharding: signature checks of the validation calls are split over its ranks

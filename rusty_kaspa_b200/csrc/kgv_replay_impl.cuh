@@ -15,10 +15,10 @@
 //               signature checks per launch).  Spent outputs come from the UTXO table or, when the output is created inside
 //               the window, from the creating transaction (found through a window hash map  tx id -> tx index  built on the
 //               device).  Which of the two exists at the spending block's position is irrelevant for the script verdict.
-//   in-order    one persistent single-CTA kernel walks the blocks: populate from the table (now position dependent),
-//               UTXO-context rules, accept = context ok && scripts ok, erase spent / insert created entries, next block.
-//               Three CTA barriers per block instead of >= 15 kernel launches; slots of the next block are prefetched
-//               into L2 while the current block is decided.
+//   in-order    whatever depends only on the outpoint is resolved for the whole window in parallel; one persistent
+//               single-CTA kernel then walks the blocks deciding only whether each input's outpoint still exists at its
+//               block's position (accept = context ok && scripts ok), and parallel passes erase the spent entries and insert
+//               the created ones that survive the window (see "The in-order pass" below).
 //
 // Result per transaction: the context verdict when the context rules fail, else the script verdict - the order
 // validate_populated_transaction_and_get_fee reports them in (tx_validation_in_utxo_context.rs:34-61).
@@ -51,37 +51,6 @@ __device__ __forceinline__ int wm_find(const uint64_t* __restrict__ ids, const u
   return -1;
 }
 
-// spent entry of every input for the pre-check: UTXO table first, else an output created inside the window
-__global__ void k_populate_window(TableView t, BatchView b, size_t n_inputs, const uint64_t* __restrict__ ids, const uint32_t* __restrict__ wm, uint64_t wm_mask,
-                                  DevEntry* __restrict__ out) {
-  size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n_inputs) return;
-  const kgv_input& in = b.inputs[i];
-  uint32_t k[9];
-  input_key(k, in);
-  SlotHead h;
-  UtxoSlot* s = table_find(t, k, h);
-  DevEntry d;
-  if (s) head_to_entry(d, t, s, h);
-  else {
-    entry_absent(d);
-    uint64_t id[4];
-#pragma unroll
-    for (int w = 0; w < 4; w++) id[w] = (uint64_t)k[2 * w] | ((uint64_t)k[2 * w + 1] << 32);
-    int src = wm_find(ids, wm, wm_mask, id);
-    if (src >= 0) {
-      const kgv_tx& stx = b.txs[src];
-      if (in.prev_index < stx.n_outputs) {
-        const kgv_output& o = b.outputs[stx.first_output + in.prev_index];
-        d.amount = o.value; d.script = b.bytes + o.script_off; d.script_len = o.script_len; d.spk_version = o.spk_version;
-        d.is_coinbase = tx_is_coinbase(stx) ? 1 : 0;
-        d.found = 1;
-      }
-    }
-  }
-  out[i] = d;
-}
-
 // per-transaction block index and the pre-check's starting status
 #define KGV_PRE_SKIPPED 0xFEu  // not script-checked in the pre-pass (coinbase position, SkipScriptChecks block)
 __global__ void k_replay_tx_block(const kgv_replay_block* __restrict__ blocks, uint32_t n_blocks, uint32_t* __restrict__ tx_block) {
@@ -106,10 +75,7 @@ __global__ void k_replay_pre_status(BatchView b, uint32_t n_txs, const kgv_repla
   }
   pre[ti] = r;
 }
-// ---------------------------------------------------------------------------------------------
-// the in-order pass: ONE CTA, blocks in sequence
-// ---------------------------------------------------------------------------------------------
-// per-block ranges, computed in parallel before the walk so that the in-order kernel never chases tx records to find them
+// per-block ranges, computed in parallel before the walk so that it never chases tx records to find them
 struct __align__(16) ReplayRange {  // 48 bytes: a whole number of 16-byte units (the walk fetches these with bulk copies)
   uint32_t t0, t1, i0, i1, o0, o1, flags, pad_;
   uint64_t pov;
@@ -131,230 +97,8 @@ __global__ void k_replay_ranges(const kgv_replay_block* __restrict__ blocks, uin
   out[b] = r;
 }
 
-struct ReplayArgs {
-  TableView t;
-  BatchView b;              // b.entries = dent (written here: the entry every input finds AT ITS BLOCK'S POSITION)
-  DevEntry* dent;
-  uint8_t* spent_scripts;   // 72 bytes per input: copy of an inline script (the slot may be reused later in the window)
-  UtxoSlot** slotp;         // slot of every input (for the erase)
-  const uint64_t* ids;
-  const uint32_t* itx;
-  const uint32_t* otx;
-  const ReplayRange* ranges;
-  uint32_t n_blocks;
-  kgv_params prm;
-  const kgv_tx_result* pre; // script verdicts of the pre-check
-  kgv_tx_result* res;       // final verdicts
-  uint8_t* accept;
-  unsigned long long* stats; // [0] accepted transactions
-  unsigned long long* timers; // KGV_DEBUG only: cycles per phase (stage, scripts, A, B, C)
-};
-
-// L2 prefetch of the 128-byte lines covering [p, p + bytes), dealt to the threads from the TOP of the CTA downwards (the low
-// threads carry the per-input / per-transaction work of the current block)
-__device__ __forceinline__ void prefetch_range(const void* p, size_t bytes, uint32_t rtid, uint32_t nth) {
-  if (!bytes) return;
-  const uintptr_t lo = (uintptr_t)p & ~(uintptr_t)127, hi = (uintptr_t)p + bytes;
-  for (uintptr_t q = lo + 128 * (uintptr_t)rtid; q < hi; q += 128 * (uintptr_t)nth) prefetch_l2((const void*)q);
-}
-
-// The walk is a chain of dependent memory accesses per block (record -> key -> slot -> entry -> verdict -> slot update).  Left in global
-// memory every link costs an L2 round trip or a DRAM miss, and ~40 dependent links per block add up to many microseconds per block.
-// So each block is STAGED in shared memory first: all 1024 threads copy its transaction / input / output records, tx ids, script verdicts
-// and index maps with independent 8-byte loads (one memory latency for everything), then the output scripts the inserts will store; the
-// three phases then run out of shared memory and touch global memory only for the table itself (probe, claim, store) and for the results.
-// Record ranges are prefetched into L2 two blocks ahead (by address range only: a prefetch that itself needs dependent loads - e.g. the
-// table slots of the next block - was measured to cost more on the critical path than the miss it hides).  Blocks too large for the staging area take the
-// same code path with the pointers left on the global arrays.
-#define RP_MAXT 320u
-#define RP_MAXI 640u
-#define RP_MAXO 768u
-#define RP_SCR 40u  // staged bytes per output script (standard scripts are 34 / 35 bytes)
-struct ReplaySmem {
-  kgv_tx txs[RP_MAXT];
-  kgv_input inputs[RP_MAXI];
-  kgv_output outputs[RP_MAXO];
-  uint64_t ids[4 * RP_MAXT];
-  kgv_tx_result pre[RP_MAXT];
-  DevEntry dent[RP_MAXI];
-  UtxoSlot* slot[RP_MAXI];
-  uint32_t itx[RP_MAXI + 2];  // staged from an 8-byte aligned start: one word of slack on either side
-  uint32_t otx[RP_MAXO + 2];
-  uint32_t scr[RP_MAXO][RP_SCR / 4];
-  uint8_t acc[RP_MAXT];
-};
-
-__device__ __forceinline__ void copy8(void* dst, const void* src, size_t bytes, uint32_t tid, uint32_t nth) {  // both 8-byte aligned
-  const size_t n = bytes >> 3;
-  const uint64_t* s = (const uint64_t*)src;
-  uint64_t* d = (uint64_t*)dst;
-  for (size_t i = tid; i < n; i += nth) d[i] = s[i];
-}
-__device__ __forceinline__ void copy4(void* dst, const void* src, size_t bytes, uint32_t tid, uint32_t nth) {
-  const size_t n = bytes >> 2;
-  const uint32_t* s = (const uint32_t*)src;
-  uint32_t* d = (uint32_t*)dst;
-  for (size_t i = tid; i < n; i += nth) d[i] = s[i];
-}
-
-__global__ void __launch_bounds__(1024, 1) k_replay_inorder(ReplayArgs a) {
-  extern __shared__ __align__(16) uint8_t smem_raw[];
-  ReplaySmem& S = *reinterpret_cast<ReplaySmem*>(smem_raw);
-  const uint32_t tid = threadIdx.x, nth = blockDim.x, rtid = nth - 1 - tid;
-  __shared__ unsigned long long s_acc;
-  __shared__ int s_live, s_tomb;  // table counter deltas of this launch (one global atomic at the end instead of one per entry)
-  if (tid == 0) { s_acc = 0; s_live = 0; s_tomb = 0; }
-  auto prefetch_records = [&](uint32_t bi) {
-    if (bi >= a.n_blocks) return;
-    const ReplayRange r = a.ranges[bi];
-    prefetch_range(a.b.txs + r.t0, (size_t)(r.t1 - r.t0) * sizeof(kgv_tx), rtid, nth);
-    prefetch_range(a.b.inputs + r.i0, (size_t)(r.i1 - r.i0) * sizeof(kgv_input), rtid, nth);
-    prefetch_range(a.b.outputs + r.o0, (size_t)(r.o1 - r.o0) * sizeof(kgv_output), rtid, nth);
-    prefetch_range(a.ids + 4 * (size_t)r.t0, (size_t)(r.t1 - r.t0) * 32, rtid, nth);
-    prefetch_range(a.pre + r.t0, (size_t)(r.t1 - r.t0) * sizeof(kgv_tx_result), rtid, nth);
-    prefetch_range(a.itx + r.i0, (size_t)(r.i1 - r.i0) * 4, rtid, nth);
-    prefetch_range(a.otx + r.o0, (size_t)(r.o1 - r.o0) * 4, rtid, nth);
-  };
-  prefetch_records(0);
-  prefetch_records(1);
-  __syncthreads();
-  long long tk[6] = {0, 0, 0, 0, 0, 0}, c0 = 0;  // KGV_DEBUG: cycles per phase, as seen by thread 0
-#define RP_TICK(k) do { if (a.timers && tid == 0) { long long c1 = clock64(); tk[k] += c1 - c0; c0 = c1; } } while (0)
-  if (a.timers && tid == 0) c0 = clock64();
-  for (uint32_t bi = 0; bi < a.n_blocks; bi++) {
-    const ReplayRange bl = a.ranges[bi];
-    prefetch_records(bi + 2);
-    if (bl.t1 == bl.t0) continue;
-    const uint32_t t0 = bl.t0, t1 = bl.t1, i0 = bl.i0, i1 = bl.i1, o0 = bl.o0, o1 = bl.o1;
-    const bool staged = t1 - t0 <= RP_MAXT && i1 - i0 <= RP_MAXI && o1 - o0 <= RP_MAXO;
-    // absolute-index views of this block's data: shared memory when staged, the global arrays otherwise
-    const kgv_tx* p_txs = a.b.txs;
-    const kgv_input* p_in = a.b.inputs;
-    const kgv_output* p_out = a.b.outputs;
-    const uint64_t* p_ids = a.ids;
-    const kgv_tx_result* p_pre = a.pre;
-    const uint32_t *p_itx = a.itx, *p_otx = a.otx;
-    DevEntry* p_dent = a.dent;
-    UtxoSlot** p_slot = a.slotp;
-    uint8_t* p_acc = a.accept;
-    if (staged) {
-      // plain range-after-range copies: measured FASTER on the single SM than one flat, batched copy (the index arithmetic of the flat form costs
-      // more issue slots over 32 warps than the serialised latencies it removes: 13.6 k vs 8.0 k cycles per block)
-      copy8(S.txs, a.b.txs + t0, (size_t)(t1 - t0) * sizeof(kgv_tx), tid, nth);
-      copy8(S.inputs, a.b.inputs + i0, (size_t)(i1 - i0) * sizeof(kgv_input), tid, nth);
-      copy8(S.outputs, a.b.outputs + o0, (size_t)(o1 - o0) * sizeof(kgv_output), tid, nth);
-      copy8(S.ids, a.ids + 4 * (size_t)t0, (size_t)(t1 - t0) * 32, tid, nth);
-      copy8(S.pre, a.pre + t0, (size_t)(t1 - t0) * sizeof(kgv_tx_result), tid, nth);
-      copy8(S.itx, a.itx + (i0 & ~1u), (size_t)((i1 - (i0 & ~1u) + 1u) / 2u) * 8, tid, nth);
-      copy8(S.otx, a.otx + (o0 & ~1u), (size_t)((o1 - (o0 & ~1u) + 1u) / 2u) * 8, tid, nth);
-      p_txs = S.txs - t0; p_in = S.inputs - i0; p_out = S.outputs - o0; p_ids = S.ids - 4 * (size_t)t0; p_pre = S.pre - t0;
-      p_itx = S.itx - (i0 & ~1u); p_otx = S.otx - (o0 & ~1u); p_dent = S.dent - i0; p_slot = S.slot - i0; p_acc = S.acc - t0;
-      __syncthreads();
-      RP_TICK(0);
-      if (!(bl.flags & KGV_REPLAY_VERIFY_ONLY))  // scripts the inserts will store (consumed in phase C, two barriers from here)
-        for (uint32_t o = o0 + rtid; o < o1; o += nth) {
-          const kgv_output& out = p_out[o];
-          if (out.script_len <= RP_SCR) {
-            uint32_t w[17];
-            load_script_words(w, a.b.bytes + out.script_off, out.script_len);
-#pragma unroll
-            for (int q = 0; q < (int)(RP_SCR / 4); q++) S.scr[o - o0][q] = w[q];
-          }
-        }
-    }
-    RP_TICK(1);
-    // ---- A: populate from the table as it stands after the previous block (utxo_validation.rs:319-327)
-    for (uint32_t i = i0 + tid; i < i1; i += nth) {
-      uint32_t k[9];
-      input_key(k, p_in[i]);
-      SlotHead h;
-      UtxoSlot* s = table_find(a.t, k, h);
-      DevEntry d;
-      if (s) {
-        head_to_entry(d, a.t, s, h);
-        if (d.script_len <= INLINE_SCRIPT) {  // keep the bytes: MuHash / diff consumers read them after the slot may have been reused
-          uint32_t* dst = (uint32_t*)(a.spent_scripts + 72 * (size_t)i);
-          const uint32_t* src = (const uint32_t*)((const uint8_t*)s + 64);
-          dst[0] = h.w[15];
-          const uint32_t nw = (d.script_len + 3) >> 2;
-          for (uint32_t w = 1; w < nw; w++) dst[w] = __ldcg(src + (w - 1));
-          d.script = (const uint8_t*)dst;
-        }
-      } else entry_absent(d);
-      p_dent[i] = d;
-      p_slot[i] = s;
-      if (staged) a.dent[i] = d;  // the global copy feeds kgv_replay_muhash
-    }
-    __syncthreads();
-    RP_TICK(2);
-    // ---- B: context rules and the acceptance decision
-    {
-      const BatchView sb{p_txs, p_in, p_out, p_dent, a.b.bytes};
-      for (uint32_t ti = t0 + tid; ti < t1; ti += nth) {
-        const bool cb = ti == t0 || tx_is_coinbase(p_txs[ti]);
-        kgv_tx_result r = tx_context_rules(sb, ti, bl.pov, KGV_FLAGS_SKIP_SCRIPT_CHECKS, a.prm, cb);
-        bool acc;
-        if (cb) acc = (ti == t0) && (bl.flags & KGV_REPLAY_ACCEPT_COINBASE);
-        else {
-          acc = r.status == KGV_TX_OK;
-          if (acc && !(bl.flags & KGV_REPLAY_SKIP_SCRIPTS)) {
-            const kgv_tx_result p = p_pre[ti];
-            if (p.status != KGV_TX_OK) { r.status = p.status; r.script_err = p.script_err; r.fail_input = p.fail_input; acc = false; }
-          }
-        }
-        if (bl.flags & KGV_REPLAY_VERIFY_ONLY) acc = false;
-        a.res[ti] = r;
-        p_acc[ti] = acc ? 1 : 0;
-        if (staged) a.accept[ti] = acc ? 1 : 0;
-        if (acc && !cb) atomicAdd(&s_acc, 1ull);
-      }
-    }
-    __syncthreads();
-    RP_TICK(3);
-    // ---- C: UtxoDiff::add_transaction straight into the table (utxo_diff.rs:233-247).  One CTA: the barrier orders these writes
-    // before the next block's probes, no device-wide fence is needed inside the walk.
-    if (!(bl.flags & KGV_REPLAY_VERIFY_ONLY)) {
-      for (uint32_t i = i0 + tid; i < i1; i += nth) {
-        if (!p_acc[p_itx[i]]) continue;
-        UtxoSlot* s = p_slot[i];
-        if (!a.t.below) {  // plain table: the slot becomes a tombstone
-          *(volatile uint32_t*)&s->state = SLOT_TOMB;
-          atomicSub(&s_live, 1);
-          atomicAdd(&s_tomb, 1);
-        } else {           // diff layer: cancel its own entry, or record a removal marker for an entry that lives below
-          uint32_t k[9];
-          input_key(k, p_in[i]);
-          table_erase_found<false>(a.t, k, s, s >= a.t.slots && s <= a.t.slots + a.t.mask, &s_live, &s_tomb);
-        }
-      }
-      for (uint32_t o = o0 + tid; o < o1; o += nth) {
-        const uint32_t ti = p_otx[o];
-        if (!p_acc[ti]) continue;
-        const kgv_tx& tx = p_txs[ti];
-        const kgv_output& out = p_out[o];
-        uint32_t k[9];
-#pragma unroll
-        for (int w = 0; w < 4; w++) { uint64_t q = p_ids[4 * (size_t)ti + w]; k[2 * w] = (uint32_t)q; k[2 * w + 1] = (uint32_t)(q >> 32); }
-        k[8] = o - tx.first_output;
-        const uint8_t* scr = (staged && out.script_len <= RP_SCR) ? (const uint8_t*)S.scr[o - o0] : a.b.bytes + out.script_off;
-        table_put<false>(a.t, k, out.value, bl.pov, out.spk_version, (ti == t0 || tx_is_coinbase(tx)) ? 1u : 0u, scr, out.script_len, &s_live, &s_tomb);
-      }
-    }
-    __syncthreads();
-    RP_TICK(4);
-  }
-  __threadfence();
-  __syncthreads();
-  if (a.timers && tid == 0) for (int q = 0; q < 6; q++) a.timers[q] = (unsigned long long)tk[q];
-  if (tid == 0) {
-    a.stats[0] = s_acc;
-    atomicAdd(&a.t.counters[0], (unsigned long long)(long long)s_live);
-    atomicAdd(&a.t.counters[1], (unsigned long long)(long long)s_tomb);
-  }
-}
-
 // ---------------------------------------------------------------------------------------------
-// The RESOLVING walk (default): the in-order pass reduced to what is inherently sequential.
+// The in-order pass, reduced to what is inherently sequential.
 //
 // Within a window, whether an input's outpoint EXISTS at its block's position depends on the acceptance of earlier transactions - that is the
 // only sequential dependence of calculate_utxo_state.  Everything else is a function of the outpoint alone (a txid commits to its outputs, so the
@@ -366,7 +110,7 @@ __global__ void __launch_bounds__(1024, 1) k_replay_inorder(ReplayArgs a) {
 //                                  plus "needs the entry's DAA score" (spends a coinbase / carries a relative lock)
 // The walk itself (one CTA, state in shared-memory bitmaps: spent outpoints, accepted transactions) then does per block: every transaction
 // checks its inputs' flags (a few dozen instructions, no table access, no division), accepted ones set theirs after a barrier.  ~1 k cycles
-// per block instead of ~35 k for the table-walking form above (measured, DESIGN.md §4).  Afterwards, again in parallel over the window:
+// per block (measured, DESIGN.md §4).  Afterwards, again in parallel over the window:
 //   k_replay_finish_inputs   every spent entry is captured (MuHash consumers) and erased from the table
 //   k_replay_finish_outputs  every output of an accepted transaction that is still unspent at the end of the window is inserted
 //   k_replay_finish_results  verdicts are assembled (dynamic verdict, else static, else the script verdict of the pre-check)
@@ -652,7 +396,7 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
 // BM_SHARED: the four bitmaps live in shared memory (windows up to ~1.4 M flags); otherwise they are the global copies.
 template <bool BM_SHARED>
 __global__ void __launch_bounds__(RW_THREADS, 1) k_replay_walk(WalkArgs a) {
-  extern __shared__ __align__(128) uint8_t smem_raw[];
+  extern __shared__ __align__(16) uint8_t smem_raw[];  // cp.async.bulk needs 16-byte destinations; every offset below is a multiple of 16
   const uint32_t tid = threadIdx.x, nth = blockDim.x;
   uint8_t* const stage0 = smem_raw;
   uint8_t* const stage1 = smem_raw + RW_STAGE_BYTES;
@@ -879,8 +623,7 @@ extern "C" int kgv_replay_window(kgv_ctx* ctx, kgv_utxo_table* table, const kgv_
   size_t o_slp = al256(o_scr + ni * 72);
   size_t o_rng = al256(o_slp + ni * sizeof(UtxoSlot*));
   size_t o_cnt = al256(o_rng + n_blocks * sizeof(ReplayRange));
-  // state of the resolving walk
-  static const bool legacy_walk = [] { const char* e = getenv("KGV_REPLAY_WALK"); return e && !strcmp(e, "table"); }();
+  // state of the walk
   uint64_t sm_cap = 1024;
   while (sm_cap < 2 * ni) sm_cap <<= 1;
   const uint32_t words_in = (uint32_t)((ni + 31) / 32), words_out = (uint32_t)((no + 31) / 32), words_tx = (uint32_t)((nt + 31) / 32);
@@ -895,7 +638,7 @@ extern "C" int kgv_replay_window(kgv_ctx* ctx, kgv_utxo_table* table, const kgv_
   size_t o_bm = al256(o_apv + nt * 8);
   size_t o_smk = al256(o_bm + ((size_t)words_in + words_out + 2 * (size_t)words_tx) * 4);
   size_t o_smv = al256(o_smk + sm_cap * 8);
-  size_t total = legacy_walk ? al256(o_sib + nt) : al256(o_smv + sm_cap * 4);
+  size_t total = al256(o_smv + sm_cap * 4);
   rc = kgv_reserve(ctx, &ctx->d_replay, &ctx->d_replay_cap, total);
   if (rc) return rc;
   uint8_t* R = ctx->d_replay;
@@ -946,12 +689,6 @@ extern "C" int kgv_replay_window(kgv_ctx* ctx, kgv_utxo_table* table, const kgv_
   UtxoSlot** slotp = (UtxoSlot**)(R + o_slp);
   auto find_sources = [&]() -> int {
     if (!ni) return KGV_OK;
-    if (legacy_walk) {
-      k_populate_window<<<nblk(ni, 128), 128, 0, st>>>(view_of(table), v, ni, ids, wm, wm_cap - 1, dent);
-      CK(cudaGetLastError());
-      ctx->launches++;
-      return KGV_OK;
-    }
     k_replay_sources<<<nblk(ni, 128), 128, 0, st>>>(view_of(table), v, ni, ids, wm, wm_cap - 1, txb, (const ReplayRange*)(R + o_rng), dent, slotp, src);
     CK(cudaGetLastError());
     ctx->launches++;
@@ -984,104 +721,76 @@ extern "C" int kgv_replay_window(kgv_ctx* ctx, kgv_utxo_table* table, const kgv_
     rc = kgv_batch_to_device(ctx, batch, &d, false);
     if (rc) return rc;
     v = BatchView{d.txs, d.inputs, d.outputs, dent, d.bytes};
-    if (!legacy_walk && d.bytes != bytes_before) {  // window-sourced entries point at output scripts inside the staged batch
+    if (d.bytes != bytes_before) {  // window-sourced entries point at output scripts inside the staged batch
       rc = find_sources();
       if (rc) return rc;
     }
   }
   mark("host vm");
   if (stats) CK(cudaEventRecord(ctx->ev_time[1], st));
-  if (!legacy_walk) {
-    // ---- the resolving walk
-    const ReplayRange* ranges = (const ReplayRange*)(R + o_rng);
-    uint32_t* sfail = (uint32_t*)(R + o_sfl);
-    ReplayTxInfo* info = (ReplayTxInfo*)(R + o_inf);
-    uint64_t* fee = (uint64_t*)(R + o_fee);
-    uint8_t* wst = R + o_wst;
-    uint32_t* wfl = (uint32_t*)(R + o_wfl);
-    unsigned long long* apov = (unsigned long long*)(R + o_apv);
-    uint32_t* bm = (uint32_t*)(R + o_bm);
-    unsigned long long* smk = (unsigned long long*)(R + o_smk);
-    uint32_t* smv = (uint32_t*)(R + o_smv);
-    const size_t bm_words = (size_t)words_in + words_out + 2 * (size_t)words_tx;
-    CK(cudaMemsetAsync(bm, 0, bm_words * 4, st));
-    CK(cudaMemsetAsync(apov, 0, nt * 8, st));
-    if (ni) {
-      CK(cudaMemsetAsync(smk, 0, sm_cap * 8, st));
-      CK(cudaMemsetAsync(smv, 0xFF, sm_cap * 4, st));
-      k_slotmap_insert<<<nblk(ni, 256), 256, 0, st>>>(src, slotp, ni, smk, smv, sm_cap - 1);
-      CK(cudaGetLastError());
-      k_slotmap_lookup<<<nblk(ni, 256), 256, 0, st>>>(slotp, ni, smk, smv, sm_cap - 1, src);
-      CK(cudaGetLastError());
-      ctx->launches += 2;
-    }
-    mark("slot map");
-    k_replay_static<<<nblk(nt, 128), 128, 0, st>>>(v, (uint32_t)nt, *prm, ranges, txb, pre, src, ids, wm, wm_cap - 1, R + o_sib, info, fee, sfail);
+  // ---- the walk
+  const ReplayRange* ranges = (const ReplayRange*)(R + o_rng);
+  uint32_t* sfail = (uint32_t*)(R + o_sfl);
+  ReplayTxInfo* info = (ReplayTxInfo*)(R + o_inf);
+  uint64_t* fee = (uint64_t*)(R + o_fee);
+  uint8_t* wst = R + o_wst;
+  uint32_t* wfl = (uint32_t*)(R + o_wfl);
+  unsigned long long* apov = (unsigned long long*)(R + o_apv);
+  uint32_t* bm = (uint32_t*)(R + o_bm);
+  unsigned long long* smk = (unsigned long long*)(R + o_smk);
+  uint32_t* smv = (uint32_t*)(R + o_smv);
+  const size_t bm_words = (size_t)words_in + words_out + 2 * (size_t)words_tx;
+  CK(cudaMemsetAsync(bm, 0, bm_words * 4, st));
+  CK(cudaMemsetAsync(apov, 0, nt * 8, st));
+  if (ni) {
+    CK(cudaMemsetAsync(smk, 0, sm_cap * 8, st));
+    CK(cudaMemsetAsync(smv, 0xFF, sm_cap * 4, st));
+    k_slotmap_insert<<<nblk(ni, 256), 256, 0, st>>>(src, slotp, ni, smk, smv, sm_cap - 1);
     CK(cudaGetLastError());
-    ctx->launches++;
-    mark("static rules");
-    WalkArgs w;
-    w.ranges = ranges; w.n_blocks = (uint32_t)n_blocks; w.info = info; w.src = src; w.dent = dent; w.inputs = d.inputs;
-    w.acc_pov = apov; w.w_status = wst; w.w_fail = wfl; w.accept = dacc;
-    w.bm_spent_in = bm; w.bm_spent_out = bm + words_in; w.bm_accepted = bm + words_in + words_out; w.bm_exists = bm + words_in + words_out + words_tx;
-    w.words_in = words_in; w.words_out = words_out; w.words_tx = words_tx;
-    w.coinbase_maturity = prm->coinbase_maturity; w.stats = cnt;
-    const size_t stage_bytes = RW_FIXED_BYTES, walk_smem = stage_bytes + bm_words * 4;
-    w.use_smem = walk_smem <= 200 * 1024;
-    static bool walk_set = false;
-    if (!walk_set) { CK(cudaFuncSetAttribute(k_replay_walk<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024)); walk_set = true; }
-    if (w.use_smem) k_replay_walk<true><<<1, RW_THREADS, walk_smem, st>>>(w);
-    else k_replay_walk<false><<<1, RW_THREADS, stage_bytes, st>>>(w);
+    k_slotmap_lookup<<<nblk(ni, 256), 256, 0, st>>>(slotp, ni, smk, smv, sm_cap - 1, src);
     CK(cudaGetLastError());
-    ctx->launches++;
-    mark("walk");
-    k_replay_verdicts<<<nblk(nt, 256), 256, 0, st>>>((uint32_t)nt, ranges, txb, info, w.bm_exists, wst, dacc, apov);
-    CK(cudaGetLastError());
-    ctx->launches++;
-    const TableView tv = view_of(table);
-    if (ni) {
-      k_replay_finish_inputs<<<nblk(ni, 128), 128, 0, st>>>(tv, v, ni, itx, dacc, slotp, src, apov, dent, R + o_scr);
-      CK(cudaGetLastError());
-      ctx->launches++;
-    }
-    if (no) {
-      k_replay_finish_outputs<<<nblk(no, 128), 128, 0, st>>>(tv, v, no, otx, dacc, bm + words_in, ids, apov, info);
-      CK(cudaGetLastError());
-      ctx->launches++;
-    }
-    mark("finish inputs+outputs");
-    k_replay_finish_results<<<nblk(nt, 256), 256, 0, st>>>((uint32_t)nt, ranges, txb, info, wst, wfl, sfail, fee, pre, res);
-    CK(cudaGetLastError());
-    ctx->launches++;
-    mark("finish results");
-    if (stats) CK(cudaEventRecord(ctx->ev_time[2], st));
-  } else {
-  // ---- in-order pass over the table itself (KGV_REPLAY_WALK=table: the round-2a form, kept as a cross-check of the resolving walk)
-  ReplayArgs a;
-  a.t = view_of(table);
-  a.b = v;
-  a.dent = dent;
-  a.spent_scripts = R + o_scr;
-  a.slotp = (UtxoSlot**)(R + o_slp);
-  a.ids = ids; a.itx = itx; a.otx = otx;
-  a.ranges = (const ReplayRange*)(R + o_rng); a.n_blocks = (uint32_t)n_blocks;
-  a.prm = *prm;
-  a.pre = pre; a.res = res; a.accept = dacc; a.stats = cnt;
-  a.timers = kgv_debug_on() ? cnt + 2 : nullptr;
-  static bool smem_set = false;
-  if (!smem_set) { CK(cudaFuncSetAttribute(k_replay_inorder, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(ReplaySmem))); smem_set = true; }
-  k_replay_inorder<<<1, 1024, sizeof(ReplaySmem), st>>>(a);
+    ctx->launches += 2;
+  }
+  mark("slot map");
+  k_replay_static<<<nblk(nt, 128), 128, 0, st>>>(v, (uint32_t)nt, *prm, ranges, txb, pre, src, ids, wm, wm_cap - 1, R + o_sib, info, fee, sfail);
   CK(cudaGetLastError());
   ctx->launches++;
+  mark("static rules");
+  WalkArgs w;
+  w.ranges = ranges; w.n_blocks = (uint32_t)n_blocks; w.info = info; w.src = src; w.dent = dent; w.inputs = d.inputs;
+  w.acc_pov = apov; w.w_status = wst; w.w_fail = wfl; w.accept = dacc;
+  w.bm_spent_in = bm; w.bm_spent_out = bm + words_in; w.bm_accepted = bm + words_in + words_out; w.bm_exists = bm + words_in + words_out + words_tx;
+  w.words_in = words_in; w.words_out = words_out; w.words_tx = words_tx;
+  w.coinbase_maturity = prm->coinbase_maturity; w.stats = cnt;
+  const size_t stage_bytes = RW_FIXED_BYTES, walk_smem = stage_bytes + bm_words * 4;
+  w.use_smem = walk_smem <= 200 * 1024;
+  static bool walk_set = false;
+  if (!walk_set) { CK(cudaFuncSetAttribute(k_replay_walk<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024)); walk_set = true; }
+  if (w.use_smem) k_replay_walk<true><<<1, RW_THREADS, walk_smem, st>>>(w);
+  else k_replay_walk<false><<<1, RW_THREADS, stage_bytes, st>>>(w);
+  CK(cudaGetLastError());
+  ctx->launches++;
+  mark("walk");
+  k_replay_verdicts<<<nblk(nt, 256), 256, 0, st>>>((uint32_t)nt, ranges, txb, info, w.bm_exists, wst, dacc, apov);
+  CK(cudaGetLastError());
+  ctx->launches++;
+  const TableView tv = view_of(table);
+  if (ni) {
+    k_replay_finish_inputs<<<nblk(ni, 128), 128, 0, st>>>(tv, v, ni, itx, dacc, slotp, src, apov, dent, R + o_scr);
+    CK(cudaGetLastError());
+    ctx->launches++;
+  }
+  if (no) {
+    k_replay_finish_outputs<<<nblk(no, 128), 128, 0, st>>>(tv, v, no, otx, dacc, bm + words_in, ids, apov, info);
+    CK(cudaGetLastError());
+    ctx->launches++;
+  }
+  mark("finish inputs+outputs");
+  k_replay_finish_results<<<nblk(nt, 256), 256, 0, st>>>((uint32_t)nt, ranges, txb, info, wst, wfl, sfail, fee, pre, res);
+  CK(cudaGetLastError());
+  ctx->launches++;
+  mark("finish results");
   if (stats) CK(cudaEventRecord(ctx->ev_time[2], st));
-  if (kgv_debug_on()) {
-    unsigned long long tk[6];
-    CK(cudaMemcpyAsync(tk, cnt + 2, sizeof tk, cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
-    fprintf(stderr, "[kgv] in-order cycles per block: stage %.0f  scripts %.0f  A(populate+prefetch) %.0f  B(context) %.0f  C(apply) %.0f\n", (double)tk[0] / n_blocks,
-            (double)tk[1] / n_blocks, (double)tk[2] / n_blocks, (double)tk[3] / n_blocks, (double)tk[4] / n_blocks);
-  }
-  }
   STAGE("replay in-order");
   if (!marks.empty()) {
     cudaStreamSynchronize(st);
@@ -1107,7 +816,6 @@ extern "C" int kgv_replay_window(kgv_ctx* ctx, kgv_utxo_table* table, const kgv_
   ctx->last_replay.nt = nt; ctx->last_replay.ni = ni; ctx->last_replay.no = no; ctx->last_replay.n_blocks = n_blocks;
   ctx->last_replay.o_ids = o_ids; ctx->last_replay.o_itx = o_itx; ctx->last_replay.o_otx = o_otx; ctx->last_replay.o_ent = o_ent; ctx->last_replay.o_acc = o_acc;
   ctx->last_replay.o_txb = o_txb; ctx->last_replay.o_rng = o_rng;
-  ctx->last_replay.resolving = !legacy_walk;
   ctx->last_replay.o_src = o_src; ctx->last_replay.o_inf = o_inf; ctx->last_replay.o_apv = o_apv;
   if (stats) {
     stats->n_accepted = n_acc; stats->n_sig_checks = n_items; stats->n_host_vm = n_vm;
@@ -1121,7 +829,7 @@ extern "C" int kgv_replay_window(kgv_ctx* ctx, kgv_utxo_table* table, const kgv_
 // ---------------------------------------------------------------------------------------------
 // kgv_replay_muhash: MuHash::from_transaction of everything the last kgv_replay_window call accepted, combined per group of
 // blocks (the mergeset of one chain block): what calculate_utxo_state folds into ctx.multiset_hash (utxo_validation.rs:120,144).
-// Spent entries are the ones the in-order pass found at each block's position (kept in the window state with their scripts).
+// Spent entries are the ones k_replay_finish_inputs captured (kept in the window state with their scripts).
 // ---------------------------------------------------------------------------------------------
 __global__ void k_replay_tx_pov(const ReplayRange* __restrict__ ranges, const uint32_t* __restrict__ tx_block, uint32_t n_txs, uint64_t* __restrict__ tx_pov, uint8_t* __restrict__ tx_first) {
   uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
@@ -1229,7 +937,7 @@ extern "C" int kgv_replay_muhash(kgv_ctx* ctx, const uint32_t* group_first_block
 // ---------------------------------------------------------------------------------------------
 // kgv_replay_diffs: the UtxoDiff of every group of blocks of the last kgv_replay_window call - ctx.mergeset_diff of calculate_utxo_state
 // (utxo_validation.rs:119,148), i.e. UtxoDiff::add_transaction (utxo_diff.rs:224-260) over the group's accepted transactions in order.  No table
-// access: everything comes from the state the resolving walk leaves behind (source records, representative / accepted instance, accepting DAA
+// access: everything comes from the state the walk leaves behind (source records, representative / accepted instance, accepting DAA
 // score, the spent entries dent holds with their scripts captured).
 //   removal   an input of an accepted transaction, unless it spends an output whose creator was accepted in the SAME group (the pair cancels)
 //   addition  an output of the accepted instance of a transaction, unless an accepted transaction of the same group spends it
@@ -1403,7 +1111,6 @@ extern "C" int kgv_replay_diffs(kgv_ctx* ctx, const uint32_t* group_first_block,
   if (!group_first_block || n_groups == 0) { ctx->err = "kgv_replay_diffs: no groups"; return KGV_ERR_ARG; }
   if (!ctx->last_replay.valid) { ctx->err = "kgv_replay_diffs refers to the last kgv_replay_window call, and none is current (another batch was staged or the table rehashed since)"; return KGV_ERR_ARG; }
   const auto& L = ctx->last_replay;
-  if (!L.resolving) { ctx->err = "kgv_replay_diffs needs the resolving walk: the table-walking form (KGV_REPLAY_WALK=table) keeps no source records"; return KGV_ERR_ARG; }
   if (kgv_ptr_is_device(group_first_block)) { ctx->err = "group offsets must be a host array"; return KGV_ERR_ARG; }
   if (group_first_block[0] != 0 || group_first_block[n_groups] != L.n_blocks) { ctx->err = "groups must tile the blocks of the window"; return KGV_ERR_ARG; }
   for (size_t i = 0; i < n_groups; i++) if (group_first_block[i] > group_first_block[i + 1]) { ctx->err = "group offsets not monotone"; return KGV_ERR_ARG; }

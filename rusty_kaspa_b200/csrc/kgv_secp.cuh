@@ -121,17 +121,13 @@ KGV_HD void sc_reduce512(uint32_t* r, const uint32_t* t) {
   }
   sc_reduce_once(r);
 }
-// As for fe_mul / fe_sqr, the device versions are real functions (operands by value, in registers).
-// KGV_SC_ONE_BLOCK (default): ALL scalar arithmetic of the ECDSA kernel goes through ONE non-inlined function, r = a^(2^k) * (b or 1), with a
-// single copy of the 8x8 product and of the reduction (squarings use the general product: +28 multiplies each, 0.4 % more instructions per
-// verification).  Three separate blocks (multiply, square, run-of-squarings: ~19 KB of SASS next to the 25 KB of the point arithmetic) pushed
-// the kernel's hot code out of the instruction cache: ncu showed `no_instruction` stalls at 1.88 per issued instruction against 0.75 in the
-// Schnorr kernel.
-#ifndef KGV_SC_ONE_BLOCK
-#define KGV_SC_ONE_BLOCK 1
-#endif
+// As for fe_mul / fe_sqr, the device versions are real functions (operands by value, in registers): ALL scalar arithmetic of the ECDSA
+// kernel goes through ONE non-inlined function, r = a^(2^k) * (b or 1), with a single copy of the 8x8 product and of the reduction (squarings
+// use the general product: +28 multiplies each, 0.4 % more instructions per verification).  Three separate blocks (multiply, square,
+// run-of-squarings: ~19 KB of SASS next to the 25 KB of the point arithmetic) pushed the kernel's hot code out of the instruction cache: ncu
+// showed `no_instruction` stalls at 1.88 per issued instruction against 0.75 in the Schnorr kernel.  The host unit-test build inlines them.
+#if defined(__CUDACC__)
 struct sc8 { uint32_t v[8]; };
-#if defined(__CUDACC__) && KGV_NOINLINE_MUL && KGV_SC_ONE_BLOCK
 static __device__ __noinline__ sc8 sc_pow2k_mul_call(sc8 a, int k, int with_mul, sc8 b) {
   const int n = k + with_mul;
 #pragma unroll 1
@@ -170,37 +166,6 @@ KGV_HD void sc_sqr_n_mul(uint32_t* r, int k, const uint32_t* m) {
 #pragma unroll
   for (int i = 0; i < 8; i++) r[i] = z.v[i];
 }
-#elif defined(__CUDACC__) && KGV_NOINLINE_MUL
-static __device__ __noinline__ sc8 sc_mul_call(sc8 a, sc8 b) {
-  sc8 r;
-  uint32_t t[16];
-  mul_wide(t, a.v, b.v);
-  sc_reduce512(r.v, t);
-  return r;
-}
-static __device__ __noinline__ sc8 sc_sqr_call(sc8 a) {
-  sc8 r;
-  uint32_t t[16];
-  sqr_wide(t, a.v);
-  sc_reduce512(r.v, t);
-  return r;
-}
-KGV_HD void sc_mul(uint32_t* r, const uint32_t* a, const uint32_t* b) {
-  sc8 x, y;
-#pragma unroll
-  for (int i = 0; i < 8; i++) { x.v[i] = a[i]; y.v[i] = b[i]; }
-  sc8 z = sc_mul_call(x, y);
-#pragma unroll
-  for (int i = 0; i < 8; i++) r[i] = z.v[i];
-}
-KGV_HD void sc_sqr(uint32_t* r, const uint32_t* a) {
-  sc8 x;
-#pragma unroll
-  for (int i = 0; i < 8; i++) x.v[i] = a[i];
-  sc8 z = sc_sqr_call(x);
-#pragma unroll
-  for (int i = 0; i < 8; i++) r[i] = z.v[i];
-}
 #else
 KGV_HD void sc_mul(uint32_t* r, const uint32_t* a, const uint32_t* b) {
   uint32_t t[16];
@@ -212,40 +177,17 @@ KGV_HD void sc_sqr(uint32_t* r, const uint32_t* a) {
   sqr_wide(t, a);
   sc_reduce512(r, t);
 }
+KGV_HD void sc_sqr_n(uint32_t* r, int n) {
+  for (int i = 0; i < n; i++) sc_sqr(r, r);
+}
+// r = r^(2^k) * m
+KGV_HD void sc_sqr_n_mul(uint32_t* r, int k, const uint32_t* m) { sc_sqr_n(r, k); sc_mul(r, r, m); }
 #endif
 // r = a^(n-2) mod n (a != 0).  The exponent is public and identical in every lane: no divergence.  Addition chain: the 127 leading one bits
 // of n-2 through x_k = a^(2^k - 1) (k = 2, 3, 6, 8, 14, 28, 56, 112, 126: the ladder libsecp256k1's scalar inverse uses), the remaining 129 bits
 // by a sliding window over the odd powers a, a^3, a^5, a^7 (schedule derived and checked against pow(a, n-2, n) by
 // tools/derive_sc_inv_chain.py; tests/test_hostsim.py runs this very function on the host): 255 squarings + 44 multiplications instead of the 255 + 191
 // of plain square-and-multiply (ECDSA shares one inversion among KGV_ITEMS signatures; it was 11 % of an ECDSA verification).
-#if defined(__CUDACC__) && KGV_NOINLINE_MUL && KGV_SC_ONE_BLOCK
-// (sc_sqr_n_mul above)
-#else
-#if defined(__CUDACC__) && KGV_NOINLINE_MUL && KGV_SC_SQRN_CALL
-static __device__ __noinline__ sc8 sc_sqr_n_call(sc8 a, int n) {  // one call per run of squarings (see fe_sqr_n)
-#pragma unroll 1
-  for (int i = 0; i < n; i++) {
-    uint32_t t[16];
-    sqr_wide(t, a.v);
-    sc_reduce512(a.v, t);
-  }
-  return a;
-}
-KGV_HD void sc_sqr_n(uint32_t* r, int n) {
-  sc8 x;
-#pragma unroll
-  for (int i = 0; i < 8; i++) x.v[i] = r[i];
-  x = sc_sqr_n_call(x, n);
-#pragma unroll
-  for (int i = 0; i < 8; i++) r[i] = x.v[i];
-}
-#else
-KGV_HD void sc_sqr_n(uint32_t* r, int n) {
-  for (int i = 0; i < n; i++) sc_sqr(r, r);
-}
-#endif
-KGV_HD void sc_sqr_n_mul(uint32_t* r, int k, const uint32_t* m) { sc_sqr_n(r, k); sc_mul(r, r, m); }
-#endif
 KGV_HD void sc_inv(uint32_t* r, const uint32_t* a) {
   uint32_t a1[8], a3[8], a5[8], a7[8], x6[8], x14[8], t[8], u[8];
 #pragma unroll
@@ -462,11 +404,8 @@ KGV_HD bool gej_add_ge_body(gej& r, const fe& bx, const fe& by, fe* hout) {
 //  * n == 0: r += (bx,by), also returning H (the table builder needs it; it used to take it from an INLINED body:
 //    seven unrolled copies, ~160 KB of straight-line code that evicted the ladder's hot code, DESIGN.md §4 K1).
 //    The rare r == addend case falls through into the same doubling loop: no second copy of the doubling, no call.
-// The point at infinity is tested by the caller of a doubling, once per call, not inside the doubling.
-#ifndef KGV_NOINLINE_POINT
-#define KGV_NOINLINE_POINT 1
-#endif
-#if defined(__CUDACC__) && KGV_NOINLINE_POINT
+// The point at infinity is tested by the caller of a doubling, once per call, not inside the doubling.  The host unit-test build inlines it.
+#if defined(__CUDACC__)
 struct gej_h { gej r; fe h; };
 static __device__ __noinline__ gej_h gej_point_call(gej r, fe bx, fe by, int n) {
   gej_h o;

@@ -70,12 +70,9 @@ KGV_HD void u3072_acc_add16(uint32_t* acc, const uint32_t* t) {
 #endif
 }
 
-struct u3072_wide16 { uint32_t v[16]; };
-#if defined(__CUDACC__) && !defined(KGV_U3072_BLOCKMUL_MODE)
-#define KGV_U3072_BLOCKMUL_MODE 0
-#endif
-#if defined(__CUDACC__) && KGV_U3072_BLOCKMUL_MODE == 0
+#if defined(__CUDACC__)
 // same calling pattern as fe_mul_call: the carry-chain multiplier stays a real function taking / returning registers
+struct u3072_wide16 { uint32_t v[16]; };
 static __device__ __noinline__ u3072_wide16 u3072_blockmul_call(fe a, fe b) { u3072_wide16 t; mul_wide(t.v, a.v, b.v); return t; }
 KGV_HD void u3072_blockmul(uint32_t* t, const uint32_t* a, const uint32_t* b) {
   fe x, y;
@@ -85,10 +82,6 @@ KGV_HD void u3072_blockmul(uint32_t* t, const uint32_t* a, const uint32_t* b) {
 #pragma unroll
   for (int i = 0; i < 16; i++) t[i] = w.v[i];
 }
-#elif defined(__CUDACC__) && KGV_U3072_BLOCKMUL_MODE == 2
-// diagnostic variant (tools/repro): operands through memory
-static __device__ __noinline__ void u3072_blockmul_ptr(uint32_t* t, const uint32_t* a, const uint32_t* b) { mul_wide(t, a, b); }
-KGV_HD void u3072_blockmul(uint32_t* t, const uint32_t* a, const uint32_t* b) { u3072_blockmul_ptr(t, a, b); }
 #else
 KGV_HD void u3072_blockmul(uint32_t* t, const uint32_t* a, const uint32_t* b) { mul_wide(t, a, b); }
 #endif

@@ -77,7 +77,6 @@ __device__ __forceinline__ void st256(void* p, const uint32_t* w) {
                "r"(w[7]), "l"(p)
                : "memory");
 }
-__device__ __forceinline__ void prefetch_l2(const void* p) { asm volatile("prefetch.global.L2 [%0];" ::"l"(p)); }
 
 // 36-byte outpoint (txid || index LE) -> 9 words.  Key arrays handed to the library are 4-byte aligned (36 * i keeps that).
 __device__ __forceinline__ void load_key(uint32_t* k, const uint8_t* p) {
@@ -201,14 +200,12 @@ __device__ __forceinline__ void load_script_words(uint32_t* w, const uint8_t* p,
 // upsert; returns 1 inserted, 2 replaced, 0 failed (table or overflow arena full).
 // Keys inserted concurrently by one kernel must be distinct (API contract), so a slot another thread is
 // filling (BUSY) always belongs to a different key and is simply skipped: no thread ever waits on another.
-// FENCE = false: the caller is a single CTA whose barriers order the slot contents before the state word for every reader.
 // In a diff layer (t.below != nullptr) the write goes to the top layer only: an added entry becomes FULLH when a lower layer (or a removal
 // marker of this layer) holds the key, and `marker` = true stores a removal marker instead of an entry (UtxoDiff::remove_entry of an entry
 // that lives below, utxo_diff.rs:249-258).
-template <bool FENCE = true>
 __device__ __forceinline__ uint32_t table_put(const TableView& t, const uint32_t* k, uint64_t amount, uint64_t daa, uint32_t spk_version, uint32_t is_coinbase,
                                               const uint8_t* script, uint32_t script_len, int* s_live = nullptr, int* s_tomb = nullptr, bool marker = false) {
-  // s_live / s_tomb: optional shared-memory accumulators for the live / tombstone counters (a single-CTA caller flushes them once)
+  // s_live / s_tomb: optional shared-memory accumulators for the live / tombstone counters (the caller flushes them once per CTA)
   uint32_t final_state = marker ? SLOT_REMOVED : SLOT_FULL;
   if (t.below && !marker) {
     SlotHead hb;
@@ -281,7 +278,7 @@ __device__ __forceinline__ uint32_t table_put(const TableView& t, const uint32_t
   st256((uint8_t*)target + 96, w + 24);
   st256(target, w);
   if (!replace) {
-    if (FENCE) __threadfence();
+    __threadfence();
     *(volatile uint32_t*)&target->state = final_state;
     if (s_live) atomicAdd(s_live, 1); else atomicAdd(&t.counters[0], 1ull);
   }
@@ -289,10 +286,9 @@ __device__ __forceinline__ uint32_t table_put(const TableView& t, const uint32_t
 }
 // erase of an entry already located (slot s, found in the top layer or below): a plain table tombstones the slot; a diff layer turns its own
 // added entry back into nothing (FULL) or into a removal marker (FULLH), and records a removal marker for an entry that lives below.
-template <bool FENCE = true>
 __device__ __forceinline__ void table_erase_found(const TableView& t, const uint32_t* k, UtxoSlot* s, bool in_top, int* s_live = nullptr, int* s_tomb = nullptr) {
   if (!in_top) {
-    table_put<FENCE>(t, k, 0, 0, 0, 0, nullptr, 0, s_live, s_tomb, true);
+    table_put(t, k, 0, 0, 0, 0, nullptr, 0, s_live, s_tomb, true);
     return;
   }
   const uint32_t st = *(volatile uint32_t*)&s->state;

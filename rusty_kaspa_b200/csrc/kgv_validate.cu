@@ -565,13 +565,6 @@ extern "C" void kgv_utxo_destroy(kgv_ctx* ctx, kgv_utxo_table* t) {
   delete t;
 }
 
-// stage a host array on the device inside ctx->d_in at a running offset
-struct Stager {
-  kgv_ctx* ctx;
-  size_t off = 0;
-  explicit Stager(kgv_ctx* c) : ctx(c) {}
-};
-
 extern "C" int kgv_utxo_lookup(kgv_ctx* ctx, kgv_utxo_table* t, const uint8_t* keys36, size_t n, kgv_utxo_entry* entries, uint8_t* scripts_out,
                                uint32_t script_stride, uint8_t* found) {
   if (!ctx || !t) return KGV_ERR_ARG;

@@ -5,7 +5,6 @@ import copy
 import ctypes
 import os
 import subprocess
-import sys
 
 import numpy as np
 import pytest
@@ -456,29 +455,6 @@ def test_contract_sizes_errors_order_independence_and_device_outputs(gpu_ctx, or
     assert t[2].cpu().numpy()[3:].tobytes() == d1.add_keys36.tobytes() and t[3].cpu().numpy().tobytes() == d1.add_entries.tobytes()
     assert t[4].cpu().numpy()[:nb].tobytes() == d1.bytes.tobytes()
     r.close()
-
-
-def test_table_walk_form_is_refused(tmp_path):
-    """KGV_REPLAY_WALK=table keeps no source records: kgv_replay_diffs refuses it instead of returning anything"""
-    code = (
-        "import sys; sys.path.insert(0, %r); sys.path.insert(0, %r)\n"
-        "import numpy as np, rusty_kaspa_b200 as rk\n"
-        "from rusty_kaspa_b200.replay import DagReplayer\n"
-        "from rusty_kaspa_b200.simgen import SimDag\n"
-        "dag = SimDag(seed=2, n_keys=16, n_nonces=16, coinbase_maturity=1, coinbase_outputs=2)\n"
-        "blocks = [dag.make_block(3) for _ in range(4)]\n"
-        "ctx = rk.GpuContext(0)\n"
-        "r = DagReplayer(ctx, rk.Params(coinbase_maturity=1, storage_mass_parameter=dag.C), 1 << 10)\n"
-        "r.replay_windowed(blocks)\n"
-        "try:\n"
-        "    r.replay_diffs([0, 4]); print('RETURNED')\n"
-        "except rk.KgvError as e:\n"
-        "    print('REFUSED', e)\n"
-    ) % (ROOT, os.path.join(ROOT, "tests"))
-    env = dict(os.environ, KGV_REPLAY_WALK="table")
-    out = subprocess.run([sys.executable, "-c", code], env=env, capture_output=True, text=True, timeout=600)
-    assert out.returncode == 0, out.stderr[-2000:]
-    assert "REFUSED" in out.stdout and "resolving walk" in out.stdout, out.stdout
 
 
 # ------------------------------------------------------------------------------------------------ 7. C++ mirror
