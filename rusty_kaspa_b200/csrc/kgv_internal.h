@@ -26,7 +26,7 @@ struct kgv_ctx {
   cudaEvent_t ev_time[3] = {};                    // kgv_replay_window: phase timing for kgv_replay_stats
   cudaEvent_t ev_chunk[32] = {};                  // upload-complete events of the chunked host-pointer verify path
   cudaStream_t stream = nullptr;
-  uint32_t* gtab = nullptr;     // [2][65536][16] u32: v*G and v*2^128*G, affine
+  uint32_t* gtab = nullptr;     // [8][65536][16] u32: v*2^(32j)*G in table j, affine
   uint8_t* d_in = nullptr;      // staging for host-pointer calls
   size_t d_in_cap = 0;
   uint8_t* d_out = nullptr;

@@ -7,6 +7,7 @@
 
 #include <cuda_runtime.h>
 #include <cstdio>
+#include <algorithm>
 #include <cstring>
 #include <mutex>
 #include <string>
@@ -22,7 +23,24 @@ struct SmemTab {
   uint32_t* base;  // smem + threadIdx.x
   __device__ __forceinline__ void put(int e, int w, uint32_t v) { base[(e * 16 + w) * KGV_BLOCK] = v; }
   __device__ __forceinline__ uint32_t get(int e, int w) const { return base[(e * 16 + w) * KGV_BLOCK]; }
+  // the comb ladder's staging (ecmult_comb) uses the same 512 bytes as 32 chunks of 16 bytes, chunk-major / thread-minor: a warp's
+  // 16-byte copies and reads of one chunk cover 512 consecutive bytes, free of bank conflicts.  Chunk c of slot s: 4s + c.
+  __device__ __forceinline__ uint4* chunk(int q) const { return reinterpret_cast<uint4*>(base - threadIdx.x) + q * KGV_BLOCK + threadIdx.x; }
 };
+__device__ __forceinline__ void stage_fetch(SmemTab& tab, int s, const uint32_t* entry) {
+#pragma unroll
+  for (int c = 0; c < 4; c++) {
+    const uint32_t dst = (uint32_t)__cvta_generic_to_shared(tab.chunk(4 * s + c));
+    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(dst), "l"(entry + 4 * c) : "memory");
+  }
+}
+__device__ __forceinline__ void stage_commit(SmemTab&) { asm volatile("cp.async.commit_group;" ::: "memory"); }
+__device__ __forceinline__ void stage_wait(SmemTab&) { asm volatile("cp.async.wait_group 7;" ::: "memory"); }
+__device__ __forceinline__ void stage_get(SmemTab& tab, int s, fe& x, fe& y) {
+  const uint4 a = *tab.chunk(4 * s), b = *tab.chunk(4 * s + 1), c = *tab.chunk(4 * s + 2), d = *tab.chunk(4 * s + 3);
+  x.v[0] = a.x; x.v[1] = a.y; x.v[2] = a.z; x.v[3] = a.w; x.v[4] = b.x; x.v[5] = b.y; x.v[6] = b.z; x.v[7] = b.w;
+  y.v[0] = c.x; y.v[1] = c.y; y.v[2] = c.z; y.v[3] = c.w; y.v[4] = d.x; y.v[5] = d.y; y.v[6] = d.z; y.v[7] = d.w;
+}
 
 // 256-bit read-only load: sm_90 has no 256-bit LDG, so two 128-bit loads of the same 32-byte sector, issued back to back
 __device__ __forceinline__ void ldg256(uint32_t* w, const void* p) {
@@ -66,7 +84,7 @@ __device__ __forceinline__ void load_be32(uint32_t* w, const uint8_t* p) {
 // ---------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(128) k_build_gtab(uint32_t* __restrict__ gtab) {
   uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
-  if (t >= 2u * 65536u) return;
+  if (t >= 8u * 65536u) return;
   uint32_t v = t & 0xFFFFu;
   uint32_t which = t >> 16;
   uint32_t* out = gtab + (size_t)t * 16;
@@ -75,21 +93,30 @@ __global__ void __launch_bounds__(128) k_build_gtab(uint32_t* __restrict__ gtab)
     for (int i = 0; i < 16; i++) out[i] = 0;
     return;
   }
-  const fe gx = {KGV_GX_LIMBS}, gy = {KGV_GY_LIMBS}, hx = {KGV_G128X_LIMBS}, hy = {KGV_G128Y_LIMBS};
-  fe x, y;
-  if (which == 0) gtab_entry(x, y, v, gx, gy);
-  else gtab_entry(x, y, v, hx, hy);
+  fe bx, by, x, y;
+  gtab_base(bx, by, (int)which);
+  gtab_entry(x, y, v, bx, by);
 #pragma unroll
   for (int i = 0; i < 8; i++) { out[i] = x.v[i]; out[8 + i] = y.v[i]; }
 }
 
 // ---- per-launch key cache: the key part of a verification done once per distinct public key of a verify launch ----
-// Records per launch at most (2^17 x 560 B = 73 MB).
+// Records per launch at most (2^17 x 2112 B = 277 MB of comb records, 2^17 x 560 B = 73 MB of plain ones).
 #define KGV_KEY_RECORDS_MAX (1u << 17)
-// A launch uses records when its keys are used twice on average (at most n/2 distinct keys) and fit the cap; then EVERY key has one.  A
-// warp pays for the inline key path of any of its lanes, so records for the repeated keys alone leave singleton lanes costing whole
-// warps; a batch of mostly distinct keys makes no records at all and pays only the dedup pass.
-__device__ __forceinline__ bool key_records_on(uint32_t n_rec, size_t n) { return n_rec <= KGV_KEY_RECORDS_MAX && 2 * (size_t)n_rec <= n; }
+// Fewest uses per key on average for comb records: the comb's preparation (~1 800 products per key against ~400) must be paid back by
+// its shorter ladder (~700 products fewer per verify); measured +20 % at 10 uses per key (DESIGN.md §5), not below.
+#ifndef KGV_COMB_USES
+#define KGV_COMB_USES 8
+#endif
+enum { KGV_KEYS_INLINE = 0, KGV_KEYS_PLAIN = 1, KGV_KEYS_COMB = 2 };
+// The form of a launch's key part, uniform over the launch: records when its keys are used twice on average (at most n/2 distinct keys)
+// and fit the cap; then EVERY key has one.  A warp pays for the inline key path of any of its lanes, so records for the repeated keys
+// alone leave singleton lanes costing whole warps; a batch of mostly distinct keys makes no records at all and pays only the dedup pass.
+// Comb records (key_comb_build, ecmult_comb) when the keys are used at least KGV_COMB_USES times on average, plain ones (key_rec_build) below.
+__device__ __forceinline__ int key_form(uint32_t n_rec, size_t n) {
+  if (n_rec > KGV_KEY_RECORDS_MAX || 2 * (size_t)n_rec > n) return KGV_KEYS_INLINE;
+  return (size_t)KGV_COMB_USES * n_rec <= n ? KGV_KEYS_COMB : KGV_KEYS_PLAIN;
+}
 
 // Slot of the open-addressed key table: key = fingerprint << 32 | (representative item + 1), 0 = empty; rec = the key's record + 1.
 struct KeySlot {
@@ -99,12 +126,15 @@ struct KeySlot {
 struct KeyCacheView {
   const KeySlot* table;
   const uint32_t* item_slot;  // item -> table slot (only the items the launch verifies are set)
-  const uint32_t* recs;       // records, KGV_KR_WORDS words each
+  const uint32_t* recs;       // records, KGV_KR_WORDS or KGV_KC_WORDS words each
   const uint32_t* n_rec;      // distinct keys of the launch; nullptr: no key cache
+  __device__ __forceinline__ bool comb(size_t n) const { return n_rec && key_form(*n_rec, n) == KGV_KEYS_COMB; }
   // the record of item i, or nullptr (the launch makes no records)
   __device__ __forceinline__ const uint32_t* rec_of(size_t i, size_t n) const {
-    if (!n_rec || !key_records_on(*n_rec, n)) return nullptr;
-    return recs + (size_t)(table[item_slot[i]].rec - 1) * KGV_KR_WORDS;
+    if (!n_rec) return nullptr;
+    const int f = key_form(*n_rec, n);
+    if (f == KGV_KEYS_INLINE) return nullptr;
+    return recs + (size_t)(table[item_slot[i]].rec - 1) * (f == KGV_KEYS_COMB ? KGV_KC_WORDS : KGV_KR_WORDS);
   }
 };
 
@@ -130,7 +160,7 @@ __device__ __forceinline__ uint64_t key_hash(const uint32_t* w, int nw) {
 }
 
 // One thread per item: find or claim the key's slot; a claimed slot gets the next record index.  Whichever item's atomicCAS claims the
-// slot becomes its representative: the record depends on the key bytes alone.  Once the launch has more keys than key_records_on allows,
+// slot becomes its representative: the record depends on the key bytes alone.  Once the launch has more keys than records allow (key_form),
 // the remaining items stop (the verify kernels then take the inline key path for every item).
 template <bool ALIGNED, bool ECDSA>
 __global__ void __launch_bounds__(256) k_key_dedup(const uint8_t* __restrict__ pk, size_t n_arg, const uint32_t* __restrict__ index,
@@ -138,7 +168,7 @@ __global__ void __launch_bounds__(256) k_key_dedup(const uint8_t* __restrict__ p
                                                    uint32_t* __restrict__ item_slot, uint32_t* __restrict__ rec_rep, uint32_t* n_rec) {
   const size_t n = n_dev ? (size_t)*n_dev : n_arg;
   const size_t t = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (t >= n || !key_records_on(*(volatile uint32_t*)n_rec, n)) return;
+  if (t >= n || key_form(*(volatile uint32_t*)n_rec, n) == KGV_KEYS_INLINE) return;
   const size_t i = index ? index[t] : t;
   const int nw = ECDSA ? 9 : 8;
   uint32_t w[9];
@@ -167,7 +197,7 @@ __global__ void __launch_bounds__(256) k_key_dedup(const uint8_t* __restrict__ p
   base = __shfl_sync(act, base, leader);
   if (won) {
     const uint32_t r = base + __popc(ball & ((1u << lane) - 1));
-    if (key_records_on(r + 1, n)) {  // (r < the host's bound of the rec_rep / record arrays)
+    if (key_form(r + 1, n) != KGV_KEYS_INLINE) {  // (r < the host's bound of the rec_rep / record arrays)
       rec_rep[r] = (uint32_t)i;
       table[s].rec = r + 1;
     }
@@ -175,18 +205,20 @@ __global__ void __launch_bounds__(256) k_key_dedup(const uint8_t* __restrict__ p
   item_slot[i] = s;
 }
 
-// One thread per record: the key's verdict, and for a good key its odd-multiples table and zs (key_rec_build).  The verify kernels'
-// occupancy (168 registers): unbounded, ptxas takes 255 and two blocks per SM.
+// One thread per record: the key's verdict, and for a good key its comb (key_comb_build) or its odd-multiples table and zs (key_rec_build).
+// The verify kernels' occupancy (168 registers): unbounded, ptxas takes 255 and two blocks per SM.
 template <bool ECDSA>
 __global__ void __launch_bounds__(KGV_BLOCK, KGV_BLOCKS_PER_SM) k_key_prepare(const uint8_t* __restrict__ pk, size_t n_arg, const uint32_t* __restrict__ n_dev,
                                                                               const uint32_t* __restrict__ rec_rep, const uint32_t* __restrict__ n_rec,
                                                                               uint32_t* __restrict__ recs) {
   const size_t n = n_dev ? (size_t)*n_dev : n_arg;
   const uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
-  if (r >= *n_rec || !key_records_on(*n_rec, n)) return;
+  const int f = key_form(*n_rec, n);
+  if (r >= *n_rec || f == KGV_KEYS_INLINE) return;
   uint32_t w[9];
   key_words<false, ECDSA>(w, pk, rec_rep[r]);
-  key_rec_build(recs + (size_t)r * KGV_KR_WORDS, ECDSA ? w[8] : 2u, w);
+  if (f == KGV_KEYS_COMB) key_comb_build(recs + (size_t)r * KGV_KC_WORDS, ECDSA ? w[8] : 2u, w);
+  else key_rec_build(recs + (size_t)r * KGV_KR_WORDS, ECDSA ? w[8] : 2u, w);
 }
 
 // Each thread verifies KGV_ITEMS consecutive-stride items (i = tid + j * total_threads: coalesced) and shares
@@ -226,7 +258,7 @@ k_schnorr_verify(const uint8_t* __restrict__ pk, const uint8_t* __restrict__ msg
     load_be32<ALIGNED>(sw, sig + 64 * i);
     load_be32<ALIGNED>(sw + 8, sig + 64 * i + 32);
     fe x, y, zt, rx;
-    uint8_t s1 = schnorr_phase1(x, y, zt, rx, pkw, mw, sw, tab, gtab, GLoadDev(), kc.rec_of(i, n));
+    uint8_t s1 = schnorr_phase1(x, y, zt, rx, pkw, mw, sw, tab, gtab, GLoadDev(), kc.rec_of(i, n), kc.comb(n));
     st[j] = s1;
     if (s1 == KGV_ST_PENDING) {
       X[j] = x; Y[j] = y; ZT[j] = zt; RX[j] = rx;
@@ -291,7 +323,7 @@ k_ecdsa_verify(const uint8_t* __restrict__ pk, const uint8_t* __restrict__ msg, 
     fe qx, qy;
     uint32_t r[8], s[8], m[8];
     const uint32_t* krec = kc.rec_of(i, n);
-    uint8_t s1 = ecdsa_phase1(qx, qy, r, s, m, tag, pkw, mw, sw, krec);
+    uint8_t s1 = ecdsa_phase1(qx, qy, r, s, m, tag, pkw, mw, sw, krec, kc.comb(n));
     st[j] = s1;
     if (s1 == KGV_ST_PENDING) {
       QX[j] = qx; QY[j] = qy; KR[j] = krec;
@@ -310,7 +342,7 @@ k_ecdsa_verify(const uint8_t* __restrict__ pk, const uint8_t* __restrict__ msg, 
       uint32_t sn[8];
       sc_mul(sn, inv, pre[j].v);
       sc_mul(inv, inv, S_[j].v);
-      st[j] = ecdsa_phase2(QX[j], QY[j], R_[j].v, sn, M_[j].v, tab, gtab, GLoadDev(), KR[j]);
+      st[j] = ecdsa_phase2(QX[j], QY[j], R_[j].v, sn, M_[j].v, tab, gtab, GLoadDev(), KR[j], kc.comb(n));
     }
   }
 #pragma unroll 1
@@ -462,8 +494,8 @@ extern "C" int kgv_create(int device, uint32_t flags, kgv_ctx** out) {
     CK(cudaStreamCreateWithFlags(&ctx->aux_stream, cudaStreamNonBlocking));
     CK(cudaEventCreateWithFlags(&ctx->ev_fork, cudaEventDisableTiming));
     CK(cudaEventCreateWithFlags(&ctx->ev_join, cudaEventDisableTiming));
-    CK(cudaMalloc((void**)&ctx->gtab, (size_t)2 * 65536 * 16 * sizeof(uint32_t)));
-    k_build_gtab<<<(2 * 65536) / 128, 128, 0, ctx->stream>>>(ctx->gtab);
+    CK(cudaMalloc((void**)&ctx->gtab, (size_t)8 * 65536 * 16 * sizeof(uint32_t)));
+    k_build_gtab<<<(8 * 65536) / 128, 128, 0, ctx->stream>>>(ctx->gtab);
     CK(cudaGetLastError());
     ctx->launches++;
     const int smem = KGV_BLOCK * 128 * (int)sizeof(uint32_t);
@@ -555,10 +587,12 @@ static int key_cache_launch(kgv_ctx* ctx, const uint8_t* dpk, size_t n, bool ecd
                             const uint32_t* n_dev, KeyCacheView* kc) {
   uint32_t slots = 64;
   while (slots < 2 * n) slots <<= 1;                       // load factor <= 1/2
-  const uint32_t cap = (uint32_t)(n / 2 < KGV_KEY_RECORDS_MAX ? n / 2 : KGV_KEY_RECORDS_MAX);  // key_records_on's bound
+  const uint32_t cap = (uint32_t)(n / 2 < KGV_KEY_RECORDS_MAX ? n / 2 : KGV_KEY_RECORDS_MAX);  // key_form's bounds
+  const size_t cap_comb = n / KGV_COMB_USES < KGV_KEY_RECORDS_MAX ? n / KGV_COMB_USES : KGV_KEY_RECORDS_MAX;
+  const size_t rec_bytes = std::max((size_t)cap * KGV_KR_WORDS, cap_comb * KGV_KC_WORDS) * 4;
   const size_t o_tab = 256, o_item = o_tab + (size_t)slots * sizeof(KeySlot);
   const size_t o_rep = (o_item + n * 4 + 255) & ~(size_t)255, o_rec = (o_rep + (size_t)cap * 4 + 255) & ~(size_t)255;
-  int rc = kgv_reserve(ctx, &ctx->d_keys[ecdsa], &ctx->d_keys_cap[ecdsa], o_rec + (size_t)cap * KGV_KR_WORDS * 4);
+  int rc = kgv_reserve(ctx, &ctx->d_keys[ecdsa], &ctx->d_keys_cap[ecdsa], o_rec + rec_bytes);
   if (rc) return rc;
   uint8_t* K = ctx->d_keys[ecdsa];
   uint32_t* n_rec = (uint32_t*)K;
@@ -765,7 +799,7 @@ extern "C" int kgv_gtable_entry(kgv_ctx* ctx, int which, uint32_t v, uint8_t out
   if ((which != 0 && which != 1) || v == 0 || v > 65535 || !out_xy) return fail_arg(ctx, "bad table index");
   CK(cudaSetDevice(ctx->device));
   uint32_t w[16];
-  CK(cudaMemcpyAsync(w, ctx->gtab + ((size_t)which * 65536 + v) * 16, sizeof w, cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaMemcpyAsync(w, ctx->gtab + ((size_t)which * 4 * 65536 + v) * 16, sizeof w, cudaMemcpyDeviceToHost, ctx->stream));  // v*G, v*2^128*G
   CK(cudaStreamSynchronize(ctx->stream));
   for (int c = 0; c < 2; c++)
     for (int i = 0; i < 8; i++) {

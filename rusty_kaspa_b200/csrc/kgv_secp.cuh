@@ -8,8 +8,9 @@
 //     (33 digits each, never zero), 8-entry table {1,3,..,15}*P per thread in shared memory,
 //     built on an isomorphic curve so the entries are affine ("effective affine")
 //   * G part: kG = lo + 2^128*hi, unsigned 16-bit windows into two 65536-entry affine tables
-//     (G and 2^128*G, 8 MiB total, L2 resident), 16 mixed additions
+//     (G and 2^128*G of the eight 2^(32j)*G tables, L2 resident), 16 mixed additions
 //   * 128 shared doublings
+// ecmult_comb is the same product for a key prepared once per launch as a four-tooth comb (keys that repeat often): 32 doublings.
 #pragma once
 #include "kgv_arith.cuh"
 
@@ -513,7 +514,7 @@ KGV_HD void build_odd_table(Tab& tab, fe& zs, const fe& px, const fe& py) {
 // R = kP * P + kG * G     (result on the isomorphic curve; true Z = R.z * zs)
 // ------------------------------------------------------------------------------------------
 // tab, zs: P's odd-multiples table and its Z scale, as build_odd_table leaves them (built by the caller, or copied from a key record).
-// gtab: [2][65536][16] u32 — affine (x limbs, y limbs) of v*G and v*2^128*G; entry 0 unused.
+// gtab: [8][65536][16] u32 — table j holds the affine (x limbs, y limbs) of v*2^(32j)*G; entry 0 unused.  This ladder reads j = 0 and 4.
 // GLoad is a functor  void operator()(fe& x, fe& y, const uint32_t* entry)  (vectorised loads on device).
 template <class Tab, class GLoad, class Trace = NoTrace>
 KGV_HD void ecmult_double(gej& R, const fe& zs, const uint32_t* kP, const uint32_t* kG, Tab& tab, const uint32_t* gtab, GLoad gload,
@@ -563,7 +564,7 @@ KGV_HD void ecmult_double(gej& R, const fe& zs, const uint32_t* kP, const uint32
         gej_add_ge(R, ex, ey);
       }
       if (dhi) {
-        gload(ex, ey, gtab + ((size_t)65536 + dhi) * 16);
+        gload(ex, ey, gtab + ((size_t)4 * 65536 + dhi) * 16);
         fe_mul(ex, ex, zs2);
         fe_mul(ey, ey, zs3);
         gej_add_ge(R, ex, ey);
@@ -585,6 +586,100 @@ KGV_HD void ecmult_double(gej& R, const fe& zs, const uint32_t* kP, const uint32
     for (int w = 0; w < 8; w++) { ex.v[w] = tab.get(0, w); ey.v[w] = tab.get(0, 8 + w); }
     fe_mul(ex, ex, beta);
     if (!neg2) fe_neg(ey, ey);
+    gej_add_ge(R, ex, ey);
+  }
+}
+
+// ------------------------------------------------------------------------------------------
+// R = kP * P + kG * G from a four-tooth comb of P     (result with true Z)
+// ------------------------------------------------------------------------------------------
+// rec: entry 8t + e (16 words at word 16(8t + e)) is (2e+1) * 2^(32t) * P, true affine (key_comb_build, kgv_verify.cuh).
+// gtab: as for ecmult_double, all eight tables.
+// Digit i (0..32) of a recoded GLV half weighs 16^i = 2^(32t) * 16^w with t = i / 8, w = i % 8, except the top digit (i = 32:
+// t = 3, w = 8).  So the ladder runs windows w = 8..0 with four doublings between them and adds, at window w, digit 8t + w of both halves
+// from tooth t (33 additions per half, as ecmult_double); the generator adds bits 32j + 16..32j + 31 of kG from table j at window 4
+// and bits 32j..32j + 15 at window 0 (16 additions).  32 doublings instead of 128.
+// The key entries are staged through the thread's Tab slot: slot s = 2t + half holds one entry; after the addition that consumes
+// slot s, the copy of its entry for the next window starts (one commit group per slot and window), so each copy has seven additions and
+// the window's doublings to land.  stage_wait returns once all but the 7 most recent groups have landed.  The defaults below copy
+// synchronously (host build); the device's shared-memory table overloads them with cp.async (SmemTab, kgv_lib.cu).
+template <class Tab>
+KGV_HD void stage_fetch(Tab& tab, int s, const uint32_t* entry) {
+  for (int w = 0; w < 16; w++) tab.put(s, w, entry[w]);
+}
+template <class Tab>
+KGV_HD void stage_commit(Tab&) {}
+template <class Tab>
+KGV_HD void stage_wait(Tab&) {}
+template <class Tab>
+KGV_HD void stage_get(Tab& tab, int s, fe& x, fe& y) {
+  for (int w = 0; w < 8; w++) { x.v[w] = tab.get(s, w); y.v[w] = tab.get(s, 8 + w); }
+}
+KGV_HD const uint32_t* comb_entry(const uint32_t* rec, const uint32_t* h, int i, bool& neg) {
+  uint32_t idx;
+  recoded_digit(h, i, idx, neg);
+  return rec + (8 * (i < 32 ? i >> 3 : 3) + idx) * 16;  // (the top digit: tooth 3)
+}
+template <class Tab, class GLoad>
+KGV_HD void ecmult_comb(gej& R, const uint32_t* kP, const uint32_t* kG, const uint32_t* rec, Tab& tab, const uint32_t* gtab, GLoad gload) {
+  const fe beta = {KGV_BETA_LIMBS};
+  uint32_t m[2][5], h[2][5];
+  bool ng[2], fix[2];
+  glv_split(m[0], ng[0], m[1], ng[1], kP);
+  recode_signed_odd(h[0], fix[0], m[0]);
+  recode_signed_odd(h[1], fix[1], m[1]);
+  bool dn;
+#pragma unroll 1
+  for (int s = 0; s < 8; s++) {
+    stage_fetch(tab, s, comb_entry(rec, h[s & 1], 8 * (s >> 1) + 7, dn));
+    stage_commit(tab);
+  }
+  R.inf = true;
+  fe_set_zero(R.x); fe_set_zero(R.y); fe_set_zero(R.z);
+  fe ex, ey;
+  // window 8: the top digits, from tooth 3 (read directly while window 7's entries are on their way)
+#pragma unroll 1
+  for (int half = 0; half < 2; half++) {
+    gload(ex, ey, comb_entry(rec, h[half], 32, dn));
+    if (half) fe_mul(ex, ex, beta);
+    if (dn != ng[half]) fe_neg(ey, ey);
+    gej_add_ge(R, ex, ey);
+  }
+#pragma unroll 1
+  for (int w = 7; w >= 0; w--) {
+    gej_double_n(R, 4);
+#pragma unroll 1
+    for (int s = 0; s < 8; s++) {
+      const int half = s & 1, i = 8 * (s >> 1) + w;
+      uint32_t idx;
+      recoded_digit(h[half], i, idx, dn);
+      stage_wait(tab);
+      stage_get(tab, s, ex, ey);
+      if (half) fe_mul(ex, ex, beta);
+      if (dn != ng[half]) fe_neg(ey, ey);
+      gej_add_ge(R, ex, ey);
+      bool dn1;
+      if (w) stage_fetch(tab, s, comb_entry(rec, h[half], i - 1, dn1));
+      stage_commit(tab);  // (empty in the last window: keeps stage_wait's count)
+    }
+    if ((w & 3) == 0) {
+#pragma unroll 1
+      for (int j = 0; j < 8; j++) {
+        const uint32_t d = (kG[j] >> (w ? 16 : 0)) & 0xFFFFu;
+        if (d) {
+          gload(ex, ey, gtab + ((size_t)j * 65536 + d) * 16);
+          gej_add_ge(R, ex, ey);
+        }
+      }
+    }
+  }
+  // parity corrections as in ecmult_double: subtract P (entry 0 of tooth 0), resp. lambda*P
+#pragma unroll 1
+  for (int half = 0; half < 2; half++) {
+    if (!fix[half]) continue;
+    gload(ex, ey, rec);
+    if (half) fe_mul(ex, ex, beta);
+    if (!ng[half]) fe_neg(ey, ey);
     gej_add_ge(R, ex, ey);
   }
 }

@@ -38,6 +38,12 @@ KGV_HD bool key_lift(fe& x, fe& y, uint32_t tag, const uint32_t* pkw) {
 #define KGV_KR_ZS 128
 #define KGV_KR_STATUS 136
 #define KGV_KR_WORDS 140  // 560 bytes
+// Comb key record, for launches whose keys repeat often (key_form, kgv_lib.cu; ecmult_comb): four teeth of odd multiples, true affine.
+// Words, 64-byte entries, records 64-byte aligned:
+//   [0, 512)   entry 8t + e = (2e+1) * 2^(32t) * P for tooth t = 0..3, e = 0..7, at word 16(8t + e): x limbs, then y limbs
+//   512        the key's verdict, as KGV_KR_STATUS
+#define KGV_KC_STATUS 512
+#define KGV_KC_WORDS 528  // 2112 bytes
 
 // Tab accessor over a key record in global memory (the preparation kernel builds the table in place)
 struct RecTab {
@@ -80,16 +86,64 @@ KGV_HD void key_rec_build(uint32_t* rec, uint32_t tag, const uint32_t* pkw) {
   }
   rec[KGV_KR_STATUS] = st;
 }
+// fills a comb key record: the tooth bases 2^(32t) * P by 96 doublings; each tooth's table as build_odd_table builds one, from the base's
+// Jacobian X, Y (affine on the curve with Z scale Z: the table's scale is then zs * Z); one inversion of the four scales' product
+// (Montgomery's trick) brings all 32 entries to true affine.
+KGV_HD void key_comb_build(uint32_t* rec, uint32_t tag, const uint32_t* pkw) {
+  fe x, y;
+  uint8_t st = KGV_ST_PK_PARSE;
+  if (key_lift(x, y, tag, pkw)) {
+    gej b;
+    b.x = x; b.y = y; fe_set_u32(b.z, 1); b.inf = false;
+    fe zs[4], pre[4], inv;
+#pragma unroll 1
+    for (int t = 0; t < 4; t++) {
+      if (t) gej_double_n(b, 32);
+      RecTab tab{rec + 128 * t};
+      fe z;
+      build_odd_table(tab, z, b.x, b.y);
+      fe_mul(zs[t], z, b.z);
+      if (t) fe_mul(pre[t], pre[t - 1], zs[t]);
+      else pre[0] = zs[0];
+    }
+    fe_inv(inv, pre[3]);
+#pragma unroll 1
+    for (int t = 3; t >= 0; t--) {
+      fe zi, zi2, zi3;
+      if (t) {
+        fe_mul(zi, inv, pre[t - 1]);
+        fe_mul(inv, inv, zs[t]);
+      } else {
+        zi = inv;
+      }
+      fe_sqr(zi2, zi);
+      fe_mul(zi3, zi2, zi);
+#pragma unroll 1
+      for (int e = 0; e < 8; e++) {
+        uint32_t* en = rec + 16 * (8 * t + e);
+        fe ex, ey;
+#pragma unroll
+        for (int w = 0; w < 8; w++) { ex.v[w] = en[w]; ey.v[w] = en[8 + w]; }
+        fe_mul(ex, ex, zi2);
+        fe_mul(ey, ey, zi3);
+#pragma unroll
+        for (int w = 0; w < 8; w++) { en[w] = ex.v[w]; en[8 + w] = ey.v[w]; }
+      }
+    }
+    st = KGV_ST_VALID;
+  }
+  rec[KGV_KC_STATUS] = st;
+}
 
 // BIP-340 verification, phase 1: everything up to the projective result R = s*G - e*P.
-// pkw/mw: 8 big-endian words, sigw: 16 big-endian words (r || s).  krec: the key's record, or nullptr (the key part is computed here).
-// Returns a final verdict, or KGV_ST_PENDING with (X, Y, zt = true Z, rx) filled in.
+// pkw/mw: 8 big-endian words, sigw: 16 big-endian words (r || s).  krec: the key's record, or nullptr (the key part is computed here);
+// comb: krec is a comb record.  Returns a final verdict, or KGV_ST_PENDING with (X, Y, zt = true Z, rx) filled in.
 template <class Tab, class GLoad, class Trace = NoTrace>
 KGV_HD uint8_t schnorr_phase1(fe& X, fe& Y, fe& zt, fe& rx, const uint32_t* pkw, const uint32_t* mw, const uint32_t* sigw, Tab& tab,
-                              const uint32_t* gtab, GLoad gload, const uint32_t* krec, Trace trace = Trace()) {
+                              const uint32_t* gtab, GLoad gload, const uint32_t* krec, bool comb, Trace trace = Trace()) {
   fe px, py;
   if (krec) {
-    if (krec[KGV_KR_STATUS] != KGV_ST_VALID) return KGV_ST_PK_PARSE;
+    if (krec[comb ? KGV_KC_STATUS : KGV_KR_STATUS] != KGV_ST_VALID) return KGV_ST_PK_PARSE;
   } else {
     limbs_from_be_words(px.v, pkw);
     if (!fe_words_lt_p(px.v)) return KGV_ST_PK_PARSE;      // x >= p
@@ -110,15 +164,20 @@ KGV_HD uint8_t schnorr_phase1(fe& X, fe& Y, fe& zt, fe& rx, const uint32_t* pkw,
   trace(3, e, 8); trace(4, k, 8); trace(5, s, 8);
   gej R;
   fe zs;
-  if (krec) key_rec_load(tab, zs, krec);
-  else build_odd_table(tab, zs, px, py);
-  ecmult_double(R, zs, k, s, tab, gtab, gload, trace);
+  if (comb) {
+    ecmult_comb(R, k, s, krec, tab, gtab, gload);
+  } else {
+    if (krec) key_rec_load(tab, zs, krec);
+    else build_odd_table(tab, zs, px, py);
+    ecmult_double(R, zs, k, s, tab, gtab, gload, trace);
+  }
   { uint32_t f[1] = {R.inf}; trace(18, f, 1); }
   if (R.inf) return KGV_ST_INVALID;
   trace(19, R.x.v, 8); trace(20, R.y.v, 8); trace(21, R.z.v, 8);
   X = R.x;
   Y = R.y;
-  fe_mul(zt, R.z, zs);
+  if (comb) zt = R.z;
+  else fe_mul(zt, R.z, zs);
   return KGV_ST_PENDING;
 }
 // phase 2: zi = 1/zt. Valid iff y(R) is even and x(R) == r.
@@ -141,21 +200,21 @@ KGV_HD uint8_t schnorr_phase2(const fe& X, const fe& Y, const fe& zi, const fe& 
 // single-signature form (audit kernel, host unit tests)
 template <class Tab, class GLoad, class Trace = NoTrace>
 KGV_HD uint8_t schnorr_verify_core(const uint32_t* pkw, const uint32_t* mw, const uint32_t* sigw, Tab& tab, const uint32_t* gtab,
-                                   GLoad gload, Trace trace = Trace(), const uint32_t* krec = nullptr) {
+                                   GLoad gload, Trace trace = Trace(), const uint32_t* krec = nullptr, bool comb = false) {
   fe X, Y, zt, rx, zi;
-  uint8_t st = schnorr_phase1(X, Y, zt, rx, pkw, mw, sigw, tab, gtab, gload, krec, trace);
+  uint8_t st = schnorr_phase1(X, Y, zt, rx, pkw, mw, sigw, tab, gtab, gload, krec, comb, trace);
   if (st != KGV_ST_PENDING) return st;
   fe_inv(zi, zt);
   return schnorr_phase2(X, Y, zi, rx, trace);
 }
 
 // ECDSA verification with libsecp256k1 semantics, phase 1: parsing and range checks.
-// pkw: 8 big-endian words of x, tag = first key byte, krec: the key's record or nullptr.  Returns a final verdict or KGV_ST_PENDING with
-// the key (qx,qy; unset with a record), r, s (to be inverted, possibly batched) and the reduced message m.
+// pkw: 8 big-endian words of x, tag = first key byte, krec: the key's record or nullptr (comb: a comb record).  Returns a final verdict or
+// KGV_ST_PENDING with the key (qx,qy; unset with a record), r, s (to be inverted, possibly batched) and the reduced message m.
 KGV_HD uint8_t ecdsa_phase1(fe& qx, fe& qy, uint32_t* r, uint32_t* s, uint32_t* m, uint32_t tag, const uint32_t* pkw, const uint32_t* mw,
-                            const uint32_t* sigw, const uint32_t* krec) {
+                            const uint32_t* sigw, const uint32_t* krec, bool comb) {
   if (krec) {
-    if (krec[KGV_KR_STATUS] != KGV_ST_VALID) return KGV_ST_PK_PARSE;
+    if (krec[comb ? KGV_KC_STATUS : KGV_KR_STATUS] != KGV_ST_VALID) return KGV_ST_PK_PARSE;
   } else if (!key_lift(qx, qy, tag, pkw)) {
     return KGV_ST_PK_PARSE;
   }
@@ -171,19 +230,24 @@ KGV_HD uint8_t ecdsa_phase1(fe& qx, fe& qy, uint32_t* r, uint32_t* s, uint32_t* 
 // phase 2: sn = s^-1 mod n.  R = (m/s)*G + (r/s)*Q, valid iff x(R) mod n == r.
 template <class Tab, class GLoad>
 KGV_HD uint8_t ecdsa_phase2(const fe& qx, const fe& qy, const uint32_t* r, const uint32_t* sn, const uint32_t* m, Tab& tab, const uint32_t* gtab,
-                            GLoad gload, const uint32_t* krec) {
+                            GLoad gload, const uint32_t* krec, bool comb) {
   uint32_t u1[8], u2[8];
   sc_mul(u1, sn, m);
   sc_mul(u2, sn, r);
   gej R;
-  fe zs;
-  if (krec) key_rec_load(tab, zs, krec);
-  else build_odd_table(tab, zs, qx, qy);
-  ecmult_double(R, zs, u2, u1, tab, gtab, gload);
+  fe zs, zt;
+  if (comb) {
+    ecmult_comb(R, u2, u1, krec, tab, gtab, gload);
+  } else {
+    if (krec) key_rec_load(tab, zs, krec);
+    else build_odd_table(tab, zs, qx, qy);
+    ecmult_double(R, zs, u2, u1, tab, gtab, gload);
+  }
   if (R.inf) return KGV_ST_INVALID;
   // x(R) mod n == r  <=>  X == r*Zt^2  or  (r + n < p and X == (r+n)*Zt^2)
-  fe zt, zt2, t, rf;
-  fe_mul(zt, R.z, zs);
+  fe zt2, t, rf;
+  if (comb) zt = R.z;
+  else fe_mul(zt, R.z, zs);
   fe_sqr(zt2, zt);
 #pragma unroll
   for (int i = 0; i < 8; i++) rf.v[i] = r[i];
@@ -200,13 +264,13 @@ KGV_HD uint8_t ecdsa_phase2(const fe& qx, const fe& qy, const uint32_t* r, const
 }
 template <class Tab, class GLoad>
 KGV_HD uint8_t ecdsa_verify_core(uint32_t tag, const uint32_t* pkw, const uint32_t* mw, const uint32_t* sigw, Tab& tab,
-                                 const uint32_t* gtab, GLoad gload, const uint32_t* krec = nullptr) {
+                                 const uint32_t* gtab, GLoad gload, const uint32_t* krec = nullptr, bool comb = false) {
   fe qx, qy;
   uint32_t r[8], s[8], m[8], sn[8];
-  uint8_t st = ecdsa_phase1(qx, qy, r, s, m, tag, pkw, mw, sigw, krec);
+  uint8_t st = ecdsa_phase1(qx, qy, r, s, m, tag, pkw, mw, sigw, krec, comb);
   if (st != KGV_ST_PENDING) return st;
   sc_inv(sn, s);
-  return ecdsa_phase2(qx, qy, r, sn, m, tab, gtab, gload, krec);
+  return ecdsa_phase2(qx, qy, r, sn, m, tab, gtab, gload, krec, comb);
 }
 
 // One entry of the generator tables: v * B for v in [1, 65535], B affine; result affine.
@@ -233,5 +297,25 @@ KGV_HD void gtab_entry(fe& ox, fe& oy, uint32_t v, const fe& bx, const fe& by) {
 // 2^128 * G (tools/derive_constants.py)
 #define KGV_G128X_LIMBS {0x9EC4C0DAu, 0x1B7B444Cu, 0x723EA335u, 0xE88C5678u, 0x981F162Eu, 0x9239C1ADu, 0xF63B5F33u, 0x8F68B9D2u}
 #define KGV_G128Y_LIMBS {0x501FFF82u, 0xF23CBF79u, 0x95510BFDu, 0xBBEA2CFEu, 0xB6BE215Du, 0xDE1D90C2u, 0xBA063986u, 0x662A9F2Du}
+// 2^(32j) * G for the other generator tables (oracle/pyref.py: pt_mul(2**(32*j), G); tests/test_hostsim_comb.py checks them)
+#define KGV_G32X_LIMBS {0x39A48DB0u, 0xEFD7835Bu, 0x9B3C03BFu, 0x9F1215A2u, 0x9B7BDE45u, 0x2791D0A0u, 0x696E7167u, 0x100F44DAu}
+#define KGV_G32Y_LIMBS {0x2BC65A09u, 0x0FBD5CD6u, 0xFF5195ACu, 0xB7FF4A18u, 0x0C090666u, 0x2EC8F330u, 0x92A00B77u, 0xCDD9E131u}
+#define KGV_G64X_LIMBS {0x42D0E6BDu, 0x13B7E0E7u, 0xDB0F5E53u, 0xF774D163u, 0x104D6ECBu, 0x82A2147Cu, 0x243C4E25u, 0x3322D401u}
+#define KGV_G64Y_LIMBS {0x6C28B2A0u, 0x24F3A2E9u, 0xA2873AF6u, 0x2805F63Eu, 0x4DDAF9B7u, 0xBFB019BCu, 0xE9664EF5u, 0x56E70797u}
+#define KGV_G96X_LIMBS {0x40FB27B6u, 0x32427E28u, 0xBE430576u, 0xC76E3DB2u, 0x61686AA5u, 0x10F238ADu, 0xBE778B1Bu, 0xFEA74E3Du}
+#define KGV_G96Y_LIMBS {0xF23CB96Fu, 0x701D3DB7u, 0x973F7B77u, 0x126B596Bu, 0xCCB6AF93u, 0x7CF674DEu, 0x9B0B1329u, 0x6E0568DBu}
+#define KGV_G160X_LIMBS {0xAC1F98CDu, 0xCBFC99C8u, 0x4D7F0308u, 0x52348905u, 0x1CC66021u, 0xFAED8A9Cu, 0x4A474870u, 0x9C3919A8u}
+#define KGV_G160Y_LIMBS {0xD4FC599Du, 0xBE7E5E03u, 0x6C64C8E6u, 0x905326F7u, 0xF260E641u, 0x584F044Bu, 0x4A4DDD57u, 0xDDB84F0Fu}
+#define KGV_G192X_LIMBS {0x2120E2B3u, 0x7F3B58FAu, 0x7F47F9AAu, 0x7A58FDCEu, 0x4CE6E521u, 0xE7BE4AE3u, 0x1F51BDBAu, 0xEAA649F2u}
+#define KGV_G192Y_LIMBS {0xBA5AD93Du, 0xD47A5305u, 0xF13F7E59u, 0x01A6B965u, 0x9879AA5Au, 0xC69A80F8u, 0x5BBBB03Au, 0xBE3279EDu}
+#define KGV_G224X_LIMBS {0x9475B7BAu, 0x884FDFF0u, 0xE4918B3Du, 0xE039E730u, 0xF5018CDBu, 0x3D3E57EDu, 0x1943785Cu, 0x95939698u}
+#define KGV_G224Y_LIMBS {0x7524F2FDu, 0xE9B8ABF8u, 0xC8709385u, 0x9C653F64u, 0x4B9CD684u, 0x8BA0386Au, 0x88C331DDu, 0x2E7E5528u}
+// base of generator table j (0..7): 2^(32j) * G
+KGV_HD void gtab_base(fe& x, fe& y, int j) {
+  const fe bx[8] = {{KGV_GX_LIMBS}, {KGV_G32X_LIMBS}, {KGV_G64X_LIMBS}, {KGV_G96X_LIMBS}, {KGV_G128X_LIMBS}, {KGV_G160X_LIMBS}, {KGV_G192X_LIMBS}, {KGV_G224X_LIMBS}};
+  const fe by[8] = {{KGV_GY_LIMBS}, {KGV_G32Y_LIMBS}, {KGV_G64Y_LIMBS}, {KGV_G96Y_LIMBS}, {KGV_G128Y_LIMBS}, {KGV_G160Y_LIMBS}, {KGV_G192Y_LIMBS}, {KGV_G224Y_LIMBS}};
+  x = bx[j];
+  y = by[j];
+}
 
 }  // namespace kgv

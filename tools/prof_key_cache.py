@@ -6,9 +6,11 @@
 Legs (device-resident triples, L2 flushed before every timed call, CUDA events around each kgv_schnorr_verify call):
   bench     bench.py's workload: N triples over 65 536 keys (each key about 16 times)
   distinct  N triples drawn over N keys (about 0.64 N distinct): too many keys for records, so only the dedup pass is added
+  sweep     N triples over N/64 ... N/2 distinct keys (a base set over about that many keys, tiled to N): where the comb records
+            (at most N/COMB_USES keys) start to pay against the plain ones
 Each leg prints one JSON line: ms per call (mean, min, max), verifies/s, the distinct keys, the keys used at least twice and the records a
-launch makes (every distinct key when there are at most n/2 and at most 2^17 of them, else none: key_records_on in kgv_lib.cu; counted
-from the keys on the host).
+launch makes and their form (every distinct key when there are at most n/2 and at most 2^17 of them, else none; comb records when there
+are at most n/COMB_USES: key_form in kgv_lib.cu; counted from the keys on the host).
 --profile DIR: a separate torch.profiler run of 3 calls per leg; the device time of every kernel and memset, summed per name, goes to
 the JSON line (and the trace to DIR).  KGV_LIB selects the build of libkgv.so, so an older build can be timed the same way.
 The generated triples are cached under the system's temporary directory (1 Mi distinct keys take a minute to generate).
@@ -26,6 +28,14 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
 RECORDS_MAX = 1 << 17
+COMB_USES = 8  # KGV_COMB_USES in kgv_lib.cu
+SWEEP = (64, 32, 16, 12, 10, 8, 6, 4, 3, 2)
+
+
+def form(n, d):
+    if d > min(n // 2, RECORDS_MAX):
+        return "inline"
+    return "comb" if COMB_USES * d <= n else "plain"
 
 
 def triples(n, n_keys, seed):
@@ -56,10 +66,18 @@ def main():
     ctx.use_stream(stream.cuda_stream)
     props = torch.cuda.get_device_properties(dev)
     flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)
+    legs = []
     for leg in args.legs.split(","):
-        n_keys = {"bench": 65536, "distinct": args.n}[leg]
+        legs += [(f"sweep_n/{u}", u) for u in SWEEP] if leg == "sweep" else [(leg, None)]
+    for leg, u in legs:
         t0 = time.perf_counter()
-        pk, msg, sig, kind = triples(args.n, n_keys, 0x6B61737061)
+        if u is None:
+            n_keys = {"bench": 65536, "distinct": args.n}[leg]
+            pk, msg, sig, kind = triples(args.n, n_keys, 0x6B61737061)
+        else:  # a base set of 1.5 items per key over n_keys keys (about 0.78 n_keys distinct), tiled to n
+            from rusty_kaspa_b200 import workload as W
+            n_keys = int(args.n / u / 0.78)
+            pk, msg, sig, kind = W.tile_triples(*triples(n_keys * 3 // 2, n_keys, 0x6B61737061), args.n)
         gen_s = time.perf_counter() - t0
         _, counts = np.unique(pk, axis=0, return_counts=True)
         repeated = int((counts >= 2).sum())
@@ -89,7 +107,7 @@ def main():
                     for _ in range(3):
                         call()
                     stream.synchronize()
-                prof.export_chrome_trace(os.path.join(args.profile, f"key_cache_{leg}.json"))
+                prof.export_chrome_trace(os.path.join(args.profile, f"key_cache_{leg.replace('/', '_')}.json"))
                 kernels = {}
                 for ev in prof.events():
                     if ev.device_type.name == "CUDA":
@@ -97,7 +115,8 @@ def main():
                         kernels[k] = kernels.get(k, 0.0) + ev.device_time / 1e3 / 3
                 kernels = {k: round(v, 4) for k, v in sorted(kernels.items(), key=lambda kv: -kv[1])}
         print(json.dumps({"leg": leg, "n": args.n, "n_keys": n_keys, "distinct_keys": int(len(counts)), "keys_used_twice_or_more": repeated,
-                          "records_per_launch": len(counts) if len(counts) <= min(args.n // 2, RECORDS_MAX) else 0, "ms_mean": round(float(np.mean(ms)), 4), "ms_min": round(float(np.min(ms)), 4),
+                          "records_per_launch": len(counts) if len(counts) <= min(args.n // 2, RECORDS_MAX) else 0,
+                          "form": form(args.n, len(counts)), "ms_mean": round(float(np.mean(ms)), 4), "ms_min": round(float(np.min(ms)), 4),
                           "ms_max": round(float(np.max(ms)), 4), "verifies_per_s": args.n / (float(np.mean(ms)) * 1e-3),
                           "kernel_ms_per_call": kernels, "lib": os.environ.get("KGV_LIB", "libkgv.so"), "gpu": props.name, "generation_s": round(gen_s, 1)}),
               flush=True)
