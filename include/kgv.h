@@ -580,6 +580,27 @@ int kgv_gtable_entry(kgv_ctx* ctx, int which, uint32_t v, uint8_t out_xy[64]);
 int kgv_debug_schnorr_trace(kgv_ctx* ctx, const uint8_t* pk32, const uint8_t* msg32, const uint8_t* sig64, uint32_t* trace_words,
                             uint8_t* status);
 
+/* Test / audit hook: which key form the last verify launch of one kind took.  A verify launch
+ * decides on the device, from the number of distinct keys it counts, whether every item computes
+ * its key part inline, reads a plain key record, or reads a four-tooth comb record; that choice
+ * selects the scalar-multiplication ladder.  ecdsa: 0 = the last kgv_schnorr_verify launch, 1 =
+ * the last kgv_ecdsa_verify launch, including launches made by the validation calls when they do
+ * not go through a signature cache.  Synchronises the stream that launch ran on (which must still
+ * exist) and copies one counter back: not for timed paths.  distinct_keys is the count of the
+ * launch's key-deduplication pass; once it exceeds what the records allow the pass stops
+ * counting, so it is then a lower bound.  KGV_ERR_ARG if no launch of that kind was made. */
+#define KGV_KEY_FORM_NO_CACHE 0 /* at most one item per thread: no key deduplication ran      */
+#define KGV_KEY_FORM_INLINE 1   /* deduplication ran, too many distinct keys: no records       */
+#define KGV_KEY_FORM_PLAIN 2    /* one odd-multiples record per key (128-doubling ladder)     */
+#define KGV_KEY_FORM_COMB 3     /* one four-tooth comb record per key (32-doubling ladder)     */
+typedef struct kgv_key_form_info {
+  uint64_t n_items;       /* items of the launch                                  */
+  uint64_t threads;       /* threads of its grid (blocks x threads per block)     */
+  uint32_t distinct_keys; /* distinct keys counted on the device (0 without cache) */
+  int32_t form;           /* KGV_KEY_FORM_*                                       */
+} kgv_key_form_info;
+int kgv_debug_key_form(kgv_ctx* ctx, int ecdsa, kgv_key_form_info* out);
+
 /* Test / audit hook: runs one arithmetic primitive (its PTX body) on n operand pairs on the device.
  * in_words / out_words: n x 16 u32 (a[8] || b[8] little-endian limbs in; result limbs out).
  * op: 0 mul_wide 1 sqr_wide 2 fe_mul 3 fe_sqr 4 sc_mul 5 sc_sqr 6 sc_inv 7 fe_inv 8 fe_add 9 fe_sub

@@ -85,8 +85,14 @@ SYMBOLS = [
     ("kgv_gtable_entry", _c.c_int, [_c.c_void_p, _c.c_int, _c.c_uint32, _u8p]),
     ("kgv_debug_selftest", _c.c_int, [_c.c_void_p, _c.c_int, _u8p, _u8p, _c.c_size_t]),
     ("kgv_debug_schnorr_trace", _c.c_int, [_c.c_void_p, _u8p, _u8p, _u8p, _u8p, _u8p]),
+    ("kgv_debug_key_form", _c.c_int, [_c.c_void_p, _c.c_int, _c.c_void_p]),
 ]
 TRACE_STAGES = 32
+KEY_FORMS = ("no-cache", "inline", "plain", "comb")  # KGV_KEY_FORM_* in include/kgv.h
+
+
+class KeyFormInfo(_c.Structure):
+    _fields_ = [("n_items", _c.c_uint64), ("threads", _c.c_uint64), ("distinct_keys", _c.c_uint32), ("form", _c.c_int32)]
 
 _lib = None
 

@@ -71,6 +71,13 @@ struct kgv_ctx {
   struct kgv_comm* shard_comm = nullptr;  // kgv_set_sharding: signature checks of the validation calls are split over its ranks
   std::vector<uint8_t*> parked;  // outgrown per-call buffers, released when the caller synchronises / destroys the context (kgv_reserve)
   uint64_t launches = 0;
+  // the last non-indexed verify launch of each kind ([0] Schnorr, [1] ECDSA), for kgv_debug_key_form
+  struct {
+    size_t n = 0;
+    unsigned blocks = 0;
+    bool key_cache = false;
+    cudaStream_t stream = nullptr;
+  } last_verify[2];
   int resident_blocks = 132 * KGV_BLOCKS_PER_SM;  // verification kernels: blocks that fit the device at once (persistent grid)
   std::recursive_mutex mu;  // recursive: the host-VM resolution inside a validation call re-enters the ABI (kgv_sighash, kgv_*_verify)
   std::string err;

@@ -113,7 +113,8 @@ enum { KGV_KEYS_INLINE = 0, KGV_KEYS_PLAIN = 1, KGV_KEYS_COMB = 2 };
 // and fit the cap; then EVERY key has one.  A warp pays for the inline key path of any of its lanes, so records for the repeated keys
 // alone leave singleton lanes costing whole warps; a batch of mostly distinct keys makes no records at all and pays only the dedup pass.
 // Comb records (key_comb_build, ecmult_comb) when the keys are used at least KGV_COMB_USES times on average, plain ones (key_rec_build) below.
-__device__ __forceinline__ int key_form(uint32_t n_rec, size_t n) {
+// Host-callable too: kgv_debug_key_form reports the form a launch took by this same rule.
+__host__ __device__ __forceinline__ int key_form(uint32_t n_rec, size_t n) {
   if (n_rec > KGV_KEY_RECORDS_MAX || 2 * (size_t)n_rec > n) return KGV_KEYS_INLINE;
   return (size_t)KGV_COMB_USES * n_rec <= n ? KGV_KEYS_COMB : KGV_KEYS_PLAIN;
 }
@@ -630,9 +631,14 @@ int kgv_launch_verify(kgv_ctx* ctx, const uint8_t* dpk, const uint8_t* dmsg, con
   // The key cache pays off when threads verify several items: in a launch of at most one item per thread the preparation's latency
   // comes on top of a verify that shortens by the same latency (small batches measured 10 % slower with it).
   KeyCacheView kc{};
-  if (n > (size_t)ctx->resident_blocks * KGV_BLOCK) {
+  const bool key_cache = n > (size_t)ctx->resident_blocks * KGV_BLOCK;
+  if (key_cache) {
     int rc = key_cache_launch(ctx, dpk, n, ecdsa, aligned, st, index, n_dev, &kc);
     if (rc) return rc;
+  }
+  if (!index) {
+    auto& lv = ctx->last_verify[ecdsa];
+    lv.n = n; lv.blocks = blocks; lv.key_cache = key_cache; lv.stream = st;
   }
   if (ecdsa) {
     if (index) {
@@ -772,6 +778,27 @@ extern "C" int kgv_debug_schnorr_trace(kgv_ctx* ctx, const uint8_t* pk32, const 
   CK(cudaMemcpyAsync(trace_words, ctx->d_out, tw, cudaMemcpyDeviceToHost, ctx->stream));
   CK(cudaMemcpyAsync(status, ctx->d_out + tw, 1, cudaMemcpyDeviceToHost, ctx->stream));
   CK(cudaStreamSynchronize(ctx->stream));
+  return KGV_OK;
+}
+
+extern "C" int kgv_debug_key_form(kgv_ctx* ctx, int ecdsa, kgv_key_form_info* out) {
+  if (!ctx) return KGV_ERR_ARG;
+  std::lock_guard<std::recursive_mutex> g(ctx->mu);
+  if (!out) return fail_arg(ctx, "null buffer");
+  const auto& lv = ctx->last_verify[ecdsa ? 1 : 0];
+  if (lv.n == 0) return fail_arg(ctx, "no verify launch of that kind yet");
+  CK(cudaSetDevice(ctx->device));
+  CK(cudaStreamSynchronize(lv.stream));
+  uint32_t n_rec = 0;
+  if (lv.key_cache) CK(cudaMemcpy(&n_rec, ctx->d_keys[ecdsa ? 1 : 0], sizeof n_rec, cudaMemcpyDeviceToHost));
+  out->n_items = lv.n;
+  out->threads = (uint64_t)lv.blocks * KGV_BLOCK;
+  out->distinct_keys = n_rec;
+  if (!lv.key_cache) out->form = KGV_KEY_FORM_NO_CACHE;
+  else {
+    const int f = key_form(n_rec, lv.n);
+    out->form = f == KGV_KEYS_COMB ? KGV_KEY_FORM_COMB : f == KGV_KEYS_PLAIN ? KGV_KEY_FORM_PLAIN : KGV_KEY_FORM_INLINE;
+  }
   return KGV_OK;
 }
 

@@ -207,6 +207,14 @@ class GpuContext:
                                                       tr.ctypes.data, st.ctypes.data))
         return int(st[0]), tr
 
+    def debug_key_form(self, ecdsa=False):
+        """Key form of the last non-indexed verify launch of one kind (audit hook, synchronises): dict with n_items, threads,
+        distinct_keys and form, one of "no-cache", "inline", "plain", "comb" (KGV_KEY_FORM_* in include/kgv.h)."""
+        info = _lib.KeyFormInfo()
+        self._check(self._lib.kgv_debug_key_form(self._h, 1 if ecdsa else 0, ctypes.byref(info)))
+        return {"n_items": int(info.n_items), "threads": int(info.threads), "distinct_keys": int(info.distinct_keys),
+                "form": _lib.KEY_FORMS[info.form]}
+
     def gtable_entry(self, which, v):
         out = (ctypes.c_uint8 * 64)()
         self._check(self._lib.kgv_gtable_entry(self._h, which, v, ctypes.addressof(out)))

@@ -5,6 +5,7 @@ import numpy as np
 import pytest
 
 from conftest import oracle_ecdsa_batch
+from ladder_model import crafted_ecdsa_edge_cases
 from rusty_kaspa_b200 import workload as W
 
 pytestmark = pytest.mark.gpu
@@ -30,48 +31,13 @@ def test_ecdsa_ragged_sizes(gpu_ctx, oracle, n):
         assert (got == oracle_ecdsa_batch(oracle, pk, msg, sig)).all()
 
 
-def _crafted_ecdsa_edge_cases():
-    """Triples built for the branches random data never reaches (big-integer arithmetic of oracle/pyref.py, no GPU / C code involved):
-      * x(R) >= n, so that r = x(R) - n and the verifier must try r + n < p  (Q is SOLVED for: Q = r^-1 (s R - m G), no discrete log needed)
-      * s exactly (n-1)/2 (the largest low S: valid) and (n+1)/2 (the smallest high S: rejected although the equation holds)
-      * 33-byte keys with the uncompressed / hybrid tags 04, 06, 07 (PublicKey::from_slice fails on a 33-byte slice with those tags)"""
-    import pyref
-    N, P, G = pyref.N, pyref.P, pyref.G
-    rng = np.random.default_rng(77)
-    out = []  # (pk33, msg32, sig64, expected status, label)
-    comp = lambda pt: bytes([2 + (pt[1] & 1)]) + pt[0].to_bytes(32, "big")
-    j = 0
-    while len([o for o in out if o[4] == "wrap"]) < 12:
-        j += 1
-        R = pyref.lift_x(N + int(rng.integers(1, 2**62)) * 7 + j)
-        if R is None:
-            continue
-        r = R[0] - N
-        s = int.from_bytes(rng.bytes(32), "big") % (N // 2 - 1) + 1  # low S
-        m = int.from_bytes(rng.bytes(32), "big") % N
-        Q = pyref.pt_mul(pow(r, -1, N), pyref.pt_add(pyref.pt_mul(s, R), pyref.pt_mul((N - m) % N, G)))
-        sig = r.to_bytes(32, "big") + s.to_bytes(32, "big")
-        out.append((comp(Q), m.to_bytes(32, "big"), sig, 1, "wrap"))
-        out.append((comp(Q), ((m + 1) % N).to_bytes(32, "big"), sig, 0, "wrap-wrong-msg"))
-    for target, exp in (((N - 1) // 2, 1), ((N + 1) // 2, 0), ((N - 1) // 2 - 1, 1), ((N + 1) // 2 + 1, 0)):
-        for _ in range(6):
-            d, k = int.from_bytes(rng.bytes(32), "big") % (N - 1) + 1, int.from_bytes(rng.bytes(32), "big") % (N - 1) + 1
-            r = pyref.pt_mul(k, G)[0] % N
-            m = (target * k - r * d) % N  # s = k^-1 (m + r d) = target
-            out.append((comp(pyref.pt_mul(d, G)), m.to_bytes(32, "big"), r.to_bytes(32, "big") + target.to_bytes(32, "big"), exp, f"s={'low' if exp else 'high'}-boundary"))
-    base = out[0]
-    for tag in (0x04, 0x06, 0x07, 0x00, 0x05):
-        out.append((bytes([tag]) + base[0][1:], base[1], base[2], 2, f"tag {tag:02x}"))
-    return out
-
-
 def test_ecdsa_crafted_edge_cases(gpu_ctx, oracle):
     """r + n < p wrap-around, the low-S boundary and foreign key tags: GPU == oracle == pyref == construction, and OpenSSL agrees where it has an opinion"""
     import pyref
     from cryptography.exceptions import InvalidSignature
     from cryptography.hazmat.primitives import hashes
     from cryptography.hazmat.primitives.asymmetric import ec, utils
-    cases = _crafted_ecdsa_edge_cases()
+    cases = crafted_ecdsa_edge_cases()
     pk = np.frombuffer(b"".join(c[0] for c in cases), dtype=np.uint8).reshape(-1, 33).copy()
     msg = np.frombuffer(b"".join(c[1] for c in cases), dtype=np.uint8).reshape(-1, 32).copy()
     sig = np.frombuffer(b"".join(c[2] for c in cases), dtype=np.uint8).reshape(-1, 64).copy()

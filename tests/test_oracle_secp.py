@@ -124,11 +124,8 @@ def test_fast_cpu_port_equals_the_plain_checker(oracle):
     assert (a == b).all() and set(a) == {0, 1, 2, 3}
     bpk, bmsg, bsig, exp, _ = bip340_vectors()
     assert _batch(oracle.ok_schnorr_verify_batch_fast, bpk, bmsg, bsig).tolist() == exp
-    sys_path_tests = __import__("os").path.dirname(__import__("os").path.abspath(__file__))
-    import importlib.util
-    spec = importlib.util.spec_from_file_location("t_gpu_ecdsa", __import__("os").path.join(sys_path_tests, "test_gpu_ecdsa.py"))
-    mod = importlib.util.module_from_spec(spec); spec.loader.exec_module(mod)
-    cases = mod._crafted_ecdsa_edge_cases()
+    from ladder_model import crafted_ecdsa_edge_cases
+    cases = crafted_ecdsa_edge_cases()
     cpk = np.frombuffer(b"".join(c[0] for c in cases), dtype=np.uint8).reshape(-1, 33).copy()
     cmsg = np.frombuffer(b"".join(c[1] for c in cases), dtype=np.uint8).reshape(-1, 32).copy()
     csig = np.frombuffer(b"".join(c[2] for c in cases), dtype=np.uint8).reshape(-1, 64).copy()
