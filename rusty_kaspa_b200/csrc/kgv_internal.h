@@ -101,10 +101,10 @@ struct kgv_dev_batch {
 // Makes the batch arrays device-resident (uploads host arrays into ctx staging; wraps device arrays).
 int kgv_batch_to_device(kgv_ctx* ctx, const kgv_tx_batch* b, kgv_dev_batch* out, bool need_entries);
 
-// Enqueue a verification kernel on device-resident SoA item arrays (no locking, no copies): used by the
+// Enqueue a verification kernel on device-resident SoA item arrays on stream st (no locking, no copies): used by the
 // fused validation path.  ecdsa: pk stride 33, else 32.
 int kgv_launch_verify(kgv_ctx* ctx, const uint8_t* dpk, const uint8_t* dmsg, const uint8_t* dsig, size_t n, uint8_t* dstatus, bool ecdsa,
-                      cudaStream_t on = nullptr, bool use_on = false, const uint32_t* index = nullptr, const uint32_t* n_dev = nullptr);
+                      cudaStream_t st, const uint32_t* index = nullptr, const uint32_t* n_dev = nullptr);
 
 // ---- MuHash product trees (kgv_muhash.cu) ----
 // Reserve the level-0 element arrays of the two trees (denominator = removed elements, numerator = added elements):

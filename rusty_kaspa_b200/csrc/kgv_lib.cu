@@ -129,13 +129,12 @@ struct KeyCacheView {
   const uint32_t* item_slot;  // item -> table slot (only the items the launch verifies are set)
   const uint32_t* recs;       // records, KGV_KR_WORDS or KGV_KC_WORDS words each
   const uint32_t* n_rec;      // distinct keys of the launch; nullptr: no key cache
-  __device__ __forceinline__ bool comb(size_t n) const { return n_rec && key_form(*n_rec, n) == KGV_KEYS_COMB; }
-  // the record of item i, or nullptr (the launch makes no records)
-  __device__ __forceinline__ const uint32_t* rec_of(size_t i, size_t n) const {
-    if (!n_rec) return nullptr;
-    const int f = key_form(*n_rec, n);
-    if (f == KGV_KEYS_INLINE) return nullptr;
-    return recs + (size_t)(table[item_slot[i]].rec - 1) * (f == KGV_KEYS_COMB ? KGV_KC_WORDS : KGV_KR_WORDS);
+  // the key source of item i: its record and the launch's form, or no record (the launch makes none)
+  __device__ __forceinline__ KeySrc key_of(size_t i, size_t n) const {
+    const int f = n_rec ? key_form(*n_rec, n) : KGV_KEYS_INLINE;
+    if (f == KGV_KEYS_INLINE) return KeySrc{nullptr, false};
+    const bool comb = f == KGV_KEYS_COMB;
+    return KeySrc{recs + (size_t)(table[item_slot[i]].rec - 1) * (comb ? KGV_KC_WORDS : KGV_KR_WORDS), comb};
   }
 };
 
@@ -226,19 +225,30 @@ __global__ void __launch_bounds__(KGV_BLOCK, KGV_BLOCKS_PER_SM) k_key_prepare(co
 // ONE modular inversion among them (Montgomery's trick): the field inversion of BIP-340's final affine
 // conversion, resp. the scalar inversion s^-1 of ECDSA, drops from 1 to 1/KGV_ITEMS per signature with no
 // cross-thread synchronisation.  Pending state sits in (L1-resident) local memory between the phases.
-template <bool ALIGNED, bool INDEXED>
-__global__ void __launch_bounds__(KGV_BLOCK, KGV_BLOCKS_PER_SM)
-k_schnorr_verify(const uint8_t* __restrict__ pk, const uint8_t* __restrict__ msg, const uint8_t* __restrict__ sig, size_t n_arg,
-                 uint8_t* __restrict__ status, const uint32_t* __restrict__ gtab, const uint32_t* __restrict__ index, const uint32_t* __restrict__ n_dev,
-                 KeyCacheView kc) {
-  // INDEXED: verify only the listed items (the signature-cache misses), their count read on the device.  A separate instantiation: the two
-  // extra pointers live across the whole kernel cost the plain form 3 % (register pressure at the 168-register cap, measured).
+// The product of the trick: in the field for Schnorr, mod n for ECDSA.
+template <bool ECDSA>
+__device__ __forceinline__ void batch_mul(fe& r, const fe& a, const fe& b) {
+  if constexpr (ECDSA) sc_mul(r.v, a.v, b.v);
+  else fe_mul(r, a, b);
+}
+// The body of both verify kernels.  INDEXED: verify only the listed items (the signature-cache misses), their count read on the device.
+// A separate instantiation: the two extra pointers live across the whole kernel cost the plain form 3 % (register pressure at the
+// 168-register cap, measured).
+template <bool ECDSA, bool ALIGNED, bool INDEXED>
+__device__ __forceinline__ void verify_body(const uint8_t* __restrict__ pk, const uint8_t* __restrict__ msg, const uint8_t* __restrict__ sig,
+                                            size_t n_arg, uint8_t* __restrict__ status, const uint32_t* __restrict__ gtab,
+                                            const uint32_t* __restrict__ index, const uint32_t* __restrict__ n_dev, KeyCacheView kc) {
   extern __shared__ uint32_t smem[];
   const size_t n = (INDEXED && n_dev) ? (size_t)*n_dev : n_arg;
   const size_t total = (size_t)gridDim.x * KGV_BLOCK;
   const size_t tid = (size_t)blockIdx.x * KGV_BLOCK + threadIdx.x;
   SmemTab tab{smem + threadIdx.x};
-  fe X[KGV_ITEMS], Y[KGV_ITEMS], ZT[KGV_ITEMS], RX[KGV_ITEMS], pre[KGV_ITEMS];
+  // pending items: D, the value to invert (Schnorr: the true Z of R; ECDSA: s), and pre, the product of the earlier items' D;
+  // X, Y: R before its affine conversion (Schnorr) or the key (ECDSA, inline key path); RX: r.  M, KR: ECDSA's m and key record, and
+  // comb its form, the same for every item of a launch (a flag per item cost 32 B of stack)
+  fe X[KGV_ITEMS], Y[KGV_ITEMS], RX[KGV_ITEMS], D[KGV_ITEMS], pre[KGV_ITEMS], M[KGV_ITEMS];
+  const uint32_t* KR[KGV_ITEMS];
+  bool comb = false;
   uint8_t st[KGV_ITEMS];
   // persistent grid (one resident wave): every thread walks the batch with stride total*KGV_ITEMS, so all
   // SM slots finish within one item of each other whatever n is (no wave quantisation)
@@ -253,31 +263,37 @@ k_schnorr_verify(const uint8_t* __restrict__ pk, const uint8_t* __restrict__ msg
     st[j] = KGV_ST_INVALID;
     if (i >= n) continue;
     if (INDEXED) i = index[i];
-    uint32_t pkw[8], mw[8], sw[16];
-    load_be32<ALIGNED>(pkw, pk + 32 * i);
+    uint32_t pkw[9], mw[8], sw[16];
+    key_words<ALIGNED, ECDSA>(pkw, pk, i);
     load_be32<ALIGNED>(mw, msg + 32 * i);
     load_be32<ALIGNED>(sw, sig + 64 * i);
     load_be32<ALIGNED>(sw + 8, sig + 64 * i + 32);
-    fe x, y, zt, rx;
-    uint8_t s1 = schnorr_phase1(x, y, zt, rx, pkw, mw, sw, tab, gtab, GLoadDev(), kc.rec_of(i, n), kc.comb(n));
+    const KeySrc key = kc.key_of(i, n);
+    fe x, y, rx, d, m;
+    uint8_t s1;
+    if constexpr (ECDSA) s1 = ecdsa_phase1(x, y, rx.v, d.v, m.v, pkw[8], pkw, mw, sw, key);
+    else s1 = schnorr_phase1(x, y, d, rx, pkw, mw, sw, tab, gtab, GLoadDev(), key);
     st[j] = s1;
     if (s1 == KGV_ST_PENDING) {
-      X[j] = x; Y[j] = y; ZT[j] = zt; RX[j] = rx;
+      X[j] = x; Y[j] = y; RX[j] = rx; D[j] = d;
+      if constexpr (ECDSA) { M[j] = m; KR[j] = key.rec; comb = key.comb; }
       pre[j] = acc;
-      fe_mul(acc, acc, zt);
+      batch_mul<ECDSA>(acc, acc, d);
       any = true;
     }
   }
   if (any) {
     fe inv;
-    fe_inv(inv, acc);
+    if constexpr (ECDSA) sc_inv(inv.v, acc.v);
+    else fe_inv(inv, acc);
 #pragma unroll 1
     for (int j = KGV_ITEMS - 1; j >= 0; j--) {
       if (st[j] != KGV_ST_PENDING) continue;
-      fe zi;
-      fe_mul(zi, inv, pre[j]);
-      fe_mul(inv, inv, ZT[j]);
-      st[j] = schnorr_phase2(X[j], Y[j], zi, RX[j]);
+      fe di;  // 1 / D[j]
+      batch_mul<ECDSA>(di, inv, pre[j]);
+      batch_mul<ECDSA>(inv, inv, D[j]);
+      if constexpr (ECDSA) st[j] = ecdsa_phase2(X[j], Y[j], RX[j].v, di.v, M[j].v, tab, gtab, GLoadDev(), KeySrc{KR[j], comb});
+      else st[j] = schnorr_phase2(X[j], Y[j], di, RX[j]);
     }
   }
 #pragma unroll 1
@@ -288,71 +304,26 @@ k_schnorr_verify(const uint8_t* __restrict__ pk, const uint8_t* __restrict__ msg
   }
 }
 
-struct sc_words { uint32_t v[8]; };
-
+template <bool ALIGNED, bool INDEXED>
+__global__ void __launch_bounds__(KGV_BLOCK, KGV_BLOCKS_PER_SM)
+k_schnorr_verify(const uint8_t* __restrict__ pk, const uint8_t* __restrict__ msg, const uint8_t* __restrict__ sig, size_t n_arg,
+                 uint8_t* __restrict__ status, const uint32_t* __restrict__ gtab, const uint32_t* __restrict__ index, const uint32_t* __restrict__ n_dev,
+                 KeyCacheView kc) {
+  verify_body<false, ALIGNED, INDEXED>(pk, msg, sig, n_arg, status, gtab, index, n_dev, kc);
+}
 template <bool ALIGNED, bool INDEXED>
 __global__ void __launch_bounds__(KGV_BLOCK, KGV_BLOCKS_PER_SM)
 k_ecdsa_verify(const uint8_t* __restrict__ pk, const uint8_t* __restrict__ msg, const uint8_t* __restrict__ sig, size_t n_arg,
                uint8_t* __restrict__ status, const uint32_t* __restrict__ gtab, const uint32_t* __restrict__ index, const uint32_t* __restrict__ n_dev,
                KeyCacheView kc) {
-  extern __shared__ uint32_t smem[];
-  const size_t n = (INDEXED && n_dev) ? (size_t)*n_dev : n_arg;
-  const size_t total = (size_t)gridDim.x * KGV_BLOCK;
-  const size_t tid = (size_t)blockIdx.x * KGV_BLOCK + threadIdx.x;
-  SmemTab tab{smem + threadIdx.x};
-  fe QX[KGV_ITEMS], QY[KGV_ITEMS];
-  sc_words R_[KGV_ITEMS], S_[KGV_ITEMS], M_[KGV_ITEMS], pre[KGV_ITEMS];
-  const uint32_t* KR[KGV_ITEMS];
-  uint8_t st[KGV_ITEMS];
-#pragma unroll 1
-  for (size_t base = 0; base < n; base += total * KGV_ITEMS) {
-  uint32_t acc[8] = {1, 0, 0, 0, 0, 0, 0, 0};
-  bool any = false;
-#pragma unroll 1
-  for (int j = 0; j < KGV_ITEMS; j++) {
-    size_t i = base + tid + (size_t)j * total;
-    st[j] = KGV_ST_INVALID;
-    if (i >= n) continue;
-    if (INDEXED) i = index[i];
-    uint32_t pkw[8], mw[8], sw[16];
-    const uint8_t* kp = pk + 33 * i;  // 33-byte stride: never word aligned
-    uint32_t tag = kp[0];
-    load_be32<false>(pkw, kp + 1);
-    load_be32<ALIGNED>(mw, msg + 32 * i);
-    load_be32<ALIGNED>(sw, sig + 64 * i);
-    load_be32<ALIGNED>(sw + 8, sig + 64 * i + 32);
-    fe qx, qy;
-    uint32_t r[8], s[8], m[8];
-    const uint32_t* krec = kc.rec_of(i, n);
-    uint8_t s1 = ecdsa_phase1(qx, qy, r, s, m, tag, pkw, mw, sw, krec, kc.comb(n));
-    st[j] = s1;
-    if (s1 == KGV_ST_PENDING) {
-      QX[j] = qx; QY[j] = qy; KR[j] = krec;
-#pragma unroll
-      for (int w = 0; w < 8; w++) { R_[j].v[w] = r[w]; S_[j].v[w] = s[w]; M_[j].v[w] = m[w]; pre[j].v[w] = acc[w]; }
-      sc_mul(acc, acc, s);
-      any = true;
-    }
-  }
-  if (any) {
-    uint32_t inv[8];
-    sc_inv(inv, acc);
-#pragma unroll 1
-    for (int j = KGV_ITEMS - 1; j >= 0; j--) {
-      if (st[j] != KGV_ST_PENDING) continue;
-      uint32_t sn[8];
-      sc_mul(sn, inv, pre[j].v);
-      sc_mul(inv, inv, S_[j].v);
-      st[j] = ecdsa_phase2(QX[j], QY[j], R_[j].v, sn, M_[j].v, tab, gtab, GLoadDev(), KR[j], kc.comb(n));
-    }
-  }
-#pragma unroll 1
-  for (int j = 0; j < KGV_ITEMS; j++) {
-    size_t i = base + tid + (size_t)j * total;
-    if (i < n) status[INDEXED ? index[i] : i] = st[j];
-  }
-  }
+  verify_body<true, ALIGNED, INDEXED>(pk, msg, sig, n_arg, status, gtab, index, n_dev, kc);
 }
+using VerifyKernel = void (*)(const uint8_t*, const uint8_t*, const uint8_t*, size_t, uint8_t*, const uint32_t*, const uint32_t*, const uint32_t*,
+                              KeyCacheView);
+// every verify instantiation, [ecdsa][indexed][aligned]
+static const VerifyKernel k_verify[2][2][2] = {
+    {{k_schnorr_verify<false, false>, k_schnorr_verify<true, false>}, {k_schnorr_verify<false, true>, k_schnorr_verify<true, true>}},
+    {{k_ecdsa_verify<false, false>, k_ecdsa_verify<true, false>}, {k_ecdsa_verify<false, true>, k_ecdsa_verify<true, true>}}};
 
 // audit/debug: one signature, every traced intermediate written to dbg[stage*16 ..]
 struct DevTrace {
@@ -500,16 +471,11 @@ extern "C" int kgv_create(int device, uint32_t flags, kgv_ctx** out) {
     CK(cudaGetLastError());
     ctx->launches++;
     const int smem = KGV_BLOCK * 128 * (int)sizeof(uint32_t);
-    CK(cudaFuncSetAttribute(k_schnorr_verify<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    CK(cudaFuncSetAttribute(k_schnorr_verify<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    CK(cudaFuncSetAttribute(k_schnorr_verify<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    CK(cudaFuncSetAttribute(k_schnorr_verify<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    CK(cudaFuncSetAttribute(k_ecdsa_verify<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    CK(cudaFuncSetAttribute(k_ecdsa_verify<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    CK(cudaFuncSetAttribute(k_ecdsa_verify<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    CK(cudaFuncSetAttribute(k_ecdsa_verify<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    for (const auto& kind : k_verify)
+      for (const auto& form : kind)
+        for (VerifyKernel k : form) CK(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
     int per_sm = 0, sms = 0;
-    CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_schnorr_verify<true, false>, KGV_BLOCK, smem));
+    CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_verify[0][0][1], KGV_BLOCK, smem));
     CK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device));
     ctx->resident_blocks = per_sm * sms > 0 ? per_sm * sms : 132 * KGV_BLOCKS_PER_SM;  // 132 SMs: H100 SXM
     CK(cudaStreamSynchronize(ctx->stream));
@@ -601,15 +567,15 @@ static int key_cache_launch(kgv_ctx* ctx, const uint8_t* dpk, size_t n, bool ecd
   uint32_t *item_slot = (uint32_t*)(K + o_item), *rec_rep = (uint32_t*)(K + o_rep), *recs = (uint32_t*)(K + o_rec);
   CK(cudaMemsetAsync(K, 0, o_item, st));
   const unsigned gd = (unsigned)((n + 255) / 256);
-  if (ecdsa) k_key_dedup<false, true><<<gd, 256, 0, st>>>(dpk, n, index, n_dev, table, slots - 1, item_slot, rec_rep, n_rec);
-  else if (aligned) k_key_dedup<true, false><<<gd, 256, 0, st>>>(dpk, n, index, n_dev, table, slots - 1, item_slot, rec_rep, n_rec);
-  else k_key_dedup<false, false><<<gd, 256, 0, st>>>(dpk, n, index, n_dev, table, slots - 1, item_slot, rec_rep, n_rec);
+  // (ECDSA keys, at a 33-byte stride, are never word aligned)
+  const auto dedup = ecdsa ? k_key_dedup<false, true> : aligned ? k_key_dedup<true, false> : k_key_dedup<false, false>;
+  dedup<<<gd, 256, 0, st>>>(dpk, n, index, n_dev, table, slots - 1, item_slot, rec_rep, n_rec);
   CK(cudaGetLastError());
   ctx->launches++;
   if (cap) {
     const unsigned gp = (cap + KGV_BLOCK - 1) / KGV_BLOCK;
-    if (ecdsa) k_key_prepare<true><<<gp, KGV_BLOCK, 0, st>>>(dpk, n, n_dev, rec_rep, n_rec, recs);
-    else k_key_prepare<false><<<gp, KGV_BLOCK, 0, st>>>(dpk, n, n_dev, rec_rep, n_rec, recs);
+    const auto prepare = ecdsa ? k_key_prepare<true> : k_key_prepare<false>;
+    prepare<<<gp, KGV_BLOCK, 0, st>>>(dpk, n, n_dev, rec_rep, n_rec, recs);
     CK(cudaGetLastError());
     ctx->launches++;
   }
@@ -618,10 +584,9 @@ static int key_cache_launch(kgv_ctx* ctx, const uint8_t* dpk, size_t n, bool ecd
 }
 
 int kgv_launch_verify(kgv_ctx* ctx, const uint8_t* dpk, const uint8_t* dmsg, const uint8_t* dsig, size_t n, uint8_t* dst, bool ecdsa,
-                      cudaStream_t on, bool use_on, const uint32_t* index, const uint32_t* n_dev) {
+                      cudaStream_t st, const uint32_t* index, const uint32_t* n_dev) {
   if (n == 0) return KGV_OK;
   if (n >= 0x7FFFFFFFu) return fail_arg(ctx, "verify launch of 2^31 or more items");
-  cudaStream_t st = use_on ? on : ctx->stream;
   const int smem = KGV_BLOCK * 128 * (int)sizeof(uint32_t);
   // one resident wave, persistent; items are strided by the grid size, so a batch smaller than the wave still
   // spreads over every SM (one item per thread) instead of packing KGV_ITEMS items into a quarter of the threads
@@ -640,23 +605,7 @@ int kgv_launch_verify(kgv_ctx* ctx, const uint8_t* dpk, const uint8_t* dmsg, con
     auto& lv = ctx->last_verify[ecdsa];
     lv.n = n; lv.blocks = blocks; lv.key_cache = key_cache; lv.stream = st;
   }
-  if (ecdsa) {
-    if (index) {
-      if (aligned) k_ecdsa_verify<true, true><<<blocks, KGV_BLOCK, smem, st>>>(dpk, dmsg, dsig, n, dst, ctx->gtab, index, n_dev, kc);
-      else k_ecdsa_verify<false, true><<<blocks, KGV_BLOCK, smem, st>>>(dpk, dmsg, dsig, n, dst, ctx->gtab, index, n_dev, kc);
-    } else {
-      if (aligned) k_ecdsa_verify<true, false><<<blocks, KGV_BLOCK, smem, st>>>(dpk, dmsg, dsig, n, dst, ctx->gtab, nullptr, nullptr, kc);
-      else k_ecdsa_verify<false, false><<<blocks, KGV_BLOCK, smem, st>>>(dpk, dmsg, dsig, n, dst, ctx->gtab, nullptr, nullptr, kc);
-    }
-  } else {
-    if (index) {
-      if (aligned) k_schnorr_verify<true, true><<<blocks, KGV_BLOCK, smem, st>>>(dpk, dmsg, dsig, n, dst, ctx->gtab, index, n_dev, kc);
-      else k_schnorr_verify<false, true><<<blocks, KGV_BLOCK, smem, st>>>(dpk, dmsg, dsig, n, dst, ctx->gtab, index, n_dev, kc);
-    } else {
-      if (aligned) k_schnorr_verify<true, false><<<blocks, KGV_BLOCK, smem, st>>>(dpk, dmsg, dsig, n, dst, ctx->gtab, nullptr, nullptr, kc);
-      else k_schnorr_verify<false, false><<<blocks, KGV_BLOCK, smem, st>>>(dpk, dmsg, dsig, n, dst, ctx->gtab, nullptr, nullptr, kc);
-    }
-  }
+  k_verify[ecdsa][index != nullptr][aligned]<<<blocks, KGV_BLOCK, smem, st>>>(dpk, dmsg, dsig, n, dst, ctx->gtab, index, n_dev, kc);
   CK(cudaGetLastError());
   ctx->launches++;
   return KGV_OK;
@@ -697,7 +646,7 @@ static int verify_common(kgv_ctx* ctx, const uint8_t* pk, size_t pk_stride, cons
         CK(cudaMemcpyAsync(ctx->d_in + off_sig + 64 * a, sig + 64 * a, 64 * m, cudaMemcpyHostToDevice, ctx->aux_stream));
         CK(cudaEventRecord(ctx->ev_chunk[c], ctx->aux_stream));
         CK(cudaStreamWaitEvent(ctx->stream, ctx->ev_chunk[c], 0));
-        int rc2 = kgv_launch_verify(ctx, dpk + pk_stride * a, dmsg + 32 * a, dsig + 64 * a, m, dst + a, ecdsa);
+        int rc2 = kgv_launch_verify(ctx, dpk + pk_stride * a, dmsg + 32 * a, dsig + 64 * a, m, dst + a, ecdsa, ctx->stream);
         if (rc2) return rc2;
       }
       CK(cudaMemcpyAsync(status, dst, n, cudaMemcpyDeviceToHost, ctx->stream));
@@ -709,7 +658,7 @@ static int verify_common(kgv_ctx* ctx, const uint8_t* pk, size_t pk_stride, cons
     CK(cudaMemcpyAsync(ctx->d_in + off_sig, sig, 64 * n, cudaMemcpyHostToDevice, ctx->stream));
   }
   {
-    int rc = kgv_launch_verify(ctx, dpk, dmsg, dsig, n, dst, ecdsa);
+    int rc = kgv_launch_verify(ctx, dpk, dmsg, dsig, n, dst, ecdsa, ctx->stream);
     if (rc) return rc;
   }
   if (!dev) {

@@ -18,6 +18,7 @@
 #include "kgv_utxo.cuh"
 #include "kgv_context.cuh"
 
+#include <algorithm>
 #include <cstdio>
 #include <vector>
 
@@ -794,54 +795,64 @@ int kgv_scripts_phase(kgv_ctx* ctx, const BatchView& v, size_t nt, size_t ni, co
   size_t ns = totals[0], ne = totals[1];
   if (n_items_out) *n_items_out = ns + ne;
   if (kgv_debug_on()) fprintf(stderr, "[kgv] items: schnorr %zu ecdsa %zu\n", ns, ne);
-  // multi-GPU (kgv_set_sharding): the candidate pairs are split into n_ranks contiguous ranges; this rank verifies one and the
-  // status bytes are exchanged before the scripts are resolved.  per_* = range length (the status arrays are padded to nr * per)
+  // multi-GPU (kgv_set_sharding): the candidate pairs of each kind are split into n_ranks contiguous ranges; this rank verifies one and
+  // the status bytes are exchanged before the scripts are resolved
   int nr = 1, rk = 0;
   if (ctx->shard_comm) nr = kgv_comm_ranks(ctx->shard_comm, &rk);
-  auto per_of = [&](size_t n) { size_t p = (n + nr - 1) / nr; return (p + 255) & ~(size_t)255; };
-  const size_t per_s = nr > 1 ? per_of(ns) : ns, per_e = nr > 1 ? per_of(ne) : ne;
-  const size_t s_lo = nr > 1 ? (rk * per_s < ns ? rk * per_s : ns) : 0, s_hi = nr > 1 ? ((rk + 1) * per_s < ns ? (rk + 1) * per_s : ns) : ns;
-  const size_t e_lo = nr > 1 ? (rk * per_e < ne ? rk * per_e : ne) : 0, e_hi = nr > 1 ? ((rk + 1) * per_e < ne ? (rk + 1) * per_e : ne) : ne;
-  // item arrays live in d_in (pk/sig/msg, status, refs)
-  size_t i_pks = 0, i_sigs = al256(i_pks + ns * 32), i_msgs = al256(i_sigs + ns * 64), i_refs = al256(i_msgs + ns * 32), i_sts = al256(i_refs + ns * sizeof(ItemRef));
-  size_t i_pke = al256(i_sts + (nr > 1 ? nr * per_s : ns)), i_sige = al256(i_pke + ne * 33), i_msge = al256(i_sige + ne * 64), i_refe = al256(i_msge + ne * 32),
-         i_ste = al256(i_refe + ne * sizeof(ItemRef));
-  // signature cache (kgv_set_sigcache; not combined with sharding): digests, miss lists and miss counts of the two item kinds
+  // signature cache (kgv_set_sigcache; not combined with sharding)
   kgv_sigcache* sc = nr == 1 ? ctx->sigcache : nullptr;
-  size_t i_digs = al256(i_ste + (nr > 1 ? nr * per_e : ne) + 64), i_idxs = al256(i_digs + (sc ? ns * 32 : 0)), i_dige = al256(i_idxs + (sc ? ns * 4 : 0)),
-         i_idxe = al256(i_dige + (sc ? ne * 32 : 0)), i_nm = al256(i_idxe + (sc ? ne * 4 : 0));
-  size_t total2 = al256(i_nm + 64);
+  // item arrays of the two kinds ([0] Schnorr, [1] ECDSA) in d_in: pk, sig, msg, refs, status (padded to nr * per), and with the signature
+  // cache the digests, the miss list and the miss count
+  struct ItemKind {
+    size_t n, per, lo, hi;                       // items, range length per rank, this rank's range [lo, hi)
+    size_t pk, sig, msg, ref, st, dig, idx, nm;  // offsets in d_in
+  } kind[2];
+  size_t total2 = 0;
+  for (int e = 0; e < 2; e++) {
+    ItemKind& k = kind[e];
+    k.n = e ? ne : ns;
+    k.per = nr > 1 ? al256((k.n + nr - 1) / nr) : k.n;
+    k.lo = std::min(rk * k.per, k.n);
+    k.hi = std::min((rk + 1) * k.per, k.n);
+    k.pk = total2; k.sig = al256(k.pk + k.n * (e ? 33 : 32)); k.msg = al256(k.sig + k.n * 64); k.ref = al256(k.msg + k.n * 32);
+    k.st = al256(k.ref + k.n * sizeof(ItemRef)); k.dig = al256(k.st + nr * k.per + 64);
+    k.idx = al256(k.dig + (sc ? k.n * 32 : 0)); k.nm = al256(k.idx + (sc ? k.n * 4 : 0));
+    total2 = al256(k.nm + 64);
+  }
   rc = kgv_reserve(ctx, &ctx->d_in, &ctx->d_in_cap, total2);
   if (rc) return rc;
   uint8_t* I = ctx->d_in;
   if (ns + ne) {
-    k_emit_items<<<nblk(ni, 128), 128, 0, st>>>(v, ni, plans, os, oe, I + i_pks, I + i_sigs, (ItemRef*)(I + i_refs), I + i_pke, I + i_sige, (ItemRef*)(I + i_refe));
+    k_emit_items<<<nblk(ni, 128), 128, 0, st>>>(v, ni, plans, os, oe, I + kind[0].pk, I + kind[0].sig, (ItemRef*)(I + kind[0].ref), I + kind[1].pk,
+                                                I + kind[1].sig, (ItemRef*)(I + kind[1].ref));
     CK(cudaGetLastError());
     k_sighash_reused_v<<<nblk(nt, 128), 128, 0, st>>>(v, (uint32_t)nt, dres, reu);
     CK(cudaGetLastError());
     ctx->launches += 2;
     STAGE("emit+reused");
   }
+  // one kind's messages and verdicts on stream s, for this rank's range
+  auto verify_kind = [&](bool ecdsa, cudaStream_t s) -> int {
+    const ItemKind& k = kind[ecdsa];
+    if (k.hi <= k.lo) return KGV_OK;
+    const size_t m = k.hi - k.lo;
+    k_item_msgs<<<nblk(m, 128), 128, 0, s>>>(v, reu, itx, plans, (const ItemRef*)(I + k.ref) + k.lo, m, ecdsa, (uint32_t*)(I + k.msg) + 8 * k.lo);
+    CK(cudaGetLastError());
+    ctx->launches++;
+    STAGE(ecdsa ? "msgs ecdsa" : "msgs schnorr");
+    if (!sc) return kgv_launch_verify(ctx, I + k.pk + (ecdsa ? 33 : 32) * k.lo, I + k.msg + 32 * k.lo, I + k.sig + 64 * k.lo, m, I + k.st + k.lo, ecdsa, s);
+    // hits are answered from the table, only the misses are verified (and remembered)
+    uint32_t *idx = (uint32_t*)(I + k.idx), *nm = (uint32_t*)(I + k.nm);
+    int r = kgv_sigcache_lookup(ctx, sc, I + k.pk, I + k.msg, I + k.sig, k.n, ecdsa, I + k.st, I + k.dig, idx, nm, s);
+    if (!r) r = kgv_launch_verify(ctx, I + k.pk, I + k.msg, I + k.sig, k.n, I + k.st, ecdsa, s, idx, nm);
+    if (!r) r = kgv_sigcache_insert(ctx, sc, I + k.st, I + k.dig, idx, nm, k.n, s);
+    return r;
+  };
   if (ns && ne) CK(cudaEventRecord(ctx->ev_fork, st));  // fork point: everything both item kinds depend on is queued
   if (ns) {
-    if (s_hi > s_lo) {
-      k_item_msgs<<<nblk(s_hi - s_lo, 128), 128, 0, st>>>(v, reu, itx, plans, (const ItemRef*)(I + i_refs) + s_lo, s_hi - s_lo, false, (uint32_t*)(I + i_msgs) + 8 * s_lo);
-      CK(cudaGetLastError());
-      ctx->launches++;
-      STAGE("msgs schnorr");
-      if (sc) {  // hits are answered from the table, only the misses are verified (and remembered)
-        rc = kgv_sigcache_lookup(ctx, sc, I + i_pks, I + i_msgs, I + i_sigs, ns, false, I + i_sts, I + i_digs, (uint32_t*)(I + i_idxs), (uint32_t*)(I + i_nm), st);
-        if (rc) return rc;
-        rc = kgv_launch_verify(ctx, I + i_pks, I + i_msgs, I + i_sigs, ns, I + i_sts, false, nullptr, false, (const uint32_t*)(I + i_idxs), (const uint32_t*)(I + i_nm));
-        if (rc) return rc;
-        rc = kgv_sigcache_insert(ctx, sc, I + i_sts, I + i_digs, (const uint32_t*)(I + i_idxs), (const uint32_t*)(I + i_nm), ns, st);
-        if (rc) return rc;
-      } else {
-        rc = kgv_launch_verify(ctx, I + i_pks + 32 * s_lo, I + i_msgs + 32 * s_lo, I + i_sigs + 64 * s_lo, s_hi - s_lo, I + i_sts + s_lo, false);
-        if (rc) return rc;
-      }
-      STAGE("verify schnorr");
-    }
+    rc = verify_kind(false, st);
+    if (rc) return rc;
+    STAGE("verify schnorr");
   }
   if (ne) {
     // with both kinds present the ECDSA items run on the side stream so the two (often sub-wave) verify
@@ -849,23 +860,8 @@ int kgv_scripts_phase(kgv_ctx* ctx, const BatchView& v, size_t nt, size_t ni, co
     const bool fork = ns != 0 && !kgv_debug_on();
     cudaStream_t se = fork ? ctx->aux_stream : st;
     if (fork) CK(cudaStreamWaitEvent(se, ctx->ev_fork, 0));
-    if (e_hi > e_lo) {
-      k_item_msgs<<<nblk(e_hi - e_lo, 128), 128, 0, se>>>(v, reu, itx, plans, (const ItemRef*)(I + i_refe) + e_lo, e_hi - e_lo, true, (uint32_t*)(I + i_msge) + 8 * e_lo);
-      CK(cudaGetLastError());
-      ctx->launches++;
-      STAGE("msgs ecdsa");
-      if (sc) {
-        rc = kgv_sigcache_lookup(ctx, sc, I + i_pke, I + i_msge, I + i_sige, ne, true, I + i_ste, I + i_dige, (uint32_t*)(I + i_idxe), (uint32_t*)(I + i_nm) + 1, se);
-        if (rc) return rc;
-        rc = kgv_launch_verify(ctx, I + i_pke, I + i_msge, I + i_sige, ne, I + i_ste, true, se, true, (const uint32_t*)(I + i_idxe), (const uint32_t*)(I + i_nm) + 1);
-        if (rc) return rc;
-        rc = kgv_sigcache_insert(ctx, sc, I + i_ste, I + i_dige, (const uint32_t*)(I + i_idxe), (const uint32_t*)(I + i_nm) + 1, ne, se);
-        if (rc) return rc;
-      } else {
-        rc = kgv_launch_verify(ctx, I + i_pke + 33 * e_lo, I + i_msge + 32 * e_lo, I + i_sige + 64 * e_lo, e_hi - e_lo, I + i_ste + e_lo, true, se, true);
-        if (rc) return rc;
-      }
-    }
+    rc = verify_kind(true, se);
+    if (rc) return rc;
     if (fork) {
       CK(cudaEventRecord(ctx->ev_join, se));
       CK(cudaStreamWaitEvent(st, ctx->ev_join, 0));
@@ -873,11 +869,11 @@ int kgv_scripts_phase(kgv_ctx* ctx, const BatchView& v, size_t nt, size_t ni, co
     STAGE("verify ecdsa");
   }
   if (nr > 1) {
-    if (ns) { rc = kgv_comm_exchange_slices(ctx, ctx->shard_comm, I + i_sts, per_s); if (rc) return rc; }
-    if (ne) { rc = kgv_comm_exchange_slices(ctx, ctx->shard_comm, I + i_ste, per_e); if (rc) return rc; }
+    for (const ItemKind& k : kind)
+      if (k.n) { rc = kgv_comm_exchange_slices(ctx, ctx->shard_comm, I + k.st, k.per); if (rc) return rc; }
     STAGE("verdict exchange");
   }
-  k_resolve<<<nblk(ni, 128), 128, 0, st>>>(v, ni, itx, dres, plans, I + i_sts, I + i_ste, ierr);
+  k_resolve<<<nblk(ni, 128), 128, 0, st>>>(v, ni, itx, dres, plans, I + kind[0].st, I + kind[1].st, ierr);
   CK(cudaGetLastError());
   STAGE("resolve");
   k_tx_finalize<<<nblk(nt, 128), 128, 0, st>>>(v, (uint32_t)nt, ierr, dres);

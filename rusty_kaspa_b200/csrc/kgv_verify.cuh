@@ -135,15 +135,40 @@ KGV_HD void key_comb_build(uint32_t* rec, uint32_t tag, const uint32_t* pkw) {
   rec[KGV_KC_STATUS] = st;
 }
 
+// Where the key part of a verification comes from: the key's comb record (comb), its plain record, or none (rec == nullptr: the key is
+// lifted and its odd-multiples table built per signature).
+struct KeySrc {
+  const uint32_t* rec;
+  bool comb;
+};
+// a prepared key's verdict: false when the key does not parse
+KGV_HD bool key_rec_valid(const KeySrc& key) { return key.rec[key.comb ? KGV_KC_STATUS : KGV_KR_STATUS] == KGV_ST_VALID; }
+// R = kP*P + kG*G and zt, the true Z of R (unset when R is infinity).  px, py: the key, read on the inline path only.
+template <class Tab, class GLoad, class Trace = NoTrace>
+KGV_HD void ecmult_key(gej& R, fe& zt, const KeySrc& key, const fe& px, const fe& py, const uint32_t* kP, const uint32_t* kG, Tab& tab,
+                       const uint32_t* gtab, GLoad gload, Trace trace = Trace()) {
+  fe zs;
+  if (key.comb) {
+    ecmult_comb(R, kP, kG, key.rec, tab, gtab, gload);
+  } else {
+    if (key.rec) key_rec_load(tab, zs, key.rec);
+    else build_odd_table(tab, zs, px, py);
+    ecmult_double(R, zs, kP, kG, tab, gtab, gload, trace);
+  }
+  if (R.inf) return;
+  if (key.comb) zt = R.z;  // comb entries are true affine
+  else fe_mul(zt, R.z, zs);
+}
+
 // BIP-340 verification, phase 1: everything up to the projective result R = s*G - e*P.
-// pkw/mw: 8 big-endian words, sigw: 16 big-endian words (r || s).  krec: the key's record, or nullptr (the key part is computed here);
-// comb: krec is a comb record.  Returns a final verdict, or KGV_ST_PENDING with (X, Y, zt = true Z, rx) filled in.
+// pkw/mw: 8 big-endian words, sigw: 16 big-endian words (r || s).  Returns a final verdict, or KGV_ST_PENDING with (X, Y, zt = true Z, rx)
+// filled in.
 template <class Tab, class GLoad, class Trace = NoTrace>
 KGV_HD uint8_t schnorr_phase1(fe& X, fe& Y, fe& zt, fe& rx, const uint32_t* pkw, const uint32_t* mw, const uint32_t* sigw, Tab& tab,
-                              const uint32_t* gtab, GLoad gload, const uint32_t* krec, bool comb, Trace trace = Trace()) {
+                              const uint32_t* gtab, GLoad gload, const KeySrc& key, Trace trace = Trace()) {
   fe px, py;
-  if (krec) {
-    if (krec[comb ? KGV_KC_STATUS : KGV_KR_STATUS] != KGV_ST_VALID) return KGV_ST_PK_PARSE;
+  if (key.rec) {
+    if (!key_rec_valid(key)) return KGV_ST_PK_PARSE;
   } else {
     limbs_from_be_words(px.v, pkw);
     if (!fe_words_lt_p(px.v)) return KGV_ST_PK_PARSE;      // x >= p
@@ -163,21 +188,12 @@ KGV_HD uint8_t schnorr_phase1(fe& X, fe& Y, fe& zt, fe& rx, const uint32_t* pkw,
   sc_neg(k, e);                                           // R = s*G - e*P
   trace(3, e, 8); trace(4, k, 8); trace(5, s, 8);
   gej R;
-  fe zs;
-  if (comb) {
-    ecmult_comb(R, k, s, krec, tab, gtab, gload);
-  } else {
-    if (krec) key_rec_load(tab, zs, krec);
-    else build_odd_table(tab, zs, px, py);
-    ecmult_double(R, zs, k, s, tab, gtab, gload, trace);
-  }
+  ecmult_key(R, zt, key, px, py, k, s, tab, gtab, gload, trace);
   { uint32_t f[1] = {R.inf}; trace(18, f, 1); }
   if (R.inf) return KGV_ST_INVALID;
   trace(19, R.x.v, 8); trace(20, R.y.v, 8); trace(21, R.z.v, 8);
   X = R.x;
   Y = R.y;
-  if (comb) zt = R.z;
-  else fe_mul(zt, R.z, zs);
   return KGV_ST_PENDING;
 }
 // phase 2: zi = 1/zt. Valid iff y(R) is even and x(R) == r.
@@ -200,21 +216,21 @@ KGV_HD uint8_t schnorr_phase2(const fe& X, const fe& Y, const fe& zi, const fe& 
 // single-signature form (audit kernel, host unit tests)
 template <class Tab, class GLoad, class Trace = NoTrace>
 KGV_HD uint8_t schnorr_verify_core(const uint32_t* pkw, const uint32_t* mw, const uint32_t* sigw, Tab& tab, const uint32_t* gtab,
-                                   GLoad gload, Trace trace = Trace(), const uint32_t* krec = nullptr, bool comb = false) {
+                                   GLoad gload, Trace trace = Trace(), KeySrc key = KeySrc{nullptr, false}) {
   fe X, Y, zt, rx, zi;
-  uint8_t st = schnorr_phase1(X, Y, zt, rx, pkw, mw, sigw, tab, gtab, gload, krec, comb, trace);
+  uint8_t st = schnorr_phase1(X, Y, zt, rx, pkw, mw, sigw, tab, gtab, gload, key, trace);
   if (st != KGV_ST_PENDING) return st;
   fe_inv(zi, zt);
   return schnorr_phase2(X, Y, zi, rx, trace);
 }
 
 // ECDSA verification with libsecp256k1 semantics, phase 1: parsing and range checks.
-// pkw: 8 big-endian words of x, tag = first key byte, krec: the key's record or nullptr (comb: a comb record).  Returns a final verdict or
-// KGV_ST_PENDING with the key (qx,qy; unset with a record), r, s (to be inverted, possibly batched) and the reduced message m.
+// pkw: 8 big-endian words of x, tag = first key byte.  Returns a final verdict or KGV_ST_PENDING with the key (qx,qy; unset with a record),
+// r, s (to be inverted, possibly batched) and the reduced message m.
 KGV_HD uint8_t ecdsa_phase1(fe& qx, fe& qy, uint32_t* r, uint32_t* s, uint32_t* m, uint32_t tag, const uint32_t* pkw, const uint32_t* mw,
-                            const uint32_t* sigw, const uint32_t* krec, bool comb) {
-  if (krec) {
-    if (krec[comb ? KGV_KC_STATUS : KGV_KR_STATUS] != KGV_ST_VALID) return KGV_ST_PK_PARSE;
+                            const uint32_t* sigw, const KeySrc& key) {
+  if (key.rec) {
+    if (!key_rec_valid(key)) return KGV_ST_PK_PARSE;
   } else if (!key_lift(qx, qy, tag, pkw)) {
     return KGV_ST_PK_PARSE;
   }
@@ -230,24 +246,16 @@ KGV_HD uint8_t ecdsa_phase1(fe& qx, fe& qy, uint32_t* r, uint32_t* s, uint32_t* 
 // phase 2: sn = s^-1 mod n.  R = (m/s)*G + (r/s)*Q, valid iff x(R) mod n == r.
 template <class Tab, class GLoad>
 KGV_HD uint8_t ecdsa_phase2(const fe& qx, const fe& qy, const uint32_t* r, const uint32_t* sn, const uint32_t* m, Tab& tab, const uint32_t* gtab,
-                            GLoad gload, const uint32_t* krec, bool comb) {
+                            GLoad gload, const KeySrc& key) {
   uint32_t u1[8], u2[8];
   sc_mul(u1, sn, m);
   sc_mul(u2, sn, r);
   gej R;
-  fe zs, zt;
-  if (comb) {
-    ecmult_comb(R, u2, u1, krec, tab, gtab, gload);
-  } else {
-    if (krec) key_rec_load(tab, zs, krec);
-    else build_odd_table(tab, zs, qx, qy);
-    ecmult_double(R, zs, u2, u1, tab, gtab, gload);
-  }
+  fe zt;
+  ecmult_key(R, zt, key, qx, qy, u2, u1, tab, gtab, gload);
   if (R.inf) return KGV_ST_INVALID;
   // x(R) mod n == r  <=>  X == r*Zt^2  or  (r + n < p and X == (r+n)*Zt^2)
   fe zt2, t, rf;
-  if (comb) zt = R.z;
-  else fe_mul(zt, R.z, zs);
   fe_sqr(zt2, zt);
 #pragma unroll
   for (int i = 0; i < 8; i++) rf.v[i] = r[i];
@@ -264,13 +272,13 @@ KGV_HD uint8_t ecdsa_phase2(const fe& qx, const fe& qy, const uint32_t* r, const
 }
 template <class Tab, class GLoad>
 KGV_HD uint8_t ecdsa_verify_core(uint32_t tag, const uint32_t* pkw, const uint32_t* mw, const uint32_t* sigw, Tab& tab,
-                                 const uint32_t* gtab, GLoad gload, const uint32_t* krec = nullptr, bool comb = false) {
+                                 const uint32_t* gtab, GLoad gload, KeySrc key = KeySrc{nullptr, false}) {
   fe qx, qy;
   uint32_t r[8], s[8], m[8], sn[8];
-  uint8_t st = ecdsa_phase1(qx, qy, r, s, m, tag, pkw, mw, sigw, krec, comb);
+  uint8_t st = ecdsa_phase1(qx, qy, r, s, m, tag, pkw, mw, sigw, key);
   if (st != KGV_ST_PENDING) return st;
   sc_inv(sn, s);
-  return ecdsa_phase2(qx, qy, r, sn, m, tab, gtab, gload, krec, comb);
+  return ecdsa_phase2(qx, qy, r, sn, m, tab, gtab, gload, key);
 }
 
 // One entry of the generator tables: v * B for v in [1, 65535], B affine; result affine.
