@@ -168,6 +168,7 @@ int kgv_sighash(kgv_ctx* ctx, const kgv_tx_batch* batch, const kgv_sighash_item*
 #define KGV_TX_NEEDS_HOST_VM 11         /* an input is not one of the GPU fast-path script classes: the host
                                            script engine must decide this transaction (all context checks passed) */
 #define KGV_TX_SKIPPED_COINBASE 12      /* coinbase transactions are skipped (utxo_validation.rs:273) */
+#define KGV_TX_FEERATE_TOO_LOW 13       /* FeerateTooLow (kgv_validate_mempool_txs only) */
 /* script errors = TxScriptError variants the standard classes can produce (crypto/txscript/errors) */
 #define KGV_SCRIPT_OK 0
 #define KGV_SCRIPT_EVAL_FALSE 1
@@ -301,6 +302,32 @@ int kgv_validate_txs(kgv_ctx* ctx, kgv_utxo_table* t, const kgv_tx_batch* batch,
  * accept[i] != 0: spent outpoints are erased, outputs inserted with block_daa_score = pov_daa_score and
  * is_coinbase of the tx (tx ids are computed on the device). */
 int kgv_utxo_apply_accepted(kgv_ctx* ctx, kgv_utxo_table* t, const kgv_tx_batch* batch, const uint8_t* accept, uint64_t pov_daa_score);
+
+/* validate_mempool_transaction_in_utxo_context (consensus/src/pipeline/virtual_processor/utxo_validation.rs:341-397) for every tx of a
+ * batch against the virtual UTXO view `virtual_view` (a table or a composed view):
+ *   populate   an input keeps the entry the caller supplies (batch->entries[i] with pad_[0] == 0: e.g. an in-mempool parent's output, whose
+ *              block_daa_score is UNACCEPTED_DAA_SCORE = u64::MAX); only the inputs without one are looked up, and every input is tried
+ *              (:348-358).  batch->entries may be NULL: everything is looked up.
+ *   rules      missing outpoints -> storage mass (MassIncomputable) -> coinbase maturity -> input amounts -> spend -> sequence lock ->
+ *              feerate -> scripts.  The committed mass is not checked (SkipMassCheck, :392); the computed one is returned.
+ *   feerate    with args[i].feerate_threshold not NaN: fee as f64 / max(storage mass, args[i].non_contextual_mass) as f64 <= threshold is
+ *              KGV_TX_FEERATE_TOO_LOW (tx_validation_in_utxo_context.rs:63-73).  It comes before the scripts, so such a transaction's
+ *              signatures are never verified nor cached.  A threshold whose divisor is 0 makes the call fail with KGV_ERR_ARG (the reference
+ *              asserts it is not zero).  args == NULL: no thresholds.
+ * Non-standard scripts are decided inside the call by the host script engine, as in kgv_validate_txs; coinbases give KGV_TX_SKIPPED_COINBASE.
+ * results: n_txs records (fee set once the amounts pass); storage_mass: n_txs values (0 when the mass was not reached).
+ * entries_out (n_inputs records, may be NULL): every input's final entry - the caller's, the one found, or absent-marked (pad_[0] = 1) when
+ * neither - with script_off into scripts_out (scripts_cap bytes).  *scripts_used (may be NULL) receives the bytes those scripts take; when
+ * entries_out is given and they exceed scripts_cap the call returns KGV_ERR_NOMEM before any signature is verified, with *scripts_used set
+ * (script_off is 32 bits: scripts above 4 GiB in all give KGV_ERR_ARG when entries_out is given).  The entries are written before the script
+ * phase runs.  Every data pointer (batch, args, outputs) host or every one device; a mix gives KGV_ERR_ARG. */
+typedef struct {
+  double feerate_threshold;     /* NaN: None */
+  uint64_t non_contextual_mass; /* max(compute mass, transient mass) the caller computed in isolation */
+} kgv_mempool_tx_args;          /* 16 bytes */
+int kgv_validate_mempool_txs(kgv_ctx* ctx, kgv_utxo_table* virtual_view, const kgv_tx_batch* batch, uint64_t virtual_daa_score, const kgv_params* params,
+                             const kgv_mempool_tx_args* args, kgv_tx_result* results, uint64_t* storage_mass, kgv_utxo_entry* entries_out,
+                             uint8_t* scripts_out, size_t scripts_cap, size_t* scripts_used);
 
 /* ------------------------------------------------------------------------------------------------
  * SigCache: Cache<SigCacheKey, bool> (crypto/txscript/src/caches.rs:14-55; consulted at crypto/txscript/src/lib.rs:589-603, 624-638;

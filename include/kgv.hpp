@@ -507,10 +507,50 @@ class TransactionValidator {
     c_.check(kgv_batch_prefetch(c_.get(), &v));
   }
   // validate_mempool_transactions_in_parallel (consensus/src/pipeline/virtual_processor/processor.rs:853-878): same kernels, but every
-  // outcome is returned (Vec<TxResult<()>>); `fee` feeds the host-side feerate check (tx_validation_in_utxo_context.rs:63-73)
+  // outcome is returned (Vec<TxResult<()>>); `fee` feeds the host-side feerate check (tx_validation_in_utxo_context.rs:63-73).
+  // validate_mempool_transactions_in_utxo_context is the mempool's own rule set: caller entries first, mass computed, feerate threshold.
   std::vector<kgv_tx_result> validate_mempool_transactions_in_parallel(UtxoSet& virtual_utxo_view, const TxBatch& b, uint64_t virtual_daa_score,
                                                                      TxValidationFlags flags = TxValidationFlags::Full) {
     return validate_transactions_in_parallel(virtual_utxo_view, b, virtual_daa_score, flags);
+  }
+  // validate_mempool_transaction_in_utxo_context (utxo_validation.rs:341-397) for a batch (kgv_validate_mempool_txs).  The entries the batch
+  // was pushed with win (an in-mempool parent's output: block_daa_score = u64::MAX); nullptr elements, or a batch pushed without entries, are
+  // looked up in the view.  args: empty (no feerate thresholds) or one per transaction.  entries[i] = input i's final entry, or nothing.
+  struct MempoolValidation {
+    std::vector<kgv_tx_result> results;
+    std::vector<uint64_t> storage_mass;
+    std::vector<std::pair<bool, UtxoEntry>> entries;  // (found, entry) per input of the batch
+  };
+  MempoolValidation validate_mempool_transactions_in_utxo_context(UtxoSet& virtual_utxo_view, const TxBatch& b, uint64_t virtual_daa_score,
+                                                                  const std::vector<kgv_mempool_tx_args>& args = {}) {
+    if (!args.empty() && args.size() != b.len()) throw Error(KGV_ERR_ARG, "kgv: one kgv_mempool_tx_args per transaction");
+    MempoolValidation out;
+    out.results.resize(b.len());
+    out.storage_mass.resize(b.len());
+    std::vector<kgv_utxo_entry> ent(b.n_inputs() + 1);
+    kgv_tx_batch v = b.view(true);
+    size_t used = 0;
+    std::vector<uint8_t> scripts(v.n_bytes + 128 * b.n_inputs() + 8);  // caller scripts come from the arena; a looked-up one usually fits 128 bytes
+    auto call = [&] {
+      return kgv_validate_mempool_txs(c_.get(), virtual_utxo_view.get(), &v, virtual_daa_score, &p_, args.empty() ? nullptr : args.data(), out.results.data(),
+                                      out.storage_mass.data(), ent.data(), scripts.data(), scripts.size(), &used);
+    };
+    int rc = call();
+    if (rc == KGV_ERR_NOMEM && used > scripts.size()) {  // reported before any signature is verified
+      scripts.resize(used);
+      rc = call();
+    }
+    c_.check(rc);
+    out.entries.resize(b.n_inputs());
+    for (size_t i = 0; i < b.n_inputs(); i++) {
+      if (ent[i].pad_[0]) continue;
+      UtxoEntry& e = out.entries[i].second;
+      out.entries[i].first = true;
+      e.amount = ent[i].amount; e.block_daa_score = ent[i].block_daa_score; e.is_coinbase = ent[i].is_coinbase != 0;
+      e.script_public_key.version = ent[i].spk_version;
+      e.script_public_key.script.assign(scripts.begin() + ent[i].script_off, scripts.begin() + ent[i].script_off + ent[i].script_len);
+    }
+    return out;
   }
   std::pair<std::vector<kgv_tx_result>, MuHash> validate_transactions_with_muhash_in_parallel(UtxoSet& utxo_view, const TxBatch& b, uint64_t pov_daa_score,
                                                                                             TxValidationFlags flags = TxValidationFlags::Full) {

@@ -197,6 +197,69 @@ __global__ void k_tx_context(BatchView b, uint32_t n_txs, uint64_t pov, uint32_t
   res[ti] = tx_context_rules(b, ti, pov, flags, prm, tx_is_coinbase(b.txs[ti]));
 }
 
+// populate_mempool_transaction_in_utxo_context (utxo_validation.rs:341-363): an entry the caller supplies (given[i].pad_[0] == 0; its script in
+// the batch arena) is kept, every other input is looked up.  len[i] = script bytes of the final entry (0 when absent); *total = their sum in
+// 64 bits (the 32-bit offsets of the scan are only used when it fits).  Launched with whole warps: every lane reaches the reduction.
+__global__ void k_populate_mempool(TableView t, const kgv_input* __restrict__ inputs, const kgv_utxo_entry* __restrict__ given, const uint8_t* __restrict__ bytes,
+                                   size_t n, DevEntry* __restrict__ out, uint32_t* __restrict__ len, unsigned long long* __restrict__ total) {
+  size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  unsigned long long l = 0;
+  if (i < n) {
+    DevEntry d;
+    if (given && !given[i].pad_[0]) {
+      const kgv_utxo_entry e = given[i];
+      d.amount = e.amount; d.block_daa_score = e.block_daa_score; d.script = bytes + e.script_off; d.script_len = e.script_len;
+      d.spk_version = e.spk_version; d.is_coinbase = e.is_coinbase; d.found = 1;
+    } else {
+      uint32_t k[9];
+      input_key(k, inputs[i]);
+      SlotHead h;
+      UtxoSlot* s = table_find(t, k, h);
+      if (s) head_to_entry(d, t, s, h);
+      else entry_absent(d);
+    }
+    out[i] = d;
+    l = d.found ? d.script_len : 0;
+    len[i] = (uint32_t)l;
+  }
+#pragma unroll
+  for (int o = 16; o; o >>= 1) l += __shfl_down_sync(0xFFFFFFFFu, l, o);
+  if ((threadIdx.x & 31) == 0 && l) atomicAdd(total, l);
+}
+
+// the context rules of a mempool batch (mempool_context_rules); *bad counts thresholds with a zero divisor
+__global__ void k_tx_mempool_context(BatchView b, uint32_t n_txs, uint64_t pov, kgv_params prm, const kgv_mempool_tx_args* __restrict__ args,
+                                     kgv_tx_result* __restrict__ res, uint64_t* __restrict__ mass, unsigned long long* __restrict__ bad) {
+  uint32_t ti = blockIdx.x * blockDim.x + threadIdx.x;
+  if (ti >= n_txs) return;
+  double thr = __longlong_as_double(0x7FF8000000000000ll);  // NaN: no threshold
+  uint64_t nc = 0;
+  if (args) { thr = args[ti].feerate_threshold; nc = args[ti].non_contextual_mass; }
+  uint64_t m;
+  bool bad_thr;
+  res[ti] = mempool_context_rules(b, ti, pov, prm, thr, nc, m, bad_thr);
+  mass[ti] = m;
+  if (bad_thr) atomicAdd(bad, 1ull);
+}
+
+// every input's final entry, its script at off[i] (exclusive prefix of the lengths) of `scripts`; absent: zero, pad_[0] = 1
+__global__ void k_mempool_entries_out(const DevEntry* __restrict__ dent, const uint32_t* __restrict__ off, size_t n, kgv_utxo_entry* __restrict__ out,
+                                      uint8_t* __restrict__ scripts) {
+  size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const DevEntry d = dent[i];
+  kgv_utxo_entry e;
+  memset(&e, 0, sizeof e);
+  e.script_off = off[i];
+  if (d.found) {
+    e.amount = d.amount; e.block_daa_score = d.block_daa_score; e.script_len = d.script_len; e.spk_version = d.spk_version; e.is_coinbase = d.is_coinbase;
+    for (uint32_t k = 0; k < d.script_len; k++) scripts[e.script_off + k] = d.script[k];
+  } else {
+    e.pad_[0] = 1;
+  }
+  out[i] = e;
+}
+
 // plan: one thread per input. counts[0][i] = Schnorr items, counts[1][i] = ECDSA items (0 when the tx already failed).
 __global__ void k_plan(BatchView b, size_t n_inputs, const uint32_t* __restrict__ input_tx, const kgv_tx_result* __restrict__ res,
                        InputPlan* __restrict__ plans, uint32_t* __restrict__ cnt_s, uint32_t* __restrict__ cnt_e) {
@@ -995,6 +1058,26 @@ __global__ void k_count_status(const kgv_tx_result* __restrict__ res, uint32_t n
   if ((threadIdx.x & 31) == 0 && m) atomicAdd(out, (unsigned long long)__popc(m));
 }
 
+// The script phase of a validation call against a table (kgv_validate_txs, kgv_validate_mempool_txs), then the host script engine for what it
+// left undecided: utxo_validation.rs:282-309 accepts ANY transaction whose scripts execute successfully, so a non-standard spend must not leave
+// the call undecided, and only the library can read the entries it was populated with.
+static int scripts_with_host_vm(kgv_ctx* ctx, kgv_utxo_table* table, const kgv_tx_batch* batch, const kgv_dev_batch& d, const BatchView& v, const uint32_t* itx,
+                                kgv_tx_result* dres) {
+  const size_t nt = d.n_txs;
+  int rc = kgv_scripts_phase(ctx, v, nt, d.n_inputs, itx, dres, nullptr);
+  if (rc) return rc;
+  cudaStream_t st = ctx->stream;
+  unsigned long long* cnt = table->counters + 4;
+  unsigned long long n_vm = 0;
+  CK(cudaMemsetAsync(cnt, 0, 8, st));
+  k_count_status<<<nblk(nt, 256), 256, 0, st>>>(dres, (uint32_t)nt, KGV_TX_NEEDS_HOST_VM, cnt);
+  CK(cudaGetLastError());
+  ctx->launches++;
+  CK(cudaMemcpyAsync(&n_vm, cnt, 8, cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  return n_vm ? kgv_host_vm_resolve(ctx, batch, d, v.entries, dres) : KGV_OK;
+}
+
 // shared core of kgv_validate_populated / kgv_validate_txs
 static int validate_core(kgv_ctx* ctx, kgv_utxo_table* table, const kgv_tx_batch* batch, uint64_t pov, uint32_t flags, const kgv_params* prm,
                          kgv_tx_result* results) {
@@ -1032,24 +1115,8 @@ static int validate_core(kgv_ctx* ctx, kgv_utxo_table* table, const kgv_tx_batch
   ctx->launches++;
   STAGE("tx_context");
   if (flags != KGV_FLAGS_SKIP_SCRIPT_CHECKS && ni) {
-    rc = kgv_scripts_phase(ctx, v, nt, ni, itx, dres, nullptr);
+    rc = table ? scripts_with_host_vm(ctx, table, batch, d, v, itx, dres) : kgv_scripts_phase(ctx, v, nt, ni, itx, dres, nullptr);
     if (rc) return rc;
-    if (table) {
-      // utxo_validation.rs:282-309 accepts ANY transaction whose scripts execute successfully: a non-standard spend must not
-      // leave this call undecided, and only the library can read the entries it was populated with
-      unsigned long long* cnt = table->counters + 4;
-      unsigned long long n_vm = 0;
-      CK(cudaMemsetAsync(cnt, 0, 8, st));
-      k_count_status<<<nblk(nt, 256), 256, 0, st>>>(dres, (uint32_t)nt, KGV_TX_NEEDS_HOST_VM, cnt);
-      CK(cudaGetLastError());
-      ctx->launches++;
-      CK(cudaMemcpyAsync(&n_vm, cnt, 8, cudaMemcpyDeviceToHost, st));
-      CK(cudaStreamSynchronize(st));
-      if (n_vm) {
-        rc = kgv_host_vm_resolve(ctx, batch, d, dent, dres);
-        if (rc) return rc;
-      }
-    }
   }
   if (kgv_ptr_is_device(results)) {
     CK(cudaMemcpyAsync(results, dres, nt * sizeof(kgv_tx_result), cudaMemcpyDeviceToDevice, st));
@@ -1071,6 +1138,104 @@ extern "C" int kgv_validate_txs(kgv_ctx* ctx, kgv_utxo_table* t, const kgv_tx_ba
   if (!ctx || !t) return KGV_ERR_ARG;
   std::lock_guard<std::recursive_mutex> g(ctx->mu);
   return validate_core(ctx, t, batch, pov_daa_score, flags, params, results);
+}
+
+// validate_mempool_transaction_in_utxo_context for a batch (utxo_validation.rs:341-397): populate (caller's entries first), the mempool rule
+// order with the storage mass computed and the feerate threshold (k_tx_mempool_context), the final entries written out, then the script phase
+// of kgv_validate_txs.  The entries go out BEFORE the script phase: a caller entry's script points into the staged batch, which the host script
+// engine's own calls may restage.  One synchronisation before the script phase reads the script bytes and the zero-divisor count.
+extern "C" int kgv_validate_mempool_txs(kgv_ctx* ctx, kgv_utxo_table* t, const kgv_tx_batch* batch, uint64_t virtual_daa_score, const kgv_params* prm,
+                                        const kgv_mempool_tx_args* args, kgv_tx_result* results, uint64_t* storage_mass, kgv_utxo_entry* entries_out,
+                                        uint8_t* scripts_out, size_t scripts_cap, size_t* scripts_used) {
+  if (!ctx || !t) return KGV_ERR_ARG;
+  std::lock_guard<std::recursive_mutex> g(ctx->mu);
+  if (scripts_used) *scripts_used = 0;
+  if (!batch || !prm || (batch->n_txs && (!results || !storage_mass)) || (entries_out && scripts_cap && !scripts_out)) { ctx->err = "null argument"; return KGV_ERR_ARG; }
+  if (batch->n_txs == 0) return KGV_OK;
+  CK(cudaSetDevice(ctx->device));
+  const bool dev = kgv_ptr_is_device(results) != 0;
+  for (const void* p : {(const void*)batch->txs, (const void*)args, (const void*)storage_mass, (const void*)entries_out, (const void*)(scripts_cap ? scripts_out : nullptr)})
+    if (p && (kgv_ptr_is_device(p) != 0) != dev) { ctx->err = "kgv_validate_mempool_txs: the batch, args and outputs must all be host or all be device pointers"; return KGV_ERR_ARG; }
+  kgv_dev_batch d;
+  int rc = kgv_batch_to_device(ctx, batch, &d, false);
+  if (rc) return rc;
+  const size_t nt = d.n_txs, ni = d.n_inputs;
+  // d_work: populated entries, input -> tx, verdicts, masses, script lengths and their offsets, the uploaded thresholds,
+  // counters [script bytes (64-bit), zero divisors, the scan's 32-bit total]
+  size_t o_ent = 0;
+  size_t o_itx = al256(o_ent + ni * sizeof(DevEntry));
+  size_t o_res = al256(o_itx + ni * 4);
+  size_t o_mass = al256(o_res + nt * sizeof(kgv_tx_result));
+  size_t o_len = al256(o_mass + nt * 8);
+  size_t o_off = al256(o_len + ni * 4);
+  size_t o_args = al256(o_off + ni * 4);
+  size_t o_cnt = al256(o_args + (args ? nt * sizeof(kgv_mempool_tx_args) : 0));
+  rc = kgv_reserve(ctx, &ctx->d_work, &ctx->d_work_cap, al256(o_cnt + 32));
+  if (rc) return rc;
+  uint8_t* S = ctx->d_work;
+  DevEntry* dent = (DevEntry*)(S + o_ent);
+  uint32_t *itx = (uint32_t*)(S + o_itx), *len = (uint32_t*)(S + o_len), *off = (uint32_t*)(S + o_off);
+  unsigned long long* cnt = (unsigned long long*)(S + o_cnt);
+  kgv_tx_result* dres = (kgv_tx_result*)(S + o_res);
+  uint64_t* dmass = (uint64_t*)(S + o_mass);
+  cudaStream_t st = ctx->stream;
+  const kgv_mempool_tx_args* dargs = args;
+  if (args && !dev) {
+    CK(cudaMemcpyAsync(S + o_args, args, nt * sizeof(kgv_mempool_tx_args), cudaMemcpyHostToDevice, st));
+    dargs = (const kgv_mempool_tx_args*)(S + o_args);
+  }
+  CK(cudaMemsetAsync(cnt, 0, 32, st));
+  if (ni) {
+    k_populate_mempool<<<nblk(ni, 128), 128, 0, st>>>(view_of(t), d.inputs, d.entries, d.bytes, ni, dent, len, cnt);
+    CK(cudaGetLastError());
+    k_input_tx_index<<<nblk(nt, 128), 128, 0, st>>>(d.txs, (uint32_t)nt, itx);
+    CK(cudaGetLastError());
+    k_exclusive_scan2<<<1, 1024, 0, st>>>(len, off, nullptr, nullptr, ni, (uint32_t*)(cnt + 2));  // block 0 only: one array
+    CK(cudaGetLastError());
+    ctx->launches += 3;
+  }
+  STAGE("populate");
+  BatchView v{d.txs, d.inputs, d.outputs, dent, d.bytes};
+  k_tx_mempool_context<<<nblk(nt, 128), 128, 0, st>>>(v, (uint32_t)nt, virtual_daa_score, *prm, dargs, dres, dmass, cnt + 1);
+  CK(cudaGetLastError());
+  ctx->launches++;
+  STAGE("mempool context");
+  unsigned long long c[2];
+  CK(cudaMemcpyAsync(c, cnt, sizeof c, cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  const uint64_t n_script = c[0];
+  if (scripts_used) *scripts_used = (size_t)n_script;
+  if (c[1]) { ctx->err = "kgv_validate_mempool_txs: a feerate threshold with max(storage mass, non_contextual_mass) == 0"; return KGV_ERR_ARG; }
+  if (entries_out && n_script > 0xFFFFFFFFull) { ctx->err = "kgv_validate_mempool_txs: the entries' scripts exceed the 32-bit script_off range"; return KGV_ERR_ARG; }
+  if (entries_out && n_script > scripts_cap) { ctx->err = "kgv_validate_mempool_txs: scripts_out is too small (size returned)"; return KGV_ERR_NOMEM; }
+  if (entries_out && ni) {
+    kgv_utxo_entry* de = entries_out;
+    uint8_t* ds = scripts_out;
+    if (!dev) {
+      const size_t o_s = al256(ni * sizeof(kgv_utxo_entry));
+      rc = kgv_reserve(ctx, &ctx->d_out, &ctx->d_out_cap, o_s + n_script + 16);
+      if (rc) return rc;
+      de = (kgv_utxo_entry*)ctx->d_out;
+      ds = ctx->d_out + o_s;
+    }
+    k_mempool_entries_out<<<nblk(ni, 128), 128, 0, st>>>(dent, off, ni, de, ds);
+    CK(cudaGetLastError());
+    ctx->launches++;
+    if (!dev) {
+      CK(cudaMemcpyAsync(entries_out, de, ni * sizeof(kgv_utxo_entry), cudaMemcpyDeviceToHost, st));
+      if (n_script) CK(cudaMemcpyAsync(scripts_out, ds, n_script, cudaMemcpyDeviceToHost, st));
+      CK(cudaStreamSynchronize(st));  // the script phase may reuse d_out
+    }
+  }
+  if (ni) {
+    rc = scripts_with_host_vm(ctx, t, batch, d, v, itx, dres);
+    if (rc) return rc;
+  }
+  const cudaMemcpyKind k = dev ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost;
+  CK(cudaMemcpyAsync(results, dres, nt * sizeof(kgv_tx_result), k, st));
+  CK(cudaMemcpyAsync(storage_mass, dmass, nt * 8, k, st));
+  if (!dev) CK(cudaStreamSynchronize(st));
+  return KGV_OK;
 }
 
 extern "C" int kgv_utxo_apply_accepted(kgv_ctx* ctx, kgv_utxo_table* t, const kgv_tx_batch* batch, const uint8_t* accept, uint64_t pov_daa_score) {

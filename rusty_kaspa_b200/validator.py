@@ -6,6 +6,8 @@
         (consensus/core/src/utxo/utxo_view.rs:5-7, consensus/src/model/stores/utxo_set.rs:107-112,143-152)
     TransactionValidator.validate_transactions_in_parallel  <->  VirtualStateProcessor::validate_transactions_in_parallel
         (consensus/src/pipeline/virtual_processor/utxo_validation.rs:262-278)
+    TransactionValidator.validate_mempool_transactions_in_utxo_context  <->  validate_mempool_transaction_in_utxo_context
+        (utxo_validation.rs:341-397), for a batch
     GpuUtxoSet.add_transactions                              <->  UtxoDiff::add_transaction (utxo_diff.rs:233-247)
 """
 import ctypes
@@ -13,15 +15,18 @@ import ctypes
 import numpy as np
 
 from . import _lib
-from .txbatch import ENTRY_DTYPE
+from .txbatch import ENTRY_DTYPE, TxBatch
 from .verifier import _c_batch
 
 RESULT_DTYPE = np.dtype([("fee", "<u8"), ("fail_input", "<u4"), ("status", "u1"), ("script_err", "u1"), ("pad_", "u1", (2,))])
 assert RESULT_DTYPE.itemsize == 16
+MEMPOOL_ARGS_DTYPE = np.dtype([("feerate_threshold", "<f8"), ("non_contextual_mass", "<u8")])  # kgv_mempool_tx_args
+assert MEMPOOL_ARGS_DTYPE.itemsize == 16
 
 FLAGS_FULL, FLAGS_SKIP_SCRIPT_CHECKS, FLAGS_SKIP_MASS_CHECK, FLAGS_SCRIPTS_ONLY = 0, 1, 2, 3
 MAX_SOMPI = 29_000_000_000 * 100_000_000
-TX_OK, TX_NEEDS_HOST_VM, TX_SKIPPED_COINBASE = 0, 11, 12
+TX_OK, TX_NEEDS_HOST_VM, TX_SKIPPED_COINBASE, TX_FEERATE_TOO_LOW = 0, 11, 12, 13
+ERR_NOMEM = -3
 
 
 class Params(ctypes.Structure):
@@ -206,8 +211,46 @@ class TransactionValidator:
         mempool transactions against the virtual UTXO set; unlike the block path the per-transaction outcome is RETURNED
         (Vec<TxResult<()>>), not filtered: status / script_err / fail_input say why, `fee` feeds the host-side feerate check
         (tx_validation_in_utxo_context.rs:63-73, f64, stays on the host).  Partially populated transactions (orphans) show up as
-        MISSING_OUTPOINTS.  Below a few hundred signature checks per call the CPU path is faster (DESIGN.md §5)."""
+        MISSING_OUTPOINTS.  Below a few hundred signature checks per call the CPU path is faster (DESIGN.md §5).
+        validate_mempool_transactions_in_utxo_context is the mempool's own rule set: caller entries first, mass computed, feerate threshold."""
         return self.validate_transactions_in_parallel(utxo_set, batch, virtual_daa_score, flags)
+
+    def validate_mempool_transactions_in_utxo_context(self, utxo_set, batch, virtual_daa_score, feerate_threshold=None, non_contextual_mass=None,
+                                                      supplied=None):
+        """validate_mempool_transaction_in_utxo_context (utxo_validation.rs:341-397) for a batch, through kgv_validate_mempool_txs.
+        supplied: None (every input is looked up in `utxo_set`; batch.entries is NOT read, since build_batch fills it with zero records that
+        would pass for present entries) or one bool per input: True keeps batch.entries[i] (e.g. an in-mempool parent's output with
+        block_daa_score = UNACCEPTED_DAA_SCORE = 2**64 - 1), False looks the input up.
+        feerate_threshold: None, or one float per transaction (NaN: None); non_contextual_mass: one value per transaction, the
+        max(compute, transient) mass computed in isolation.  Fee / max(storage mass, non_contextual_mass) <= threshold is FeerateTooLow (13).
+        Returns (RESULT_DTYPE[n_txs], storage masses u64[n_txs], every input's final entry ENTRY_DTYPE[n_inputs] (pad_[0] = 1: absent),
+        the byte arena the entries' script_off points into)."""
+        n, ni = batch.n_txs, batch.n_inputs
+        if supplied is not None:
+            given = batch.entries.copy()
+            given["pad_"][:, 0] = np.where(np.asarray(supplied, dtype=bool), 0, 1)
+            batch = TxBatch(batch.txs, batch.inputs, batch.outputs, given, batch.arena)
+        cb = _c_batch(batch, with_entries=supplied is not None)
+        args = None
+        if feerate_threshold is not None:
+            args = np.zeros(n, dtype=MEMPOOL_ARGS_DTYPE)
+            args["feerate_threshold"] = feerate_threshold
+            args["non_contextual_mass"] = 0 if non_contextual_mass is None else non_contextual_mass
+        res = np.zeros(n, dtype=RESULT_DTYPE)
+        mass = np.zeros(n, dtype=np.uint64)
+        ent = np.zeros(max(ni, 1), dtype=ENTRY_DTYPE)
+        used = ctypes.c_size_t()
+        cap = len(batch.arena) + 128 * ni  # caller scripts come from the arena; a looked-up one usually fits 128 bytes
+        for _ in range(2):  # the call reports the size it needs before any signature is verified
+            arena = np.zeros(max(cap, 8), dtype=np.uint8)
+            rc = self._lib.kgv_validate_mempool_txs(self.ctx._h, utxo_set._h, ctypes.byref(cb), int(virtual_daa_score), ctypes.byref(self.params),
+                                                    None if args is None else args.ctypes.data, res.ctypes.data, mass.ctypes.data, ent.ctypes.data,
+                                                    arena.ctypes.data, len(arena), ctypes.byref(used))
+            if rc != ERR_NOMEM or used.value <= cap:
+                break
+            cap = used.value
+        self.ctx._check(rc)
+        return res, mass, ent[:ni], arena[:used.value]
 
     def validate_transactions_with_muhash_in_parallel(self, utxo_set, batch, pov_daa_score, flags=FLAGS_FULL):
         """utxo_validation.rs:282-309: as validate_transactions_in_parallel, plus the combined MuHash::from_transaction of the
