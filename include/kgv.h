@@ -631,7 +631,9 @@ int kgv_debug_key_form(kgv_ctx* ctx, int ecdsa, kgv_key_form_info* out);
 /* Test / audit hook: runs one arithmetic primitive (its PTX body) on n operand pairs on the device.
  * in_words / out_words: n x 16 u32 (a[8] || b[8] little-endian limbs in; result limbs out).
  * op: 0 mul_wide 1 sqr_wide 2 fe_mul 3 fe_sqr 4 sc_mul 5 sc_sqr 6 sc_inv 7 fe_inv 8 fe_add 9 fe_sub
- *     10 mul_wide+reduce mod n  11 glv_split. */
+ *     10 mul_wide+reduce mod n  11 glv_split
+ *     12 fe_mul_lanes 13 fe_sqr_lanes: the eight-lane forms (one item per group of eight lanes, lane k holding limb k;
+ *        weakly reduced results, like 2 and 3). */
 int kgv_debug_selftest(kgv_ctx* ctx, int op, const uint32_t* in_words, uint32_t* out_words, size_t n);
 
 #ifdef __cplusplus

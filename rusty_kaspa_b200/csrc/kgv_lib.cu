@@ -4,6 +4,7 @@
 #include "../../include/kgv.h"
 #include "kgv_internal.h"
 #include "kgv_verify.cuh"
+#include "kgv_lanes.cuh"
 
 #include <cuda_runtime.h>
 #include <cstdio>
@@ -376,6 +377,23 @@ __global__ void k_selftest(int op, const uint32_t* __restrict__ in, uint32_t* __
   }
 #pragma unroll
   for (int k = 0; k < 16; k++) out[i * 16 + k] = r[k];
+}
+
+// audit/debug: the eight-lane field primitives (kgv_lanes.cuh), one item per group of eight lanes, same in/out layout
+// as k_selftest.  A group past n leaves as a whole group (n * 8 threads, groups never straddle the bound).
+__global__ void k_selftest_lanes(int op, const uint32_t* __restrict__ in, uint32_t* __restrict__ out, int n) {
+  const int i = (int)((blockIdx.x * blockDim.x + threadIdx.x) >> 3);
+  if (i >= n) return;
+  const lane_grp g = lane_group();
+  const uint32_t a = in[i * 16 + g.k], b = in[i * 16 + 8 + g.k];
+  uint32_t r = 0;
+  switch (op) {
+    case 12: r = fe_mul_lanes(a, b, g); break;
+    case 13: r = fe_sqr_lanes(a, g); break;
+    default: break;
+  }
+  out[i * 16 + g.k] = r;
+  out[i * 16 + 8 + g.k] = 0;
 }
 
 __global__ void k_status_to_bitmap(const uint8_t* __restrict__ status, size_t n, uint8_t* __restrict__ bitmap) {
@@ -761,7 +779,10 @@ extern "C" int kgv_debug_selftest(kgv_ctx* ctx, int op, const uint32_t* in_words
   rc = kgv_reserve(ctx, &ctx->d_out, &ctx->d_out_cap, n * 64);
   if (rc) return rc;
   CK(cudaMemcpyAsync(ctx->d_in, in_words, n * 64, cudaMemcpyHostToDevice, ctx->stream));
-  k_selftest<<<(unsigned)((n + 63) / 64), 64, 0, ctx->stream>>>(op, (const uint32_t*)ctx->d_in, (uint32_t*)ctx->d_out, (int)n);
+  if (op >= 12)
+    k_selftest_lanes<<<(unsigned)((n * 8 + 63) / 64), 64, 0, ctx->stream>>>(op, (const uint32_t*)ctx->d_in, (uint32_t*)ctx->d_out, (int)n);
+  else
+    k_selftest<<<(unsigned)((n + 63) / 64), 64, 0, ctx->stream>>>(op, (const uint32_t*)ctx->d_in, (uint32_t*)ctx->d_out, (int)n);
   CK(cudaGetLastError());
   ctx->launches++;
   CK(cudaMemcpyAsync(out_words, ctx->d_out, n * 64, cudaMemcpyDeviceToHost, ctx->stream));

@@ -1,15 +1,19 @@
 // Latency/throughput probe of the field multiply and square subroutines (the exact code the verify kernels
 // call) as a function of resident warps per SM sub-partition: a chain of dependent fe_mul / fe_sqr per thread,
 // one block per SM with 128*W threads.  Prints cycles per call per warp and calls/clk/SM.
+// The lane modes run the eight-lane product of kgv_lanes.cuh: each group of eight lanes carries one dependent chain, so
+// at one warp per scheduler "cycles per call per warp" is the latency of one cooperative call.
 #include <cstdio>
 #include <cstdint>
 #include <cuda_runtime.h>
 #include "../../rusty_kaspa_b200/csrc/kgv_arith.cuh"
+#include "../../rusty_kaspa_b200/csrc/kgv_lanes.cuh"
 using namespace kgv;
 
 template <int MODE>
 __global__ void probe(uint32_t* out, int iters) {
   fe a, b;
+  const lane_grp g = lane_group();
   for (int i = 0; i < 8; i++) { a.v[i] = 0x9E3779B9u * (threadIdx.x + 1 + i) + blockIdx.x; b.v[i] = 0x85EBCA6Bu * (threadIdx.x + 7 + i); }
 #pragma unroll 1
   for (int it = 0; it < iters; it++) {
@@ -18,6 +22,8 @@ __global__ void probe(uint32_t* out, int iters) {
     else if (MODE == 2) { fe_mul(a, a, b); fe_sqr(b, b); }          // two independent chains
     else if (MODE == 3) { fe_add(a, a, b); }
     else if (MODE == 4) { fe_sub(a, a, b); }
+    else if (MODE == 5) { a.v[0] = fe_mul_lanes(a.v[0], b.v[0], g); }
+    else if (MODE == 6) { a.v[0] = fe_sqr_lanes(a.v[0], g); }
   }
   uint32_t acc = 0;
   for (int i = 0; i < 8; i++) acc ^= a.v[i] ^ b.v[i];
@@ -52,5 +58,7 @@ int main() {
   run<2>("fe_mul + fe_sqr indep", 2, p.multiProcessorCount, out, ghz);
   run<3>("fe_add chain", 1, p.multiProcessorCount, out, ghz);
   run<4>("fe_sub chain", 1, p.multiProcessorCount, out, ghz);
+  run<5>("fe_mul_lanes chain", 1, p.multiProcessorCount, out, ghz);
+  run<6>("fe_sqr_lanes chain", 1, p.multiProcessorCount, out, ghz);
   return 0;
 }
