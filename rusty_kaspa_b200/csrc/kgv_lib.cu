@@ -24,7 +24,7 @@ struct SmemTab {
   uint32_t* base;  // smem + threadIdx.x
   __device__ __forceinline__ void put(int e, int w, uint32_t v) { base[(e * 16 + w) * KGV_BLOCK] = v; }
   __device__ __forceinline__ uint32_t get(int e, int w) const { return base[(e * 16 + w) * KGV_BLOCK]; }
-  // the comb ladder's staging (ecmult_comb) uses the same 512 bytes as 32 chunks of 16 bytes, chunk-major / thread-minor: a warp's
+  // the comb ladder's staging (ecmult_joint) uses the same 512 bytes as 32 chunks of 16 bytes, chunk-major / thread-minor: a warp's
   // 16-byte copies and reads of one chunk cover 512 consecutive bytes, free of bank conflicts.  Chunk c of slot s: 4s + c.
   __device__ __forceinline__ uint4* chunk(int q) const { return reinterpret_cast<uint4*>(base - threadIdx.x) + q * KGV_BLOCK + threadIdx.x; }
 };
@@ -102,10 +102,11 @@ __global__ void __launch_bounds__(128) k_build_gtab(uint32_t* __restrict__ gtab)
 }
 
 // ---- per-launch key cache: the key part of a verification done once per distinct public key of a verify launch ----
-// Records per launch at most (2^17 x 2112 B = 277 MB of comb records, 2^17 x 560 B = 73 MB of plain ones).
+// Records per launch at most (2^17 x 10304 B = 1.35 GB of comb records with their joint tables, 2^17 x 560 B = 73 MB of plain ones).
 #define KGV_KEY_RECORDS_MAX (1u << 17)
-// Fewest uses per key on average for comb records: the comb's preparation (~1 800 products per key against ~400) must be paid back by
-// its shorter ladder (~700 products fewer per verify); measured +20 % at 10 uses per key (DESIGN.md §5), not below.
+// Fewest uses per key on average for comb records: the comb's preparation (~1 800 products per key against ~400, ~2 700 with the joint
+// table) must be paid back by its shorter ladder (~700, with the joint table ~1 000 products fewer per verify); measured +20 % at 10 uses
+// per key before the joint table and faster still with it at 8 to 50 uses (DESIGN.md §5), not below.
 #ifndef KGV_COMB_USES
 #define KGV_COMB_USES 8
 #endif
@@ -113,7 +114,7 @@ enum { KGV_KEYS_INLINE = 0, KGV_KEYS_PLAIN = 1, KGV_KEYS_COMB = 2 };
 // The form of a launch's key part, uniform over the launch: records when its keys are used twice on average (at most n/2 distinct keys)
 // and fit the cap; then EVERY key has one.  A warp pays for the inline key path of any of its lanes, so records for the repeated keys
 // alone leave singleton lanes costing whole warps; a batch of mostly distinct keys makes no records at all and pays only the dedup pass.
-// Comb records (key_comb_build, ecmult_comb) when the keys are used at least KGV_COMB_USES times on average, plain ones (key_rec_build) below.
+// Comb records (key_comb_build + key_joint_build, ecmult_joint) when the keys are used at least KGV_COMB_USES times on average, plain ones (key_rec_build) below.
 // Host-callable too: kgv_debug_key_form reports the form a launch took by this same rule.
 __host__ __device__ __forceinline__ int key_form(uint32_t n_rec, size_t n) {
   if (n_rec > KGV_KEY_RECORDS_MAX || 2 * (size_t)n_rec > n) return KGV_KEYS_INLINE;
@@ -128,14 +129,14 @@ struct KeySlot {
 struct KeyCacheView {
   const KeySlot* table;
   const uint32_t* item_slot;  // item -> table slot (only the items the launch verifies are set)
-  const uint32_t* recs;       // records, KGV_KR_WORDS or KGV_KC_WORDS words each
+  const uint32_t* recs;       // records, KGV_KR_WORDS or KGV_KJ_WORDS words each
   const uint32_t* n_rec;      // distinct keys of the launch; nullptr: no key cache
   // the key source of item i: its record and the launch's form, or no record (the launch makes none)
   __device__ __forceinline__ KeySrc key_of(size_t i, size_t n) const {
     const int f = n_rec ? key_form(*n_rec, n) : KGV_KEYS_INLINE;
     if (f == KGV_KEYS_INLINE) return KeySrc{nullptr, false};
     const bool comb = f == KGV_KEYS_COMB;
-    return KeySrc{recs + (size_t)(table[item_slot[i]].rec - 1) * (comb ? KGV_KC_WORDS : KGV_KR_WORDS), comb};
+    return KeySrc{recs + (size_t)(table[item_slot[i]].rec - 1) * (comb ? KGV_KJ_WORDS : KGV_KR_WORDS), comb};
   }
 };
 
@@ -206,7 +207,7 @@ __global__ void __launch_bounds__(256) k_key_dedup(const uint8_t* __restrict__ p
   item_slot[i] = s;
 }
 
-// One thread per record: the key's verdict, and for a good key its comb (key_comb_build) or its odd-multiples table and zs (key_rec_build).
+// One thread per record: the key's verdict, and for a good key its comb and joint table (key_comb_build, key_joint_build) or its odd-multiples table and zs (key_rec_build).
 // The verify kernels' occupancy (168 registers): unbounded, ptxas takes 255 and two blocks per SM.
 template <bool ECDSA>
 __global__ void __launch_bounds__(KGV_BLOCK, KGV_BLOCKS_PER_SM) k_key_prepare(const uint8_t* __restrict__ pk, size_t n_arg, const uint32_t* __restrict__ n_dev,
@@ -218,8 +219,11 @@ __global__ void __launch_bounds__(KGV_BLOCK, KGV_BLOCKS_PER_SM) k_key_prepare(co
   if (r >= *n_rec || f == KGV_KEYS_INLINE) return;
   uint32_t w[9];
   key_words<false, ECDSA>(w, pk, rec_rep[r]);
-  if (f == KGV_KEYS_COMB) key_comb_build(recs + (size_t)r * KGV_KC_WORDS, ECDSA ? w[8] : 2u, w);
-  else key_rec_build(recs + (size_t)r * KGV_KR_WORDS, ECDSA ? w[8] : 2u, w);
+  if (f == KGV_KEYS_COMB) {
+    uint32_t* rec = recs + (size_t)r * KGV_KJ_WORDS;
+    key_comb_build(rec, ECDSA ? w[8] : 2u, w);
+    if (rec[KGV_KC_STATUS] == KGV_ST_VALID) key_joint_build(rec);
+  } else key_rec_build(recs + (size_t)r * KGV_KR_WORDS, ECDSA ? w[8] : 2u, w);
 }
 
 // Each thread verifies KGV_ITEMS consecutive-stride items (i = tid + j * total_threads: coalesced) and shares
@@ -574,7 +578,7 @@ static int key_cache_launch(kgv_ctx* ctx, const uint8_t* dpk, size_t n, bool ecd
   while (slots < 2 * n) slots <<= 1;                       // load factor <= 1/2
   const uint32_t cap = (uint32_t)(n / 2 < KGV_KEY_RECORDS_MAX ? n / 2 : KGV_KEY_RECORDS_MAX);  // key_form's bounds
   const size_t cap_comb = n / KGV_COMB_USES < KGV_KEY_RECORDS_MAX ? n / KGV_COMB_USES : KGV_KEY_RECORDS_MAX;
-  const size_t rec_bytes = std::max((size_t)cap * KGV_KR_WORDS, cap_comb * KGV_KC_WORDS) * 4;
+  const size_t rec_bytes = std::max((size_t)cap * KGV_KR_WORDS, cap_comb * KGV_KJ_WORDS) * 4;
   const size_t o_tab = 256, o_item = o_tab + (size_t)slots * sizeof(KeySlot);
   const size_t o_rep = (o_item + n * 4 + 255) & ~(size_t)255, o_rec = (o_rep + (size_t)cap * 4 + 255) & ~(size_t)255;
   int rc = kgv_reserve(ctx, &ctx->d_keys[ecdsa], &ctx->d_keys_cap[ecdsa], o_rec + rec_bytes);

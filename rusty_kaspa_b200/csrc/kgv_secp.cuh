@@ -11,6 +11,8 @@
 //     (G and 2^128*G of the eight 2^(32j)*G tables, L2 resident), 16 mixed additions
 //   * 128 shared doublings
 // ecmult_comb is the same product for a key prepared once per launch as a four-tooth comb (keys that repeat often): 32 doublings.
+// ecmult_joint (the device's ladder for such keys) reads joint entries a*T + b*lambda*T of the same teeth: one addition per digit pair of
+// both GLV halves, 44 instead of 66, and 30 doublings.  ecmult_comb stays as the host-checked reference it is compared with.
 #pragma once
 #include "kgv_arith.cuh"
 
@@ -677,6 +679,129 @@ KGV_HD void ecmult_comb(gej& R, const uint32_t* kP, const uint32_t* kG, const ui
 #pragma unroll 1
   for (int half = 0; half < 2; half++) {
     if (!fix[half]) continue;
+    gload(ex, ey, rec);
+    if (half) fe_mul(ex, ex, beta);
+    if (!ng[half]) fe_neg(ey, ey);
+    gej_add_ge(R, ex, ey);
+  }
+}
+
+// ------------------------------------------------------------------------------------------
+// R = kP * P + kG * G from the joint table of a comb record     (result with true Z)
+// ------------------------------------------------------------------------------------------
+// Joint recoding of one GLV half m (5 limbs), after the parity fix m -> m + 1 of an even m (`fix`, as recode_signed_odd):
+//   m = sum_t c_t 2^(32t), t = 0..3, every c_t odd with |c_t| < 2^33: from the low tooth up, c_t = r mod 2^32, minus 2^32 (and one more
+//   carry) when the quotient would be even, so every quotient stays odd; c_3 is the last quotient;
+//   c_t = sum_w d_w 8^w, w = 0..10, d_w odd in {+-1, +-3, +-5, +-7}: v = (c_t + 2^33 - 1) / 2, d_w = 2 ((v >> 3w) & 7) - 7.
+// glv_split's halves are below 2^128: |k1| <= (a1 + a2)/2 + 1 and |k2| <= (|b1| + b2)/2 + 1 (each rounding error of c1, c2 is at most
+// 1/2 + 2^-128; a1 b2 - a2 b1 = n), and both bounds are below 2^128 (tests/test_hostsim_joint.py evaluates them).  So c_3 <= 2^32 + 1.
+// Digit 11t + w is stored as the 3-bit v field in bits 3(i % 10) of word i / 10 (44 digits, 5 words).
+KGV_HD void recode_joint(uint32_t* h, bool& fix, const uint32_t* m) {
+  fix = (m[0] & 1u) == 0;
+  uint64_t v[4], carry = fix ? 1 : 0;  // r_t = (m >> 32t) + carry, odd
+#pragma unroll
+  for (int t = 0; t < 3; t++) {
+    const uint64_t x = (uint64_t)m[t] + carry;
+    const uint32_t lo = (uint32_t)x, hi = (uint32_t)(x >> 32);  // lo: the low word of r_t, odd
+    const uint32_t borrow = ((m[t + 1] + hi) & 1u) ^ 1u;         // the quotient would be even: c_t = lo - 2^32
+    v[t] = (uint64_t)(lo >> 1) + (borrow ? (1ull << 31) : (1ull << 32));
+    carry = hi + borrow;
+  }
+  const uint64_t c3 = (uint64_t)m[3] + ((uint64_t)m[4] << 32) + carry;  // odd, positive
+  v[3] = (c3 >> 1) + (1ull << 32);
+#pragma unroll
+  for (int q = 0; q < 5; q++) h[q] = 0;
+#pragma unroll
+  for (int i = 0; i < 44; i++) h[i / 10] |= (uint32_t)((v[i / 11] >> (3 * (i % 11))) & 7u) << (3 * (i % 10));
+}
+// the v field (0..7, d = 2v - 7) of digit i = 11t + w
+KGV_HD uint32_t joint_digit(const uint32_t* h, int i) { return (h[i / 10] >> (3 * (i % 10))) & 7u; }
+// jt: the joint table, entry 32t + 8a + k (16 words at word 16(32t + 8a + k)) = (2a+1) T + (2k-7) lambda T, T = 2^(32t) P, true affine
+// (key_joint_build, kgv_verify.cuh).  The entry for digit i of both halves, with the GLV signs ng folded in: e0 T + e1 lambda T =
+// sign(e0) (|e0| T + sign(e0) e1 lambda T); neg: negate its y.
+KGV_HD const uint32_t* joint_entry(const uint32_t* jt, const uint32_t (*h)[5], const bool* ng, int i, bool& neg) {
+  const uint32_t u0 = joint_digit(h[0], i), u1 = joint_digit(h[1], i);
+  neg = (u0 < 4u) != ng[0];
+  const uint32_t a = u0 < 4u ? 3u - u0 : u0 - 4u;   // (|d0| - 1) / 2
+  const uint32_t k = neg != ng[1] ? 7u - u1 : u1;   // b = sign(e0) e1 = 2k - 7
+  return jt + 16 * (32 * (i / 11) + 8 * a + k);
+}
+// the eight generator additions of 16-bit fields at bits 32j + sh of kG, from table j (zero fields skipped)
+template <class GLoad>
+KGV_HD void gen_fields(gej& R, const uint32_t* kG, int sh, const uint32_t* gtab, GLoad gload) {
+  fe ex, ey;
+#pragma unroll 1
+  for (int j = 0; j < 8; j++) {
+    const uint32_t d = (kG[j] >> sh) & 0xFFFFu;
+    if (d) {
+      gload(ex, ey, gtab + ((size_t)j * 65536 + d) * 16);
+      gej_add_ge(R, ex, ey);
+    }
+  }
+}
+// rec: the comb record (entry 0 = P); jt: its joint table.  gtab: as for ecmult_comb.
+// Windows w = 10..0 with three doublings between them (30 in all); window w adds, per tooth t, ONE joint entry for digit 11t + w of both
+// halves (44 key additions, no beta products).  The generator's fields at bits 32j..32j+15 weigh 1 (after window 0); those at bits
+// 32j+16..32j+31 weigh 2^16 = 2 * 2^(3*5): window 5's three doublings are split 2 + 1 around them.  Both use the eight tables of ecmult_comb
+// (32 MiB, L2 resident), none more.
+// Staging as in ecmult_comb: window 10 is read directly; window w's entry of tooth t sits in slot 4(w & 1) + t; after the addition that
+// consumes it, the copy of the entry of window w - 2 starts into the same slot (one commit group per addition, empty ones in windows 1, 0).
+// Between a copy's commit and its read lie 3 - t + 4 + t = 7 newer groups: stage_wait's count.
+template <class Tab, class GLoad>
+KGV_HD void ecmult_joint(gej& R, const uint32_t* kP, const uint32_t* kG, const uint32_t* rec, const uint32_t* jt, Tab& tab, const uint32_t* gtab,
+                         GLoad gload) {
+  const fe beta = {KGV_BETA_LIMBS};
+  uint32_t m[2][5], h[2][5];
+  bool ng[2], fix[2], neg;
+  glv_split(m[0], ng[0], m[1], ng[1], kP);
+  recode_joint(h[0], fix[0], m[0]);
+  recode_joint(h[1], fix[1], m[1]);
+#pragma unroll 1
+  for (int s = 0; s < 8; s++) {  // window 9 into slots 4..7, then window 8 into slots 0..3
+    const int w = 9 - (s >> 2), t = s & 3;
+    stage_fetch(tab, 4 * (w & 1) + t, joint_entry(jt, h, ng, 11 * t + w, neg));
+    stage_commit(tab);
+  }
+  R.inf = true;
+  fe_set_zero(R.x); fe_set_zero(R.y); fe_set_zero(R.z);
+  fe ex, ey;
+#pragma unroll 1
+  for (int t = 0; t < 4; t++) {
+    gload(ex, ey, joint_entry(jt, h, ng, 11 * t + 10, neg));
+    if (neg) fe_neg(ey, ey);
+    gej_add_ge(R, ex, ey);
+  }
+#pragma unroll 1
+  for (int w = 9; w >= 0; w--) {
+    if (w == 5) {
+      gej_double_n(R, 2);
+      gen_fields(R, kG, 16, gtab, gload);
+      gej_double_n(R, 1);
+    } else {
+      gej_double_n(R, 3);
+    }
+#pragma unroll 1
+    for (int t = 0; t < 4; t++) {
+      const int s = 4 * (w & 1) + t;
+      (void)joint_entry(jt, h, ng, 11 * t + w, neg);
+      stage_wait(tab);
+      stage_get(tab, s, ex, ey);
+      if (neg) fe_neg(ey, ey);
+      gej_add_ge(R, ex, ey);
+      bool neg2;
+      if (w >= 2) stage_fetch(tab, s, joint_entry(jt, h, ng, 11 * t + w - 2, neg2));
+      stage_commit(tab);  // (empty in windows 1 and 0: keeps stage_wait's count)
+    }
+  }
+  gen_fields(R, kG, 0, gtab, gload);
+  // parity corrections, at most one addition: -(s0 P + s1 lambda P) = -s0 (P + s0 s1 lambda P) is joint entry (a = 1, b = s0 s1) of
+  // tooth 0; one of them alone is comb entry 0, times beta for the lambda half
+  if (fix[0] && fix[1]) {
+    gload(ex, ey, jt + 16 * (ng[0] == ng[1] ? 4 : 3));
+    if (!ng[0]) fe_neg(ey, ey);
+    gej_add_ge(R, ex, ey);
+  } else if (fix[0] || fix[1]) {
+    const int half = fix[1] ? 1 : 0;
     gload(ex, ey, rec);
     if (half) fe_mul(ex, ex, beta);
     if (!ng[half]) fe_neg(ey, ey);

@@ -44,6 +44,11 @@ KGV_HD bool key_lift(fe& x, fe& y, uint32_t tag, const uint32_t* pkw) {
 //   512        the key's verdict, as KGV_KR_STATUS
 #define KGV_KC_STATUS 512
 #define KGV_KC_WORDS 528  // 2112 bytes
+// The comb form's record as the verify kernels use it (ecmult_joint): the comb record above, then the joint table
+//   [528, 2576) entry 32t + 8a + k = (2a+1) * T + (2k-7) * lambda * T, T = 2^(32t) * P, for t = 0..3, a = 0..3, k = 0..7, at word
+//               528 + 16(32t + 8a + k): x limbs, then y limbs, true affine
+#define KGV_KJ_JOINT KGV_KC_WORDS
+#define KGV_KJ_WORDS (KGV_KJ_JOINT + 4 * 32 * 16)  // 2576 words, 10304 bytes
 
 // Tab accessor over a key record in global memory (the preparation kernel builds the table in place)
 struct RecTab {
@@ -57,6 +62,23 @@ KGV_HD void ldg128(uint32_t* w, const uint32_t* p) {
   asm volatile("ld.global.nc.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(w[0]), "=r"(w[1]), "=r"(w[2]), "=r"(w[3]) : "l"(p));
 #else
   for (int i = 0; i < 4; i++) w[i] = p[i];
+#endif
+}
+// a field element at p (16-byte aligned) of a record the same thread writes: two 128-bit accesses (coherent, not the read-only path)
+KGV_HD void fe_ld(fe& x, const uint32_t* p) {
+#ifdef __CUDA_ARCH__
+  const uint4 a = reinterpret_cast<const uint4*>(p)[0], b = reinterpret_cast<const uint4*>(p)[1];
+  x.v[0] = a.x; x.v[1] = a.y; x.v[2] = a.z; x.v[3] = a.w; x.v[4] = b.x; x.v[5] = b.y; x.v[6] = b.z; x.v[7] = b.w;
+#else
+  for (int w = 0; w < 8; w++) x.v[w] = p[w];
+#endif
+}
+KGV_HD void fe_st(uint32_t* p, const fe& x) {
+#ifdef __CUDA_ARCH__
+  reinterpret_cast<uint4*>(p)[0] = make_uint4(x.v[0], x.v[1], x.v[2], x.v[3]);
+  reinterpret_cast<uint4*>(p)[1] = make_uint4(x.v[4], x.v[5], x.v[6], x.v[7]);
+#else
+  for (int w = 0; w < 8; w++) p[w] = x.v[w];
 #endif
 }
 // table and zs of a prepared key (its verdict is KGV_ST_VALID)
@@ -122,17 +144,100 @@ KGV_HD void key_comb_build(uint32_t* rec, uint32_t tag, const uint32_t* pkw) {
       for (int e = 0; e < 8; e++) {
         uint32_t* en = rec + 16 * (8 * t + e);
         fe ex, ey;
-#pragma unroll
-        for (int w = 0; w < 8; w++) { ex.v[w] = en[w]; ey.v[w] = en[8 + w]; }
+        fe_ld(ex, en);
+        fe_ld(ey, en + 8);
         fe_mul(ex, ex, zi2);
         fe_mul(ey, ey, zi3);
-#pragma unroll
-        for (int w = 0; w < 8; w++) { en[w] = ex.v[w]; en[8 + w] = ey.v[w]; }
+        fe_st(en, ex);
+        fe_st(en + 8, ey);
       }
     }
     st = KGV_ST_VALID;
   }
   rec[KGV_KC_STATUS] = st;
+}
+
+// fills the joint table of a comb record whose verdict is KGV_ST_VALID (after key_comb_build, same thread).  Per tooth t and pair
+// p = (a, j): A = (2a+1) T (comb entry 8t + a) and B = (2j+1) lambda T = (beta x_j, y_j) of comb entry 8t + j; A + B is entry k = j + 4,
+// A - B entry k = 3 - j, both affine additions over the one denominator beta x_j - x_A.  The 64 denominators share one inversion
+// (Montgomery's trick), with the joint area itself as scratch: beta x_j of tooth t in words 0..7 of entry (t, 0, 3 - j) and the prefix
+// product of pairs 0..p (p = 16t + 4a + j) in words 0..7 of entry (t, a, j + 4), each read before the pass going back down overwrites it.
+// No denominator is zero for a key that parses: A = +-B means (2a+1) = +-(2j+1) lambda (mod n), so (2a+1)^3 = +-(2j+1)^3 (mod n) with
+// both cubes below 7^3 < n, hence 2a+1 = 2j+1 as integers and lambda = +-1, which it is not.
+// About 860 products: 16 by beta, 63 + 126 for the trick, 6 per pair, one fe_inv.
+// Each thread owns a 10 KB record, so a warp's accesses are 32 lanes at a 10 KB stride: all of them go through fe_ld / fe_st (128-bit),
+// and every operand is loaded once per loop level that needs it.
+KGV_HD void key_joint_build(uint32_t* rec) {
+  const fe beta = {KGV_BETA_LIMBS};
+  uint32_t* jt = rec + KGV_KJ_JOINT;
+#pragma unroll 1
+  for (int t = 0; t < 4; t++) {
+#pragma unroll 1
+    for (int j = 0; j < 4; j++) {
+      fe bx;
+      fe_ld(bx, rec + 16 * (8 * t + j));
+      fe_mul(bx, bx, beta);
+      fe_st(jt + 16 * (32 * t + 3 - j), bx);
+    }
+  }
+  fe acc;
+  fe_set_u32(acc, 1);
+#pragma unroll 1
+  for (int ta = 0; ta < 16; ta++) {  // pairs p = 4 ta + j
+    const int t = ta >> 2, a = ta & 3;
+    fe xa;
+    fe_ld(xa, rec + 16 * (8 * t + a));
+#pragma unroll 1
+    for (int j = 0; j < 4; j++) {
+      fe bx, d;
+      fe_ld(bx, jt + 16 * (32 * t + 3 - j));
+      fe_sub(d, bx, xa);
+      fe_mul(acc, acc, d);
+      fe_st(jt + 16 * (32 * t + 8 * a + j + 4), acc);
+    }
+  }
+  fe inv;
+  fe_inv(inv, acc);
+#pragma unroll 1
+  for (int ta = 15; ta >= 0; ta--) {
+    const int t = ta >> 2, a = ta & 3;
+    fe xa, ya;
+    fe_ld(xa, rec + 16 * (8 * t + a));
+    fe_ld(ya, rec + 16 * (8 * t + a) + 8);
+#pragma unroll 1
+    for (int j = 3; j >= 0; j--) {
+      const int p = 4 * ta + j, q = p - 1;
+      fe bx, yb, d, di;
+      fe_ld(bx, jt + 16 * (32 * t + 3 - j));
+      fe_ld(yb, rec + 16 * (8 * t + j) + 8);
+      if (p) {
+        fe pre;
+        fe_ld(pre, jt + 16 * (32 * (q >> 4) + 8 * ((q >> 2) & 3) + (q & 3) + 4));
+        fe_sub(d, bx, xa);
+        fe_mul(di, inv, pre);
+        fe_mul(inv, inv, d);
+      } else {
+        di = inv;
+      }
+#pragma unroll 1
+      for (int sgn = 0; sgn < 2; sgn++) {  // A + B (k = j + 4), then A - B (k = 3 - j)
+        fe l, x3, y3, t1;
+        if (sgn) fe_neg(t1, yb);
+        else t1 = yb;
+        fe_sub(t1, t1, ya);
+        fe_mul(l, t1, di);                 // slope
+        fe_sqr(x3, l);
+        fe_sub(x3, x3, xa);
+        fe_sub(x3, x3, bx);                // x3 = l^2 - xA - xB
+        fe_sub(t1, xa, x3);
+        fe_mul(y3, l, t1);
+        fe_sub(y3, y3, ya);                // y3 = l (xA - x3) - yA
+        uint32_t* en = jt + 16 * (32 * t + 8 * a + (sgn ? 3 - j : j + 4));
+        fe_st(en, x3);
+        fe_st(en + 8, y3);
+      }
+    }
+  }
 }
 
 // Where the key part of a verification comes from: the key's comb record (comb), its plain record, or none (rec == nullptr: the key is
@@ -149,7 +254,7 @@ KGV_HD void ecmult_key(gej& R, fe& zt, const KeySrc& key, const fe& px, const fe
                        const uint32_t* gtab, GLoad gload, Trace trace = Trace()) {
   fe zs;
   if (key.comb) {
-    ecmult_comb(R, kP, kG, key.rec, tab, gtab, gload);
+    ecmult_joint(R, kP, kG, key.rec, key.rec + KGV_KJ_JOINT, tab, gtab, gload);
   } else {
     if (key.rec) key_rec_load(tab, zs, key.rec);
     else build_odd_table(tab, zs, px, py);
