@@ -294,7 +294,7 @@ int kgv_utxo_set_max_load(kgv_ctx* ctx, kgv_utxo_table* t, uint32_t max_load_per
 /* validate_transactions_in_parallel (utxo_validation.rs:262-278) against the table: populate every input
  * by table lookup (:319-327), then as kgv_validate_populated.  batch->entries is ignored.
  * Unlike kgv_validate_populated this call never reports KGV_TX_NEEDS_HOST_VM: transactions with non-standard scripts are
- * decided inside the call by the host script engine on the entries the table returned (the reference accepts ANY
+ * decided inside the call by the full script engine on the GPU (kgv_check_scripts) on the entries the table returned (the reference accepts ANY
  * transaction whose scripts execute successfully, utxo_validation.rs:282-309). */
 int kgv_validate_txs(kgv_ctx* ctx, kgv_utxo_table* t, const kgv_tx_batch* batch, uint64_t pov_daa_score, uint32_t flags, const kgv_params* params,
                      kgv_tx_result* results);
@@ -314,7 +314,7 @@ int kgv_utxo_apply_accepted(kgv_ctx* ctx, kgv_utxo_table* t, const kgv_tx_batch*
  *              KGV_TX_FEERATE_TOO_LOW (tx_validation_in_utxo_context.rs:63-73).  It comes before the scripts, so such a transaction's
  *              signatures are never verified nor cached.  A threshold whose divisor is 0 makes the call fail with KGV_ERR_ARG (the reference
  *              asserts it is not zero).  args == NULL: no thresholds.
- * Non-standard scripts are decided inside the call by the host script engine, as in kgv_validate_txs; coinbases give KGV_TX_SKIPPED_COINBASE.
+ * Non-standard scripts are decided inside the call by the device script engine, as in kgv_validate_txs; coinbases give KGV_TX_SKIPPED_COINBASE.
  * results: n_txs records (fee set once the amounts pass); storage_mass: n_txs values (0 when the mass was not reached).
  * entries_out (n_inputs records, may be NULL): every input's final entry - the caller's, the one found, or absent-marked (pad_[0] = 1) when
  * neither - with script_off into scripts_out (scripts_cap bytes).  *scripts_used (may be NULL) receives the bytes those scripts take; when
@@ -412,7 +412,7 @@ typedef struct {
 typedef struct {
   uint64_t n_accepted;   /* accepted non-coinbase transactions */
   uint64_t n_sig_checks; /* candidate (signature, key) pairs verified in the pre-check */
-  uint64_t n_host_vm;    /* transactions decided by the host script engine */
+  uint64_t n_host_vm;    /* transactions the fast path declined, decided by the full script engine */
   float pre_check_ms;    /* device time of the batched script pre-check (tx ids, window map, populate, sighash, verify, resolve) */
   float in_order_ms;     /* device time from the end of the pre-check to the end of the finishing passes (slot map, static rules, walk,
                             verdicts, table updates, results) */
@@ -579,6 +579,14 @@ int kgv_script_execute(const kgv_tx_batch* batch, uint32_t tx, uint32_t input_in
  * results[i] belongs to tx_indices[i]: status KGV_TX_OK / KGV_TX_SIGNATURE_INVALID / KGV_TX_SIGNATURE_EMPTY. */
 int kgv_check_scripts_host(kgv_ctx* ctx, const kgv_tx_batch* batch, const uint32_t* tx_indices, size_t n, kgv_tx_result* results);
 
+/* The same check_scripts with the full script engine on the device: the same results as kgv_check_scripts_host for every input, but
+ * the populated batch may be host OR device memory, and tx_indices / results may each be host or device memory.  Every input of a listed
+ * transaction runs on the GPU; the signature checks its scripts reach are hashed and verified in rounds (through the attached SigCache,
+ * if any), one synchronisation per round, at most 256 rounds.  This is what a caller runs after kgv_validate_populated reports
+ * KGV_TX_NEEDS_HOST_VM for a device-resident batch; the table-backed calls (kgv_validate_txs, kgv_validate_mempool_txs,
+ * kgv_replay_window) run the same engine internally. */
+int kgv_check_scripts(kgv_ctx* ctx, const kgv_tx_batch* batch, const uint32_t* tx_indices, size_t n, kgv_tx_result* results);
+
 /* ------------------------------------------------------------------------------------------------
  * Persistence formats either side of the path (SURVEY.md §8f-4): the RocksDB rows of DbUtxoSetStore.  Host functions (the store lives on
  * the host): what a shim runs between the database and kgv_utxo_apply_diff / kgv_utxo_lookup (write_diff_batch utxo_set.rs:107-112, the
@@ -627,6 +635,9 @@ typedef struct kgv_key_form_info {
   int32_t form;           /* KGV_KEY_FORM_*                                       */
 } kgv_key_form_info;
 int kgv_debug_key_form(kgv_ctx* ctx, int ecdsa, kgv_key_form_info* out);
+/* Signature verification rounds of the last run of the device script engine on this context (kgv_check_scripts, or the engine inside
+ * kgv_validate_txs / kgv_validate_mempool_txs / kgv_replay_window); 0 when it had nothing to verify. */
+int kgv_debug_script_rounds(const kgv_ctx* ctx, uint32_t* rounds);
 
 /* Test / audit hook: runs one arithmetic primitive (its PTX body) on n operand pairs on the device.
  * in_words / out_words: n x 16 u32 (a[8] || b[8] little-endian limbs in; result limbs out).

@@ -564,6 +564,18 @@ class TransactionValidator {
     return {std::move(res), MuHash(c_, num, den)};
   }
 
+  // check_scripts with the full script engine on the GPU (kgv_check_scripts) for every tx of `res` reported KGV_TX_NEEDS_HOST_VM; the
+  // results of the host engine, fee kept.  b must carry the populated entries.
+  void check_scripts(const TxBatch& b, std::vector<kgv_tx_result>& res) {
+    std::vector<uint32_t> idx;
+    for (size_t i = 0; i < res.size(); i++) if (res[i].status == KGV_TX_NEEDS_HOST_VM) idx.push_back((uint32_t)i);
+    if (idx.empty()) return;
+    kgv_tx_batch v = b.view(true);
+    std::vector<kgv_tx_result> out(idx.size());
+    c_.check(kgv_check_scripts(c_.get(), &v, idx.data(), idx.size(), out.data()));
+    for (size_t k = 0; k < idx.size(); k++) { uint64_t fee = res[idx[k]].fee; res[idx[k]] = out[k]; res[idx[k]].fee = fee; }
+  }
+
  private:
   void check_scripts_host(const kgv_tx_batch& v, std::vector<kgv_tx_result>& res) {
     std::vector<uint32_t> idx;

@@ -82,12 +82,14 @@ SYMBOLS = [
     ("kgv_utxo_muhash", _c.c_int, [_c.c_void_p, _c.c_void_p, _u8p]),
     ("kgv_script_execute", _c.c_int, [_c.c_void_p, _c.c_uint32, _c.c_uint32, _c.c_void_p, _c.c_void_p, _u8p]),
     ("kgv_check_scripts_host", _c.c_int, [_c.c_void_p, _c.c_void_p, _u8p, _c.c_size_t, _u8p]),
+    ("kgv_check_scripts", _c.c_int, [_c.c_void_p, _c.c_void_p, _u8p, _c.c_size_t, _u8p]),
     ("kgv_utxo_rows_encode", _c.c_int, [_u8p, _u8p, _u8p, _c.c_size_t, _c.c_size_t, _u8p, _u8p, _u8p, _u8p, _c.c_size_t, _c.c_size_t]),
     ("kgv_utxo_rows_decode", _c.c_int, [_u8p, _u8p, _u8p, _u8p, _c.c_size_t, _u8p, _u8p, _u8p, _c.c_size_t, _c.POINTER(_c.c_size_t)]),
     ("kgv_gtable_entry", _c.c_int, [_c.c_void_p, _c.c_int, _c.c_uint32, _u8p]),
     ("kgv_debug_selftest", _c.c_int, [_c.c_void_p, _c.c_int, _u8p, _u8p, _c.c_size_t]),
     ("kgv_debug_schnorr_trace", _c.c_int, [_c.c_void_p, _u8p, _u8p, _u8p, _u8p, _u8p]),
     ("kgv_debug_key_form", _c.c_int, [_c.c_void_p, _c.c_int, _c.c_void_p]),
+    ("kgv_debug_script_rounds", _c.c_int, [_c.c_void_p, _c.POINTER(_c.c_uint32)]),
 ]
 TRACE_STAGES = 32
 KEY_FORMS = ("no-cache", "inline", "plain", "comb")  # KGV_KEY_FORM_* in include/kgv.h

@@ -71,6 +71,7 @@ struct kgv_ctx {
   struct kgv_comm* shard_comm = nullptr;  // kgv_set_sharding: signature checks of the validation calls are split over its ranks
   std::vector<uint8_t*> parked;  // outgrown per-call buffers, released when the caller synchronises / destroys the context (kgv_reserve)
   uint64_t launches = 0;
+  uint32_t last_script_rounds = 0;  // verification rounds of the last device script engine run (kgv_debug_script_rounds)
   // the last non-indexed verify launch of each kind ([0] Schnorr, [1] ECDSA), for kgv_debug_key_form
   struct {
     size_t n = 0;
@@ -79,7 +80,7 @@ struct kgv_ctx {
     cudaStream_t stream = nullptr;
   } last_verify[2];
   int resident_blocks = 132 * KGV_BLOCKS_PER_SM;  // verification kernels: blocks that fit the device at once (persistent grid)
-  std::recursive_mutex mu;  // recursive: the host-VM resolution inside a validation call re-enters the ABI (kgv_sighash, kgv_*_verify)
+  std::recursive_mutex mu;  // recursive: an entry point may call others (kgv_check_scripts_host -> kgv_sighash, kgv_*_verify)
   std::string err;
 };
 
@@ -124,6 +125,19 @@ struct kgv_utxo_table;
 // call can newly occupy, b the long-script bytes it can append.  Returns at once when the policy is off; otherwise it may rehash the table
 // (KGV_ERR_NOMEM when that fails: the caller returns before writing anything).
 int utxo_reserve(kgv_ctx* ctx, kgv_utxo_table* t, uint64_t m, uint64_t b);
+// exclusive prefix sums of one (in1 == null) or two u32 arrays of n elements on st; totals[0] (and totals[1]) get the sums
+int kgv_scan_u32(kgv_ctx* ctx, const uint32_t* in0, uint32_t* out0, const uint32_t* in1, uint32_t* out1, size_t n, uint32_t* totals, cudaStream_t st);
+// the verification step of the script phase for n device-resident items (pk stride 33 for ECDSA, else 32; 32-byte messages, 64-byte
+// signatures -> KGV_SIG_* in st).  With a SigCache (sc) hits are answered from it and the misses verified and inserted; dig (32 B per item),
+// idx (4 B per item) and nm (one u32) are its scratch.
+int kgv_verify_items(kgv_ctx* ctx, struct kgv_sigcache* sc, const uint8_t* pk, const uint8_t* msg, const uint8_t* sig, size_t n, bool ecdsa, uint8_t* st,
+                     uint8_t* dig, uint32_t* idx, uint32_t* nm, cudaStream_t s);
+// check_scripts with the device script engine (kgv_scripts_dev.cu) for n_list transactions of a populated device batch view: dlist holds
+// their indices, or is null to take the transactions whose dres status is KGV_TX_NEEDS_HOST_VM.  patch: dres[tx] gets status / script_err /
+// fail_input (the fee stays); else dres[j] = the result of list entry j.  *rounds_out (may be null): verification rounds run.
+namespace kgv { struct BatchView; }
+int kgv_script_engine_run(kgv_ctx* ctx, const kgv::BatchView& v, size_t n_txs, const uint32_t* dlist, size_t n_list, kgv_tx_result* dres, bool patch,
+                          uint32_t* rounds_out);
 
 // ---- multi-GPU exchange used by the sharded script phase (kgv_comm.cu) ----
 // Every rank contributes `per` bytes at buf + rank * per (device memory, n_ranks * per bytes in all); on return (stream order)

@@ -713,20 +713,11 @@ extern "C" int kgv_replay_window(kgv_ctx* ctx, kgv_utxo_table* table, const kgv_
   CK(cudaMemcpyAsync(&n_vm, cnt + 1, 8, cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
   if (n_vm) {
-    // non-standard scripts: the host engine decides them on the entries the pre-check populated (kgv_host_vm_resolve)
-    rc = kgv_host_vm_resolve(ctx, batch, d, dent, pre);
+    // non-standard scripts: the device script engine decides them on the entries the pre-check populated
+    rc = kgv_script_engine_run(ctx, v, nt, nullptr, (size_t)n_vm, pre, true, nullptr);
     if (rc) return rc;
-    // the host engine's GPU rounds went through the batch staging buffer: stage the window again
-    const uint8_t* bytes_before = d.bytes;
-    rc = kgv_batch_to_device(ctx, batch, &d, false);
-    if (rc) return rc;
-    v = BatchView{d.txs, d.inputs, d.outputs, dent, d.bytes};
-    if (d.bytes != bytes_before) {  // window-sourced entries point at output scripts inside the staged batch
-      rc = find_sources();
-      if (rc) return rc;
-    }
   }
-  mark("host vm");
+  mark("script engine");
   if (stats) CK(cudaEventRecord(ctx->ev_time[1], st));
   // ---- the walk
   const ReplayRange* ranges = (const ReplayRange*)(R + o_rng);

@@ -310,6 +310,14 @@ __global__ void __launch_bounds__(1024) k_exclusive_scan2(const uint32_t* __rest
   if (threadIdx.x == 1023) totals[blockIdx.x] = part[1023];
 }
 
+// one array (in1 == null: one block) or two, for the other translation units
+int kgv_scan_u32(kgv_ctx* ctx, const uint32_t* in0, uint32_t* out0, const uint32_t* in1, uint32_t* out1, size_t n, uint32_t* totals, cudaStream_t st) {
+  k_exclusive_scan2<<<in1 ? 2 : 1, 1024, 0, st>>>(in0, out0, in1, out1, n, totals);
+  CK(cudaGetLastError());
+  ctx->launches++;
+  return KGV_OK;
+}
+
 struct ItemRef { uint32_t input; uint32_t k; };  // which input / which candidate pair
 
 __global__ void k_emit_items(BatchView b, size_t n_inputs, InputPlan* __restrict__ plans, const uint32_t* __restrict__ off_s, const uint32_t* __restrict__ off_e,
@@ -822,6 +830,17 @@ extern "C" int kgv_utxo_digest(kgv_ctx* ctx, kgv_utxo_table* t, uint8_t out32[32
   return KGV_OK;
 }
 
+// The verification step of a list of items on stream s: without a SigCache every item is verified; with one, hits are answered from the
+// table and only the misses are verified (and remembered).  dig / idx / nm: the cache's digests, miss list and miss count (unused without).
+int kgv_verify_items(kgv_ctx* ctx, kgv_sigcache* sc, const uint8_t* pk, const uint8_t* msg, const uint8_t* sig, size_t n, bool ecdsa, uint8_t* st, uint8_t* dig,
+                     uint32_t* idx, uint32_t* nm, cudaStream_t s) {
+  if (!sc) return kgv_launch_verify(ctx, pk, msg, sig, n, st, ecdsa, s);
+  int r = kgv_sigcache_lookup(ctx, sc, pk, msg, sig, n, ecdsa, st, dig, idx, nm, s);
+  if (!r) r = kgv_launch_verify(ctx, pk, msg, sig, n, st, ecdsa, s, idx, nm);
+  if (!r) r = kgv_sigcache_insert(ctx, sc, st, dig, idx, nm, n, s);
+  return r;
+}
+
 // The script phase of check_scripts (tx_validation_in_utxo_context.rs:162-200) for every transaction whose dres[].status is
 // KGV_TX_OK: plan -> scan -> emit -> sighash -> verify -> resolve -> finalize, all enqueued on ctx->stream (the ECDSA items on
 // the side stream).  v.entries must be populated.  Uses ctx->d_scratch (plans, counts, offsets, sub-hashes) and ctx->d_in
@@ -903,13 +922,9 @@ int kgv_scripts_phase(kgv_ctx* ctx, const BatchView& v, size_t nt, size_t ni, co
     CK(cudaGetLastError());
     ctx->launches++;
     STAGE(ecdsa ? "msgs ecdsa" : "msgs schnorr");
-    if (!sc) return kgv_launch_verify(ctx, I + k.pk + (ecdsa ? 33 : 32) * k.lo, I + k.msg + 32 * k.lo, I + k.sig + 64 * k.lo, m, I + k.st + k.lo, ecdsa, s);
-    // hits are answered from the table, only the misses are verified (and remembered)
-    uint32_t *idx = (uint32_t*)(I + k.idx), *nm = (uint32_t*)(I + k.nm);
-    int r = kgv_sigcache_lookup(ctx, sc, I + k.pk, I + k.msg, I + k.sig, k.n, ecdsa, I + k.st, I + k.dig, idx, nm, s);
-    if (!r) r = kgv_launch_verify(ctx, I + k.pk, I + k.msg, I + k.sig, k.n, I + k.st, ecdsa, s, idx, nm);
-    if (!r) r = kgv_sigcache_insert(ctx, sc, I + k.st, I + k.dig, idx, nm, k.n, s);
-    return r;
+    // (with the cache there is one rank: lo = 0, m = n)
+    return kgv_verify_items(ctx, sc, I + k.pk + (ecdsa ? 33 : 32) * k.lo, I + k.msg + 32 * k.lo, I + k.sig + 64 * k.lo, m, ecdsa, I + k.st + k.lo, I + k.dig,
+                            (uint32_t*)(I + k.idx), (uint32_t*)(I + k.nm), s);
   };
   if (ns && ne) CK(cudaEventRecord(ctx->ev_fork, st));  // fork point: everything both item kinds depend on is queued
   if (ns) {
@@ -945,112 +960,6 @@ int kgv_scripts_phase(kgv_ctx* ctx, const BatchView& v, size_t nt, size_t ni, co
   return KGV_OK;
 }
 
-// ---------------------------------------------------------------------------------------------
-// Non-standard scripts behind the table: the host script engine needs the populated entries, which only the library can
-// see.  For every transaction reported KGV_TX_NEEDS_HOST_VM the entries the device populated (dent) are gathered at their
-// TRUE script length (no stride, no truncation), a host-resident populated batch is assembled and kgv_check_scripts_host
-// decides (its signature checks go back to the GPU in batches).  `dres` is patched in place (device array of n_txs).
-// Rare path: a few synchronous copies.
-// ---------------------------------------------------------------------------------------------
-__global__ void k_gather_entry_meta(const DevEntry* __restrict__ dent, const uint32_t* __restrict__ list, uint32_t n, kgv_utxo_entry* __restrict__ out) {
-  uint32_t j = blockIdx.x * blockDim.x + threadIdx.x;
-  if (j >= n) return;
-  DevEntry d = dent[list[j]];
-  kgv_utxo_entry e;
-  memset(&e, 0, sizeof e);
-  e.amount = d.amount; e.block_daa_score = d.block_daa_score; e.script_len = d.found ? d.script_len : 0; e.spk_version = d.spk_version; e.is_coinbase = d.is_coinbase;
-  e.pad_[0] = d.found ? 0 : 1;
-  out[j] = e;
-}
-__global__ void k_gather_entry_scripts(const DevEntry* __restrict__ dent, const uint32_t* __restrict__ list, uint32_t n, const uint64_t* __restrict__ off,
-                                       uint8_t* __restrict__ out) {
-  uint32_t j = blockIdx.x;
-  if (j >= n) return;
-  DevEntry d = dent[list[j]];
-  if (!d.found) return;
-  for (uint32_t b = threadIdx.x; b < d.script_len; b += blockDim.x) out[off[j] + b] = d.script[b];
-}
-
-int kgv_host_vm_resolve(kgv_ctx* ctx, const kgv_tx_batch* batch, const kgv_dev_batch& d, const DevEntry* dent, kgv_tx_result* dres) {
-  const size_t nt = d.n_txs, ni = d.n_inputs;
-  cudaStream_t st = ctx->stream;
-  std::vector<kgv_tx_result> hres(nt);
-  CK(cudaMemcpyAsync(hres.data(), dres, nt * sizeof(kgv_tx_result), cudaMemcpyDeviceToHost, st));
-  CK(cudaStreamSynchronize(st));
-  std::vector<uint32_t> idx;
-  for (size_t i = 0; i < nt; i++) if (hres[i].status == KGV_TX_NEEDS_HOST_VM) idx.push_back((uint32_t)i);
-  if (idx.empty()) return KGV_OK;
-  // host copy of the batch
-  std::vector<kgv_tx> htx; std::vector<kgv_input> hin; std::vector<kgv_output> hout; std::vector<uint8_t> hby;
-  const kgv_tx* txs = batch->txs; const kgv_input* ins = batch->inputs; const kgv_output* outs = batch->outputs; const uint8_t* by = batch->bytes;
-  const void* probe = batch->n_txs ? (const void*)batch->txs : (const void*)batch->bytes;
-  if (probe && kgv_ptr_is_device(probe)) {
-    htx.resize(nt); hin.resize(ni); hout.resize(d.n_outputs); hby.resize(d.n_bytes);
-    CK(cudaMemcpyAsync(htx.data(), d.txs, nt * sizeof(kgv_tx), cudaMemcpyDeviceToHost, st));
-    if (ni) CK(cudaMemcpyAsync(hin.data(), d.inputs, ni * sizeof(kgv_input), cudaMemcpyDeviceToHost, st));
-    if (d.n_outputs) CK(cudaMemcpyAsync(hout.data(), d.outputs, d.n_outputs * sizeof(kgv_output), cudaMemcpyDeviceToHost, st));
-    if (d.n_bytes) CK(cudaMemcpyAsync(hby.data(), d.bytes, d.n_bytes, cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
-    txs = htx.data(); ins = hin.data(); outs = hout.data(); by = hby.data();
-  }
-  std::vector<uint32_t> list;
-  for (uint32_t ti : idx)
-    for (uint32_t k = 0; k < txs[ti].n_inputs; k++) list.push_back(txs[ti].first_input + k);
-  const size_t nl = list.size();
-  std::vector<kgv_utxo_entry> ents(ni);
-  for (auto& e : ents) { memset(&e, 0, sizeof e); e.pad_[0] = 1; }
-  std::vector<uint8_t> arena(by, by + d.n_bytes);
-  if (nl) {
-    size_t o_list = 0, o_meta = al256(nl * 4), o_off = al256(o_meta + nl * sizeof(kgv_utxo_entry));
-    int rc = kgv_reserve(ctx, &ctx->d_out, &ctx->d_out_cap, al256(o_off + nl * 8));
-    if (rc) return rc;
-    uint8_t* O = ctx->d_out;
-    CK(cudaMemcpyAsync(O + o_list, list.data(), nl * 4, cudaMemcpyHostToDevice, st));
-    k_gather_entry_meta<<<nblk(nl, 128), 128, 0, st>>>(dent, (const uint32_t*)(O + o_list), (uint32_t)nl, (kgv_utxo_entry*)(O + o_meta));
-    CK(cudaGetLastError());
-    ctx->launches++;
-    std::vector<kgv_utxo_entry> meta(nl);
-    CK(cudaMemcpyAsync(meta.data(), O + o_meta, nl * sizeof(kgv_utxo_entry), cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
-    std::vector<uint64_t> off(nl);
-    uint64_t run = 0;
-    for (size_t j = 0; j < nl; j++) { off[j] = run; run += (meta[j].script_len + 7u) & ~7u; }
-    if (d.n_bytes + run > 0xFFFFFFF0ull) { ctx->err = "populated scripts do not fit a 32-bit arena offset"; return KGV_ERR_ARG; }
-    std::vector<uint8_t> scripts(run + 8);
-    if (run) {
-      // d_scratch is free again at this point (the script phase of this call has completed)
-      rc = kgv_reserve(ctx, &ctx->d_scratch, &ctx->d_scratch_cap, run + 256);
-      if (rc) return rc;
-      CK(cudaMemcpyAsync(O + o_off, off.data(), nl * 8, cudaMemcpyHostToDevice, st));
-      k_gather_entry_scripts<<<(unsigned)nl, 64, 0, st>>>(dent, (const uint32_t*)(O + o_list), (uint32_t)nl, (const uint64_t*)(O + o_off), ctx->d_scratch);
-      CK(cudaGetLastError());
-      ctx->launches++;
-      CK(cudaMemcpyAsync(scripts.data(), ctx->d_scratch, run, cudaMemcpyDeviceToHost, st));
-      CK(cudaStreamSynchronize(st));
-    }
-    const size_t base = arena.size();
-    arena.insert(arena.end(), scripts.begin(), scripts.end());
-    for (size_t j = 0; j < nl; j++) {
-      kgv_utxo_entry e = meta[j];
-      e.script_off = (uint32_t)(base + off[j]);
-      ents[list[j]] = e;
-    }
-  }
-  // a transaction with an absent entry never reaches the script phase (MissingTxOutpoints comes first), so every listed entry is present
-  kgv_tx_batch hb;
-  hb.txs = txs; hb.n_txs = nt; hb.inputs = ins; hb.n_inputs = ni; hb.outputs = outs; hb.n_outputs = d.n_outputs; hb.entries = ents.data();
-  hb.bytes = arena.data(); hb.n_bytes = arena.size();
-  std::vector<kgv_tx_result> out(idx.size());
-  int rc = kgv_check_scripts_host(ctx, &hb, idx.data(), idx.size(), out.data());
-  if (rc) return rc;
-  for (size_t j = 0; j < idx.size(); j++) {
-    kgv_tx_result& r = hres[idx[j]];
-    r.status = out[j].status; r.script_err = out[j].script_err; r.fail_input = out[j].fail_input;
-  }
-  CK(cudaMemcpyAsync(dres, hres.data(), nt * sizeof(kgv_tx_result), cudaMemcpyHostToDevice, st));
-  CK(cudaStreamSynchronize(st));
-  return KGV_OK;
-}
 __global__ void k_count_status(const kgv_tx_result* __restrict__ res, uint32_t n, uint8_t what, unsigned long long* __restrict__ out) {
   uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
   bool hit = i < n && res[i].status == what;
@@ -1058,11 +967,10 @@ __global__ void k_count_status(const kgv_tx_result* __restrict__ res, uint32_t n
   if ((threadIdx.x & 31) == 0 && m) atomicAdd(out, (unsigned long long)__popc(m));
 }
 
-// The script phase of a validation call against a table (kgv_validate_txs, kgv_validate_mempool_txs), then the host script engine for what it
-// left undecided: utxo_validation.rs:282-309 accepts ANY transaction whose scripts execute successfully, so a non-standard spend must not leave
-// the call undecided, and only the library can read the entries it was populated with.
-static int scripts_with_host_vm(kgv_ctx* ctx, kgv_utxo_table* table, const kgv_tx_batch* batch, const kgv_dev_batch& d, const BatchView& v, const uint32_t* itx,
-                                kgv_tx_result* dres) {
+// The script phase of a validation call against a table (kgv_validate_txs, kgv_validate_mempool_txs), then the device script engine for what
+// it declined: utxo_validation.rs:282-309 accepts ANY transaction whose scripts execute successfully, so a non-standard spend must not leave
+// the call undecided.  The engine runs on the entries the call populated (v.entries), long scripts in the table's overflow arena included.
+static int scripts_with_engine(kgv_ctx* ctx, kgv_utxo_table* table, const kgv_dev_batch& d, const BatchView& v, const uint32_t* itx, kgv_tx_result* dres) {
   const size_t nt = d.n_txs;
   int rc = kgv_scripts_phase(ctx, v, nt, d.n_inputs, itx, dres, nullptr);
   if (rc) return rc;
@@ -1075,7 +983,7 @@ static int scripts_with_host_vm(kgv_ctx* ctx, kgv_utxo_table* table, const kgv_t
   ctx->launches++;
   CK(cudaMemcpyAsync(&n_vm, cnt, 8, cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
-  return n_vm ? kgv_host_vm_resolve(ctx, batch, d, v.entries, dres) : KGV_OK;
+  return n_vm ? kgv_script_engine_run(ctx, v, nt, nullptr, (size_t)n_vm, dres, true, nullptr) : KGV_OK;
 }
 
 // shared core of kgv_validate_populated / kgv_validate_txs
@@ -1115,7 +1023,7 @@ static int validate_core(kgv_ctx* ctx, kgv_utxo_table* table, const kgv_tx_batch
   ctx->launches++;
   STAGE("tx_context");
   if (flags != KGV_FLAGS_SKIP_SCRIPT_CHECKS && ni) {
-    rc = table ? scripts_with_host_vm(ctx, table, batch, d, v, itx, dres) : kgv_scripts_phase(ctx, v, nt, ni, itx, dres, nullptr);
+    rc = table ? scripts_with_engine(ctx, table, d, v, itx, dres) : kgv_scripts_phase(ctx, v, nt, ni, itx, dres, nullptr);
     if (rc) return rc;
   }
   if (kgv_ptr_is_device(results)) {
@@ -1142,8 +1050,8 @@ extern "C" int kgv_validate_txs(kgv_ctx* ctx, kgv_utxo_table* t, const kgv_tx_ba
 
 // validate_mempool_transaction_in_utxo_context for a batch (utxo_validation.rs:341-397): populate (caller's entries first), the mempool rule
 // order with the storage mass computed and the feerate threshold (k_tx_mempool_context), the final entries written out, then the script phase
-// of kgv_validate_txs.  The entries go out BEFORE the script phase: a caller entry's script points into the staged batch, which the host script
-// engine's own calls may restage.  One synchronisation before the script phase reads the script bytes and the zero-divisor count.
+// of kgv_validate_txs.  The entries go out BEFORE the script phase, so a too small scripts_out is reported before any signature is verified.
+// One synchronisation before the script phase reads the script bytes and the zero-divisor count.
 extern "C" int kgv_validate_mempool_txs(kgv_ctx* ctx, kgv_utxo_table* t, const kgv_tx_batch* batch, uint64_t virtual_daa_score, const kgv_params* prm,
                                         const kgv_mempool_tx_args* args, kgv_tx_result* results, uint64_t* storage_mass, kgv_utxo_entry* entries_out,
                                         uint8_t* scripts_out, size_t scripts_cap, size_t* scripts_used) {
@@ -1228,7 +1136,7 @@ extern "C" int kgv_validate_mempool_txs(kgv_ctx* ctx, kgv_utxo_table* t, const k
     }
   }
   if (ni) {
-    rc = scripts_with_host_vm(ctx, t, batch, d, v, itx, dres);
+    rc = scripts_with_engine(ctx, t, d, v, itx, dres);
     if (rc) return rc;
   }
   const cudaMemcpyKind k = dev ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost;

@@ -206,6 +206,20 @@ class TransactionValidator:
         results["fee"][idx] = fees
         return results
 
+    def check_scripts(self, batch, results):
+        """check_scripts with the full script engine ON THE GPU (kgv_check_scripts) for every tx whose status is NEEDS_HOST_VM; the same
+        results as check_scripts_host.  Updates `results` in place (the fee stays)."""
+        idx = np.nonzero(results["status"] == TX_NEEDS_HOST_VM)[0].astype(np.uint32)
+        if len(idx) == 0:
+            return results
+        out = np.zeros(len(idx), dtype=RESULT_DTYPE)
+        cb = _c_batch(batch, with_entries=True)
+        self.ctx._check(self._lib.kgv_check_scripts(self.ctx._h, ctypes.byref(cb), idx.ctypes.data, len(idx), out.ctypes.data))
+        fees = results["fee"][idx]
+        results[idx] = out
+        results["fee"][idx] = fees
+        return results
+
     def validate_mempool_transactions_in_parallel(self, utxo_set, batch, virtual_daa_score, flags=FLAGS_FULL):
         """consensus/src/pipeline/virtual_processor/processor.rs:853-878: the same UTXO-context validation run for a batch of
         mempool transactions against the virtual UTXO set; unlike the block path the per-transaction outcome is RETURNED
