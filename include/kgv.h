@@ -169,6 +169,26 @@ int kgv_sighash(kgv_ctx* ctx, const kgv_tx_batch* batch, const kgv_sighash_item*
                                            script engine must decide this transaction (all context checks passed) */
 #define KGV_TX_SKIPPED_COINBASE 12      /* coinbase transactions are skipped (utxo_validation.rs:273) */
 #define KGV_TX_FEERATE_TOO_LOW 13       /* FeerateTooLow (kgv_validate_mempool_txs only) */
+/* validate_tx_in_isolation (tx_validation_in_isolation.rs:16-26) and the lock-time finality of validate_tx_in_header_context
+ * (tx_validation_in_header_context.rs): kgv_validate_txs_in_isolation and kgv_validate_mempool_txs_in_parallel only */
+#define KGV_TX_NO_TX_INPUTS 14                         /* NoTxInputs                          */
+#define KGV_TX_TOO_MANY_INPUTS 15                      /* TooManyInputs                       */
+#define KGV_TX_TOO_BIG_SIGNATURE_SCRIPT 16             /* TooBigSignatureScript(fail_input)   */
+#define KGV_TX_TOO_MANY_OUTPUTS 17                     /* TooManyOutputs                      */
+#define KGV_TX_TOO_BIG_SCRIPT_PUBLIC_KEY 18            /* TooBigScriptPublicKey(output)       */
+#define KGV_TX_COINBASE_HAS_INPUTS 19                  /* CoinbaseHasInputs                   */
+#define KGV_TX_COINBASE_NON_ZERO_MASS_COMMITMENT 20    /* CoinbaseNonZeroMassCommitment       */
+#define KGV_TX_COINBASE_TOO_MANY_OUTPUTS 21            /* CoinbaseTooManyOutputs              */
+#define KGV_TX_COINBASE_SCRIPT_PUBLIC_KEY_TOO_LONG 22  /* CoinbaseScriptPublicKeyTooLong(output) */
+#define KGV_TX_TX_OUT_ZERO 23                          /* TxOutZero(output)                   */
+#define KGV_TX_TX_OUT_TOO_HIGH 24                      /* TxOutTooHigh(output)                */
+#define KGV_TX_OUTPUTS_VALUE_OVERFLOW 25               /* OutputsValueOverflow                */
+#define KGV_TX_TOTAL_TX_OUT_TOO_HIGH 26                /* TotalTxOutTooHigh                   */
+#define KGV_TX_DUPLICATE_INPUTS 27                     /* TxDuplicateInputs                   */
+#define KGV_TX_HAS_GAS 28                              /* TxHasGas                            */
+#define KGV_TX_SUBNETWORKS_DISABLED 29                 /* SubnetworksDisabled                 */
+#define KGV_TX_UNKNOWN_TX_VERSION 30                   /* UnknownTxVersion                    */
+#define KGV_TX_NOT_FINALIZED 31                        /* NotFinalized(fail_input)            */
 /* script errors = TxScriptError variants the standard classes can produce (crypto/txscript/errors) */
 #define KGV_SCRIPT_OK 0
 #define KGV_SCRIPT_EVAL_FALSE 1
@@ -196,7 +216,8 @@ typedef struct {
 } kgv_params;
 typedef struct {
   uint64_t fee;        /* calculated_fee (valid when status == KGV_TX_OK) */
-  uint32_t fail_input; /* first failing input (index within the tx) for status 2, 9, 10, 11 */
+  uint32_t fail_input; /* first failing input (index within the tx) for status 2, 9, 10, 11, 16, 31; the first failing OUTPUT (index
+                          within the tx) for status 18, 22, 23, 24 */
   uint8_t status;      /* KGV_TX_*     */
   uint8_t script_err;  /* KGV_SCRIPT_* */
   uint8_t pad_[2];
@@ -328,6 +349,49 @@ typedef struct {
 int kgv_validate_mempool_txs(kgv_ctx* ctx, kgv_utxo_table* virtual_view, const kgv_tx_batch* batch, uint64_t virtual_daa_score, const kgv_params* params,
                              const kgv_mempool_tx_args* args, kgv_tx_result* results, uint64_t* storage_mass, kgv_utxo_entry* entries_out,
                              uint8_t* scripts_out, size_t scripts_cap, size_t* scripts_used);
+
+/* The per-transaction rules that need no UTXO context: validate_tx_in_isolation (tx_validation_in_isolation.rs:16-26), the lock-time
+ * finality of validate_tx_in_header_context_with_args (tx_validation_in_header_context.rs) and calc_non_contextual_masses
+ * (consensus/core/src/mass/mod.rs:248-269).  The fields are the reference's Params of the same names (kgv_params is frozen). */
+typedef struct {
+  uint64_t max_tx_inputs;
+  uint64_t max_tx_outputs;
+  uint64_t max_signature_script_len;
+  uint64_t max_script_public_key_len;
+  uint64_t mass_per_tx_byte;
+  uint64_t mass_per_script_pub_key_byte;
+  uint64_t mass_per_sig_op;
+  uint64_t ghostdag_k;                                 /* a coinbase may have ghostdag_k + 2 outputs */
+  uint64_t coinbase_payload_script_public_key_max_len;
+} kgv_tx_rules; /* 72 bytes */
+typedef struct {
+  uint64_t compute_mass;   /* NonContextualMasses::compute_mass   */
+  uint64_t transient_mass; /* NonContextualMasses::transient_mass */
+} kgv_tx_masses; /* 16 bytes */
+#define KGV_ISOLATION_SKIP_FINALITY 1u /* run validate_tx_in_isolation alone */
+
+/* validate_tx_in_isolation then validate_tx_in_header_context_with_args(tx, ctx_daa_score, ctx_past_median_time) for every tx of a batch
+ * (batch->entries is not read).  The checks run in the reference's order and the first failing one gives the status (KGV_TX_OK or 14..31),
+ * with fail_input set for the indexed variants; fee and script_err are 0.  A tx is a coinbase when its subnetwork_id is the coinbase
+ * subnetwork id (kgv_tx.flags is not read).  MAX_SOMPI and LOCK_TIME_THRESHOLD are the consensus constants.  Finality: lock_time 0 is
+ * final; a lock_time below 500 000 000 000 is compared with ctx_daa_score, any other with ctx_past_median_time; lock_time < that value is
+ * final; otherwise the first input whose sequence is not u64::MAX gives KGV_TX_NOT_FINALIZED.  flags: KGV_ISOLATION_SKIP_FINALITY or 0.
+ * results: n_txs records.  masses (may be NULL): n_txs calc_non_contextual_masses records, computed for every tx whatever its status, in
+ * wrapping u64 arithmetic ((0, 0) for a coinbase).  Every data pointer host or every one device. */
+int kgv_validate_txs_in_isolation(kgv_ctx* ctx, const kgv_tx_batch* batch, const kgv_tx_rules* rules, uint64_t ctx_daa_score, uint64_t ctx_past_median_time,
+                                  uint32_t flags, kgv_tx_result* results, kgv_tx_masses* masses);
+
+/* validate_mempool_transactions_in_parallel (processor.rs:853-878): per tx, what validate_mempool_transaction_impl (:823-839) does -
+ * kgv_validate_txs_in_isolation's checks with (virtual_daa_score, virtual_past_median_time), then kgv_validate_mempool_txs.  A tx that
+ * fails isolation or finality gets that status, storage_mass 0, and is never looked up: its entries_out rows are the caller's entries
+ * where batch->entries supplies them and absent-marked otherwise; it reaches neither the context rules nor the scripts nor the SigCache.
+ * The feerate divisor is max(storage mass, compute mass, transient mass) with the masses computed here (what the mempool stores in
+ * calculated_non_contextual_masses before it validates): args[i].non_contextual_mass is IGNORED, only feerate_threshold is read.
+ * masses (may be NULL): n_txs records as in kgv_validate_txs_in_isolation.  Everything else as kgv_validate_mempool_txs. */
+int kgv_validate_mempool_txs_in_parallel(kgv_ctx* ctx, kgv_utxo_table* virtual_view, const kgv_tx_batch* batch, uint64_t virtual_daa_score,
+                                         uint64_t virtual_past_median_time, const kgv_params* params, const kgv_tx_rules* rules,
+                                         const kgv_mempool_tx_args* args, kgv_tx_result* results, uint64_t* storage_mass, kgv_tx_masses* masses,
+                                         kgv_utxo_entry* entries_out, uint8_t* scripts_out, size_t scripts_cap, size_t* scripts_used);
 
 /* ------------------------------------------------------------------------------------------------
  * SigCache: Cache<SigCacheKey, bool> (crypto/txscript/src/caches.rs:14-55; consulted at crypto/txscript/src/lib.rs:589-603, 624-638;

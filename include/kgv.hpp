@@ -443,6 +443,10 @@ struct Params {
   uint64_t coinbase_maturity = 100, storage_mass_parameter = 1000000000000ull, max_sompi = 2900000000000000000ull;  // consensus/core/src/config/params.rs, constants.rs
 };
 enum class TxValidationFlags : uint32_t { Full = KGV_FLAGS_FULL, SkipScriptChecks = KGV_FLAGS_SKIP_SCRIPT_CHECKS, SkipMassCheck = KGV_FLAGS_SKIP_MASS_CHECK };
+// parameters of the isolation rules and the non-contextual masses: mainnet's (MAINNET_PARAMS, consensus/core/src/config/params.rs; ghostdag_k of 10 BPS)
+struct TxRules : kgv_tx_rules {
+  TxRules() : kgv_tx_rules{1000, 1000, 10000, 10000, 1, 10, 1000, 124, 150} {}
+};
 
 class TransactionValidator {
  public:
@@ -537,6 +541,57 @@ class TransactionValidator {
     };
     int rc = call();
     if (rc == KGV_ERR_NOMEM && used > scripts.size()) {  // reported before any signature is verified
+      scripts.resize(used);
+      rc = call();
+    }
+    c_.check(rc);
+    out.entries.resize(b.n_inputs());
+    for (size_t i = 0; i < b.n_inputs(); i++) {
+      if (ent[i].pad_[0]) continue;
+      UtxoEntry& e = out.entries[i].second;
+      out.entries[i].first = true;
+      e.amount = ent[i].amount; e.block_daa_score = ent[i].block_daa_score; e.is_coinbase = ent[i].is_coinbase != 0;
+      e.script_public_key.version = ent[i].spk_version;
+      e.script_public_key.script.assign(scripts.begin() + ent[i].script_off, scripts.begin() + ent[i].script_off + ent[i].script_len);
+    }
+    return out;
+  }
+  // validate_tx_in_isolation, then (finality) validate_tx_in_header_context_with_args(tx, ctx_daa_score, ctx_past_median_time), for every
+  // transaction of the batch (kgv_validate_txs_in_isolation); masses receives calc_non_contextual_masses of each when given
+  std::vector<kgv_tx_result> validate_tx_in_isolation(const TxBatch& b, const TxRules& rules = TxRules(), uint64_t ctx_daa_score = 0,
+                                                      uint64_t ctx_past_median_time = 0, bool finality = true, std::vector<kgv_tx_masses>* masses = nullptr) {
+    std::vector<kgv_tx_result> res(b.len());
+    if (masses) masses->assign(b.len(), kgv_tx_masses{});
+    kgv_tx_batch v = b.view(false);
+    c_.check(kgv_validate_txs_in_isolation(c_.get(), &v, &rules, ctx_daa_score, ctx_past_median_time, finality ? 0u : KGV_ISOLATION_SKIP_FINALITY, res.data(),
+                                           masses ? masses->data() : nullptr));
+    return res;
+  }
+  // validate_mempool_transactions_in_parallel (processor.rs:853-878; kgv_validate_mempool_txs_in_parallel): per transaction isolation,
+  // finality, then validate_mempool_transactions_in_utxo_context.  Only args[i].feerate_threshold is read: the feerate divisor uses the
+  // non-contextual masses computed in the call, returned in `masses`.
+  struct FullMempoolValidation : MempoolValidation {
+    std::vector<kgv_tx_masses> masses;
+  };
+  FullMempoolValidation validate_mempool_transactions_in_parallel_full(UtxoSet& virtual_utxo_view, const TxBatch& b, uint64_t virtual_daa_score,
+                                                                       uint64_t virtual_past_median_time, const TxRules& rules = TxRules(),
+                                                                       const std::vector<kgv_mempool_tx_args>& args = {}) {
+    if (!args.empty() && args.size() != b.len()) throw Error(KGV_ERR_ARG, "kgv: one kgv_mempool_tx_args per transaction");
+    FullMempoolValidation out;
+    out.results.resize(b.len());
+    out.storage_mass.resize(b.len());
+    out.masses.resize(b.len());
+    std::vector<kgv_utxo_entry> ent(b.n_inputs() + 1);
+    kgv_tx_batch v = b.view(true);
+    size_t used = 0;
+    std::vector<uint8_t> scripts(v.n_bytes + 128 * b.n_inputs() + 8);
+    auto call = [&] {
+      return kgv_validate_mempool_txs_in_parallel(c_.get(), virtual_utxo_view.get(), &v, virtual_daa_score, virtual_past_median_time, &p_, &rules,
+                                                  args.empty() ? nullptr : args.data(), out.results.data(), out.storage_mass.data(), out.masses.data(), ent.data(),
+                                                  scripts.data(), scripts.size(), &used);
+    };
+    int rc = call();
+    if (rc == KGV_ERR_NOMEM && used > scripts.size()) {
       scripts.resize(used);
       rc = call();
     }

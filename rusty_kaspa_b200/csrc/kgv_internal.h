@@ -139,6 +139,12 @@ namespace kgv { struct BatchView; }
 int kgv_script_engine_run(kgv_ctx* ctx, const kgv::BatchView& v, size_t n_txs, const uint32_t* dlist, size_t n_list, kgv_tx_result* dres, bool patch,
                           uint32_t* rounds_out);
 
+// ---- isolation rules, finality and non-contextual masses (kgv_isolation.cu) ----
+// Enqueues on st, for every tx of a device batch: dres = the first failing isolation / finality rule (finality == false skips it),
+// dmasses = calc_non_contextual_masses and dnc = max(compute, transient) (either may be null).  dlist: scratch of n_txs + 1 u32.
+int kgv_isolation_run(kgv_ctx* ctx, const kgv_dev_batch& d, const kgv_tx_rules& rules, uint64_t daa, uint64_t pmt, bool finality, kgv_tx_result* dres,
+                      kgv_tx_masses* dmasses, uint64_t* dnc, uint32_t* dlist, cudaStream_t st);
+
 // ---- multi-GPU exchange used by the sharded script phase (kgv_comm.cu) ----
 // Every rank contributes `per` bytes at buf + rank * per (device memory, n_ranks * per bytes in all); on return (stream order)
 // buf holds all ranks' contributions.  Peer transport if the communicator is connected, else NCCL (in place).

@@ -200,8 +200,10 @@ __global__ void k_tx_context(BatchView b, uint32_t n_txs, uint64_t pov, uint32_t
 // populate_mempool_transaction_in_utxo_context (utxo_validation.rs:341-363): an entry the caller supplies (given[i].pad_[0] == 0; its script in
 // the batch arena) is kept, every other input is looked up.  len[i] = script bytes of the final entry (0 when absent); *total = their sum in
 // 64 bits (the 32-bit offsets of the scan are only used when it fits).  Launched with whole warps: every lane reaches the reduction.
+// gate (may be null): the isolation verdicts; an input of a transaction that failed them is never looked up (absent unless supplied).
 __global__ void k_populate_mempool(TableView t, const kgv_input* __restrict__ inputs, const kgv_utxo_entry* __restrict__ given, const uint8_t* __restrict__ bytes,
-                                   size_t n, DevEntry* __restrict__ out, uint32_t* __restrict__ len, unsigned long long* __restrict__ total) {
+                                   size_t n, DevEntry* __restrict__ out, uint32_t* __restrict__ len, unsigned long long* __restrict__ total,
+                                   const kgv_tx_result* __restrict__ gate, const uint32_t* __restrict__ input_tx) {
   size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   unsigned long long l = 0;
   if (i < n) {
@@ -210,6 +212,8 @@ __global__ void k_populate_mempool(TableView t, const kgv_input* __restrict__ in
       const kgv_utxo_entry e = given[i];
       d.amount = e.amount; d.block_daa_score = e.block_daa_score; d.script = bytes + e.script_off; d.script_len = e.script_len;
       d.spk_version = e.spk_version; d.is_coinbase = e.is_coinbase; d.found = 1;
+    } else if (gate && gate[input_tx[i]].status != KGV_TX_OK) {
+      entry_absent(d);
     } else {
       uint32_t k[9];
       input_key(k, inputs[i]);
@@ -227,14 +231,19 @@ __global__ void k_populate_mempool(TableView t, const kgv_input* __restrict__ in
   if ((threadIdx.x & 31) == 0 && l) atomicAdd(total, l);
 }
 
-// the context rules of a mempool batch (mempool_context_rules); *bad counts thresholds with a zero divisor
+// the context rules of a mempool batch (mempool_context_rules); *bad counts thresholds with a zero divisor.  gate (may be null): a
+// transaction that failed isolation or finality keeps that verdict and a storage mass of 0; nc_mass (may be null) replaces the
+// caller's args[ti].non_contextual_mass.
 __global__ void k_tx_mempool_context(BatchView b, uint32_t n_txs, uint64_t pov, kgv_params prm, const kgv_mempool_tx_args* __restrict__ args,
-                                     kgv_tx_result* __restrict__ res, uint64_t* __restrict__ mass, unsigned long long* __restrict__ bad) {
+                                     kgv_tx_result* __restrict__ res, uint64_t* __restrict__ mass, unsigned long long* __restrict__ bad,
+                                     const kgv_tx_result* __restrict__ gate, const uint64_t* __restrict__ nc_mass) {
   uint32_t ti = blockIdx.x * blockDim.x + threadIdx.x;
   if (ti >= n_txs) return;
+  if (gate && gate[ti].status != KGV_TX_OK) { res[ti] = gate[ti]; mass[ti] = 0; return; }
   double thr = __longlong_as_double(0x7FF8000000000000ll);  // NaN: no threshold
   uint64_t nc = 0;
   if (args) { thr = args[ti].feerate_threshold; nc = args[ti].non_contextual_mass; }
+  if (nc_mass) nc = nc_mass[ti];
   uint64_t m;
   bool bad_thr;
   res[ti] = mempool_context_rules(b, ti, pov, prm, thr, nc, m, bad_thr);
@@ -1052,17 +1061,27 @@ extern "C" int kgv_validate_txs(kgv_ctx* ctx, kgv_utxo_table* t, const kgv_tx_ba
 // order with the storage mass computed and the feerate threshold (k_tx_mempool_context), the final entries written out, then the script phase
 // of kgv_validate_txs.  The entries go out BEFORE the script phase, so a too small scripts_out is reported before any signature is verified.
 // One synchronisation before the script phase reads the script bytes and the zero-divisor count.
-extern "C" int kgv_validate_mempool_txs(kgv_ctx* ctx, kgv_utxo_table* t, const kgv_tx_batch* batch, uint64_t virtual_daa_score, const kgv_params* prm,
-                                        const kgv_mempool_tx_args* args, kgv_tx_result* results, uint64_t* storage_mass, kgv_utxo_entry* entries_out,
-                                        uint8_t* scripts_out, size_t scripts_cap, size_t* scripts_used) {
-  if (!ctx || !t) return KGV_ERR_ARG;
-  std::lock_guard<std::recursive_mutex> g(ctx->mu);
+// iso (kgv_validate_mempool_txs_in_parallel): the isolation and finality rules run first, on the device; their verdicts gate the lookups
+// and the context rules, and their masses replace args[i].non_contextual_mass.  iso == null is kgv_validate_mempool_txs.
+struct MempoolIso {
+  const kgv_tx_rules* rules;
+  uint64_t past_median_time;
+  kgv_tx_masses* masses;  // caller's output, may be null
+};
+static int mempool_core(kgv_ctx* ctx, kgv_utxo_table* t, const kgv_tx_batch* batch, uint64_t virtual_daa_score, const kgv_params* prm,
+                        const kgv_mempool_tx_args* args, kgv_tx_result* results, uint64_t* storage_mass, kgv_utxo_entry* entries_out,
+                        uint8_t* scripts_out, size_t scripts_cap, size_t* scripts_used, const MempoolIso* iso) {
   if (scripts_used) *scripts_used = 0;
-  if (!batch || !prm || (batch->n_txs && (!results || !storage_mass)) || (entries_out && scripts_cap && !scripts_out)) { ctx->err = "null argument"; return KGV_ERR_ARG; }
+  if (!batch || !prm || (batch->n_txs && (!results || !storage_mass)) || (entries_out && scripts_cap && !scripts_out) || (iso && !iso->rules)) {
+    ctx->err = "null argument";
+    return KGV_ERR_ARG;
+  }
   if (batch->n_txs == 0) return KGV_OK;
+  if (iso && batch->n_txs > 0xFFFFFFFFull) { ctx->err = "kgv_validate_mempool_txs_in_parallel: more than 2^32 - 1 transactions"; return KGV_ERR_ARG; }
   CK(cudaSetDevice(ctx->device));
   const bool dev = kgv_ptr_is_device(results) != 0;
-  for (const void* p : {(const void*)batch->txs, (const void*)args, (const void*)storage_mass, (const void*)entries_out, (const void*)(scripts_cap ? scripts_out : nullptr)})
+  for (const void* p : {(const void*)batch->txs, (const void*)args, (const void*)storage_mass, (const void*)entries_out, (const void*)(scripts_cap ? scripts_out : nullptr),
+                        (const void*)(iso ? iso->masses : nullptr)})
     if (p && (kgv_ptr_is_device(p) != 0) != dev) { ctx->err = "kgv_validate_mempool_txs: the batch, args and outputs must all be host or all be device pointers"; return KGV_ERR_ARG; }
   kgv_dev_batch d;
   int rc = kgv_batch_to_device(ctx, batch, &d, false);
@@ -1078,7 +1097,12 @@ extern "C" int kgv_validate_mempool_txs(kgv_ctx* ctx, kgv_utxo_table* t, const k
   size_t o_off = al256(o_len + ni * 4);
   size_t o_args = al256(o_off + ni * 4);
   size_t o_cnt = al256(o_args + (args ? nt * sizeof(kgv_mempool_tx_args) : 0));
-  rc = kgv_reserve(ctx, &ctx->d_work, &ctx->d_work_cap, al256(o_cnt + 32));
+  // with iso: its verdicts, max(compute, transient) per tx, the masses for a host caller, the large-transaction list
+  size_t o_iso = al256(o_cnt + 32);
+  size_t o_nc = al256(o_iso + (iso ? nt * sizeof(kgv_tx_result) : 0));
+  size_t o_ism = al256(o_nc + (iso ? nt * 8 : 0));
+  size_t o_lst = al256(o_ism + (iso && iso->masses && !dev ? nt * sizeof(kgv_tx_masses) : 0));
+  rc = kgv_reserve(ctx, &ctx->d_work, &ctx->d_work_cap, iso ? al256(o_lst + (nt + 1) * 4) : al256(o_cnt + 32));
   if (rc) return rc;
   uint8_t* S = ctx->d_work;
   DevEntry* dent = (DevEntry*)(S + o_ent);
@@ -1093,10 +1117,21 @@ extern "C" int kgv_validate_mempool_txs(kgv_ctx* ctx, kgv_utxo_table* t, const k
     dargs = (const kgv_mempool_tx_args*)(S + o_args);
   }
   CK(cudaMemsetAsync(cnt, 0, 32, st));
+  kgv_tx_result* gate = nullptr;
+  uint64_t* dnc = nullptr;
+  kgv_tx_masses* dism = nullptr;
+  if (iso) {
+    gate = (kgv_tx_result*)(S + o_iso);
+    dnc = (uint64_t*)(S + o_nc);
+    dism = dev ? iso->masses : (iso->masses ? (kgv_tx_masses*)(S + o_ism) : nullptr);
+    rc = kgv_isolation_run(ctx, d, *iso->rules, virtual_daa_score, iso->past_median_time, true, gate, dism, dnc, (uint32_t*)(S + o_lst), st);
+    if (rc) return rc;
+    STAGE("isolation");
+  }
   if (ni) {
-    k_populate_mempool<<<nblk(ni, 128), 128, 0, st>>>(view_of(t), d.inputs, d.entries, d.bytes, ni, dent, len, cnt);
-    CK(cudaGetLastError());
     k_input_tx_index<<<nblk(nt, 128), 128, 0, st>>>(d.txs, (uint32_t)nt, itx);
+    CK(cudaGetLastError());
+    k_populate_mempool<<<nblk(ni, 128), 128, 0, st>>>(view_of(t), d.inputs, d.entries, d.bytes, ni, dent, len, cnt, gate, itx);
     CK(cudaGetLastError());
     k_exclusive_scan2<<<1, 1024, 0, st>>>(len, off, nullptr, nullptr, ni, (uint32_t*)(cnt + 2));  // block 0 only: one array
     CK(cudaGetLastError());
@@ -1104,7 +1139,7 @@ extern "C" int kgv_validate_mempool_txs(kgv_ctx* ctx, kgv_utxo_table* t, const k
   }
   STAGE("populate");
   BatchView v{d.txs, d.inputs, d.outputs, dent, d.bytes};
-  k_tx_mempool_context<<<nblk(nt, 128), 128, 0, st>>>(v, (uint32_t)nt, virtual_daa_score, *prm, dargs, dres, dmass, cnt + 1);
+  k_tx_mempool_context<<<nblk(nt, 128), 128, 0, st>>>(v, (uint32_t)nt, virtual_daa_score, *prm, dargs, dres, dmass, cnt + 1, gate, dnc);
   CK(cudaGetLastError());
   ctx->launches++;
   STAGE("mempool context");
@@ -1142,8 +1177,28 @@ extern "C" int kgv_validate_mempool_txs(kgv_ctx* ctx, kgv_utxo_table* t, const k
   const cudaMemcpyKind k = dev ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost;
   CK(cudaMemcpyAsync(results, dres, nt * sizeof(kgv_tx_result), k, st));
   CK(cudaMemcpyAsync(storage_mass, dmass, nt * 8, k, st));
+  if (dism && !dev) CK(cudaMemcpyAsync(iso->masses, dism, nt * sizeof(kgv_tx_masses), k, st));
   if (!dev) CK(cudaStreamSynchronize(st));
   return KGV_OK;
+}
+
+extern "C" int kgv_validate_mempool_txs(kgv_ctx* ctx, kgv_utxo_table* t, const kgv_tx_batch* batch, uint64_t virtual_daa_score, const kgv_params* prm,
+                                        const kgv_mempool_tx_args* args, kgv_tx_result* results, uint64_t* storage_mass, kgv_utxo_entry* entries_out,
+                                        uint8_t* scripts_out, size_t scripts_cap, size_t* scripts_used) {
+  if (!ctx || !t) return KGV_ERR_ARG;
+  std::lock_guard<std::recursive_mutex> g(ctx->mu);
+  return mempool_core(ctx, t, batch, virtual_daa_score, prm, args, results, storage_mass, entries_out, scripts_out, scripts_cap, scripts_used, nullptr);
+}
+
+// validate_mempool_transaction_impl (processor.rs:823-839) for a batch: isolation -> finality -> the UTXO-context pipeline above
+extern "C" int kgv_validate_mempool_txs_in_parallel(kgv_ctx* ctx, kgv_utxo_table* t, const kgv_tx_batch* batch, uint64_t virtual_daa_score,
+                                                    uint64_t virtual_past_median_time, const kgv_params* prm, const kgv_tx_rules* rules,
+                                                    const kgv_mempool_tx_args* args, kgv_tx_result* results, uint64_t* storage_mass, kgv_tx_masses* masses,
+                                                    kgv_utxo_entry* entries_out, uint8_t* scripts_out, size_t scripts_cap, size_t* scripts_used) {
+  if (!ctx || !t) return KGV_ERR_ARG;
+  std::lock_guard<std::recursive_mutex> g(ctx->mu);
+  const MempoolIso iso{rules, virtual_past_median_time, masses};
+  return mempool_core(ctx, t, batch, virtual_daa_score, prm, args, results, storage_mass, entries_out, scripts_out, scripts_cap, scripts_used, &iso);
 }
 
 extern "C" int kgv_utxo_apply_accepted(kgv_ctx* ctx, kgv_utxo_table* t, const kgv_tx_batch* batch, const uint8_t* accept, uint64_t pov_daa_score) {

@@ -8,6 +8,10 @@
         (consensus/src/pipeline/virtual_processor/utxo_validation.rs:262-278)
     TransactionValidator.validate_mempool_transactions_in_utxo_context  <->  validate_mempool_transaction_in_utxo_context
         (utxo_validation.rs:341-397), for a batch
+    TransactionValidator.validate_txs_in_isolation           <->  validate_tx_in_isolation + validate_tx_in_header_context_with_args
+        (tx_validation_in_isolation.rs:16-26, tx_validation_in_header_context.rs) and calc_non_contextual_masses (mass/mod.rs:248-269)
+    TransactionValidator.validate_mempool_transactions_in_parallel_full  <->  validate_mempool_transactions_in_parallel
+        (processor.rs:853-878): isolation -> finality -> UTXO context, per transaction
     GpuUtxoSet.add_transactions                              <->  UtxoDiff::add_transaction (utxo_diff.rs:233-247)
 """
 import ctypes
@@ -22,6 +26,15 @@ RESULT_DTYPE = np.dtype([("fee", "<u8"), ("fail_input", "<u4"), ("status", "u1")
 assert RESULT_DTYPE.itemsize == 16
 MEMPOOL_ARGS_DTYPE = np.dtype([("feerate_threshold", "<f8"), ("non_contextual_mass", "<u8")])  # kgv_mempool_tx_args
 assert MEMPOOL_ARGS_DTYPE.itemsize == 16
+TX_MASSES_DTYPE = np.dtype([("compute_mass", "<u8"), ("transient_mass", "<u8")])  # kgv_tx_masses
+assert TX_MASSES_DTYPE.itemsize == 16
+ISOLATION_SKIP_FINALITY = 1
+# KGV_TX_* verdicts of the isolation and finality rules (include/kgv.h), by the reference's TxRuleError names
+ISOLATION_STATUS = {14: "NoTxInputs", 15: "TooManyInputs", 16: "TooBigSignatureScript", 17: "TooManyOutputs", 18: "TooBigScriptPublicKey",
+                    19: "CoinbaseHasInputs", 20: "CoinbaseNonZeroMassCommitment", 21: "CoinbaseTooManyOutputs",
+                    22: "CoinbaseScriptPublicKeyTooLong", 23: "TxOutZero", 24: "TxOutTooHigh", 25: "OutputsValueOverflow",
+                    26: "TotalTxOutTooHigh", 27: "TxDuplicateInputs", 28: "TxHasGas", 29: "SubnetworksDisabled", 30: "UnknownTxVersion",
+                    31: "NotFinalized"}
 
 FLAGS_FULL, FLAGS_SKIP_SCRIPT_CHECKS, FLAGS_SKIP_MASS_CHECK, FLAGS_SCRIPTS_ONLY = 0, 1, 2, 3
 MAX_SOMPI = 29_000_000_000 * 100_000_000
@@ -35,6 +48,25 @@ class Params(ctypes.Structure):
 
     def __init__(self, coinbase_maturity=100, storage_mass_parameter=10**12, max_sompi=MAX_SOMPI):
         super().__init__(coinbase_maturity, storage_mass_parameter, max_sompi)
+
+
+class TxRules(ctypes.Structure):
+    """kgv_tx_rules: the parameters of the isolation rules and the non-contextual masses.  The defaults are mainnet's
+    (MAINNET_PARAMS, consensus/core/src/config/params.rs; ghostdag_k of the 10 BPS blockrate)."""
+    _fields_ = [(n, ctypes.c_uint64) for n in ("max_tx_inputs", "max_tx_outputs", "max_signature_script_len", "max_script_public_key_len",
+                                               "mass_per_tx_byte", "mass_per_script_pub_key_byte", "mass_per_sig_op", "ghostdag_k",
+                                               "coinbase_payload_script_public_key_max_len")]
+    MAINNET = dict(max_tx_inputs=1000, max_tx_outputs=1000, max_signature_script_len=10_000, max_script_public_key_len=10_000, mass_per_tx_byte=1,
+                   mass_per_script_pub_key_byte=10, mass_per_sig_op=1000, ghostdag_k=124, coinbase_payload_script_public_key_max_len=150)
+
+    def __init__(self, **overrides):
+        unknown = set(overrides) - set(self.MAINNET)
+        if unknown:
+            raise TypeError("unknown rule parameters: %s" % sorted(unknown))
+        super().__init__(**{**self.MAINNET, **overrides})
+
+
+assert ctypes.sizeof(TxRules) == 72
 
 
 class SigRequest(ctypes.Structure):
@@ -265,6 +297,54 @@ class TransactionValidator:
             cap = used.value
         self.ctx._check(rc)
         return res, mass, ent[:ni], arena[:used.value]
+
+    def validate_txs_in_isolation(self, batch, rules=None, ctx_daa_score=0, ctx_past_median_time=0, finality=True):
+        """validate_tx_in_isolation, then (finality=True) the lock-time finality of validate_tx_in_header_context_with_args, for every tx of
+        the batch (kgv_validate_txs_in_isolation).  Returns (RESULT_DTYPE[n_txs]: status 0 or 14..31, fail_input for the indexed
+        variants; TX_MASSES_DTYPE[n_txs]: calc_non_contextual_masses of every tx)."""
+        rules = rules or TxRules()
+        res = np.zeros(batch.n_txs, dtype=RESULT_DTYPE)
+        masses = np.zeros(batch.n_txs, dtype=TX_MASSES_DTYPE)
+        cb = _c_batch(batch, with_entries=False)
+        self.ctx._check(self._lib.kgv_validate_txs_in_isolation(self.ctx._h, ctypes.byref(cb), ctypes.byref(rules), int(ctx_daa_score), int(ctx_past_median_time),
+                                                                0 if finality else ISOLATION_SKIP_FINALITY, res.ctypes.data, masses.ctypes.data))
+        return res, masses
+
+    def validate_mempool_transactions_in_parallel_full(self, utxo_set, batch, virtual_daa_score, virtual_past_median_time, rules=None,
+                                                       feerate_threshold=None, supplied=None):
+        """validate_mempool_transactions_in_parallel (processor.rs:853-878) through kgv_validate_mempool_txs_in_parallel: per tx, the
+        isolation rules, lock-time finality, then validate_mempool_transactions_in_utxo_context.  A tx rejected by the first two is never
+        looked up and gets storage mass 0.  The feerate divisor uses the non-contextual masses computed on the device.  `supplied` and
+        `feerate_threshold` as in validate_mempool_transactions_in_utxo_context.  Returns (RESULT_DTYPE[n_txs], storage masses u64[n_txs],
+        TX_MASSES_DTYPE[n_txs], every input's final entry ENTRY_DTYPE[n_inputs], the byte arena of their scripts)."""
+        rules = rules or TxRules()
+        n, ni = batch.n_txs, batch.n_inputs
+        if supplied is not None:
+            given = batch.entries.copy()
+            given["pad_"][:, 0] = np.where(np.asarray(supplied, dtype=bool), 0, 1)
+            batch = TxBatch(batch.txs, batch.inputs, batch.outputs, given, batch.arena)
+        cb = _c_batch(batch, with_entries=supplied is not None)
+        args = None
+        if feerate_threshold is not None:
+            args = np.zeros(n, dtype=MEMPOOL_ARGS_DTYPE)
+            args["feerate_threshold"] = feerate_threshold
+        res = np.zeros(n, dtype=RESULT_DTYPE)
+        mass = np.zeros(n, dtype=np.uint64)
+        masses = np.zeros(n, dtype=TX_MASSES_DTYPE)
+        ent = np.zeros(max(ni, 1), dtype=ENTRY_DTYPE)
+        used = ctypes.c_size_t()
+        cap = len(batch.arena) + 128 * ni
+        for _ in range(2):  # the call reports the size it needs before any signature is verified
+            arena = np.zeros(max(cap, 8), dtype=np.uint8)
+            rc = self._lib.kgv_validate_mempool_txs_in_parallel(self.ctx._h, utxo_set._h, ctypes.byref(cb), int(virtual_daa_score), int(virtual_past_median_time),
+                                                                ctypes.byref(self.params), ctypes.byref(rules), None if args is None else args.ctypes.data,
+                                                                res.ctypes.data, mass.ctypes.data, masses.ctypes.data, ent.ctypes.data, arena.ctypes.data,
+                                                                len(arena), ctypes.byref(used))
+            if rc != ERR_NOMEM or used.value <= cap:
+                break
+            cap = used.value
+        self.ctx._check(rc)
+        return res, mass, masses, ent[:ni], arena[:used.value]
 
     def validate_transactions_with_muhash_in_parallel(self, utxo_set, batch, pov_daa_score, flags=FLAGS_FULL):
         """utxo_validation.rs:282-309: as validate_transactions_in_parallel, plus the combined MuHash::from_transaction of the
