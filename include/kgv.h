@@ -569,14 +569,17 @@ int kgv_muhash_combine(kgv_ctx* ctx, uint8_t* numerator_a, uint8_t* denominator_
  * hash = BLAKE2b-256 keyed "MuHashFinalize".  Sequential by nature (one modular inversion: 3 072 dependent squarings);
  * the reference calls it once per chain block outside the parallel section.  serialized384 may be NULL. */
 int kgv_muhash_finalize(kgv_ctx* ctx, const uint8_t* numerator384, const uint8_t* denominator384, uint8_t* serialized384, uint8_t* hash32);
-/* n finalizations at once: hashes32[i] = MuHash{numerator_i, denominator_i}.finalize() (lib.rs:98-115); value i sits pitch_bytes after value
- * i - 1 (384 for plain arrays, 768 for (numerator || denominator) records).  ONE modular inversion for the whole batch (Montgomery's
- * trick over prefix / suffix products built by parallel scans): a chain block's commitment costs five multiplications instead of
- * 3 072 squarings.  serialized384 (n * 384 contiguous bytes) may be NULL. */
+/* n finalizations at once: hashes32[i] = MuHash{numerator_i, denominator_i}.finalize() (lib.rs:98-115) for NONZERO denominators (every
+ * denominator_i mod p != 0, which a product of hashed elements always is); value i sits pitch_bytes after value i - 1 (384 for plain
+ * arrays, 768 for (numerator || denominator) records).  ONE modular inversion for the whole batch (Montgomery's trick over prefix /
+ * suffix products built by parallel scans): a chain block's commitment costs five multiplications instead of 3 072 squarings.
+ * serialized384 (n * 384 contiguous bytes) may be NULL.  KGV_ERR_ARG unless pitch_bytes >= 384 is a multiple of 16 and, for device
+ * pointers, numerators384 is 16-byte aligned and hashes32 / serialized384 are 4-byte aligned. */
 int kgv_muhash_finalize_batch(kgv_ctx* ctx, const uint8_t* numerators384, const uint8_t* denominators384, size_t n, size_t pitch_bytes, uint8_t* serialized384,
                               uint8_t* hashes32);
 /* The MuHash::combine chain of a replay (utxo_validation.rs:144): values768 holds n (numerator || denominator) records; on return record i is
- * init * record 0 * ... * record i (canonical).  init768 may be NULL (= the empty MuHash). */
+ * init * record 0 * ... * record i (canonical).  init768 may be NULL (= the empty MuHash).  A device values768 must be 16-byte aligned
+ * (KGV_ERR_ARG otherwise). */
 int kgv_muhash_prefix_combine(kgv_ctx* ctx, const uint8_t* init768, uint8_t* values768, size_t n);
 /* MuHash::add_utxo (consensus/core/src/muhash.rs:28-33) over every live entry of the table: the UTXO-set commitment
  * numerator (denominator 1). */
@@ -710,6 +713,11 @@ int kgv_debug_script_rounds(const kgv_ctx* ctx, uint32_t* rounds);
  *     12 fe_mul_lanes 13 fe_sqr_lanes: the eight-lane forms (one item per group of eight lanes, lane k holding limb k;
  *        weakly reduced results, like 2 and 3). */
 int kgv_debug_selftest(kgv_ctx* ctx, int op, const uint32_t* in_words, uint32_t* out_words, size_t n);
+/* Test / audit hook: one level of the MuHash product tree on n_in caller values, by the library's own level kernel: coop = 0 the
+ * one-thread-per-product multiplier, coop = 1 the 16-lane cooperative one (reduce_one otherwise picks by level size).  Host pointers
+ * only; in384: n_in contiguous 384-byte little-endian values below 2^3072; out384: the (n_in + 1) / 2 raw results in[2t] * in[2t + 1]
+ * folded below 2^3072 but not reduced mod p, the odd last value copied.  1 <= n_in <= 2^20. */
+int kgv_debug_u3072_level(kgv_ctx* ctx, int coop, const uint8_t* in384, size_t n_in, uint8_t* out384);
 
 #ifdef __cplusplus
 }

@@ -90,6 +90,7 @@ SYMBOLS = [
     ("kgv_utxo_rows_decode", _c.c_int, [_u8p, _u8p, _u8p, _u8p, _c.c_size_t, _u8p, _u8p, _u8p, _c.c_size_t, _c.POINTER(_c.c_size_t)]),
     ("kgv_gtable_entry", _c.c_int, [_c.c_void_p, _c.c_int, _c.c_uint32, _u8p]),
     ("kgv_debug_selftest", _c.c_int, [_c.c_void_p, _c.c_int, _u8p, _u8p, _c.c_size_t]),
+    ("kgv_debug_u3072_level", _c.c_int, [_c.c_void_p, _c.c_int, _u8p, _c.c_size_t, _u8p]),
     ("kgv_debug_schnorr_trace", _c.c_int, [_c.c_void_p, _u8p, _u8p, _u8p, _u8p, _u8p]),
     ("kgv_debug_key_form", _c.c_int, [_c.c_void_p, _c.c_int, _c.c_void_p]),
     ("kgv_debug_script_rounds", _c.c_int, [_c.c_void_p, _c.POINTER(_c.c_uint32)]),

@@ -187,6 +187,32 @@ extern "C" int kgv_muhash_elements(kgv_ctx* ctx, const uint8_t* data, const uint
   return kgv_mu_reduce(ctx, n, n, numerator384, denominator384);
 }
 
+// Test / audit hook: one product-tree level on caller values, by the same two level kernels reduce_one launches
+extern "C" int kgv_debug_u3072_level(kgv_ctx* ctx, int coop, const uint8_t* in384, size_t n_in, uint8_t* out384) {
+  if (!ctx) return KGV_ERR_ARG;
+  std::lock_guard<std::recursive_mutex> g(ctx->mu);
+  if (!in384 || !out384 || n_in == 0 || n_in > ((size_t)1 << 20) || (coop != 0 && coop != 1)) { ctx->err = "bad u3072 level arguments"; return KGV_ERR_ARG; }
+  if (kgv_ptr_is_device(in384) || kgv_ptr_is_device(out384)) { ctx->err = "kgv_debug_u3072_level takes host pointers"; return KGV_ERR_ARG; }
+  CK(cudaSetDevice(ctx->device));
+  const size_t h = (n_in + 1) / 2;
+  const size_t o_out = al256(n_in * 384), o_wide = al256(o_out + h * 384);
+  int rc = kgv_reserve(ctx, &ctx->d_mu, &ctx->d_mu_cap, al256(o_wide + h * 768));
+  if (rc) return rc;
+  uint8_t* M = ctx->d_mu;
+  cudaStream_t st = ctx->stream;
+  // contiguous values -> block-transposed level (limb block i of element e at (i * n_in + e) * 32 bytes) and back
+  for (int i = 0; i < KGV_U3072_BLOCKS; i++)
+    CK(cudaMemcpy2DAsync(M + (size_t)i * n_in * 32, 32, in384 + 32 * i, 384, 32, n_in, cudaMemcpyHostToDevice, st));
+  if (coop) k_u3072_tree_level_coop<<<nblk(h, KGV_COOP_GROUPS), 128, 0, st>>>((const uint32_t*)M, n_in, (uint32_t*)(M + o_out));
+  else k_u3072_tree_level<<<nblk(h, 128), 128, 0, st>>>((const uint32_t*)M, n_in, (uint32_t*)(M + o_out), (uint32_t*)(M + o_wide));
+  CK(cudaGetLastError());
+  ctx->launches++;
+  for (int i = 0; i < KGV_U3072_BLOCKS; i++)
+    CK(cudaMemcpy2DAsync(out384 + 32 * i, 384, M + o_out + (size_t)i * h * 32, 32, 32, h, cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  return KGV_OK;
+}
+
 // a <- a * b for both fields (crypto/muhash/src/lib.rs:91-96 combine); all four are 384-byte little-endian residues
 __global__ void k_muhash_combine(uint32_t* __restrict__ w) {  // w: [a_num | a_den | b_num | b_den] contiguous words; one warp: group 0 numerators, group 1 denominators
   __shared__ U3072Coop sm[2];
@@ -470,10 +496,15 @@ extern "C" int kgv_muhash_finalize_batch(kgv_ctx* ctx, const uint8_t* numerators
   if (!ctx) return KGV_ERR_ARG;
   std::lock_guard<std::recursive_mutex> g(ctx->mu);
   if (n == 0) return KGV_OK;
-  if (!numerators384 || !denominators384 || !hashes32 || pitch_bytes < 384 || (pitch_bytes & 3)) { ctx->err = "bad argument"; return KGV_ERR_ARG; }
+  // k_muhash_divide_all reads numerator k with 16-byte loads at numerators384 + k * pitch_bytes; the hash / serialize kernel stores words
+  if (!numerators384 || !denominators384 || !hashes32 || pitch_bytes < 384 || (pitch_bytes & 15)) { ctx->err = "bad argument (pitch_bytes must be >= 384 and a multiple of 16)"; return KGV_ERR_ARG; }
   CK(cudaSetDevice(ctx->device));
   const bool dev = kgv_ptr_is_device(numerators384);
   if (kgv_ptr_is_device(denominators384) != dev || kgv_ptr_is_device(hashes32) != dev) { ctx->err = "all buffers of one call must be host pointers or all device pointers"; return KGV_ERR_ARG; }
+  if (dev && (((uintptr_t)numerators384 & 15) || ((uintptr_t)hashes32 & 3) || ((uintptr_t)serialized384 & 3))) {
+    ctx->err = "device numerators384 must be 16-byte aligned, hashes32 and serialized384 4-byte aligned";
+    return KGV_ERR_ARG;
+  }
   const size_t n_chunks = (n + KGV_SCAN_CHUNK - 1) / KGV_SCAN_CHUNK;
   // layout: [num in (host path only)] [P n] [S n] [out n] [tot chunks] [inverse scratch 3] [hashes n*32 (host path)] [serialized (host path)]
   const size_t span = (n - 1) * pitch_bytes + 384;
@@ -523,6 +554,7 @@ extern "C" int kgv_muhash_prefix_combine(kgv_ctx* ctx, const uint8_t* init768, u
   if (!values768) { ctx->err = "null argument"; return KGV_ERR_ARG; }
   CK(cudaSetDevice(ctx->device));
   const bool dev = kgv_ptr_is_device(values768);
+  if (dev && ((uintptr_t)values768 & 15)) { ctx->err = "device values768 must be 16-byte aligned"; return KGV_ERR_ARG; }  // scanned in place with 16-byte loads
   const size_t n_chunks = (n + KGV_SCAN_CHUNK - 1) / KGV_SCAN_CHUNK;
   size_t o_v = 0, o_tot = al256(dev ? 0 : n * 768), o_init = al256(o_tot + n_chunks * 384);
   int rc = kgv_reserve(ctx, &ctx->d_mu, &ctx->d_mu_cap, al256(o_init + 768));

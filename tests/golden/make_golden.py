@@ -16,6 +16,7 @@ retyped by hand — and each fixture records the file:line range it came from:
   testing/integration/testdata/dags_for_json_tests/goref-1060-tx-265-blocks/blocks.json.gz
                                                            simpa-generated DAG: 224 signed inputs, all valid
   crypto/muhash/src/lib.rs:17-21,189-238,290-327,430-444   MuHash known answers (empty, 3 vectors, pre-computed, serialize, parse)
+  crypto/muhash/src/u3072.rs:455-555                       MuHash field edge cases (overflowing values, (p-1)^2, inverse edge case)
   consensus/core/src/utxo/utxo_diff.rs:270-568             UtxoDiff algebra rule table (diff_from / with_diff)
 """
 import gzip
@@ -327,13 +328,27 @@ def muhash():
     ser_src = src[src.index("fn test_serialize()"):]
     ser = ints(re.search(r"let expected = \[(.*?)\];", ser_src, re.S).group(1))
     assert len(ser) == 384
-    prime_diff = int(re.search(r"pub const PRIME_DIFF: Limb = (\d+);", read("crypto/muhash/src/u3072.rs")).group(1))
+    u3072 = read("crypto/muhash/src/u3072.rs")
+    prime_diff = int(re.search(r"pub const PRIME_DIFF: Limb = (\d+);", u3072).group(1))
+    # the field's own edge tests (u3072.rs:455-555): 64-bit limbs, little-endian
+    limbs = lambda txt: [int(x) for x in re.findall(r"\d+", txt)]
+    edge = limbs(re.search(r"fn test_inverse_edge_case\(\) \{.*?limbs: \[(.*?)\],", u3072, re.S).group(1))
+    assert len(edge) == 48
+    assert "limbs[0] = Limb::MAX - i;" in u3072 and "(0..PRIME_DIFF).into_par_iter()" in u3072  # exhuastive_test_div_overflow
+    assert "max.limbs[0] -= u3072::PRIME_DIFF;" in u3072 and "max *= copy_max;" in u3072  # test_mul_max
     dump("muhash.json", {"source": "crypto/muhash/src/lib.rs:17-21 (EMPTY_MUHASH), :189-238 (TEST_VECTORS), :290-298 (test_new_pre_computed), "
                                    ":301-327 (test_serialize), :430-444 (test_parse_muhash_fail); crypto/muhash/src/u3072.rs:22 (PRIME_DIFF)",
                          "prime_diff": prime_diff, "empty_muhash": empty.hex(), "test_vectors": vecs,
                          "pre_computed": {"add": ["00" + "00" * 31, "01" + "00" * 31], "remove": ["02" + "00" * 31], "finalized": pre},
                          "serialize": {"add": ["01" + "00" * 31, "02" + "00" * 31], "serialized": ser.hex()},
-                         "parse_fail": {"overflow": "9b28ef" + "ff" * 381, "ok": "0028ef" + "ff" * 381, "all_ff_overflows": True}})
+                         "parse_fail": {"overflow": "9b28ef" + "ff" * 381, "ok": "0028ef" + "ff" * 381, "all_ff_overflows": True},
+                         "u3072_edges": {
+                             "source": "crypto/muhash/src/u3072.rs:455-484 (exhuastive_test_div_overflow), :486-493 (test_mul_max), "
+                                       ":521-555 (test_inverse_edge_case)",
+                             "inverse_edge_case": b"".join(x.to_bytes(8, "little") for x in edge).hex(),
+                             "mul_max": {"a": ((2**3072 - 1) - prime_diff).to_bytes(384, "little").hex(), "a_times_a": "01" + "00" * 383},
+                             "div_overflow": {"x_i": "2^3072 - 1 - i for i in 0..prime_diff", "x_over_1": "prime_diff - 1 - i",
+                                              "x_over_x": "1 for every i but prime_diff - 1 (x = p, which is 0)"}}})
 
 
 # ------------------------------------------------------------------------------------ utxo diff algebra
