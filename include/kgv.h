@@ -538,13 +538,90 @@ int kgv_block_hash_merkle_roots(kgv_ctx* ctx, const kgv_tx_batch* batch, const u
 /* Block-body set checks of validate_body_in_isolation (body_validation_in_isolation.rs:13-23,95-131) for many blocks at
  * once: check_duplicate_transactions, check_block_double_spends, check_no_chained_transactions, in that order; the
  * reported item is the first offender in the reference's iteration order (the tx index for duplicates, the absolute
- * input index otherwise).  grid y dimension = n_blocks (<= 65535 per call). */
+ * input index otherwise).  Linear work per block (the hashed sets of kgv_validate_block_bodies); any number of blocks per call. */
 #define KGV_BLOCK_OK 0u
 #define KGV_BLOCK_DUPLICATE_TRANSACTIONS 1u      /* RuleError::DuplicateTransactions(tx id of txs[index]) */
 #define KGV_BLOCK_DOUBLE_SPEND_IN_SAME_BLOCK 2u  /* RuleError::DoubleSpendInSameBlock(inputs[index].previous_outpoint) */
 #define KGV_BLOCK_CHAINED_TRANSACTION 3u         /* RuleError::ChainedTransaction(inputs[index].previous_outpoint) */
 typedef struct kgv_block_check { uint32_t status, index; } kgv_block_check;
 int kgv_block_set_checks(kgv_ctx* ctx, const kgv_tx_batch* batch, const uint32_t* block_first_tx, uint32_t n_blocks, kgv_block_check* out);
+
+/* BlockBodyProcessor::validate_body_in_isolation (body_validation_in_isolation.rs:13-131) and validate_body_in_context
+ * (body_validation_in_context.rs:20-80) for a window of blocks in one call.  Block b = transactions [block_first_tx[b], block_first_tx[b+1])
+ * of the batch (HOST array of n_blocks + 1 offsets, monotone, from 0 to batch->n_txs), with headers[b] holding what the rules read from its
+ * header and from the stores.  expected_subsidy is calc_block_subsidy(daa_score): the caller looks it up in the subsidy table it holds.
+ * past_median_time is read only for a transaction whose lock time is a timestamp.  check_parent_bodies_exist is a query of the statuses
+ * store and stays with the caller, before this call.
+ *
+ * The status of a block is its FIRST failing rule in the reference's order; a later rule is never visible when an earlier one fails:
+ *   1 check_has_transactions                  NO_TRANSACTIONS
+ *   2 check_hash_merkle_root                  BAD_MERKLE_ROOT          (the computed root: roots32)
+ *   3 check_only_one_coinbase                 FIRST_TX_NOT_COINBASE; MULTIPLE_COINBASES with index = position in transactions[1..]
+ *   4 check_transactions_in_isolation         TX_IN_ISOLATION_FAILED   index = first failing tx of the block (position in the block),
+ *                                                                      tx_status = KGV_TX_* 14..30, fail_input as kgv_tx_result
+ *   5 check_block_mass                        EXCEEDS_COMPUTE / TRANSIENT / STORAGE_MASS_LIMIT: index = position of the tx at which a
+ *                                             running total first passes max_block_mass (at one tx compute is tested before transient
+ *                                             before storage), a = that saturating total, b = max_block_mass
+ *   6 check_duplicate_transactions, check_block_double_spends, check_no_chained_transactions
+ *                                             DUPLICATE_TRANSACTIONS / DOUBLE_SPEND_IN_SAME_BLOCK / CHAINED_TRANSACTION, index exactly as
+ *                                             kgv_block_set_checks reports it (tx resp. input index within the BATCH)
+ *   7 check_coinbase_blue_score_and_subsidy   BAD_COINBASE_PAYLOAD (tx_status = KGV_COINBASE_PAYLOAD_*, a and b the CoinbaseError's two
+ *                                             numbers), BAD_COINBASE_PAYLOAD_BLUE_SCORE (a payload's, b header's), WRONG_SUBSIDY
+ *                                             (a expected, b payload's)
+ *   8 check_block_transactions_in_context     TX_IN_CONTEXT_FAILED     index = first tx (position in the block) not finalized under ITS
+ *                                                                      block's daa_score / past_median_time, tx_status =
+ *                                                                      KGV_TX_NOT_FINALIZED, fail_input
+ * flags: 0 runs both stages, KGV_BODY_ISOLATION_ONLY stops after rule 6 (what validate_body_in_isolation returns).
+ * masses (may be NULL): the returned Mass of each block - calc_non_contextual_masses and the storage mass commitments (kgv_tx.mass), each
+ * summed with saturating_add - and zeros unless the status is KGV_BODY_OK.  roots32 (may be NULL): n_blocks computed hash merkle roots
+ * (bytes, any alignment).
+ * rules->coinbase_payload_script_public_key_max_len also bounds the payload's script.  Every data pointer (batch, headers, results,
+ * masses, roots32) host or every one device; with device pointers the call only enqueues work on the context's stream. */
+typedef struct {
+  uint8_t hash_merkle_root[32]; /* header.hash_merkle_root */
+  uint64_t daa_score;           /* header.daa_score        */
+  uint64_t blue_score;          /* header.blue_score       */
+  uint64_t past_median_time;    /* calc_past_median_time_for_known_hash(block) */
+  uint64_t expected_subsidy;    /* calc_block_subsidy(header.daa_score) */
+} kgv_block_header_ctx; /* 64 bytes */
+typedef struct {
+  uint64_t max_block_mass;           /* Params::max_block_mass */
+  uint64_t max_coinbase_payload_len; /* Params::max_coinbase_payload_len */
+} kgv_body_rules; /* 16 bytes */
+typedef struct {
+  uint32_t status;     /* KGV_BODY_* */
+  uint32_t index;
+  uint32_t tx_status;
+  uint32_t fail_input;
+  uint64_t a, b;
+} kgv_body_result; /* 32 bytes */
+typedef struct {
+  uint64_t compute_mass, transient_mass, storage_mass;
+} kgv_block_masses; /* 24 bytes */
+#define KGV_BODY_OK 0u
+#define KGV_BODY_NO_TRANSACTIONS 1u                  /* RuleError::NoTransactions */
+#define KGV_BODY_BAD_MERKLE_ROOT 2u                  /* RuleError::BadMerkleRoot(header's, computed) */
+#define KGV_BODY_FIRST_TX_NOT_COINBASE 3u            /* RuleError::FirstTxNotCoinbase */
+#define KGV_BODY_MULTIPLE_COINBASES 4u               /* RuleError::MultipleCoinbases(index) */
+#define KGV_BODY_TX_IN_ISOLATION_FAILED 5u           /* RuleError::TxInIsolationValidationFailed(tx id, tx_status) */
+#define KGV_BODY_EXCEEDS_COMPUTE_MASS_LIMIT 6u       /* RuleError::ExceedsComputeMassLimit(a, b) */
+#define KGV_BODY_EXCEEDS_TRANSIENT_MASS_LIMIT 7u     /* RuleError::ExceedsTransientMassLimit(a, b) */
+#define KGV_BODY_EXCEEDS_STORAGE_MASS_LIMIT 8u       /* RuleError::ExceedsStorageMassLimit(a, b) */
+#define KGV_BODY_DUPLICATE_TRANSACTIONS 9u           /* RuleError::DuplicateTransactions */
+#define KGV_BODY_DOUBLE_SPEND_IN_SAME_BLOCK 10u      /* RuleError::DoubleSpendInSameBlock */
+#define KGV_BODY_CHAINED_TRANSACTION 11u             /* RuleError::ChainedTransaction */
+#define KGV_BODY_BAD_COINBASE_PAYLOAD 12u            /* RuleError::BadCoinbasePayload(tx_status) */
+#define KGV_BODY_BAD_COINBASE_PAYLOAD_BLUE_SCORE 13u /* RuleError::BadCoinbasePayloadBlueScore(a, b) */
+#define KGV_BODY_WRONG_SUBSIDY 14u                   /* RuleError::WrongSubsidy(a, b) */
+#define KGV_BODY_TX_IN_CONTEXT_FAILED 15u            /* RuleError::TxInContextFailed(tx id, NotFinalized(fail_input)) */
+#define KGV_COINBASE_PAYLOAD_LEN_BELOW_MIN 1u        /* CoinbaseError::PayloadLenBelowMin(a = length, b = 19) */
+#define KGV_COINBASE_PAYLOAD_LEN_ABOVE_MAX 2u        /* CoinbaseError::PayloadLenAboveMax(a = length, b = max_coinbase_payload_len) */
+#define KGV_COINBASE_PAYLOAD_SPK_LEN_ABOVE_MAX 3u    /* CoinbaseError::PayloadScriptPublicKeyLenAboveMax(a = script length, b = maximum) */
+#define KGV_COINBASE_PAYLOAD_CANT_CONTAIN_SPK 4u     /* CoinbaseError::PayloadCantContainScriptPublicKey(a = length, b = 19 + script length) */
+#define KGV_BODY_ISOLATION_ONLY 1u
+int kgv_validate_block_bodies(kgv_ctx* ctx, const kgv_tx_batch* batch, const uint32_t* block_first_tx, uint32_t n_blocks,
+                              const kgv_block_header_ctx* headers, const kgv_tx_rules* rules, const kgv_body_rules* body_rules, uint32_t flags,
+                              kgv_body_result* results, kgv_block_masses* masses, uint8_t* roots32);
 
 /* ------------------------------------------------------------------------------------------------
  * K8 MuHash (SURVEY.md §8f-1): crypto/muhash/src/lib.rs, u3072.rs; consensus/core/src/muhash.rs.

@@ -12,6 +12,8 @@
 //   kgv::SigVerifier (check_schnorr_signatures / check_ecdsa_signatures)    crypto/txscript/src/lib.rs:574-643, batched
 //   kgv::UtxoDiff (with_diff / diff_from / add_transaction)                 consensus/core/src/utxo/utxo_diff.rs:15-262
 //   kgv::calc_hash_merkle_roots, kgv::check_block_bodies                    consensus/core/src/merkle.rs:5-7, body_validation_in_isolation.rs:95-131
+//   kgv::BlockBodyProcessor (validate_body_in_isolation / validate_body_in_context / validate_bodies)  consensus/src/pipeline/body_processor/
+//                                                                           body_validation_in_isolation.rs:13-131, body_validation_in_context.rs:20-80
 // (* batched: one verdict per transaction.)  Verdicts are data (status codes of kgv.h); only transport failures throw.
 // There is no CPU execution path behind any of this: without libkgv.so + a CUDA device, Context's constructor throws.
 #pragma once
@@ -657,5 +659,42 @@ inline std::vector<kgv_block_check> check_block_bodies(Context& c, const TxBatch
   c.check(kgv_block_set_checks(c.get(), &v, block_first_tx.data(), (uint32_t)out.size(), out.data()));
   return out;
 }
+
+// ---- BlockBodyProcessor: every body rule for a window of blocks in one call (kgv_validate_block_bodies) ----
+struct BodyRules : kgv_body_rules {
+  BodyRules() : kgv_body_rules{500000, 204} {}  // MAINNET_PARAMS: max_block_mass, max_coinbase_payload_len
+};
+struct BlockBodyVerdicts {
+  std::vector<kgv_body_result> results;  // the first failing rule of each block (KGV_BODY_*); a verdict is data, never an exception
+  std::vector<kgv_block_masses> masses;  // the block's Mass; zeros unless the block is KGV_BODY_OK
+  std::vector<Hash> hash_merkle_roots;   // calc_hash_merkle_root of each block, for RuleError::BadMerkleRoot(header's, calculated)
+};
+class BlockBodyProcessor {
+ public:
+  explicit BlockBodyProcessor(Context& c, const TxRules& rules = TxRules(), const BodyRules& body_rules = BodyRules()) : c_(c), rules_(rules), body_(body_rules) {}
+  // block k = transactions [block_first_tx[k], block_first_tx[k + 1]) of b; headers[k]: what the rules read from its header and the stores.
+  // check_parent_bodies_exist is a statuses-store query and stays with the caller.
+  BlockBodyVerdicts validate_body_in_isolation(const TxBatch& b, const std::vector<uint32_t>& block_first_tx, const std::vector<kgv_block_header_ctx>& headers) {
+    return validate_bodies(b, block_first_tx, headers, KGV_BODY_ISOLATION_ONLY);
+  }
+  // the whole order: a block failing an isolation rule reports that rule, as the reference never reaches the context stage for it
+  BlockBodyVerdicts validate_body_in_context(const TxBatch& b, const std::vector<uint32_t>& block_first_tx, const std::vector<kgv_block_header_ctx>& headers) {
+    return validate_bodies(b, block_first_tx, headers, 0);
+  }
+  BlockBodyVerdicts validate_bodies(const TxBatch& b, const std::vector<uint32_t>& block_first_tx, const std::vector<kgv_block_header_ctx>& headers, uint32_t flags) {
+    if (block_first_tx.empty() || headers.size() != block_first_tx.size() - 1) throw Error(KGV_ERR_ARG, "BlockBodyProcessor: one header record per block");
+    const size_t n = headers.size();
+    BlockBodyVerdicts v{std::vector<kgv_body_result>(n), std::vector<kgv_block_masses>(n), std::vector<Hash>(n)};
+    kgv_tx_batch view = b.view(false);
+    c_.check(kgv_validate_block_bodies(c_.get(), &view, block_first_tx.data(), (uint32_t)n, headers.data(), &rules_, &body_, flags, v.results.data(), v.masses.data(),
+                                       n ? v.hash_merkle_roots[0].data() : nullptr));
+    return v;
+  }
+
+ private:
+  Context& c_;
+  TxRules rules_;
+  BodyRules body_;
+};
 
 }  // namespace kgv

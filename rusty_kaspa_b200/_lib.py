@@ -73,6 +73,7 @@ SYMBOLS = [
     ("kgv_merkle_roots", _c.c_int, [_c.c_void_p, _u8p, _u8p, _c.c_uint32, _u8p]),
     ("kgv_block_hash_merkle_roots", _c.c_int, [_c.c_void_p, _c.c_void_p, _u8p, _c.c_uint32, _u8p]),
     ("kgv_block_set_checks", _c.c_int, [_c.c_void_p, _c.c_void_p, _u8p, _c.c_uint32, _u8p]),
+    ("kgv_validate_block_bodies", _c.c_int, [_c.c_void_p, _c.c_void_p, _u8p, _c.c_uint32, _u8p, _c.c_void_p, _c.c_void_p, _c.c_uint32, _u8p, _u8p, _u8p]),
     ("kgv_muhash_elements", _c.c_int, [_c.c_void_p, _u8p, _u8p, _u8p, _c.c_size_t, _u8p, _u8p]),
     ("kgv_muhash_txs", _c.c_int, [_c.c_void_p, _c.c_void_p, _c.c_void_p, _u8p, _c.c_uint64, _u8p, _u8p]),
     ("kgv_muhash_combine", _c.c_int, [_c.c_void_p, _u8p, _u8p, _u8p, _u8p]),

@@ -18,8 +18,8 @@ def _tx(t):
 
 
 def load_blocks_json(path):
-    """Returns (params dict, list of blocks); a block = {"hash", "daa_score", "hash_merkle_root", "accepted_id_merkle_root",
-    "utxo_commitment", "parents" (level 0), "transactions" (tx dicts)} in file (topological) order."""
+    """Returns (params dict, list of blocks); a block = {"hash", "daa_score", "blue_score", "hash_merkle_root",
+    "accepted_id_merkle_root", "utxo_commitment", "parents" (level 0), "transactions" (tx dicts)} in file (topological) order."""
     opener = gzip.open if str(path).endswith(".gz") else open
     with opener(path, "rt") as f:
         lines = [l for l in f.read().splitlines() if l.strip()]
@@ -28,7 +28,8 @@ def load_blocks_json(path):
     for l in lines[1:]:
         b = json.loads(l)
         h = b["header"]
-        blocks.append({"hash": bytes.fromhex(h["hash"]), "daa_score": h["daaScore"], "hash_merkle_root": bytes.fromhex(h["hashMerkleRoot"]),
+        blocks.append({"hash": bytes.fromhex(h["hash"]), "daa_score": h["daaScore"], "blue_score": h["blueScore"],
+                       "hash_merkle_root": bytes.fromhex(h["hashMerkleRoot"]),
                        "accepted_id_merkle_root": bytes.fromhex(h["acceptedIdMerkleRoot"]), "utxo_commitment": bytes.fromhex(h["utxoCommitment"]),
                        "parents": [bytes.fromhex(p) for p in (h["parentsByLevel"][0] if h["parentsByLevel"] else [])],
                        "transactions": [_tx(t) for t in b["transactions"]]})

@@ -236,6 +236,17 @@ k_sighash_items(BatchView b, const SigHashReused* __restrict__ reused, const kgv
   for (int k = 0; k < 8; k++) out[8 * i + k] = bswap32(w[k]);  // back to the digest's byte order
 }
 
+int kgv_tx_digests_run(kgv_ctx* ctx, const kgv_dev_batch& d, size_t n, uint64_t* out, bool hash) {
+  if (n == 0) return KGV_OK;
+  const BatchView v{d.txs, d.inputs, d.outputs, nullptr, d.bytes};
+  const unsigned blocks = (unsigned)((n + 127) / 128);
+  if (hash) k_tx_digest<true><<<blocks, 128, 0, ctx->stream>>>(v, (uint32_t)n, out);
+  else k_tx_digest<false><<<blocks, 128, 0, ctx->stream>>>(v, (uint32_t)n, out);
+  CK(cudaGetLastError());
+  ctx->launches++;
+  return KGV_OK;
+}
+
 // ---------------------------------------------------------------------------------------------
 static int digest_common(kgv_ctx* ctx, const kgv_tx_batch* batch, uint8_t* out32, bool hash) {
   if (!ctx) return KGV_ERR_ARG;
@@ -253,12 +264,8 @@ static int digest_common(kgv_ctx* ctx, const kgv_tx_batch* batch, uint8_t* out32
     if (rc) return rc;
     dout = ctx->d_out;
   }
-  BatchView v{d.txs, d.inputs, d.outputs, nullptr, d.bytes};
-  unsigned blocks = (unsigned)((d.n_txs + 127) / 128);
-  if (hash) k_tx_digest<true><<<blocks, 128, 0, ctx->stream>>>(v, (uint32_t)d.n_txs, (uint64_t*)dout);
-  else k_tx_digest<false><<<blocks, 128, 0, ctx->stream>>>(v, (uint32_t)d.n_txs, (uint64_t*)dout);
-  CK(cudaGetLastError());
-  ctx->launches++;
+  rc = kgv_tx_digests_run(ctx, d, d.n_txs, (uint64_t*)dout, hash);
+  if (rc) return rc;
   if (!out_dev) {
     CK(cudaMemcpyAsync(out32, dout, d.n_txs * 32, cudaMemcpyDeviceToHost, ctx->stream));
     CK(cudaStreamSynchronize(ctx->stream));
@@ -360,7 +367,7 @@ __global__ void k_merkle_collect(const uint64_t* __restrict__ cur, const uint32_
 }
 
 // dh: device array of n_total hashes (modified: used as one of the two ping-pong buffers); first_host: n_groups + 1 offsets on the HOST
-static int merkle_core(kgv_ctx* ctx, uint64_t* dh, size_t n_total, const uint32_t* first_host, uint32_t n_groups, uint64_t* droots) {
+int kgv_merkle_run(kgv_ctx* ctx, uint64_t* dh, size_t n_total, const uint32_t* first_host, uint32_t n_groups, uint64_t* droots) {
   uint32_t max_n = 0;
   if (n_groups && (first_host[0] != 0 || first_host[n_groups] != n_total)) { ctx->err = "merkle group offsets must start at 0 and end at the number of hashes"; return KGV_ERR_ARG; }
   for (uint32_t g = 0; g < n_groups; g++) {
@@ -413,7 +420,7 @@ extern "C" int kgv_merkle_roots(kgv_ctx* ctx, const uint8_t* hashes32, const uin
   uint64_t* dh = (uint64_t*)ctx->d_in;
   uint64_t* dr = (uint64_t*)(ctx->d_in + al256(n_total * 32 + 32));
   if (n_total) CK(cudaMemcpyAsync(dh, hashes32, n_total * 32, dev ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, ctx->stream));
-  rc = merkle_core(ctx, dh, n_total, first, n_groups, dr);
+  rc = kgv_merkle_run(ctx, dh, n_total, first, n_groups, dr);
   if (rc) return rc;
   CK(cudaMemcpyAsync(roots32, dr, (size_t)n_groups * 32, dev ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, ctx->stream));
   if (!dev) CK(cudaStreamSynchronize(ctx->stream));
@@ -441,13 +448,9 @@ extern "C" int kgv_block_hash_merkle_roots(kgv_ctx* ctx, const kgv_tx_batch* bat
   if (rc) return rc;
   uint64_t* dh = (uint64_t*)ctx->d_in;
   uint64_t* dr = (uint64_t*)(ctx->d_in + al256(nt * 32 + 32));
-  if (nt) {
-    BatchView v{d.txs, d.inputs, d.outputs, nullptr, d.bytes};
-    k_tx_digest<true><<<(unsigned)((nt + 127) / 128), 128, 0, ctx->stream>>>(v, (uint32_t)nt, dh);
-    CK(cudaGetLastError());
-    ctx->launches++;
-  }
-  rc = merkle_core(ctx, dh, nt, block_first_tx, n_blocks, dr);
+  rc = kgv_tx_digests_run(ctx, d, nt, dh, true);
+  if (rc) return rc;
+  rc = kgv_merkle_run(ctx, dh, nt, block_first_tx, n_blocks, dr);
   if (rc) return rc;
   const bool dev = kgv_ptr_is_device(roots32) != 0;
   CK(cudaMemcpyAsync(roots32, dr, (size_t)n_blocks * 32, dev ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, ctx->stream));
@@ -457,48 +460,10 @@ extern "C" int kgv_block_hash_merkle_roots(kgv_ctx* ctx, const kgv_tx_batch* bat
 
 // ---------------------------------------------------------------------------------------------
 // Block-body set checks (consensus/src/pipeline/body_processor/body_validation_in_isolation.rs:95-131), many blocks at
-// once.  Blocks hold a few hundred transactions, so each item simply scans the earlier items of its own block
-// (O(n^2) compares of 32/36-byte keys per block, all blocks in parallel); the FIRST offender in the reference's
-// iteration order is kept with atomicMin.
+// once: the hashed sets of kgv_block_body.cu find each check's FIRST offender in the reference's iteration order.
 // ---------------------------------------------------------------------------------------------
-struct BlockCheckAcc { unsigned int dup_tx, double_spend, chained; };
+using BlockCheckAcc = kgv_block_check_acc;
 
-__device__ __forceinline__ bool same_outpoint(const kgv_input& a, const kgv_input& b) {
-  if (a.prev_index != b.prev_index) return false;
-  const uint32_t* x = reinterpret_cast<const uint32_t*>(a.prev_txid);
-  const uint32_t* y = reinterpret_cast<const uint32_t*>(b.prev_txid);
-  bool eq = true;
-#pragma unroll
-  for (int k = 0; k < 8; k++) eq = eq && x[k] == y[k];
-  return eq;
-}
-__global__ void __launch_bounds__(128) k_block_set_checks(const kgv_tx* __restrict__ txs, const kgv_input* __restrict__ inputs, const uint64_t* __restrict__ ids,
-                                                          const uint32_t* __restrict__ block_first_tx, BlockCheckAcc* __restrict__ acc) {
-  const uint32_t b = blockIdx.y;
-  const uint32_t t0 = block_first_tx[b], t1 = block_first_tx[b + 1];
-  if (t0 == t1) return;
-  const uint32_t i0 = txs[t0].first_input, i1 = txs[t1 - 1].first_input + txs[t1 - 1].n_inputs;
-  const uint32_t item = blockIdx.x * blockDim.x + threadIdx.x;
-  // check_duplicate_transactions (:120-129): first tx whose id already occurred
-  if (item < t1 - t0) {
-    const uint32_t t = t0 + item;
-    const uint64_t a0 = ids[4 * (size_t)t], a1 = ids[4 * (size_t)t + 1], a2 = ids[4 * (size_t)t + 2], a3 = ids[4 * (size_t)t + 3];
-    for (uint32_t j = t0; j < t; j++)
-      if (ids[4 * (size_t)j] == a0 && ids[4 * (size_t)j + 1] == a1 && ids[4 * (size_t)j + 2] == a2 && ids[4 * (size_t)j + 3] == a3) { atomicMin(&acc[b].dup_tx, t); break; }
-  }
-  if (item < i1 - i0) {
-    const uint32_t i = i0 + item;
-    const kgv_input in = inputs[i];
-    // check_block_double_spends (:95-103): first input whose outpoint already occurred
-    for (uint32_t j = i0; j < i; j++)
-      if (same_outpoint(inputs[j], in)) { atomicMin(&acc[b].double_spend, i); break; }
-    // check_no_chained_transactions (:105-118): first input spending an output created in this block
-    const uint64_t* pid = reinterpret_cast<const uint64_t*>(in.prev_txid);  // 8-byte aligned: kgv_input is 56 bytes, prev_txid first
-    for (uint32_t j = t0; j < t1; j++)
-      if (in.prev_index < txs[j].n_outputs && ids[4 * (size_t)j] == pid[0] && ids[4 * (size_t)j + 1] == pid[1] && ids[4 * (size_t)j + 2] == pid[2] &&
-          ids[4 * (size_t)j + 3] == pid[3]) { atomicMin(&acc[b].chained, i); break; }
-  }
-}
 __global__ void k_block_set_checks_final(const BlockCheckAcc* __restrict__ acc, uint32_t n_blocks, kgv_block_check* __restrict__ out) {
   uint32_t b = blockIdx.x * blockDim.x + threadIdx.x;
   if (b >= n_blocks) return;
@@ -516,14 +481,11 @@ extern "C" int kgv_block_set_checks(kgv_ctx* ctx, const kgv_tx_batch* batch, con
   if (!ctx) return KGV_ERR_ARG;
   std::lock_guard<std::recursive_mutex> g(ctx->mu);
   if (n_blocks == 0) return KGV_OK;
-  if (n_blocks > 65535) { ctx->err = "at most 65535 blocks per call"; return KGV_ERR_ARG; }
   if (!batch || !block_first_tx || !out) { ctx->err = "null argument"; return KGV_ERR_ARG; }
   if (kgv_ptr_is_device(block_first_tx)) { ctx->err = "block offsets must be a host array"; return KGV_ERR_ARG; }
-  uint32_t max_tx = 0;
-  for (uint32_t b = 0; b < n_blocks; b++) {
+  if (batch->n_txs > 0x7FFFFFFFull || batch->n_inputs > 0x7FFFFFFFull) { ctx->err = "kgv_block_set_checks: more than 2^31 - 1 transactions or inputs"; return KGV_ERR_ARG; }
+  for (uint32_t b = 0; b < n_blocks; b++)
     if (block_first_tx[b + 1] < block_first_tx[b] || block_first_tx[b + 1] > batch->n_txs) { ctx->err = "block offsets not monotone / out of range"; return KGV_ERR_ARG; }
-    if (block_first_tx[b + 1] - block_first_tx[b] > max_tx) max_tx = block_first_tx[b + 1] - block_first_tx[b];
-  }
   CK(cudaSetDevice(ctx->device));
   kgv_dev_batch d;
   d.n_txs = d.n_inputs = 0;
@@ -533,34 +495,18 @@ extern "C" int kgv_block_set_checks(kgv_ctx* ctx, const kgv_tx_batch* batch, con
   }
   const size_t nt = block_first_tx[n_blocks];
   size_t o_ids = 0, o_first = al256(nt * 32 + 32), o_acc = al256(o_first + (n_blocks + 1) * 4), o_out = al256(o_acc + (size_t)n_blocks * sizeof(BlockCheckAcc));
-  int rc = kgv_reserve(ctx, &ctx->d_scratch, &ctx->d_scratch_cap, al256(o_out + (size_t)n_blocks * sizeof(kgv_block_check)));
+  const size_t o_tab = al256(o_out + (size_t)n_blocks * sizeof(kgv_block_check));
+  int rc = kgv_reserve(ctx, &ctx->d_scratch, &ctx->d_scratch_cap, al256(o_tab + kgv_body_sets_scratch(nt, d.n_inputs)));
   if (rc) return rc;
   uint8_t* S = ctx->d_scratch;
   cudaStream_t st = ctx->stream;
   CK(cudaMemcpyAsync(S + o_first, block_first_tx, (n_blocks + 1) * 4, cudaMemcpyHostToDevice, st));
   CK(cudaMemsetAsync(S + o_acc, 0xFF, (size_t)n_blocks * sizeof(BlockCheckAcc), st));
   if (nt) {
-    BatchView v{d.txs, d.inputs, d.outputs, nullptr, d.bytes};
-    k_tx_digest<false><<<(unsigned)((nt + 127) / 128), 128, 0, st>>>(v, (uint32_t)nt, (uint64_t*)(S + o_ids));
-    CK(cudaGetLastError());
-    // items per block = max(#txs, #inputs).  Host batches: exact maximum; device-resident batches: the tx records cannot be
-    // read here, so the grid covers the worst case (all inputs in one block) and the kernel bounds itself.
-    uint32_t max_items = max_tx;
-    if (!kgv_ptr_is_device(batch->txs)) {
-      for (uint32_t b = 0; b < n_blocks; b++) {
-        uint32_t t0 = block_first_tx[b], t1 = block_first_tx[b + 1];
-        if (t0 == t1) continue;
-        uint32_t ni = batch->txs[t1 - 1].first_input + batch->txs[t1 - 1].n_inputs - batch->txs[t0].first_input;
-        if (ni > max_items) max_items = ni;
-      }
-    } else if (d.n_inputs > max_items) {
-      max_items = (uint32_t)d.n_inputs;
-    }
-    if (max_items == 0) max_items = 1;
-    dim3 grid((max_items + 127) / 128, n_blocks);
-    k_block_set_checks<<<grid, 128, 0, st>>>(d.txs, d.inputs, (const uint64_t*)(S + o_ids), (const uint32_t*)(S + o_first), (BlockCheckAcc*)(S + o_acc));
-    CK(cudaGetLastError());
-    ctx->launches += 2;
+    rc = kgv_tx_digests_run(ctx, d, nt, (uint64_t*)(S + o_ids), false);
+    if (rc) return rc;
+    rc = kgv_body_sets_run(ctx, d, nt, (const uint64_t*)(S + o_ids), (const uint32_t*)(S + o_first), n_blocks, (BlockCheckAcc*)(S + o_acc), (uint32_t*)(S + o_tab), st);
+    if (rc) return rc;
   }
   k_block_set_checks_final<<<(n_blocks + 127) / 128, 128, 0, st>>>((const BlockCheckAcc*)(S + o_acc), n_blocks, (kgv_block_check*)(S + o_out));
   CK(cudaGetLastError());

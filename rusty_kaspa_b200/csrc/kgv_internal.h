@@ -142,8 +142,24 @@ int kgv_script_engine_run(kgv_ctx* ctx, const kgv::BatchView& v, size_t n_txs, c
 // ---- isolation rules, finality and non-contextual masses (kgv_isolation.cu) ----
 // Enqueues on st, for every tx of a device batch: dres = the first failing isolation / finality rule (finality == false skips it),
 // dmasses = calc_non_contextual_masses and dnc = max(compute, transient) (either may be null).  dlist: scratch of n_txs + 1 u32.
+// With dheaders (device, one record per block) and dtx_block (device, the block of every tx) the finality rule reads each transaction's
+// own block's daa_score / past_median_time instead of daa / pmt.
 int kgv_isolation_run(kgv_ctx* ctx, const kgv_dev_batch& d, const kgv_tx_rules& rules, uint64_t daa, uint64_t pmt, bool finality, kgv_tx_result* dres,
-                      kgv_tx_masses* dmasses, uint64_t* dnc, uint32_t* dlist, cudaStream_t st);
+                      kgv_tx_masses* dmasses, uint64_t* dnc, uint32_t* dlist, cudaStream_t st, const kgv_block_header_ctx* dheaders = nullptr,
+                      const uint32_t* dtx_block = nullptr);
+
+// ---- pieces of the block body path shared between kgv_hash.cu and kgv_block_body.cu ----
+// enqueue Transaction::id() (hash == false) or hashing::tx::hash (true) of the first n txs of a device batch into out (32 B each)
+int kgv_tx_digests_run(kgv_ctx* ctx, const kgv_dev_batch& d, size_t n, uint64_t* out, bool hash);
+// merkle roots of n_groups groups over the device hashes dh (overwritten); first_host: n_groups + 1 offsets on the host.  Uses d_scratch.
+int kgv_merkle_run(kgv_ctx* ctx, uint64_t* dh, size_t n_total, const uint32_t* first_host, uint32_t n_groups, uint64_t* droots);
+// check_duplicate_transactions / check_block_double_spends / check_no_chained_transactions of every block (kgv_block_body.cu): dacc[b] gets
+// the lowest offending tx / input / input index within the batch, 0xFFFFFFFF where a check passes.  dids: the tx ids; dfirst: the block
+// offsets on the device; dtab: scratch of kgv_body_sets_scratch(n_txs, n_inputs) bytes.
+struct kgv_block_check_acc { unsigned int dup_tx, double_spend, chained; };
+size_t kgv_body_sets_scratch(size_t n_txs, size_t n_inputs);
+int kgv_body_sets_run(kgv_ctx* ctx, const kgv_dev_batch& d, size_t n_txs, const uint64_t* dids, const uint32_t* dfirst, uint32_t n_blocks,
+                      kgv_block_check_acc* dacc, uint32_t* dtab, cudaStream_t st);
 
 // ---- multi-GPU exchange used by the sharded script phase (kgv_comm.cu) ----
 // Every rank contributes `per` bytes at buf + rank * per (device memory, n_ranks * per bytes in all); on return (stream order)

@@ -37,10 +37,11 @@ constexpr uint32_t ISO_SORT_MAX = ISO_LARGE_THREADS * ISO_LARGE_ITEMS;  // 2048 
 constexpr uint32_t ISO_PAD = 0xFFFFFFFFu;
 
 __global__ void __launch_bounds__(32 * ISO_WARPS)
-k_tx_isolation(BatchView b, uint32_t n_txs, kgv_tx_rules r, uint64_t daa, uint64_t pmt, bool finality, kgv_tx_result* __restrict__ res,
+k_tx_isolation(BatchView b, uint32_t n_txs, kgv_tx_rules r, IsoContext c, bool finality, kgv_tx_result* __restrict__ res,
                kgv_tx_masses* __restrict__ masses, uint64_t* __restrict__ nc_mass, uint32_t* __restrict__ large, uint32_t* __restrict__ n_large) {
   const uint32_t ti = blockIdx.x * ISO_WARPS + threadIdx.x / 32, lane = threadIdx.x & 31;
   if (ti >= n_txs) return;  // uniform per warp
+  const uint64_t daa = c.daa(ti), pmt = c.pmt(ti);
   const kgv_tx t = b.txs[ti];
   const bool cb = tx_is_coinbase(t);
   const kgv_tx_masses m = iso_masses(b, t, cb, r, lane);
@@ -76,7 +77,7 @@ __device__ __forceinline__ bool same_outpoint(const kgv_input* in, uint32_t a, u
 // inputs: a block radix sort of (key_hash, input) in shared memory, and every sorted neighbour run of equal hashes compared exactly.
 // Above that (only with rules beyond mainnet's input limit) each input is compared with every earlier one: quadratic, exact.
 __global__ void __launch_bounds__(ISO_LARGE_THREADS)
-k_tx_isolation_large(BatchView b, kgv_tx_rules r, uint64_t daa, uint64_t pmt, bool finality, const uint32_t* __restrict__ large,
+k_tx_isolation_large(BatchView b, kgv_tx_rules r, IsoContext c, bool finality, const uint32_t* __restrict__ large,
                      const uint32_t* __restrict__ n_large, kgv_tx_result* __restrict__ res) {
   using Sort = cub::BlockRadixSort<unsigned long long, ISO_LARGE_THREADS, ISO_LARGE_ITEMS, uint32_t>;
   __shared__ union {
@@ -134,7 +135,7 @@ k_tx_isolation_large(BatchView b, kgv_tx_rules r, uint64_t daa, uint64_t pmt, bo
     }
     __syncthreads();
     if (threadIdx.x < 32) {
-      const kgv_tx_result out = dup ? iso_result(KGV_TX_DUPLICATE_INPUTS, 0) : iso_tail(b, t, tx_is_coinbase(t), daa, pmt, finality, threadIdx.x);
+      const kgv_tx_result out = dup ? iso_result(KGV_TX_DUPLICATE_INPUTS, 0) : iso_tail(b, t, tx_is_coinbase(t), c.daa(ti), c.pmt(ti), finality, threadIdx.x);
       if (threadIdx.x == 0) res[ti] = out;
     }
     __syncthreads();  // sm and dup are reused by the next listed tx
@@ -142,18 +143,20 @@ k_tx_isolation_large(BatchView b, kgv_tx_rules r, uint64_t daa, uint64_t pmt, bo
 }
 
 int kgv_isolation_run(kgv_ctx* ctx, const kgv_dev_batch& d, const kgv_tx_rules& rules, uint64_t daa, uint64_t pmt, bool finality, kgv_tx_result* dres,
-                      kgv_tx_masses* dmasses, uint64_t* dnc, uint32_t* dlist, cudaStream_t st) {
+                      kgv_tx_masses* dmasses, uint64_t* dnc, uint32_t* dlist, cudaStream_t st, const kgv_block_header_ctx* dheaders,
+                      const uint32_t* dtx_block) {
   const size_t nt = d.n_txs;
   if (nt == 0) return KGV_OK;
+  const IsoContext c{daa, pmt, dheaders, dtx_block};
   uint32_t* n_large = dlist + nt;
   CK(cudaMemsetAsync(n_large, 0, 4, st));
   const BatchView v{d.txs, d.inputs, d.outputs, nullptr, d.bytes};
-  k_tx_isolation<<<(unsigned)((nt + ISO_WARPS - 1) / ISO_WARPS), 32 * ISO_WARPS, 0, st>>>(v, (uint32_t)nt, rules, daa, pmt, finality, dres, dmasses, dnc,
+  k_tx_isolation<<<(unsigned)((nt + ISO_WARPS - 1) / ISO_WARPS), 32 * ISO_WARPS, 0, st>>>(v, (uint32_t)nt, rules, c, finality, dres, dmasses, dnc,
                                                                                             dlist, n_large);
   CK(cudaGetLastError());
   // the list's length stays on the device: a fixed grid strides over it (blocks past its end return at once)
   const unsigned grid = (unsigned)std::min<size_t>(nt, 2 * 132);
-  k_tx_isolation_large<<<grid, ISO_LARGE_THREADS, 0, st>>>(v, rules, daa, pmt, finality, dlist, n_large, dres);
+  k_tx_isolation_large<<<grid, ISO_LARGE_THREADS, 0, st>>>(v, rules, c, finality, dlist, n_large, dres);
   CK(cudaGetLastError());
   ctx->launches += 2;
   return KGV_OK;

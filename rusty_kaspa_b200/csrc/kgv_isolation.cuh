@@ -20,6 +20,16 @@ constexpr uint16_t ISO_TX_VERSION = 0;                             // constants:
 constexpr uint32_t ISO_WARP_DUP_MAX = 32;                          // inputs a warp checks for duplicates by itself
 constexpr unsigned ISO_FULL = 0xFFFFFFFFu;
 
+// the header context the finality rule reads for transaction ti: one pair for the whole batch, or (headers != null) the values of the
+// transaction's own block
+struct IsoContext {
+  uint64_t daa_score, past_median_time;
+  const kgv_block_header_ctx* headers;
+  const uint32_t* tx_block;
+  __device__ __forceinline__ uint64_t daa(uint32_t ti) const { return headers ? headers[tx_block[ti]].daa_score : daa_score; }
+  __device__ __forceinline__ uint64_t pmt(uint32_t ti) const { return headers ? headers[tx_block[ti]].past_median_time : past_median_time; }
+};
+
 // first index in [0, n) where pred holds, n if none; n must be the same on every lane, and every lane returns the answer
 template <class P>
 __device__ __forceinline__ uint32_t warp_first(uint32_t n, uint32_t lane, P pred) {

@@ -13,6 +13,8 @@
     TransactionValidator.validate_mempool_transactions_in_parallel_full  <->  validate_mempool_transactions_in_parallel
         (processor.rs:853-878): isolation -> finality -> UTXO context, per transaction
     GpuUtxoSet.add_transactions                              <->  UtxoDiff::add_transaction (utxo_diff.rs:233-247)
+    BlockBodyProcessor.validate_body_in_isolation / validate_body_in_context / validate_bodies  <->  BlockBodyProcessor
+        (consensus/src/pipeline/body_processor/body_validation_in_isolation.rs:13-131, body_validation_in_context.rs:20-80), a window per call
 """
 import ctypes
 
@@ -35,6 +37,19 @@ ISOLATION_STATUS = {14: "NoTxInputs", 15: "TooManyInputs", 16: "TooBigSignatureS
                     22: "CoinbaseScriptPublicKeyTooLong", 23: "TxOutZero", 24: "TxOutTooHigh", 25: "OutputsValueOverflow",
                     26: "TotalTxOutTooHigh", 27: "TxDuplicateInputs", 28: "TxHasGas", 29: "SubnetworksDisabled", 30: "UnknownTxVersion",
                     31: "NotFinalized"}
+
+# kgv_block_header_ctx / kgv_body_result / kgv_block_masses
+BLOCK_HEADER_CTX_DTYPE = np.dtype([("hash_merkle_root", "u1", (32,)), ("daa_score", "<u8"), ("blue_score", "<u8"), ("past_median_time", "<u8"),
+                                   ("expected_subsidy", "<u8")])
+BODY_RESULT_DTYPE = np.dtype([("status", "<u4"), ("index", "<u4"), ("tx_status", "<u4"), ("fail_input", "<u4"), ("a", "<u8"), ("b", "<u8")])
+BLOCK_MASSES_DTYPE = np.dtype([("compute_mass", "<u8"), ("transient_mass", "<u8"), ("storage_mass", "<u8")])
+assert (BLOCK_HEADER_CTX_DTYPE.itemsize, BODY_RESULT_DTYPE.itemsize, BLOCK_MASSES_DTYPE.itemsize) == (64, 32, 24)
+BODY_ISOLATION_ONLY = 1
+# KGV_BODY_* verdicts (include/kgv.h), by the reference's RuleError names
+BODY_STATUS = {0: "Ok", 1: "NoTransactions", 2: "BadMerkleRoot", 3: "FirstTxNotCoinbase", 4: "MultipleCoinbases", 5: "TxInIsolationValidationFailed",
+               6: "ExceedsComputeMassLimit", 7: "ExceedsTransientMassLimit", 8: "ExceedsStorageMassLimit", 9: "DuplicateTransactions",
+               10: "DoubleSpendInSameBlock", 11: "ChainedTransaction", 12: "BadCoinbasePayload", 13: "BadCoinbasePayloadBlueScore", 14: "WrongSubsidy",
+               15: "TxInContextFailed"}
 
 FLAGS_FULL, FLAGS_SKIP_SCRIPT_CHECKS, FLAGS_SKIP_MASS_CHECK, FLAGS_SCRIPTS_ONLY = 0, 1, 2, 3
 MAX_SOMPI = 29_000_000_000 * 100_000_000
@@ -359,6 +374,73 @@ class TransactionValidator:
         cb = _c_batch(batch, with_entries=False)
         self.ctx._check(self._lib.kgv_validate_txs(self.ctx._h, utxo_set._h, ctypes.byref(cb), int(pov_daa_score), int(flags), ctypes.byref(self.params), res.ctypes.data))
         return res
+
+
+class BodyRules(ctypes.Structure):
+    """kgv_body_rules; the defaults are mainnet's (MAINNET_PARAMS)."""
+    _fields_ = [("max_block_mass", ctypes.c_uint64), ("max_coinbase_payload_len", ctypes.c_uint64)]
+
+    def __init__(self, max_block_mass=500_000, max_coinbase_payload_len=204):
+        super().__init__(max_block_mass, max_coinbase_payload_len)
+
+
+def block_headers(blocks, expected_subsidy, past_median_time=0):
+    """BLOCK_HEADER_CTX_DTYPE[n] from blocks_json.load_blocks_json blocks (hash_merkle_root, daa_score, blue_score).  expected_subsidy and
+    past_median_time come from the caller's stores: one value for all blocks, one per block, or expected_subsidy as a function of the
+    block's daa_score (calc_block_subsidy)."""
+    h = np.zeros(len(blocks), dtype=BLOCK_HEADER_CTX_DTYPE)
+    for k, b in enumerate(blocks):
+        h[k]["hash_merkle_root"] = np.frombuffer(bytes(b["hash_merkle_root"]), dtype=np.uint8)
+        h[k]["daa_score"], h[k]["blue_score"] = b["daa_score"], b["blue_score"]
+    h["expected_subsidy"] = [expected_subsidy(b["daa_score"]) for b in blocks] if callable(expected_subsidy) else expected_subsidy
+    h["past_median_time"] = past_median_time
+    return h
+
+
+class BlockBodyProcessor:
+    """Batch counterpart of the reference's BlockBodyProcessor: every rule of validate_body_in_isolation and validate_body_in_context
+    (but check_parent_bodies_exist, a statuses-store query) for a window of blocks in one kgv_validate_block_bodies call."""
+
+    def __init__(self, ctx, rules=None, body_rules=None):
+        self.ctx = ctx
+        self._lib = ctx._lib
+        self.rules = rules or TxRules()
+        self.body_rules = body_rules or BodyRules()
+
+    def validate_bodies(self, batch, block_first_tx, headers, isolation_only=False):
+        """batch: the transactions of all blocks, block b = txs [block_first_tx[b], block_first_tx[b+1]); headers: BLOCK_HEADER_CTX_DTYPE
+        per block.  Returns (BODY_RESULT_DTYPE[n_blocks]: the first failing rule of each block, see BODY_STATUS and include/kgv.h;
+        BLOCK_MASSES_DTYPE[n_blocks]: the block's Mass, zeros unless Ok; (n_blocks, 32) uint8: the computed hash merkle roots)."""
+        f = np.ascontiguousarray(block_first_tx, dtype=np.uint32)
+        h = np.ascontiguousarray(headers, dtype=BLOCK_HEADER_CTX_DTYPE)
+        n = len(f) - 1
+        if len(h) != n:
+            raise ValueError("one header record per block")
+        res = np.zeros(n, dtype=BODY_RESULT_DTYPE)
+        masses = np.zeros(n, dtype=BLOCK_MASSES_DTYPE)
+        roots = np.zeros((n, 32), dtype=np.uint8)
+        cb = _c_batch(batch, with_entries=False)
+        self.ctx._check(self._lib.kgv_validate_block_bodies(self.ctx._h, ctypes.byref(cb), f.ctypes.data, n, h.ctypes.data, ctypes.byref(self.rules),
+                                                            ctypes.byref(self.body_rules), BODY_ISOLATION_ONLY if isolation_only else 0,
+                                                            res.ctypes.data, masses.ctypes.data, roots.ctypes.data))
+        return res, masses, roots
+
+    def validate_blocks(self, blocks, expected_subsidy, past_median_time=0, isolation_only=False):
+        """the window form over blocks_json.load_blocks_json blocks: builds the batch and the header records, then validate_bodies"""
+        from .txbatch import build_batch
+        first = np.cumsum([0] + [len(b["transactions"]) for b in blocks]).astype(np.uint32)
+        batch = build_batch([t for b in blocks for t in b["transactions"]])
+        return self.validate_bodies(batch, first, block_headers(blocks, expected_subsidy, past_median_time), isolation_only)
+
+    def validate_body_in_isolation(self, block):
+        """validate_body_in_isolation for one block: (BODY_RESULT_DTYPE record, BLOCK_MASSES_DTYPE record)"""
+        res, masses, _ = self.validate_blocks([block], 0, isolation_only=True)
+        return res[0], masses[0]
+
+    def validate_body_in_context(self, block, expected_subsidy, past_median_time=0):
+        """validate_body_in_context for one block that passed validate_body_in_isolation: the BODY_RESULT_DTYPE record of the whole order
+        (a block failing an isolation rule reports that rule)"""
+        return self.validate_blocks([block], expected_subsidy, past_median_time)[0][0]
 
 
 class SigCache:
