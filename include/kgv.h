@@ -189,6 +189,19 @@ int kgv_sighash(kgv_ctx* ctx, const kgv_tx_batch* batch, const kgv_sighash_item*
 #define KGV_TX_SUBNETWORKS_DISABLED 29                 /* SubnetworksDisabled                 */
 #define KGV_TX_UNKNOWN_TX_VERSION 30                   /* UnknownTxVersion                    */
 #define KGV_TX_NOT_FINALIZED 31                        /* NotFinalized(fail_input)            */
+/* the mempool's standardness policy, NonStandardError (mining/errors/src/mempool.rs:100-135): the kgv_check_txs_standard_* calls and
+ * kgv_validate_mempool_txs_with_policy only.  detail = the number the variant carries beyond the index (see kgv_mempool_policy). */
+#define KGV_TX_REJECT_VERSION 32                       /* RejectVersion               detail: the version       */
+#define KGV_TX_REJECT_COMPUTE_MASS 33                  /* RejectComputeMass           detail: the compute mass  */
+#define KGV_TX_REJECT_TRANSIENT_MASS 34                /* RejectTransientMass         detail: the transient mass */
+#define KGV_TX_REJECT_SIGNATURE_SCRIPT_SIZE 35         /* RejectSignatureScriptSize(fail_input)  detail: its length */
+#define KGV_TX_REJECT_SCRIPT_PUBLIC_KEY_VERSION 36     /* RejectScriptPublicKeyVersion(output)              */
+#define KGV_TX_REJECT_OUTPUT_SCRIPT_CLASS 37           /* RejectOutputScriptClass(output)                   */
+#define KGV_TX_REJECT_DUST 38                          /* RejectDust(output)          detail: its value         */
+#define KGV_TX_REJECT_STORAGE_MASS 39                  /* RejectStorageMass           detail: the storage mass  */
+#define KGV_TX_REJECT_INPUT_SCRIPT_CLASS 40            /* RejectInputScriptClass(fail_input)                */
+#define KGV_TX_REJECT_SIGNATURE_COUNT 41               /* RejectSignatureCount(fail_input)  detail: num_sig_ops */
+#define KGV_TX_REJECT_INSUFFICIENT_FEE 42              /* RejectInsufficientFee       detail: the minimum fee   */
 /* script errors = TxScriptError variants the standard classes can produce (crypto/txscript/errors) */
 #define KGV_SCRIPT_OK 0
 #define KGV_SCRIPT_EVAL_FALSE 1
@@ -216,8 +229,8 @@ typedef struct {
 } kgv_params;
 typedef struct {
   uint64_t fee;        /* calculated_fee (valid when status == KGV_TX_OK) */
-  uint32_t fail_input; /* first failing input (index within the tx) for status 2, 9, 10, 11, 16, 31; the first failing OUTPUT (index
-                          within the tx) for status 18, 22, 23, 24 */
+  uint32_t fail_input; /* first failing input (index within the tx) for status 2, 9, 10, 11, 16, 31, 35, 40, 41; the first failing OUTPUT
+                          (index within the tx) for status 18, 22, 23, 24, 36, 37, 38 */
   uint8_t status;      /* KGV_TX_*     */
   uint8_t script_err;  /* KGV_SCRIPT_* */
   uint8_t pad_[2];
@@ -392,6 +405,54 @@ int kgv_validate_mempool_txs_in_parallel(kgv_ctx* ctx, kgv_utxo_table* virtual_v
                                          uint64_t virtual_past_median_time, const kgv_params* params, const kgv_tx_rules* rules,
                                          const kgv_mempool_tx_args* args, kgv_tx_result* results, uint64_t* storage_mass, kgv_tx_masses* masses,
                                          kgv_utxo_entry* entries_out, uint8_t* scripts_out, size_t scripts_cap, size_t* scripts_used);
+
+/* The mempool's standardness policy (mining/src/mempool/check_transaction_standard.rs), which a node that does not relay non-standard
+ * transactions (Config::accept_non_standard = false) applies to every transaction it admits.  The limits are the reference's constants:
+ * MAXIMUM_STANDARD_TRANSACTION_MASS 100 000, MAXIMUM_STANDARD_SIGNATURE_SCRIPT_SIZE 1 650, MAX_STANDARD_P2SH_SIG_OPS 15 (:13-38).
+ * The fields are mining/src/mempool/config.rs's of the same names; the defaults there are 1 000 sompi/kg and TX_VERSION (0) for both versions.
+ * detail (may be NULL, n_txs values): the number the verdict carries beyond its index (KGV_TX_REJECT_* above), 0 for any other status. */
+typedef struct {
+  uint64_t minimum_relay_transaction_fee;          /* sompi per 1 000 grams of mass */
+  uint16_t minimum_standard_transaction_version;
+  uint16_t maximum_standard_transaction_version;
+  uint8_t pad_[4];
+} kgv_mempool_policy; /* 16 bytes */
+
+/* check_transaction_standard_in_isolation (:41-105) for every tx: version range, compute mass, transient mass (masses: the caller's
+ * calculated_non_contextual_masses, n_txs records), the first input whose signature script exceeds 1 650 bytes, then the outputs in order
+ * - per output its spk version (> 0), its ScriptClass (script_class.rs:39-82: NonStandard) and dust, the first failing check of the first
+ * failing output.  results: n_txs records, status KGV_TX_OK or 32..38, fee 0.  Every data pointer host or every one device. */
+int kgv_check_txs_standard_in_isolation(kgv_ctx* ctx, const kgv_tx_batch* batch, const kgv_mempool_policy* policy, const kgv_tx_masses* masses,
+                                        kgv_tx_result* results, uint64_t* detail);
+/* check_transaction_standard_in_context (:172-211) for every tx of a batch whose entries are populated (batch->entries required):
+ * storage_mass[i] > 100 000 (tx.mass(), the storage mass the UTXO-context validation computed), then per input the entry's ScriptClass
+ * (NonStandard) and, for a P2SH entry, get_sig_op_count_upper_bound(signature script) > 15 (crypto/txscript/src/lib.rs:176-226); INSIDE
+ * that loop fee[i] (calculated_fee) < minimum_required_transaction_relay_fee(masses[i].compute_mass) (:215-231) is RejectInsufficientFee.
+ * The fee check does not depend on the input, so the order is: storage mass, input 0, the fee, inputs 1..; a tx without inputs never has
+ * its fee checked.  Where the reference's sig-op count panics (OP_16 before a multisig opcode: to_small_int's range excludes OP_16) the
+ * count takes 16, the value OP_16 stands for.  results: status KGV_TX_OK or 39..42, fee = fee[i].  A relay fee with mass * fee above
+ * u64::MAX for a tx whose fee check is reached (the reference's overflow check panics) makes the call return KGV_ERR_ARG. */
+int kgv_check_txs_standard_in_context(kgv_ctx* ctx, const kgv_tx_batch* batch, const kgv_mempool_policy* policy, const kgv_tx_masses* masses,
+                                      const uint64_t* storage_mass, const uint64_t* fee, kgv_tx_result* results, uint64_t* detail);
+/* is_transaction_output_dust (:116-163; MiningManager::is_transaction_output_dust, mining/src/manager.rs:819) for every output of the batch:
+ * is_dust[o] = 1 when the script is unspendable (a parse error anywhere, or OP_RETURN first: crypto/txscript/src/lib.rs:231-233) or
+ * value * 1000 / (3 * (8 + 2 + 8 + script_len + 148)) < minimum_relay_transaction_fee, computed exactly in 128 bits.  Scripts of any
+ * length; the version and class are not read.  is_dust: n_outputs bytes, host or device as the batch. */
+int kgv_outputs_dust(kgv_ctx* ctx, const kgv_tx_batch* batch, uint64_t minimum_relay_transaction_fee, uint8_t* is_dust);
+/* kgv_validate_mempool_txs_in_parallel with the standardness policy, in the mempool's admission order
+ * (mining/src/mempool/validate_and_insert_transaction.rs:20-33, 142-159):
+ *   1. standardness in isolation, on the non-contextual masses the call computes;
+ *   2. isolation and finality;  3. UTXO context and feerate;  4. scripts;
+ *   5. standardness in context, for the transactions whose status is still KGV_TX_OK (storage mass and fee of this call).
+ * A tx rejected in step 1 is never looked up, verified or cached, as an isolation failure (its entries_out rows likewise); one rejected in
+ * step 5 has had its signatures verified (and cached).  policy == NULL is accept_non_standard = true: the call is then exactly
+ * kgv_validate_mempool_txs_in_parallel.  detail (may be NULL): as above.  The relay-fee overflow of kgv_check_txs_standard_in_context can
+ * only occur when minimum_relay_transaction_fee > u64::MAX / 100 000; only then does a device-pointer call synchronise once more. */
+int kgv_validate_mempool_txs_with_policy(kgv_ctx* ctx, kgv_utxo_table* virtual_view, const kgv_tx_batch* batch, uint64_t virtual_daa_score,
+                                         uint64_t virtual_past_median_time, const kgv_params* params, const kgv_tx_rules* rules,
+                                         const kgv_mempool_tx_args* args, kgv_tx_result* results, uint64_t* storage_mass, kgv_tx_masses* masses,
+                                         kgv_utxo_entry* entries_out, uint8_t* scripts_out, size_t scripts_cap, size_t* scripts_used,
+                                         const kgv_mempool_policy* policy, uint64_t* detail);
 
 /* ------------------------------------------------------------------------------------------------
  * SigCache: Cache<SigCacheKey, bool> (crypto/txscript/src/caches.rs:14-55; consulted at crypto/txscript/src/lib.rs:589-603, 624-638;

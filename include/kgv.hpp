@@ -449,6 +449,13 @@ enum class TxValidationFlags : uint32_t { Full = KGV_FLAGS_FULL, SkipScriptCheck
 struct TxRules : kgv_tx_rules {
   TxRules() : kgv_tx_rules{1000, 1000, 10000, 10000, 1, 10, 1000, 124, 150} {}
 };
+// the mempool Config fields of the standardness policy; the defaults are the reference's (mining/src/mempool/config.rs: 1 000 sompi/kg,
+// TX_VERSION for both versions)
+struct MempoolPolicy : kgv_mempool_policy {
+  MempoolPolicy(uint64_t minimum_relay_transaction_fee = 1000, uint16_t minimum_standard_transaction_version = 0,
+                uint16_t maximum_standard_transaction_version = 0)
+      : kgv_mempool_policy{minimum_relay_transaction_fee, minimum_standard_transaction_version, maximum_standard_transaction_version, {0, 0, 0, 0}} {}
+};
 
 class TransactionValidator {
  public:
@@ -609,6 +616,81 @@ class TransactionValidator {
     }
     return out;
   }
+
+  // ---- the mempool's standardness policy (mining/src/mempool/check_transaction_standard.rs) ----
+  // Each verdict comes with the number its NonStandardError carries beyond the index (`detail`, 0 for any other status).
+  struct StandardResults {
+    std::vector<kgv_tx_result> results;
+    std::vector<uint64_t> detail;
+  };
+  // check_transaction_standard_in_isolation (kgv_check_txs_standard_in_isolation); masses: calculated_non_contextual_masses, one per tx
+  StandardResults check_transaction_standard_in_isolation(const TxBatch& b, const std::vector<kgv_tx_masses>& masses,
+                                                          const MempoolPolicy& policy = MempoolPolicy()) {
+    if (masses.size() != b.len()) throw Error(KGV_ERR_ARG, "kgv: one kgv_tx_masses per transaction");
+    StandardResults out{std::vector<kgv_tx_result>(b.len()), std::vector<uint64_t>(b.len())};
+    kgv_tx_batch v = b.view(false);
+    c_.check(kgv_check_txs_standard_in_isolation(c_.get(), &v, &policy, masses.data(), out.results.data(), out.detail.data()));
+    return out;
+  }
+  // check_transaction_standard_in_context (kgv_check_txs_standard_in_context) on a batch pushed with its entries: storage_mass is tx.mass(),
+  // fee the calculated_fee, one each per tx
+  StandardResults check_transaction_standard_in_context(const TxBatch& b, const std::vector<kgv_tx_masses>& masses, const std::vector<uint64_t>& storage_mass,
+                                                        const std::vector<uint64_t>& fee, const MempoolPolicy& policy = MempoolPolicy()) {
+    if (masses.size() != b.len() || storage_mass.size() != b.len() || fee.size() != b.len())
+      throw Error(KGV_ERR_ARG, "kgv: one mass record, storage mass and fee per transaction");
+    StandardResults out{std::vector<kgv_tx_result>(b.len()), std::vector<uint64_t>(b.len())};
+    kgv_tx_batch v = b.view(true);
+    c_.check(kgv_check_txs_standard_in_context(c_.get(), &v, &policy, masses.data(), storage_mass.data(), fee.data(), out.results.data(), out.detail.data()));
+    return out;
+  }
+  // is_transaction_output_dust (kgv_outputs_dust) for every output of the batch, in batch order
+  std::vector<bool> is_transaction_output_dust(const TxBatch& b, uint64_t minimum_relay_transaction_fee = 1000) {
+    kgv_tx_batch v = b.view(false);
+    std::vector<uint8_t> d(v.n_outputs + 1);
+    c_.check(kgv_outputs_dust(c_.get(), &v, minimum_relay_transaction_fee, d.data()));
+    return std::vector<bool>(d.begin(), d.begin() + v.n_outputs);
+  }
+  // validate_mempool_transactions_in_parallel_full with the standardness policy in the mempool's admission order
+  // (kgv_validate_mempool_txs_with_policy); policy == nullptr is accept_non_standard = true
+  struct PolicyMempoolValidation : FullMempoolValidation {
+    std::vector<uint64_t> detail;
+  };
+  PolicyMempoolValidation validate_mempool_transactions_with_policy(UtxoSet& virtual_utxo_view, const TxBatch& b, uint64_t virtual_daa_score,
+                                                                    uint64_t virtual_past_median_time, const MempoolPolicy* policy,
+                                                                    const TxRules& rules = TxRules(), const std::vector<kgv_mempool_tx_args>& args = {}) {
+    if (!args.empty() && args.size() != b.len()) throw Error(KGV_ERR_ARG, "kgv: one kgv_mempool_tx_args per transaction");
+    PolicyMempoolValidation out;
+    out.results.resize(b.len());
+    out.storage_mass.resize(b.len());
+    out.masses.resize(b.len());
+    out.detail.resize(b.len());
+    std::vector<kgv_utxo_entry> ent(b.n_inputs() + 1);
+    kgv_tx_batch v = b.view(true);
+    size_t used = 0;
+    std::vector<uint8_t> scripts(v.n_bytes + 128 * b.n_inputs() + 8);
+    auto call = [&] {
+      return kgv_validate_mempool_txs_with_policy(c_.get(), virtual_utxo_view.get(), &v, virtual_daa_score, virtual_past_median_time, &p_, &rules,
+                                                  args.empty() ? nullptr : args.data(), out.results.data(), out.storage_mass.data(), out.masses.data(), ent.data(),
+                                                  scripts.data(), scripts.size(), &used, policy, out.detail.data());
+    };
+    int rc = call();
+    if (rc == KGV_ERR_NOMEM && used > scripts.size()) {
+      scripts.resize(used);
+      rc = call();
+    }
+    c_.check(rc);
+    out.entries.resize(b.n_inputs());
+    for (size_t i = 0; i < b.n_inputs(); i++) {
+      if (ent[i].pad_[0]) continue;
+      UtxoEntry& e = out.entries[i].second;
+      out.entries[i].first = true;
+      e.amount = ent[i].amount; e.block_daa_score = ent[i].block_daa_score; e.is_coinbase = ent[i].is_coinbase != 0;
+      e.script_public_key.version = ent[i].spk_version;
+      e.script_public_key.script.assign(scripts.begin() + ent[i].script_off, scripts.begin() + ent[i].script_off + ent[i].script_len);
+    }
+    return out;
+  }
+
   std::pair<std::vector<kgv_tx_result>, MuHash> validate_transactions_with_muhash_in_parallel(UtxoSet& utxo_view, const TxBatch& b, uint64_t pov_daa_score,
                                                                                             TxValidationFlags flags = TxValidationFlags::Full) {
     auto res = validate_transactions_in_parallel(utxo_view, b, pov_daa_score, flags);

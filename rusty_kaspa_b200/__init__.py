@@ -5,5 +5,5 @@ into libkgv.so) and the host-side mirror of the reference interface for this pat
 """
 from ._lib import KgvError, LIB_PATH, SIG_INVALID, SIG_PK_PARSE_ERR, SIG_SIG_PARSE_ERR, SIG_VALID  # noqa: F401
 from .verifier import GpuContext  # noqa: F401
-from .validator import GpuUtxoSet, Params, TransactionValidator, TxRules  # noqa: F401
+from .validator import GpuUtxoSet, MempoolPolicy, Params, TransactionValidator, TxRules  # noqa: F401
 from .muhash import MuHash  # noqa: F401

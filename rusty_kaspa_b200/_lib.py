@@ -53,6 +53,11 @@ SYMBOLS = [
     ("kgv_validate_txs_in_isolation", _c.c_int, [_c.c_void_p, _c.c_void_p, _c.c_void_p, _c.c_uint64, _c.c_uint64, _c.c_uint32, _u8p, _u8p]),
     ("kgv_validate_mempool_txs_in_parallel", _c.c_int, [_c.c_void_p, _c.c_void_p, _c.c_void_p, _c.c_uint64, _c.c_uint64, _c.c_void_p, _c.c_void_p, _u8p, _u8p,
                                                         _u8p, _u8p, _u8p, _u8p, _c.c_size_t, _c.POINTER(_c.c_size_t)]),
+    ("kgv_check_txs_standard_in_isolation", _c.c_int, [_c.c_void_p, _c.c_void_p, _c.c_void_p, _u8p, _u8p, _u8p]),
+    ("kgv_check_txs_standard_in_context", _c.c_int, [_c.c_void_p, _c.c_void_p, _c.c_void_p, _u8p, _u8p, _u8p, _u8p, _u8p]),
+    ("kgv_outputs_dust", _c.c_int, [_c.c_void_p, _c.c_void_p, _c.c_uint64, _u8p]),
+    ("kgv_validate_mempool_txs_with_policy", _c.c_int, [_c.c_void_p, _c.c_void_p, _c.c_void_p, _c.c_uint64, _c.c_uint64, _c.c_void_p, _c.c_void_p, _u8p, _u8p,
+                                                        _u8p, _u8p, _u8p, _u8p, _c.c_size_t, _c.POINTER(_c.c_size_t), _c.c_void_p, _u8p]),
     ("kgv_sigcache_create", _c.c_int, [_c.c_void_p, _c.c_uint64, _c.POINTER(_c.c_void_p)]),
     ("kgv_sigcache_destroy", None, [_c.c_void_p]),
     ("kgv_sigcache_clear", _c.c_int, [_c.c_void_p, _c.c_void_p]),

@@ -148,6 +148,19 @@ int kgv_isolation_run(kgv_ctx* ctx, const kgv_dev_batch& d, const kgv_tx_rules& 
                       kgv_tx_masses* dmasses, uint64_t* dnc, uint32_t* dlist, cudaStream_t st, const kgv_block_header_ctx* dheaders = nullptr,
                       const uint32_t* dtx_block = nullptr);
 
+// ---- the mempool's standardness policy (kgv_standard.cu) ----
+// check_transaction_standard_in_isolation of every tx of a device batch on st: dres gets the verdict (with gate, only a failure is
+// written), ddetail (may be null) the number it carries for every tx.  dmasses: the non-contextual masses.
+int kgv_standard_isolation_run(kgv_ctx* ctx, const kgv_dev_batch& d, const kgv_mempool_policy& p, const kgv_tx_masses* dmasses, bool gate,
+                               kgv_tx_result* dres, uint64_t* ddetail, cudaStream_t st);
+// check_transaction_standard_in_context on st.  dent: the populated entries of a validation call, or null to read d.entries.  dfee: the
+// fees, or null to check only the txs whose dres status is KGV_TX_OK with their dres fee (then only failures are written).  *dflag |= 1
+// when a reached fee check's mass * fee overflows u64.
+namespace kgv { struct DevEntry; }
+int kgv_standard_context_run(kgv_ctx* ctx, const kgv_dev_batch& d, const kgv::DevEntry* dent, const kgv_mempool_policy& p, const kgv_tx_masses* dmasses,
+                             const uint64_t* dsmass, const uint64_t* dfee, kgv_tx_result* dres, uint64_t* ddetail, unsigned long long* dflag,
+                             cudaStream_t st);
+
 // ---- pieces of the block body path shared between kgv_hash.cu and kgv_block_body.cu ----
 // enqueue Transaction::id() (hash == false) or hashing::tx::hash (true) of the first n txs of a device batch into out (32 B each)
 int kgv_tx_digests_run(kgv_ctx* ctx, const kgv_dev_batch& d, size_t n, uint64_t* out, bool hash);

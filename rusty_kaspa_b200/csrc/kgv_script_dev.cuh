@@ -487,21 +487,9 @@ struct DevScriptEngine {
     uint8_t res = KGV_SCRIPT_OK;
     uint32_t pos = 0;
     while (pos < n) {
-      const uint32_t op = sc[pos++];
-      const uint8_t* data = nullptr;
-      uint32_t dlen = 0;
-      if (op >= 0x01 && op <= 0x4b) {  // macros.rs:27-41, :54-61
-        if (n - pos < op) { res = KGV_SCRIPT_MALFORMED_PUSH; break; }
-        data = sc + pos; dlen = op; pos += op;
-      } else if (op >= 0x4c && op <= 0x4e) {  // macros.rs:9-26
-        const uint32_t lb = op == 0x4c ? 1 : op == 0x4d ? 2 : 4;
-        if (n - pos < lb) { res = KGV_SCRIPT_MALFORMED_PUSH_SIZE; break; }
-        uint64_t l = 0;
-        for (uint32_t i = 0; i < lb; i++) l |= (uint64_t)sc[pos + i] << (8 * i);
-        pos += lb;
-        if ((uint64_t)(n - pos) < l) { res = KGV_SCRIPT_MALFORMED_PUSH; break; }
-        data = sc + pos; dlen = (uint32_t)l; pos += (uint32_t)l;
-      }
+      uint32_t op, doff, dlen;
+      if ((res = script_next_op(sc, n, pos, op, doff, dlen))) break;  // macros.rs:9-61 (kgv_script_std.cuh)
+      const uint8_t* data = op >= 0x01 && op <= 0x4e ? sc + doff : nullptr;
       if (se_is_disabled(op)) { res = KGV_SCRIPT_OPCODE_DISABLED; break; }
       if (op == 0x65 || op == 0x66) { res = KGV_SCRIPT_OPCODE_RESERVED; break; }
       if (verify_only_push && op > 0x60) { res = KGV_SCRIPT_NOT_PUSH_ONLY; break; }

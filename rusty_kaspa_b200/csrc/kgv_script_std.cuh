@@ -45,6 +45,28 @@ struct InputPlan {
 
 KGV_HD bool sighash_type_allowed(uint32_t t) { return t == 1 || t == 2 || t == 4 || t == 0x81 || t == 0x82 || t == 0x84; }
 
+// the next opcode of sc[0..n) at pos as parse_script deserialises it (opcodes/macros.rs:9-61): op, and its pushed data at sc[doff..doff+dlen)
+// (dlen 0 for every opcode that is not OP_DATA_1..75 / OP_PUSHDATA1/2/4, OP_0 and OP_1..OP_16 included); pos moves past both.  Returns 0,
+// or KGV_SCRIPT_MALFORMED_PUSH_SIZE / KGV_SCRIPT_MALFORMED_PUSH when the length bytes or the data run past the end - the last opcode then.
+KGV_HD uint8_t script_next_op(const uint8_t* sc, uint32_t n, uint32_t& pos, uint32_t& op, uint32_t& doff, uint32_t& dlen) {
+  op = sc[pos++];
+  doff = pos; dlen = 0;
+  if (op >= 0x01 && op <= 0x4b) {
+    if (n - pos < op) return KGV_SCRIPT_MALFORMED_PUSH;
+    dlen = op;
+  } else if (op >= 0x4c && op <= 0x4e) {
+    const uint32_t lb = op == 0x4c ? 1 : op == 0x4d ? 2 : 4;
+    if (n - pos < lb) return KGV_SCRIPT_MALFORMED_PUSH_SIZE;
+    uint64_t l = 0;
+    for (uint32_t i = 0; i < lb; i++) l |= (uint64_t)sc[pos + i] << (8 * i);
+    pos += lb;
+    if ((uint64_t)(n - pos) < l) return KGV_SCRIPT_MALFORMED_PUSH;
+    doff = pos; dlen = (uint32_t)l;
+  }
+  pos += dlen;
+  return 0;
+}
+
 // one canonical direct data push at p[0..n): returns bytes consumed (0 if not canonical), data offset/len relative to p
 KGV_HD uint32_t canonical_push(const uint8_t* p, uint32_t n, uint32_t& doff, uint32_t& dlen) {
   if (n == 0) return 0;

@@ -17,9 +17,11 @@
 #include "kgv_txhash.cuh"
 #include "kgv_utxo.cuh"
 #include "kgv_context.cuh"
+#include "kgv_standard.cuh"
 
 #include <algorithm>
 #include <cstdio>
+#include <cstring>
 #include <vector>
 
 using namespace kgv;
@@ -1063,10 +1065,14 @@ extern "C" int kgv_validate_txs(kgv_ctx* ctx, kgv_utxo_table* t, const kgv_tx_ba
 // One synchronisation before the script phase reads the script bytes and the zero-divisor count.
 // iso (kgv_validate_mempool_txs_in_parallel): the isolation and finality rules run first, on the device; their verdicts gate the lookups
 // and the context rules, and their masses replace args[i].non_contextual_mass.  iso == null is kgv_validate_mempool_txs.
+// iso->policy (kgv_validate_mempool_txs_with_policy): standardness in isolation right after the isolation rules (its failures override
+// the gate) and standardness in context after the scripts, for the txs still KGV_TX_OK.
 struct MempoolIso {
   const kgv_tx_rules* rules;
   uint64_t past_median_time;
-  kgv_tx_masses* masses;  // caller's output, may be null
+  kgv_tx_masses* masses;                     // caller's output, may be null
+  const kgv_mempool_policy* policy = nullptr;
+  uint64_t* detail = nullptr;                // caller's output, may be null
 };
 static int mempool_core(kgv_ctx* ctx, kgv_utxo_table* t, const kgv_tx_batch* batch, uint64_t virtual_daa_score, const kgv_params* prm,
                         const kgv_mempool_tx_args* args, kgv_tx_result* results, uint64_t* storage_mass, kgv_utxo_entry* entries_out,
@@ -1081,14 +1087,14 @@ static int mempool_core(kgv_ctx* ctx, kgv_utxo_table* t, const kgv_tx_batch* bat
   CK(cudaSetDevice(ctx->device));
   const bool dev = kgv_ptr_is_device(results) != 0;
   for (const void* p : {(const void*)batch->txs, (const void*)args, (const void*)storage_mass, (const void*)entries_out, (const void*)(scripts_cap ? scripts_out : nullptr),
-                        (const void*)(iso ? iso->masses : nullptr)})
+                        (const void*)(iso ? iso->masses : nullptr), (const void*)(iso ? iso->detail : nullptr)})
     if (p && (kgv_ptr_is_device(p) != 0) != dev) { ctx->err = "kgv_validate_mempool_txs: the batch, args and outputs must all be host or all be device pointers"; return KGV_ERR_ARG; }
   kgv_dev_batch d;
   int rc = kgv_batch_to_device(ctx, batch, &d, false);
   if (rc) return rc;
   const size_t nt = d.n_txs, ni = d.n_inputs;
   // d_work: populated entries, input -> tx, verdicts, masses, script lengths and their offsets, the uploaded thresholds,
-  // counters [script bytes (64-bit), zero divisors, the scan's 32-bit total]
+  // counters [script bytes (64-bit), zero divisors, the scan's 32-bit total, the relay-fee overflow flag of the standardness policy]
   size_t o_ent = 0;
   size_t o_itx = al256(o_ent + ni * sizeof(DevEntry));
   size_t o_res = al256(o_itx + ni * 4);
@@ -1097,12 +1103,17 @@ static int mempool_core(kgv_ctx* ctx, kgv_utxo_table* t, const kgv_tx_batch* bat
   size_t o_off = al256(o_len + ni * 4);
   size_t o_args = al256(o_off + ni * 4);
   size_t o_cnt = al256(o_args + (args ? nt * sizeof(kgv_mempool_tx_args) : 0));
-  // with iso: its verdicts, max(compute, transient) per tx, the masses for a host caller, the large-transaction list
+  // with iso: its verdicts, max(compute, transient) per tx, the masses (for a host caller, or for the policy when the caller takes none),
+  // the large-transaction list, the policy's details for a host caller
+  const kgv_mempool_policy* pol = iso ? iso->policy : nullptr;
+  uint64_t* detail = iso ? iso->detail : nullptr;
+  const bool own_masses = iso && (iso->masses || pol) && !(dev && iso->masses);
   size_t o_iso = al256(o_cnt + 32);
   size_t o_nc = al256(o_iso + (iso ? nt * sizeof(kgv_tx_result) : 0));
   size_t o_ism = al256(o_nc + (iso ? nt * 8 : 0));
-  size_t o_lst = al256(o_ism + (iso && iso->masses && !dev ? nt * sizeof(kgv_tx_masses) : 0));
-  rc = kgv_reserve(ctx, &ctx->d_work, &ctx->d_work_cap, iso ? al256(o_lst + (nt + 1) * 4) : al256(o_cnt + 32));
+  size_t o_lst = al256(o_ism + (own_masses ? nt * sizeof(kgv_tx_masses) : 0));
+  size_t o_det = al256(o_lst + (iso ? (nt + 1) * 4 : 0));
+  rc = kgv_reserve(ctx, &ctx->d_work, &ctx->d_work_cap, iso ? al256(o_det + (pol && detail && !dev ? nt * 8 : 0)) : al256(o_cnt + 32));
   if (rc) return rc;
   uint8_t* S = ctx->d_work;
   DevEntry* dent = (DevEntry*)(S + o_ent);
@@ -1120,13 +1131,22 @@ static int mempool_core(kgv_ctx* ctx, kgv_utxo_table* t, const kgv_tx_batch* bat
   kgv_tx_result* gate = nullptr;
   uint64_t* dnc = nullptr;
   kgv_tx_masses* dism = nullptr;
+  uint64_t* ddet = pol && detail && !dev ? (uint64_t*)(S + o_det) : detail;
   if (iso) {
     gate = (kgv_tx_result*)(S + o_iso);
     dnc = (uint64_t*)(S + o_nc);
-    dism = dev ? iso->masses : (iso->masses ? (kgv_tx_masses*)(S + o_ism) : nullptr);
+    dism = own_masses ? (kgv_tx_masses*)(S + o_ism) : iso->masses;
     rc = kgv_isolation_run(ctx, d, *iso->rules, virtual_daa_score, iso->past_median_time, true, gate, dism, dnc, (uint32_t*)(S + o_lst), st);
     if (rc) return rc;
     STAGE("isolation");
+    if (pol) {
+      // the mempool checks standardness in isolation before consensus validates the tx: its failures take the gate's place
+      if ((rc = kgv_standard_isolation_run(ctx, d, *pol, dism, true, gate, ddet, st))) return rc;
+      STAGE("standard in isolation");
+    } else if (detail) {
+      if (dev) CK(cudaMemsetAsync(detail, 0, nt * 8, st));
+      else memset(detail, 0, nt * 8);
+    }
   }
   if (ni) {
     k_input_tx_index<<<nblk(nt, 128), 128, 0, st>>>(d.txs, (uint32_t)nt, itx);
@@ -1174,11 +1194,23 @@ static int mempool_core(kgv_ctx* ctx, kgv_utxo_table* t, const kgv_tx_batch* bat
     rc = scripts_with_engine(ctx, t, d, v, itx, dres);
     if (rc) return rc;
   }
+  unsigned long long* fee_overflow = cnt + 3;
+  if (pol) {
+    if ((rc = kgv_standard_context_run(ctx, d, dent, *pol, dism, dmass, nullptr, dres, ddet, fee_overflow, st))) return rc;
+    STAGE("standard in context");
+  }
   const cudaMemcpyKind k = dev ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost;
   CK(cudaMemcpyAsync(results, dres, nt * sizeof(kgv_tx_result), k, st));
   CK(cudaMemcpyAsync(storage_mass, dmass, nt * 8, k, st));
-  if (dism && !dev) CK(cudaMemcpyAsync(iso->masses, dism, nt * sizeof(kgv_tx_masses), k, st));
-  if (!dev) CK(cudaStreamSynchronize(st));
+  if (iso && iso->masses && !dev) CK(cudaMemcpyAsync(iso->masses, dism, nt * sizeof(kgv_tx_masses), k, st));
+  // the compute mass of a tx that reaches the fee check is at most 100 000 (standardness in isolation), so only a relay fee above
+  // u64::MAX / 100 000 can overflow: a device-pointer caller waits for the flag only then
+  unsigned long long overflow = 0;
+  const bool read_flag = pol && (!dev || pol->minimum_relay_transaction_fee > ~0ull / kgv::STD_MAX_TRANSACTION_MASS);
+  if (pol && detail && !dev) CK(cudaMemcpyAsync(detail, ddet, nt * 8, k, st));
+  if (read_flag) CK(cudaMemcpyAsync(&overflow, fee_overflow, 8, cudaMemcpyDeviceToHost, st));
+  if (!dev || read_flag) CK(cudaStreamSynchronize(st));
+  if (overflow) { ctx->err = "kgv_validate_mempool_txs_with_policy: compute mass * minimum_relay_transaction_fee overflows u64"; return KGV_ERR_ARG; }
   return KGV_OK;
 }
 
@@ -1198,6 +1230,18 @@ extern "C" int kgv_validate_mempool_txs_in_parallel(kgv_ctx* ctx, kgv_utxo_table
   if (!ctx || !t) return KGV_ERR_ARG;
   std::lock_guard<std::recursive_mutex> g(ctx->mu);
   const MempoolIso iso{rules, virtual_past_median_time, masses};
+  return mempool_core(ctx, t, batch, virtual_daa_score, prm, args, results, storage_mass, entries_out, scripts_out, scripts_cap, scripts_used, &iso);
+}
+
+// the mempool's admission path (validate_and_insert_transaction.rs:20-33, 142-159) with its standardness policy around the pipeline above
+extern "C" int kgv_validate_mempool_txs_with_policy(kgv_ctx* ctx, kgv_utxo_table* t, const kgv_tx_batch* batch, uint64_t virtual_daa_score,
+                                                    uint64_t virtual_past_median_time, const kgv_params* prm, const kgv_tx_rules* rules,
+                                                    const kgv_mempool_tx_args* args, kgv_tx_result* results, uint64_t* storage_mass, kgv_tx_masses* masses,
+                                                    kgv_utxo_entry* entries_out, uint8_t* scripts_out, size_t scripts_cap, size_t* scripts_used,
+                                                    const kgv_mempool_policy* policy, uint64_t* detail) {
+  if (!ctx || !t) return KGV_ERR_ARG;
+  std::lock_guard<std::recursive_mutex> g(ctx->mu);
+  const MempoolIso iso{rules, virtual_past_median_time, masses, policy, detail};
   return mempool_core(ctx, t, batch, virtual_daa_score, prm, args, results, storage_mass, entries_out, scripts_out, scripts_cap, scripts_used, &iso);
 }
 

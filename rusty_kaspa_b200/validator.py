@@ -12,6 +12,11 @@
         (tx_validation_in_isolation.rs:16-26, tx_validation_in_header_context.rs) and calc_non_contextual_masses (mass/mod.rs:248-269)
     TransactionValidator.validate_mempool_transactions_in_parallel_full  <->  validate_mempool_transactions_in_parallel
         (processor.rs:853-878): isolation -> finality -> UTXO context, per transaction
+    TransactionValidator.check_transaction_standard_in_isolation / check_transaction_standard_in_context / is_transaction_output_dust
+        <->  Mempool::check_transaction_standard_in_isolation / _in_context / is_transaction_output_dust
+        (mining/src/mempool/check_transaction_standard.rs:41-211), for a batch
+    TransactionValidator.validate_mempool_transactions_with_policy  <->  the mempool's admission order with its standardness policy
+        (mining/src/mempool/validate_and_insert_transaction.rs:20-33, 142-159)
     GpuUtxoSet.add_transactions                              <->  UtxoDiff::add_transaction (utxo_diff.rs:233-247)
     BlockBodyProcessor.validate_body_in_isolation / validate_body_in_context / validate_bodies  <->  BlockBodyProcessor
         (consensus/src/pipeline/body_processor/body_validation_in_isolation.rs:13-131, body_validation_in_context.rs:20-80), a window per call
@@ -37,6 +42,10 @@ ISOLATION_STATUS = {14: "NoTxInputs", 15: "TooManyInputs", 16: "TooBigSignatureS
                     22: "CoinbaseScriptPublicKeyTooLong", 23: "TxOutZero", 24: "TxOutTooHigh", 25: "OutputsValueOverflow",
                     26: "TotalTxOutTooHigh", 27: "TxDuplicateInputs", 28: "TxHasGas", 29: "SubnetworksDisabled", 30: "UnknownTxVersion",
                     31: "NotFinalized"}
+# KGV_TX_* verdicts of the standardness policy (include/kgv.h), by the reference's NonStandardError names
+STANDARD_STATUS = {32: "RejectVersion", 33: "RejectComputeMass", 34: "RejectTransientMass", 35: "RejectSignatureScriptSize",
+                   36: "RejectScriptPublicKeyVersion", 37: "RejectOutputScriptClass", 38: "RejectDust", 39: "RejectStorageMass",
+                   40: "RejectInputScriptClass", 41: "RejectSignatureCount", 42: "RejectInsufficientFee"}
 
 # kgv_block_header_ctx / kgv_body_result / kgv_block_masses
 BLOCK_HEADER_CTX_DTYPE = np.dtype([("hash_merkle_root", "u1", (32,)), ("daa_score", "<u8"), ("blue_score", "<u8"), ("past_median_time", "<u8"),
@@ -82,6 +91,19 @@ class TxRules(ctypes.Structure):
 
 
 assert ctypes.sizeof(TxRules) == 72
+
+
+class MempoolPolicy(ctypes.Structure):
+    """kgv_mempool_policy: the mempool Config fields the standardness policy reads (mining/src/mempool/config.rs); the defaults are the
+    reference's (DEFAULT_MINIMUM_RELAY_TRANSACTION_FEE, and TX_VERSION for both versions)."""
+    _fields_ = [("minimum_relay_transaction_fee", ctypes.c_uint64), ("minimum_standard_transaction_version", ctypes.c_uint16),
+                ("maximum_standard_transaction_version", ctypes.c_uint16), ("pad_", ctypes.c_uint8 * 4)]
+
+    def __init__(self, minimum_relay_transaction_fee=1000, minimum_standard_transaction_version=0, maximum_standard_transaction_version=0):
+        super().__init__(minimum_relay_transaction_fee, minimum_standard_transaction_version, maximum_standard_transaction_version)
+
+
+assert ctypes.sizeof(MempoolPolicy) == 16
 
 
 class SigRequest(ctypes.Structure):
@@ -360,6 +382,79 @@ class TransactionValidator:
             cap = used.value
         self.ctx._check(rc)
         return res, mass, masses, ent[:ni], arena[:used.value]
+
+    def check_transaction_standard_in_isolation(self, batch, masses, policy=None):
+        """check_transaction_standard_in_isolation for every tx (kgv_check_txs_standard_in_isolation); masses: TX_MASSES_DTYPE[n_txs], the
+        calculated_non_contextual_masses.  Returns (RESULT_DTYPE[n_txs]: status 0 or 32..38, fail_input the input / output index of the
+        indexed variants; u64[n_txs] details: the number each verdict carries)."""
+        policy = policy or MempoolPolicy()
+        m = np.ascontiguousarray(masses, dtype=TX_MASSES_DTYPE)
+        res = np.zeros(batch.n_txs, dtype=RESULT_DTYPE)
+        det = np.zeros(batch.n_txs, dtype=np.uint64)
+        cb = _c_batch(batch, with_entries=False)
+        self.ctx._check(self._lib.kgv_check_txs_standard_in_isolation(self.ctx._h, ctypes.byref(cb), ctypes.byref(policy), m.ctypes.data, res.ctypes.data,
+                                                                      det.ctypes.data))
+        return res, det
+
+    def check_transaction_standard_in_context(self, batch, masses, storage_mass, fee, policy=None):
+        """check_transaction_standard_in_context for every tx of a populated batch (kgv_check_txs_standard_in_context): storage_mass is
+        tx.mass(), fee the calculated_fee, masses the non-contextual masses.  Returns (RESULT_DTYPE[n_txs]: status 0 or 39..42, fee echoed;
+        u64[n_txs] details)."""
+        policy = policy or MempoolPolicy()
+        m = np.ascontiguousarray(masses, dtype=TX_MASSES_DTYPE)
+        sm = np.ascontiguousarray(storage_mass, dtype=np.uint64)
+        fe = np.ascontiguousarray(fee, dtype=np.uint64)
+        res = np.zeros(batch.n_txs, dtype=RESULT_DTYPE)
+        det = np.zeros(batch.n_txs, dtype=np.uint64)
+        cb = _c_batch(batch, with_entries=True)
+        self.ctx._check(self._lib.kgv_check_txs_standard_in_context(self.ctx._h, ctypes.byref(cb), ctypes.byref(policy), m.ctypes.data, sm.ctypes.data,
+                                                                    fe.ctypes.data, res.ctypes.data, det.ctypes.data))
+        return res, det
+
+    def is_transaction_output_dust(self, batch, minimum_relay_transaction_fee=1000):
+        """is_transaction_output_dust for every output of the batch (kgv_outputs_dust).  Returns bool[n_outputs]."""
+        n = len(batch.outputs)
+        out = np.zeros(max(n, 1), dtype=np.uint8)
+        cb = _c_batch(batch, with_entries=False)
+        self.ctx._check(self._lib.kgv_outputs_dust(self.ctx._h, ctypes.byref(cb), int(minimum_relay_transaction_fee), out.ctypes.data))
+        return out[:n].astype(bool)
+
+    def validate_mempool_transactions_with_policy(self, utxo_set, batch, virtual_daa_score, virtual_past_median_time, policy=None, rules=None,
+                                                  feerate_threshold=None, supplied=None):
+        """validate_mempool_transactions_in_parallel_full with the standardness policy (kgv_validate_mempool_txs_with_policy): standardness in
+        isolation, isolation, finality, UTXO context, scripts, then standardness in context for the txs still Ok.  policy=None is
+        accept_non_standard = true.  Returns (RESULT_DTYPE[n_txs], storage masses u64[n_txs], TX_MASSES_DTYPE[n_txs], every input's final
+        entry ENTRY_DTYPE[n_inputs], the byte arena of their scripts, u64[n_txs] details)."""
+        rules = rules or TxRules()
+        n, ni = batch.n_txs, batch.n_inputs
+        if supplied is not None:
+            given = batch.entries.copy()
+            given["pad_"][:, 0] = np.where(np.asarray(supplied, dtype=bool), 0, 1)
+            batch = TxBatch(batch.txs, batch.inputs, batch.outputs, given, batch.arena)
+        cb = _c_batch(batch, with_entries=supplied is not None)
+        args = None
+        if feerate_threshold is not None:
+            args = np.zeros(n, dtype=MEMPOOL_ARGS_DTYPE)
+            args["feerate_threshold"] = feerate_threshold
+        res = np.zeros(n, dtype=RESULT_DTYPE)
+        mass = np.zeros(n, dtype=np.uint64)
+        masses = np.zeros(n, dtype=TX_MASSES_DTYPE)
+        det = np.zeros(n, dtype=np.uint64)
+        ent = np.zeros(max(ni, 1), dtype=ENTRY_DTYPE)
+        used = ctypes.c_size_t()
+        cap = len(batch.arena) + 128 * ni
+        for _ in range(2):  # the call reports the size it needs before any signature is verified
+            arena = np.zeros(max(cap, 8), dtype=np.uint8)
+            rc = self._lib.kgv_validate_mempool_txs_with_policy(self.ctx._h, utxo_set._h, ctypes.byref(cb), int(virtual_daa_score), int(virtual_past_median_time),
+                                                                ctypes.byref(self.params), ctypes.byref(rules), None if args is None else args.ctypes.data,
+                                                                res.ctypes.data, mass.ctypes.data, masses.ctypes.data, ent.ctypes.data, arena.ctypes.data,
+                                                                len(arena), ctypes.byref(used), None if policy is None else ctypes.byref(policy),
+                                                                det.ctypes.data)
+            if rc != ERR_NOMEM or used.value <= cap:
+                break
+            cap = used.value
+        self.ctx._check(rc)
+        return res, mass, masses, ent[:ni], arena[:used.value], det
 
     def validate_transactions_with_muhash_in_parallel(self, utxo_set, batch, pov_daa_score, flags=FLAGS_FULL):
         """utxo_validation.rs:282-309: as validate_transactions_in_parallel, plus the combined MuHash::from_transaction of the
