@@ -102,11 +102,12 @@ __global__ void __launch_bounds__(128) k_build_gtab(uint32_t* __restrict__ gtab)
 }
 
 // ---- per-launch key cache: the key part of a verification done once per distinct public key of a verify launch ----
-// Records per launch at most (2^17 x 10304 B = 1.35 GB of comb records with their joint tables, 2^17 x 560 B = 73 MB of plain ones).
+// Records per launch at most (2^17 x 8320 B = 1.09 GB of comb-form records, 2^17 x 560 B = 73 MB of plain ones).
 #define KGV_KEY_RECORDS_MAX (1u << 17)
 // Fewest uses per key on average for comb records: the comb's preparation (~1 800 products per key against ~400, ~2 700 with the joint
-// table) must be paid back by its shorter ladder (~700, with the joint table ~1 000 products fewer per verify); measured +20 % at 10 uses
-// per key before the joint table and faster still with it at 8 to 50 uses (DESIGN.md §5), not below.
+// table, ~2 200 for the comb-form record that keeps only P and the joint table: 2.24 ms for 70 794 keys against 2.99 ms) must be paid
+// back by its shorter ladder (~700, with the joint table ~1 000 products fewer per verify); measured +20 % at 10 uses per key before the
+// joint table and faster still with it at 8 to 50 uses (DESIGN.md §5), not below.  Not re-tuned for the cheaper preparation.
 #ifndef KGV_COMB_USES
 #define KGV_COMB_USES 8
 #endif
@@ -114,7 +115,7 @@ enum { KGV_KEYS_INLINE = 0, KGV_KEYS_PLAIN = 1, KGV_KEYS_COMB = 2 };
 // The form of a launch's key part, uniform over the launch: records when its keys are used twice on average (at most n/2 distinct keys)
 // and fit the cap; then EVERY key has one.  A warp pays for the inline key path of any of its lanes, so records for the repeated keys
 // alone leave singleton lanes costing whole warps; a batch of mostly distinct keys makes no records at all and pays only the dedup pass.
-// Comb records (key_comb_build + key_joint_build, ecmult_joint) when the keys are used at least KGV_COMB_USES times on average, plain ones (key_rec_build) below.
+// Comb-form records (key_joint_record_build, ecmult_joint) when the keys are used at least KGV_COMB_USES times on average, plain ones (key_rec_build) below.
 // Host-callable too: kgv_debug_key_form reports the form a launch took by this same rule.
 __host__ __device__ __forceinline__ int key_form(uint32_t n_rec, size_t n) {
   if (n_rec > KGV_KEY_RECORDS_MAX || 2 * (size_t)n_rec > n) return KGV_KEYS_INLINE;
@@ -129,14 +130,14 @@ struct KeySlot {
 struct KeyCacheView {
   const KeySlot* table;
   const uint32_t* item_slot;  // item -> table slot (only the items the launch verifies are set)
-  const uint32_t* recs;       // records, KGV_KR_WORDS or KGV_KJ_WORDS words each
+  const uint32_t* recs;       // records, KGV_KR_WORDS or KGV_JR_WORDS words each
   const uint32_t* n_rec;      // distinct keys of the launch; nullptr: no key cache
   // the key source of item i: its record and the launch's form, or no record (the launch makes none)
   __device__ __forceinline__ KeySrc key_of(size_t i, size_t n) const {
     const int f = n_rec ? key_form(*n_rec, n) : KGV_KEYS_INLINE;
     if (f == KGV_KEYS_INLINE) return KeySrc{nullptr, false};
     const bool comb = f == KGV_KEYS_COMB;
-    return KeySrc{recs + (size_t)(table[item_slot[i]].rec - 1) * (comb ? KGV_KJ_WORDS : KGV_KR_WORDS), comb};
+    return KeySrc{recs + (size_t)(table[item_slot[i]].rec - 1) * (comb ? KGV_JR_WORDS : KGV_KR_WORDS), comb};
   }
 };
 
@@ -207,10 +208,15 @@ __global__ void __launch_bounds__(256) k_key_dedup(const uint8_t* __restrict__ p
   item_slot[i] = s;
 }
 
-// One thread per record: the key's verdict, and for a good key its comb and joint table (key_comb_build, key_joint_build) or its odd-multiples table and zs (key_rec_build).
-// The verify kernels' occupancy (168 registers): unbounded, ptxas takes 255 and two blocks per SM.
+// One thread per record: the key's verdict, and for a good key P and its joint table (key_joint_record_build) or its odd-multiples table and zs (key_rec_build).
+// It uses no shared memory, so its occupancy is its own (unbounded, ptxas takes 255 registers and two blocks per SM).  Five blocks per SM
+// (96 registers, 84 480 resident threads: the bench shape's 70 794 records in one wave) measured 2.24 ms at the bench shape against
+// 2.43 ms at three blocks (168 registers, 1.4 waves) and 2.46 ms at four, despite the larger spill code (DESIGN.md §4 K1).
+#ifndef KGV_PREP_BLOCKS_PER_SM
+#define KGV_PREP_BLOCKS_PER_SM 5
+#endif
 template <bool ECDSA>
-__global__ void __launch_bounds__(KGV_BLOCK, KGV_BLOCKS_PER_SM) k_key_prepare(const uint8_t* __restrict__ pk, size_t n_arg, const uint32_t* __restrict__ n_dev,
+__global__ void __launch_bounds__(KGV_BLOCK, KGV_PREP_BLOCKS_PER_SM) k_key_prepare(const uint8_t* __restrict__ pk, size_t n_arg, const uint32_t* __restrict__ n_dev,
                                                                               const uint32_t* __restrict__ rec_rep, const uint32_t* __restrict__ n_rec,
                                                                               uint32_t* __restrict__ recs) {
   const size_t n = n_dev ? (size_t)*n_dev : n_arg;
@@ -219,11 +225,8 @@ __global__ void __launch_bounds__(KGV_BLOCK, KGV_BLOCKS_PER_SM) k_key_prepare(co
   if (r >= *n_rec || f == KGV_KEYS_INLINE) return;
   uint32_t w[9];
   key_words<false, ECDSA>(w, pk, rec_rep[r]);
-  if (f == KGV_KEYS_COMB) {
-    uint32_t* rec = recs + (size_t)r * KGV_KJ_WORDS;
-    key_comb_build(rec, ECDSA ? w[8] : 2u, w);
-    if (rec[KGV_KC_STATUS] == KGV_ST_VALID) key_joint_build(rec);
-  } else key_rec_build(recs + (size_t)r * KGV_KR_WORDS, ECDSA ? w[8] : 2u, w);
+  if (f == KGV_KEYS_COMB) key_joint_record_build(recs + (size_t)r * KGV_JR_WORDS, ECDSA ? w[8] : 2u, w);
+  else key_rec_build(recs + (size_t)r * KGV_KR_WORDS, ECDSA ? w[8] : 2u, w);
 }
 
 // Each thread verifies KGV_ITEMS consecutive-stride items (i = tid + j * total_threads: coalesced) and shares
@@ -578,7 +581,7 @@ static int key_cache_launch(kgv_ctx* ctx, const uint8_t* dpk, size_t n, bool ecd
   while (slots < 2 * n) slots <<= 1;                       // load factor <= 1/2
   const uint32_t cap = (uint32_t)(n / 2 < KGV_KEY_RECORDS_MAX ? n / 2 : KGV_KEY_RECORDS_MAX);  // key_form's bounds
   const size_t cap_comb = n / KGV_COMB_USES < KGV_KEY_RECORDS_MAX ? n / KGV_COMB_USES : KGV_KEY_RECORDS_MAX;
-  const size_t rec_bytes = std::max((size_t)cap * KGV_KR_WORDS, cap_comb * KGV_KJ_WORDS) * 4;
+  const size_t rec_bytes = std::max((size_t)cap * KGV_KR_WORDS, cap_comb * KGV_JR_WORDS) * 4;
   const size_t o_tab = 256, o_item = o_tab + (size_t)slots * sizeof(KeySlot);
   const size_t o_rep = (o_item + n * 4 + 255) & ~(size_t)255, o_rec = (o_rep + (size_t)cap * 4 + 255) & ~(size_t)255;
   int rc = kgv_reserve(ctx, &ctx->d_keys[ecdsa], &ctx->d_keys_cap[ecdsa], o_rec + rec_bytes);

@@ -464,13 +464,15 @@ KGV_HD bool ge_lift_x(fe& y, const fe& x, bool odd) {
 // per-thread table of odd multiples {1,3,...,15} * P, "effective affine"
 // ------------------------------------------------------------------------------------------
 // Tab is an accessor with  void put(int entry, int word, uint32_t v)  and  uint32_t get(int entry, int word)
-// (entry 0..7, word 0..15: x limbs then y limbs).
+// (entry 0..NE-1, word 0..15: x limbs then y limbs).
 //
 // After the call, entry j holds the affine coordinates of (2j+1)*P on the isomorphic curve
 // E' : y^2 = x^3 + 7*zs^6, where zs (returned) is such that a Jacobian point (X,Y,Z) on E'
 // corresponds to (X, Y, Z*zs) on secp256k1.  lambda*(entry) = (beta*x, y) also holds on E'.
-template <class Tab>
+// NE: the number of entries, 8 for the verify ladders; the comb-form record builds {1,3,5,7} * T per tooth (NE = 4).
+template <int NE = 8, class Tab>
 KGV_HD void build_odd_table(Tab& tab, fe& zs, const fe& px, const fe& py) {
+  static_assert(NE >= 2 && NE <= 8, "build_odd_table: 2 to 8 entries");
   // D = 2P (from affine input)
   gej d;
   d.x = px; d.y = py; fe_set_u32(d.z, 1); d.inf = false;
@@ -484,20 +486,20 @@ KGV_HD void build_odd_table(Tab& tab, fe& zs, const fe& px, const fe& py) {
   fe_mul(t.y, py, zd3);
   fe_set_u32(t.z, 1);
   t.inf = false;
-  fe H[7];
+  fe H[NE - 1];
 #pragma unroll
   for (int w = 0; w < 8; w++) { tab.put(0, w, t.x.v[w]); tab.put(0, 8 + w, t.y.v[w]); }
 #pragma unroll
-  for (int j = 1; j < 8; j++) {
+  for (int j = 1; j < NE; j++) {
     gej_add_ge(t, d.x, d.y, &H[j - 1]);
 #pragma unroll
     for (int w = 0; w < 8; w++) { tab.put(j, w, t.x.v[w]); tab.put(j, 8 + w, t.y.v[w]); }
   }
-  // bring every entry to the Z of the last one: entry j *= (Z_7/Z_j)^{2,3}, Z_7/Z_j = H_{j+1}...H_7
-  fe acc = H[6];
+  // bring every entry to the Z of the last one: entry j *= (Z_last/Z_j)^{2,3}, Z_last/Z_j = H_{j+1}...H_last
+  fe acc = H[NE - 2];
 #pragma unroll
-  for (int j = 6; j >= 0; j--) {
-    if (j < 6) fe_mul(acc, acc, H[j]);
+  for (int j = NE - 2; j >= 0; j--) {
+    if (j < NE - 2) fe_mul(acc, acc, H[j]);
     fe a2, a3, ex, ey;
     fe_sqr(a2, acc);
     fe_mul(a3, a2, acc);
@@ -717,7 +719,7 @@ KGV_HD void recode_joint(uint32_t* h, bool& fix, const uint32_t* m) {
 // the v field (0..7, d = 2v - 7) of digit i = 11t + w
 KGV_HD uint32_t joint_digit(const uint32_t* h, int i) { return (h[i / 10] >> (3 * (i % 10))) & 7u; }
 // jt: the joint table, entry 32t + 8a + k (16 words at word 16(32t + 8a + k)) = (2a+1) T + (2k-7) lambda T, T = 2^(32t) P, true affine
-// (key_joint_build, kgv_verify.cuh).  The entry for digit i of both halves, with the GLV signs ng folded in: e0 T + e1 lambda T =
+// (joint_table_build, kgv_verify.cuh).  The entry for digit i of both halves, with the GLV signs ng folded in: e0 T + e1 lambda T =
 // sign(e0) (|e0| T + sign(e0) e1 lambda T); neg: negate its y.
 KGV_HD const uint32_t* joint_entry(const uint32_t* jt, const uint32_t (*h)[5], const bool* ng, int i, bool& neg) {
   const uint32_t u0 = joint_digit(h[0], i), u1 = joint_digit(h[1], i);
@@ -739,7 +741,8 @@ KGV_HD void gen_fields(gej& R, const uint32_t* kG, int sh, const uint32_t* gtab,
     }
   }
 }
-// rec: the comb record (entry 0 = P); jt: its joint table.  gtab: as for ecmult_comb.
+// rec: a record whose first 16 words are P, true affine (the comb-form record, KGV_JR_*, or the reference comb record, KGV_KC_*: entry 0);
+// jt: its joint table.  gtab: as for ecmult_comb.
 // Windows w = 10..0 with three doublings between them (30 in all); window w adds, per tooth t, ONE joint entry for digit 11t + w of both
 // halves (44 key additions, no beta products).  The generator's fields at bits 32j..32j+15 weigh 1 (after window 0); those at bits
 // 32j+16..32j+31 weigh 2^16 = 2 * 2^(3*5): window 5's three doublings are split 2 + 1 around them.  Both use the eight tables of ecmult_comb
@@ -795,7 +798,7 @@ KGV_HD void ecmult_joint(gej& R, const uint32_t* kP, const uint32_t* kG, const u
   }
   gen_fields(R, kG, 0, gtab, gload);
   // parity corrections, at most one addition: -(s0 P + s1 lambda P) = -s0 (P + s0 s1 lambda P) is joint entry (a = 1, b = s0 s1) of
-  // tooth 0; one of them alone is comb entry 0, times beta for the lambda half
+  // tooth 0; one of them alone is P (rec's first 16 words), times beta for the lambda half
   if (fix[0] && fix[1]) {
     gload(ex, ey, jt + 16 * (ng[0] == ng[1] ? 4 : 3));
     if (!ng[0]) fe_neg(ey, ey);

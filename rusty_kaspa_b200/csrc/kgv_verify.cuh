@@ -38,15 +38,24 @@ KGV_HD bool key_lift(fe& x, fe& y, uint32_t tag, const uint32_t* pkw) {
 #define KGV_KR_ZS 128
 #define KGV_KR_STATUS 136
 #define KGV_KR_WORDS 140  // 560 bytes
-// Comb key record, for launches whose keys repeat often (key_form, kgv_lib.cu; ecmult_comb): four teeth of odd multiples, true affine.
-// Words, 64-byte entries, records 64-byte aligned:
+// The comb form's record, for launches whose keys repeat often (key_form, kgv_lib.cu), as k_key_prepare builds it
+// (key_joint_record_build) and the verify kernels read it (ecmult_joint).  Words, 64-byte entries, records 64-byte aligned:
+//   [0, 16)     P, true affine (x limbs, then y limbs, canonical): ecmult_joint's parity fix
+//   16          the key's verdict, as KGV_KR_STATUS; the rest of the record is unset when the key does not parse
+//   [32, 2080)  the joint table: entry 32t + 8a + k = (2a+1) * T + (2k-7) * lambda * T, T = 2^(32t) * P, for t = 0..3, a = 0..3,
+//               k = 0..7, at word 32 + 16(32t + 8a + k): x limbs, then y limbs, true affine
+#define KGV_JR_P 0
+#define KGV_JR_STATUS 16
+#define KGV_JR_JOINT 32
+#define KGV_JR_WORDS (KGV_JR_JOINT + 4 * 32 * 16)  // 2080 words, 8320 bytes
+// The host-side reference pair the comb-form record is checked against (the device builds neither record):
+// comb key record (key_comb_build; ecmult_comb): four teeth of odd multiples, true affine.  Words, 64-byte entries:
 //   [0, 512)   entry 8t + e = (2e+1) * 2^(32t) * P for tooth t = 0..3, e = 0..7, at word 16(8t + e): x limbs, then y limbs
 //   512        the key's verdict, as KGV_KR_STATUS
 #define KGV_KC_STATUS 512
 #define KGV_KC_WORDS 528  // 2112 bytes
-// The comb form's record as the verify kernels use it (ecmult_joint): the comb record above, then the joint table
-//   [528, 2576) entry 32t + 8a + k = (2a+1) * T + (2k-7) * lambda * T, T = 2^(32t) * P, for t = 0..3, a = 0..3, k = 0..7, at word
-//               528 + 16(32t + 8a + k): x limbs, then y limbs, true affine
+// the comb record above, then its joint table (key_joint_build), the same entries as the comb-form record's
+//   [528, 2576) entry 32t + 8a + k at word 528 + 16(32t + 8a + k)
 #define KGV_KJ_JOINT KGV_KC_WORDS
 #define KGV_KJ_WORDS (KGV_KJ_JOINT + 4 * 32 * 16)  // 2576 words, 10304 bytes
 
@@ -111,6 +120,7 @@ KGV_HD void key_rec_build(uint32_t* rec, uint32_t tag, const uint32_t* pkw) {
 // fills a comb key record: the tooth bases 2^(32t) * P by 96 doublings; each tooth's table as build_odd_table builds one, from the base's
 // Jacobian X, Y (affine on the curve with Z scale Z: the table's scale is then zs * Z); one inversion of the four scales' product
 // (Montgomery's trick) brings all 32 entries to true affine.
+// Host-side reference only (with key_joint_build and ecmult_comb): the device builds key_joint_record_build's record instead.
 KGV_HD void key_comb_build(uint32_t* rec, uint32_t tag, const uint32_t* pkw) {
   fe x, y;
   uint8_t st = KGV_ST_PK_PARSE;
@@ -157,7 +167,8 @@ KGV_HD void key_comb_build(uint32_t* rec, uint32_t tag, const uint32_t* pkw) {
   rec[KGV_KC_STATUS] = st;
 }
 
-// fills the joint table of a comb record whose verdict is KGV_ST_VALID (after key_comb_build, same thread).  Per tooth t and pair
+// fills the joint table of a comb record whose verdict is KGV_ST_VALID (after key_comb_build).  The host-side reference of
+// joint_table_build, which builds the same entries without the comb record.  Per tooth t and pair
 // p = (a, j): A = (2a+1) T (comb entry 8t + a) and B = (2j+1) lambda T = (beta x_j, y_j) of comb entry 8t + j; A + B is entry k = j + 4,
 // A - B entry k = 3 - j, both affine additions over the one denominator beta x_j - x_A.  The 64 denominators share one inversion
 // (Montgomery's trick), with the joint area itself as scratch: beta x_j of tooth t in words 0..7 of entry (t, 0, 3 - j) and the prefix
@@ -240,6 +251,127 @@ KGV_HD void key_joint_build(uint32_t* rec) {
   }
 }
 
+// build_odd_table's Tab over four entries of local field-element arrays (x limbs in x[e], y limbs in y[e])
+struct FeTab {
+  fe* x;
+  fe* y;
+  KGV_HD void put(int e, int w, uint32_t v) {
+    if (w < 8) x[e].v[w] = v;
+    else y[e].v[w - 8] = v;
+  }
+  KGV_HD uint32_t get(int e, int w) const { return w < 8 ? x[e].v[w] : y[e].v[w - 8]; }
+};
+// fills the joint table jt (KGV_JR_JOINT's layout) of the key P = (px, py), affine.  It builds only the tooth entries the table is made
+// of, A = (2a+1) T_t and B = (2j+1) lambda T_t for a, j < 4, and runs one inversion:
+//  1. per tooth: the base T_t = 2^(32t) P by 32 doublings, then {1,3,5,7} T_t by build_odd_table<4> in the tooth's frame: entry e is
+//     (X'_e, Y'_e) = (x_e Z_t^2, y_e Z_t^3), Z_t the table's scale times the base's Z; and beta X'_e.
+//  2. one Montgomery trick over the 64 frame denominators d'_p = beta X'_j - X'_a (pair p = 16t + 4a + j) and then the four Z_t;
+//     one fe_inv.
+//  3. going back down, the Z_t's inverses bring the 16 tooth entries and their beta X to true affine, in place (3 products each), then
+//     per pair 1 / (beta x_j - x_a) = Z_t^2 / d'_p (one product) and A + B (entry k = j + 4), A - B (k = 3 - j) as key_joint_build
+//     forms them (6 products).
+// No d'_p is zero (key_joint_build's argument; Z_t != 0).
+// All scratch (tooth entries, denominators, prefix products: 5.9 KB) is in local arrays, which the hardware interleaves across a warp's
+// lanes: a warp's access to one element is coalesced.  The record itself is 8 KB per thread, so a warp's access to it touches 32 sectors
+// at an 8 KB stride; only the 256 16-byte stores of the finished entries go there (with the scratch in the record, k_key_prepare took
+// 2.54 ms at the bench shape, 2.24 ms with it in local arrays; DESIGN.md §4 K1).
+// About 1 000 products: 16 by beta, 67 + 4 * 5 + 126 for the trick, 48 to true affine, 7 per pair (448), one fe_inv.
+KGV_HD void joint_table_build(uint32_t* jt, const fe& px, const fe& py) {
+  const fe beta = {KGV_BETA_LIMBS};
+  fe ex[16], ey[16], eb[16];  // tooth t, entry e at 4t + e: x, y, beta x (in the frame, then true affine)
+  fe dn[64], pre[64];         // d'_p and the prefix product of d'_0..d'_p
+  fe zs[4], zp[5];            // Z_t; zp[t]: the prefix product of the 64 denominators and Z_0..Z_{t-1}
+  gej b;
+  b.x = px; b.y = py; fe_set_u32(b.z, 1); b.inf = false;
+#pragma unroll 1
+  for (int t = 0; t < 4; t++) {
+    if (t) gej_double_n(b, 32);
+    FeTab tab{ex + 4 * t, ey + 4 * t};
+    fe z;
+    build_odd_table<4>(tab, z, b.x, b.y);
+    fe_mul(zs[t], z, b.z);
+#pragma unroll 1
+    for (int e = 0; e < 4; e++) fe_mul(eb[4 * t + e], ex[4 * t + e], beta);
+  }
+  fe acc;
+#pragma unroll 1
+  for (int p = 0; p < 64; p++) {
+    const int t = p >> 4, a = (p >> 2) & 3, j = p & 3;
+    fe d;
+    fe_sub(d, eb[4 * t + j], ex[4 * t + a]);
+    if (p) fe_mul(acc, acc, d);
+    else acc = d;
+    dn[p] = d;
+    pre[p] = acc;
+  }
+  zp[0] = acc;
+#pragma unroll 1
+  for (int t = 0; t < 4; t++) {
+    fe_mul(acc, acc, zs[t]);
+    zp[t + 1] = acc;
+  }
+  fe inv;
+  fe_inv(inv, acc);
+#pragma unroll 1
+  for (int t = 3; t >= 0; t--) {
+    fe zi, zi2, zi3;
+    fe_mul(zi, inv, zp[t]);
+    fe_mul(inv, inv, zs[t]);
+    fe_sqr(zi2, zi);
+    fe_mul(zi3, zi2, zi);
+    fe_sqr(zs[t], zs[t]);  // Z_t^2 from here on
+#pragma unroll 1
+    for (int e = 4 * t; e < 4 * t + 4; e++) {
+      fe_mul(ex[e], ex[e], zi2);
+      fe_mul(ey[e], ey[e], zi3);
+      fe_mul(eb[e], eb[e], zi2);
+    }
+  }
+  // inv = 1 / (d'_0 ... d'_63)
+#pragma unroll 1
+  for (int p = 63; p >= 0; p--) {
+    const int t = p >> 4, a = (p >> 2) & 3, j = p & 3;
+    fe di;
+    if (p) {
+      fe_mul(di, inv, pre[p - 1]);
+      fe_mul(inv, inv, dn[p]);
+    } else {
+      di = inv;
+    }
+    fe_mul(di, di, zs[t]);  // 1 / (beta x_j - x_a)
+    const fe xa = ex[4 * t + a], ya = ey[4 * t + a], bx = eb[4 * t + j], yb = ey[4 * t + j];
+#pragma unroll 1
+    for (int sgn = 0; sgn < 2; sgn++) {  // A + B (k = j + 4), then A - B (k = 3 - j)
+      fe l, x3, y3, t1;
+      if (sgn) fe_neg(t1, yb);
+      else t1 = yb;
+      fe_sub(t1, t1, ya);
+      fe_mul(l, t1, di);                 // slope
+      fe_sqr(x3, l);
+      fe_sub(x3, x3, xa);
+      fe_sub(x3, x3, bx);                // x3 = l^2 - xA - xB
+      fe_sub(t1, xa, x3);
+      fe_mul(y3, l, t1);
+      fe_sub(y3, y3, ya);                // y3 = l (xA - x3) - yA
+      uint32_t* en = jt + 16 * (32 * t + 8 * a + (sgn ? 3 - j : j + 4));
+      fe_st(en, x3);
+      fe_st(en + 8, y3);
+    }
+  }
+}
+// fills a comb-form record (KGV_JR_*; tag as for key_lift)
+KGV_HD void key_joint_record_build(uint32_t* rec, uint32_t tag, const uint32_t* pkw) {
+  fe x, y;
+  uint8_t st = KGV_ST_PK_PARSE;
+  if (key_lift(x, y, tag, pkw)) {
+    fe_st(rec + KGV_JR_P, x);
+    fe_st(rec + KGV_JR_P + 8, y);
+    joint_table_build(rec + KGV_JR_JOINT, x, y);
+    st = KGV_ST_VALID;
+  }
+  rec[KGV_JR_STATUS] = st;
+}
+
 // Where the key part of a verification comes from: the key's comb record (comb), its plain record, or none (rec == nullptr: the key is
 // lifted and its odd-multiples table built per signature).
 struct KeySrc {
@@ -247,14 +379,14 @@ struct KeySrc {
   bool comb;
 };
 // a prepared key's verdict: false when the key does not parse
-KGV_HD bool key_rec_valid(const KeySrc& key) { return key.rec[key.comb ? KGV_KC_STATUS : KGV_KR_STATUS] == KGV_ST_VALID; }
+KGV_HD bool key_rec_valid(const KeySrc& key) { return key.rec[key.comb ? KGV_JR_STATUS : KGV_KR_STATUS] == KGV_ST_VALID; }
 // R = kP*P + kG*G and zt, the true Z of R (unset when R is infinity).  px, py: the key, read on the inline path only.
 template <class Tab, class GLoad, class Trace = NoTrace>
 KGV_HD void ecmult_key(gej& R, fe& zt, const KeySrc& key, const fe& px, const fe& py, const uint32_t* kP, const uint32_t* kG, Tab& tab,
                        const uint32_t* gtab, GLoad gload, Trace trace = Trace()) {
   fe zs;
   if (key.comb) {
-    ecmult_joint(R, kP, kG, key.rec, key.rec + KGV_KJ_JOINT, tab, gtab, gload);
+    ecmult_joint(R, kP, kG, key.rec + KGV_JR_P, key.rec + KGV_JR_JOINT, tab, gtab, gload);
   } else {
     if (key.rec) key_rec_load(tab, zs, key.rec);
     else build_odd_table(tab, zs, px, py);
