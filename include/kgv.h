@@ -552,7 +552,8 @@ int kgv_replay_window(kgv_ctx* ctx, kgv_utxo_table* t, const kgv_tx_batch* batch
  * [group_first_block[g], group_first_block[g+1]) of that window (the mergeset of one chain block); values768[g] = (numerator || denominator) of
  * MuHash::from_transaction over the accepted transactions of the group incl. accepted coinbases (utxo_validation.rs:116-121,144; spent entries as
  * found at each block's position).  Must directly follow that kgv_replay_window call (no other batch call in between).
- * With kgv_muhash_prefix_combine and kgv_muhash_finalize_batch this yields every chain block's utxo_commitment of a window (:188-192). */
+ * With kgv_muhash_prefix_combine and kgv_muhash_finalize_batch this yields every chain block's utxo_commitment of a window (:188-192);
+ * kgv_replay_verify_chain (after kgv_validate_block_bodies below) does that and the rest of verify_expected_utxo_state in one call. */
 int kgv_replay_muhash(kgv_ctx* ctx, const uint32_t* group_first_block, size_t n_groups, uint8_t* values768);
 /* The UtxoDiff of every group of blocks of the LAST kgv_replay_window call (ctx.mergeset_diff of calculate_utxo_state, utxo_validation.rs:119,148:
  * what commit_utxo_state stores per chain block and what reorgs read back).  Groups tile the window as in kgv_replay_muhash (group_first_block:
@@ -683,6 +684,74 @@ typedef struct {
 int kgv_validate_block_bodies(kgv_ctx* ctx, const kgv_tx_batch* batch, const uint32_t* block_first_tx, uint32_t n_blocks,
                               const kgv_block_header_ctx* headers, const kgv_tx_rules* rules, const kgv_body_rules* body_rules, uint32_t flags,
                               kgv_body_result* results, kgv_block_masses* masses, uint8_t* roots32);
+
+/* verify_expected_utxo_state (utxo_validation.rs:182-228) for every chain block of the LAST kgv_replay_window call, with what
+ * calculate_utxo_state (:110-173) gathers on the way.  Group g = blocks [group_first_block[g], group_first_block[g+1]) of that window (a HOST
+ * array tiling it, as for kgv_replay_muhash) is one chain block: its first block is the selected parent (KGV_REPLAY_ACCEPT_COINBASE), then
+ * the rest of the mergeset in consensus order, and its LAST block is the chain block's own body (KGV_REPLAY_VERIFY_ONLY; its transaction 0
+ * is the coinbase being verified).  No other block of a group may be VERIFY_ONLY.  Any other layout (n_groups == 0 included), or no current window (see
+ * kgv_replay_muhash: any other batch call or a rehash ends it) gives KGV_ERR_ARG.  The call does not end the window: it, kgv_replay_muhash
+ * and kgv_replay_diffs run in any order, any number of times.
+ *
+ * Per group, in the reference's order, the first failing check gives results[g].status:
+ *   (calculate_utxo_state, per merged block in group order)
+ *     block_fee += fee overflows u64                                        REWARD_OVERFLOW
+ *     its coinbase payload fails deserialize_coinbase_payload(...).unwrap()  COINBASE_PAYLOAD_UNPARSABLE
+ *   1 finalize(init * multiset of groups 0..g) != headers[g].utxo_commitment BAD_UTXO_COMMITMENT
+ *   2 merkle_hash(selected_parent_accepted_id_merkle_root, calc_merkle_root(accepted ids)) != accepted_id_merkle_root
+ *                                                                           BAD_ACCEPTED_ID_MERKLE_ROOT
+ *   4 the chain block's payload is unparsable                               COINBASE_PAYLOAD_UNPARSABLE
+ *     a reward sum of expected_coinbase_transaction overflows               REWARD_OVERFLOW
+ *     hashing::tx::hash(coinbase) != hash(expected_coinbase_transaction)    BAD_COINBASE_TRANSACTION
+ * The REWARD_OVERFLOW and UNPARSABLE cases are the reference's panics (overflow-checks are on in its release profile; unwrap), reported at the
+ * point where it panics.  Blocks that passed body validation never reach them: a payload that parses there parses here, and fees and
+ * subsidies are bounded by the money supply.  Check 3 (the header's pruning point) sits between 4 and 5 in the reference and stays with the
+ * caller, so check 5 is not folded into the status: n_invalid_txs / n_txs count the non-coinbase transactions of the VERIFY_ONLY block whose
+ * verdict is not KGV_TX_OK, and of all of them (InvalidTransactionsInUtxoContext(n_invalid_txs, n_txs) when n_invalid_txs > 0).
+ *
+ * Accepted ids (ctx.accepted_tx_ids): the selected parent's coinbase, then every accepted transaction of the group's other positions, in
+ * window order.  Rewards (mergeset_rewards): a merged block's subsidy is its own payload's, its total_fees the sum of the fees of its accepted
+ * non-coinbase transactions.  The expected coinbase (coinbase.rs:97-142): one output of subsidy + total_fees to the block's payload script per
+ * merged block that is neither red nor non-DAA, when that sum is > 0, in group order; one output of the red blocks' rewards (a non-DAA red
+ * contributes its fees only) to the chain block's miner script when > 0; payload = blue_score, expected_subsidy and the chain block's own
+ * miner data; version 0, no inputs, lock time 0, the coinbase subnetwork, gas 0, mass 0.
+ *
+ * merged_flags: one byte of KGV_MERGED_* per window block (read for the non-VERIFY_ONLY ones); the caller knows GHOSTDAG's mergeset_reds and
+ * the daa_excluded store's mergeset_non_daa.  init768: (numerator || denominator) of the window's first selected parent's multiset.
+ * rules->coinbase_payload_script_public_key_max_len and body_rules->max_coinbase_payload_len bound the payloads (max_block_mass is not read).
+ * Outputs: results (n_groups records: the computed commitment and accepted-id root always, coinbase_hash zero when the expected coinbase could
+ * not be built); block_fees (may be NULL): total_fees of every window block, 0 for VERIFY_ONLY blocks, meaningless once its sum overflowed;
+ * multisets768 (may be NULL): the running (numerator || denominator) after each group - what the multiset store keeps per chain block, and
+ * the next window's init768.
+ * headers, merged_flags, init768, results, block_fees, multisets768: all host or all device pointers.  With device pointers the call only
+ * enqueues work on the context's stream; with host pointers it synchronises once, at the end. */
+typedef struct {
+  uint8_t utxo_commitment[32];                         /* header.utxo_commitment */
+  uint8_t accepted_id_merkle_root[32];                 /* header.accepted_id_merkle_root */
+  uint8_t selected_parent_accepted_id_merkle_root[32]; /* headers_store(selected parent).accepted_id_merkle_root (utxo_validation.rs:407) */
+  uint64_t blue_score;                                 /* ghostdag_data.blue_score */
+  uint64_t expected_subsidy;                           /* calc_block_subsidy(header.daa_score), as in kgv_block_header_ctx */
+} kgv_chain_header; /* 112 bytes */
+typedef struct {
+  uint32_t status;        /* KGV_CHAIN_* */
+  uint32_t n_invalid_txs; /* check 5: non-coinbase transactions of the chain block that are not KGV_TX_OK */
+  uint32_t n_txs;         /* non-coinbase transactions of the chain block */
+  uint32_t pad_;
+  uint8_t utxo_commitment[32];         /* computed */
+  uint8_t accepted_id_merkle_root[32]; /* computed */
+  uint8_t coinbase_hash[32];           /* hashing::tx::hash of the expected coinbase; zero if it could not be built */
+} kgv_chain_result; /* 112 bytes */
+#define KGV_CHAIN_OK 0u
+#define KGV_CHAIN_BAD_UTXO_COMMITMENT 1u          /* RuleError::BadUTXOCommitment */
+#define KGV_CHAIN_BAD_ACCEPTED_ID_MERKLE_ROOT 2u  /* RuleError::BadAcceptedIDMerkleRoot */
+#define KGV_CHAIN_BAD_COINBASE_TRANSACTION 3u     /* RuleError::BadCoinbaseTransaction */
+#define KGV_CHAIN_REWARD_OVERFLOW 4u              /* the reference panics: a u64 fee / reward sum overflows */
+#define KGV_CHAIN_COINBASE_PAYLOAD_UNPARSABLE 5u  /* the reference panics: deserialize_coinbase_payload(...).unwrap() */
+#define KGV_MERGED_RED 1u                         /* the block is in ghostdag_data.mergeset_reds */
+#define KGV_MERGED_NON_DAA 2u                     /* the block is in mergeset_non_daa */
+int kgv_replay_verify_chain(kgv_ctx* ctx, const uint32_t* group_first_block, size_t n_groups, const kgv_chain_header* headers, const uint8_t* merged_flags,
+                            const uint8_t* init768, const kgv_tx_rules* rules, const kgv_body_rules* body_rules, kgv_chain_result* results,
+                            uint64_t* block_fees, uint8_t* multisets768);
 
 /* ------------------------------------------------------------------------------------------------
  * K8 MuHash (SURVEY.md §8f-1): crypto/muhash/src/lib.rs, u3072.rs; consensus/core/src/muhash.rs.

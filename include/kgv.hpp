@@ -513,6 +513,24 @@ class TransactionValidator {
     }
     return out;
   }
+  // verify_expected_utxo_state of every chain block of the window replay_window just processed (kgv_replay_verify_chain): group g = blocks
+  // [group_first[g], group_first[g+1]), the selected parent first, the chain block's own body (KGV_REPLAY_VERIFY_ONLY) last.  One result per
+  // group; block_fees (optional) receives every block's total_fees, multisets768 (optional) the running multiset after every group.
+  std::vector<kgv_chain_result> verify_chain_blocks(const std::vector<uint32_t>& group_first, const std::vector<kgv_chain_header>& headers,
+                                                    const std::vector<uint8_t>& merged_flags, const uint8_t init768[768], const kgv_tx_rules& rules,
+                                                    const kgv_body_rules& body_rules, std::vector<uint64_t>* block_fees = nullptr,
+                                                    std::vector<uint8_t>* multisets768 = nullptr) {
+    const size_t n_groups = group_first.size() ? group_first.size() - 1 : 0;
+    // the call reads one merged-flags byte and writes one fee per window block, and reads one header per group
+    if (n_groups == 0 || merged_flags.size() != group_first.back() || headers.size() != n_groups)
+      throw Error(KGV_ERR_ARG, "verify_chain_blocks: one header per group and one merged-flags byte per window block");
+    std::vector<kgv_chain_result> res(n_groups);
+    if (block_fees) block_fees->assign(merged_flags.size(), 0);
+    if (multisets768) multisets768->assign(768 * n_groups, 0);
+    c_.check(kgv_replay_verify_chain(c_.get(), group_first.data(), n_groups, headers.data(), merged_flags.data(), init768, &rules, &body_rules, res.data(),
+                                     block_fees ? block_fees->data() : nullptr, multisets768 ? multisets768->data() : nullptr));
+    return res;
+  }
   // the NEXT window's range checks and upload under the current window's compute (kgv_batch_prefetch): call it with window i+1, then
   // replay_window with window i; `next` must stay alive and unchanged until it is replayed
   void prefetch(const TxBatch& next) {

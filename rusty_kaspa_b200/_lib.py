@@ -88,6 +88,7 @@ SYMBOLS = [
     ("kgv_replay_muhash", _c.c_int, [_c.c_void_p, _u8p, _c.c_size_t, _u8p]),
     ("kgv_replay_diffs", _c.c_int, [_c.c_void_p, _u8p, _c.c_size_t, _u8p, _u8p, _u8p, _u8p, _u8p, _u8p, _c.c_size_t, _c.c_size_t, _c.c_size_t,
                                     _c.POINTER(_c.c_size_t), _c.POINTER(_c.c_size_t), _c.POINTER(_c.c_size_t)]),
+    ("kgv_replay_verify_chain", _c.c_int, [_c.c_void_p, _u8p, _c.c_size_t, _u8p, _u8p, _u8p, _c.c_void_p, _c.c_void_p, _u8p, _u8p, _u8p]),
     ("kgv_utxo_muhash", _c.c_int, [_c.c_void_p, _c.c_void_p, _u8p]),
     ("kgv_script_execute", _c.c_int, [_c.c_void_p, _c.c_uint32, _c.c_uint32, _c.c_void_p, _c.c_void_p, _u8p]),
     ("kgv_check_scripts_host", _c.c_int, [_c.c_void_p, _c.c_void_p, _u8p, _c.c_size_t, _u8p]),

@@ -1,18 +1,16 @@
 // kgv_block_body.cuh — device pieces of the block body rules (kgv_block_body.cu): the hashed sets behind the three set checks, the
-// saturating mass triple of check_block_mass and the coinbase payload parse.
+// saturating mass triple of check_block_mass and the coinbase payload rule.
 //
 // Restates, in the reference's check order:
 //   check_block_mass / check_duplicate_transactions / check_block_double_spends / check_no_chained_transactions
 //                                          consensus/src/pipeline/body_processor/body_validation_in_isolation.rs:63-131
-//   deserialize_coinbase_payload           consensus/src/processes/coinbase.rs:185-220
 //   check_coinbase_blue_score_and_subsidy  body_validation_in_context.rs:63-80
 #pragma once
-#include "kgv_txhash.cuh"
+#include "kgv_chain.cuh"
 
 namespace kgv {
 
 constexpr uint32_t BODY_NONE = 0xFFFFFFFFu;        // no offender / empty set slot
-constexpr uint32_t BODY_MIN_PAYLOAD_LENGTH = 19;   // coinbase.rs MIN_PAYLOAD_LENGTH: blue score 8, subsidy 8, spk version 2, spk length 1
 
 // ---- open-addressed sets of item indices ----
 // A set has cap >= 2 * (items inserted) slots, so a probe walk always meets an empty slot.  A slot holds the LOWEST index among the inserted
@@ -69,25 +67,15 @@ struct BodyMassAdd {
   }
 };
 
-// ---- check_coinbase_blue_score_and_subsidy on the coinbase's payload; lengths are compared before any byte is read ----
-__device__ __forceinline__ uint64_t body_le64(const uint8_t* p) {
-  uint64_t v = 0;
-#pragma unroll
-  for (int i = 7; i >= 0; i--) v = v << 8 | p[i];
-  return v;
-}
+// ---- check_coinbase_blue_score_and_subsidy on the coinbase's payload (parsed by coinbase_payload_parse, kgv_chain.cuh) ----
 __device__ __forceinline__ void body_coinbase_payload(kgv_body_result& r, const uint8_t* payload, uint32_t len, const kgv_block_header_ctx& h, uint64_t max_payload_len,
                                                       uint64_t max_spk_len) {
-  if (len < BODY_MIN_PAYLOAD_LENGTH) { r.status = KGV_BODY_BAD_COINBASE_PAYLOAD; r.tx_status = KGV_COINBASE_PAYLOAD_LEN_BELOW_MIN; r.a = len; r.b = BODY_MIN_PAYLOAD_LENGTH; return; }
-  if (len > max_payload_len) { r.status = KGV_BODY_BAD_COINBASE_PAYLOAD; r.tx_status = KGV_COINBASE_PAYLOAD_LEN_ABOVE_MAX; r.a = len; r.b = max_payload_len; return; }
-  const uint64_t blue_score = body_le64(payload), subsidy = body_le64(payload + 8), spk_len = payload[18];
-  if (spk_len > max_spk_len) { r.status = KGV_BODY_BAD_COINBASE_PAYLOAD; r.tx_status = KGV_COINBASE_PAYLOAD_SPK_LEN_ABOVE_MAX; r.a = spk_len; r.b = max_spk_len; return; }
-  if (len - BODY_MIN_PAYLOAD_LENGTH < spk_len) {
-    r.status = KGV_BODY_BAD_COINBASE_PAYLOAD; r.tx_status = KGV_COINBASE_PAYLOAD_CANT_CONTAIN_SPK; r.a = len; r.b = BODY_MIN_PAYLOAD_LENGTH + spk_len;
-    return;
-  }
-  if (blue_score != h.blue_score) { r.status = KGV_BODY_BAD_COINBASE_PAYLOAD_BLUE_SCORE; r.a = blue_score; r.b = h.blue_score; return; }
-  if (subsidy != h.expected_subsidy) { r.status = KGV_BODY_WRONG_SUBSIDY; r.a = h.expected_subsidy; r.b = subsidy; }
+  CoinbasePayload c;
+  uint64_t a = 0, b = 0;
+  const uint32_t e = coinbase_payload_parse(c, payload, len, max_payload_len, max_spk_len, a, b);
+  if (e) { r.status = KGV_BODY_BAD_COINBASE_PAYLOAD; r.tx_status = e; r.a = a; r.b = b; return; }
+  if (c.blue_score != h.blue_score) { r.status = KGV_BODY_BAD_COINBASE_PAYLOAD_BLUE_SCORE; r.a = c.blue_score; r.b = h.blue_score; return; }
+  if (c.subsidy != h.expected_subsidy) { r.status = KGV_BODY_WRONG_SUBSIDY; r.a = h.expected_subsidy; r.b = c.subsidy; }
 }
 
 }  // namespace kgv

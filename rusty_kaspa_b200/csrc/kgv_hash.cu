@@ -330,9 +330,9 @@ __global__ void k_merkle_group_index(const uint32_t* __restrict__ first, uint32_
   for (uint32_t p = first[g]; p < first[g + 1]; p++) gid[p] = g;
 }
 __global__ void __launch_bounds__(128) k_merkle_level(const uint64_t* __restrict__ cur, uint64_t* __restrict__ nxt, const uint32_t* __restrict__ first,
-                                                      const uint32_t* __restrict__ gid, size_t n_total, uint32_t level) {
+                                                      uint32_t n_groups, const uint32_t* __restrict__ gid, size_t n_cap, uint32_t level) {
   size_t p = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (p >= n_total) return;
+  if (p >= n_cap || p >= first[n_groups]) return;
   const uint32_t g = gid[p];
   const uint32_t f = first[g], n = first[g + 1] - f;
   const uint32_t li = (uint32_t)(p - f);
@@ -366,25 +366,13 @@ __global__ void k_merkle_collect(const uint64_t* __restrict__ cur, const uint32_
   for (int k = 0; k < 4; k++) roots[4 * (size_t)g + k] = empty ? 0ull : cur[4 * (size_t)first[g] + k];  // no hashes: ZERO_HASH
 }
 
-// dh: device array of n_total hashes (modified: used as one of the two ping-pong buffers); first_host: n_groups + 1 offsets on the HOST
-int kgv_merkle_run(kgv_ctx* ctx, uint64_t* dh, size_t n_total, const uint32_t* first_host, uint32_t n_groups, uint64_t* droots) {
-  uint32_t max_n = 0;
-  if (n_groups && (first_host[0] != 0 || first_host[n_groups] != n_total)) { ctx->err = "merkle group offsets must start at 0 and end at the number of hashes"; return KGV_ERR_ARG; }
-  for (uint32_t g = 0; g < n_groups; g++) {
-    if (first_host[g + 1] < first_host[g] || first_host[g + 1] > n_total) { ctx->err = "merkle group offsets not monotone / out of range"; return KGV_ERR_ARG; }
-    uint32_t n = first_host[g + 1] - first_host[g];
-    if (n > max_n) max_n = n;
-  }
-  size_t o_first = 0, o_gid = al256((n_groups + 1) * 4), o_buf = al256(o_gid + n_total * 4);
-  int rc = kgv_reserve(ctx, &ctx->d_scratch, &ctx->d_scratch_cap, al256(o_buf + n_total * 32 + 32));
-  if (rc) return rc;
-  uint8_t* S = ctx->d_scratch;
-  uint32_t* dfirst = (uint32_t*)(S + o_first);
-  uint32_t* dgid = (uint32_t*)(S + o_gid);
-  uint64_t* other = (uint64_t*)(S + o_buf);
-  cudaStream_t st = ctx->stream;
-  CK(cudaMemcpyAsync(dfirst, first_host, (n_groups + 1) * 4, cudaMemcpyHostToDevice, st));
-  if (n_total) {
+// dh: device array of up to n_cap hashes (modified: used as one of the two ping-pong buffers); dfirst: n_groups + 1 DEVICE offsets
+size_t kgv_merkle_scratch(size_t n_cap) { return al256(n_cap * 4) + al256(n_cap * 32 + 32); }
+int kgv_merkle_levels(kgv_ctx* ctx, uint64_t* dh, size_t n_cap, const uint32_t* dfirst, uint32_t n_groups, uint32_t max_n, uint8_t* scratch, uint64_t* droots,
+                      cudaStream_t st) {
+  uint32_t* dgid = (uint32_t*)scratch;
+  uint64_t* other = (uint64_t*)(scratch + al256(n_cap * 4));
+  if (n_cap) {
     k_merkle_group_index<<<(n_groups + 127) / 128, 128, 0, st>>>(dfirst, n_groups, dgid);
     CK(cudaGetLastError());
     ctx->launches++;
@@ -392,7 +380,7 @@ int kgv_merkle_run(kgv_ctx* ctx, uint64_t* dh, size_t n_total, const uint32_t* f
   uint64_t* cur = dh;
   uint64_t* nxt = other;
   for (uint32_t level = 0; ((uint64_t)1 << level) < max_n; level++) {
-    k_merkle_level<<<(unsigned)((n_total + 127) / 128), 128, 0, st>>>(cur, nxt, dfirst, dgid, n_total, level);
+    k_merkle_level<<<(unsigned)((n_cap + 127) / 128), 128, 0, st>>>(cur, nxt, dfirst, n_groups, dgid, n_cap, level);
     CK(cudaGetLastError());
     ctx->launches++;
     uint64_t* t = cur; cur = nxt; nxt = t;
@@ -401,6 +389,24 @@ int kgv_merkle_run(kgv_ctx* ctx, uint64_t* dh, size_t n_total, const uint32_t* f
   CK(cudaGetLastError());
   ctx->launches++;
   return KGV_OK;
+}
+
+// first_host: n_groups + 1 offsets on the HOST, from 0 to n_total
+int kgv_merkle_run(kgv_ctx* ctx, uint64_t* dh, size_t n_total, const uint32_t* first_host, uint32_t n_groups, uint64_t* droots) {
+  uint32_t max_n = 0;
+  if (n_groups && (first_host[0] != 0 || first_host[n_groups] != n_total)) { ctx->err = "merkle group offsets must start at 0 and end at the number of hashes"; return KGV_ERR_ARG; }
+  for (uint32_t g = 0; g < n_groups; g++) {
+    if (first_host[g + 1] < first_host[g] || first_host[g + 1] > n_total) { ctx->err = "merkle group offsets not monotone / out of range"; return KGV_ERR_ARG; }
+    uint32_t n = first_host[g + 1] - first_host[g];
+    if (n > max_n) max_n = n;
+  }
+  const size_t o_first = 0, o_lv = al256((n_groups + 1) * 4);
+  int rc = kgv_reserve(ctx, &ctx->d_scratch, &ctx->d_scratch_cap, o_lv + kgv_merkle_scratch(n_total));
+  if (rc) return rc;
+  uint8_t* S = ctx->d_scratch;
+  uint32_t* dfirst = (uint32_t*)(S + o_first);
+  CK(cudaMemcpyAsync(dfirst, first_host, (n_groups + 1) * 4, cudaMemcpyHostToDevice, ctx->stream));
+  return kgv_merkle_levels(ctx, dh, n_total, dfirst, n_groups, max_n, S + o_lv, droots, ctx->stream);
 }
 
 extern "C" int kgv_merkle_roots(kgv_ctx* ctx, const uint8_t* hashes32, const uint32_t* first, uint32_t n_groups, uint8_t* roots32) {

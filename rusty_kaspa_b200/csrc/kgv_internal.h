@@ -59,13 +59,16 @@ struct kgv_ctx {
   size_t d_keys_cap[2] = {};
   uint8_t* d_mu = nullptr;      // MuHash element arrays, product-tree levels and wide-product scratch rows
   size_t d_mu_cap = 0;
-  // state of the last kgv_replay_window call, kept for kgv_replay_muhash / kgv_replay_diffs (cleared by any call that stages another batch)
+  // state of the last kgv_replay_window call, kept for kgv_replay_muhash / kgv_replay_diffs / kgv_replay_verify_chain (cleared by any call
+  // that stages another batch)
   struct {
     bool valid = false;
     const void *txs = nullptr, *inputs = nullptr, *outputs = nullptr, *bytes = nullptr;
     size_t nt = 0, ni = 0, no = 0, n_blocks = 0;
     size_t o_ids = 0, o_itx = 0, o_otx = 0, o_ent = 0, o_acc = 0, o_txb = 0, o_rng = 0;  // offsets into d_replay
     size_t o_src = 0, o_inf = 0, o_apv = 0;
+    size_t o_blk = 0, o_res = 0;                    // the kgv_replay_block records and the per-transaction results
+    std::vector<uint32_t> block_flags, block_n_txs;  // host copy of the blocks' flags and sizes
   } last_replay;
   struct kgv_sigcache* sigcache = nullptr;  // kgv_set_sigcache: verdicts of the validation calls are looked up / remembered here
   struct kgv_comm* shard_comm = nullptr;  // kgv_set_sharding: signature checks of the validation calls are split over its ranks
@@ -118,6 +121,20 @@ int kgv_mu_reduce(kgv_ctx* ctx, size_t n_den, size_t n_num, uint8_t* out_num384,
 int kgv_mu_range_products(kgv_ctx* ctx, const uint32_t* E, size_t stride, const uint8_t* flags, const uint32_t* flag_index, const uint32_t* lo, const uint32_t* hi, uint32_t n_segs,
                           uint32_t* out, size_t out_pitch_words, cudaStream_t st);
 int kgv_mu_canonicalize(kgv_ctx* ctx, uint32_t* vals, size_t pitch_words, size_t n, cudaStream_t st);
+// kgv_muhash_prefix_combine on device records (v: n (numerator || denominator) records, 16-byte aligned; dinit: one record or null), in place;
+// tot: kgv_mu_prefix_scratch(n) bytes
+size_t kgv_mu_prefix_scratch(size_t n);
+int kgv_mu_prefix_combine_run(kgv_ctx* ctx, const uint32_t* dinit, uint32_t* v, size_t n, uint32_t* tot, cudaStream_t st);
+// kgv_muhash_finalize_batch on device values (numerator k at dnum + k * pitch_words, 16-byte aligned); dser (may be null) / dhashes: n values
+// of 384 / 32 bytes, 4-byte aligned; scratch: kgv_mu_finalize_scratch(n) bytes, 256-byte aligned
+size_t kgv_mu_finalize_scratch(size_t n);
+int kgv_mu_finalize_run(kgv_ctx* ctx, const uint32_t* dnum, const uint32_t* dden, size_t n, size_t pitch_words, uint8_t* scratch, uint32_t* dser,
+                        uint32_t* dhashes, cudaStream_t st);
+// kgv_replay_muhash on the last window's state (kgv_validate.cu): dgf = n_groups + 1 device block offsets; vals = n_groups canonical
+// (numerator || denominator) records, 768 bytes apart, 16-byte aligned; scratch: kgv_replay_muhash_scratch(n_groups) bytes, 256-byte aligned.
+// The element arrays live in d_mu.
+size_t kgv_replay_muhash_scratch(kgv_ctx* ctx, size_t n_groups);
+int kgv_replay_muhash_run(kgv_ctx* ctx, const uint32_t* dgf, size_t n_groups, uint8_t* scratch, uint32_t* vals, cudaStream_t st);
 
 // ---- shared pieces of the validation path (kgv_validate.cu) ----
 struct kgv_utxo_table;
@@ -166,6 +183,11 @@ int kgv_standard_context_run(kgv_ctx* ctx, const kgv_dev_batch& d, const kgv::De
 int kgv_tx_digests_run(kgv_ctx* ctx, const kgv_dev_batch& d, size_t n, uint64_t* out, bool hash);
 // merkle roots of n_groups groups over the device hashes dh (overwritten); first_host: n_groups + 1 offsets on the host.  Uses d_scratch.
 int kgv_merkle_run(kgv_ctx* ctx, uint64_t* dh, size_t n_total, const uint32_t* first_host, uint32_t n_groups, uint64_t* droots);
+// the same with DEVICE offsets dfirst (n_groups + 1, from 0 to at most n_cap hashes) and max_n >= the largest group; scratch:
+// kgv_merkle_scratch(n_cap) bytes, 256-byte aligned.  Enqueued on st.
+size_t kgv_merkle_scratch(size_t n_cap);
+int kgv_merkle_levels(kgv_ctx* ctx, uint64_t* dh, size_t n_cap, const uint32_t* dfirst, uint32_t n_groups, uint32_t max_n, uint8_t* scratch, uint64_t* droots,
+                      cudaStream_t st);
 // check_duplicate_transactions / check_block_double_spends / check_no_chained_transactions of every block (kgv_block_body.cu): dacc[b] gets
 // the lowest offending tx / input / input index within the batch, 0xFFFFFFFF where a check passes.  dids: the tx ids; dfirst: the block
 // offsets on the device; dtab: scratch of kgv_body_sets_scratch(n_txs, n_inputs) bytes.

@@ -491,6 +491,32 @@ int kgv_mu_scan(kgv_ctx* ctx, uint32_t* vals, size_t pitch, size_t n, bool rev, 
   return KGV_OK;
 }
 
+// [P n] [S n] [out n] [tot chunks] [inverse scratch 3]
+size_t kgv_mu_finalize_scratch(size_t n) { return 3 * al256(n * 384) + al256((n + KGV_SCAN_CHUNK - 1) / KGV_SCAN_CHUNK * 384) + al256(3 * 384); }
+int kgv_mu_finalize_run(kgv_ctx* ctx, const uint32_t* dnum, const uint32_t* dden, size_t n, size_t pitch_words, uint8_t* scratch, uint32_t* dser,
+                        uint32_t* dhashes, cudaStream_t st) {
+  if (n == 0) return KGV_OK;
+  const size_t n_chunks = (n + KGV_SCAN_CHUNK - 1) / KGV_SCAN_CHUNK;
+  const size_t o_P = 0, o_S = al256(n * 384), o_out = o_S + al256(n * 384), o_tot = o_out + al256(n * 384), o_inv = o_tot + al256(n_chunks * 384);
+  uint32_t *P = (uint32_t*)(scratch + o_P), *S = (uint32_t*)(scratch + o_S), *out = (uint32_t*)(scratch + o_out), *tot = (uint32_t*)(scratch + o_tot),
+           *inv = (uint32_t*)(scratch + o_inv);
+  CK(cudaMemcpy2DAsync(P, 384, dden, pitch_words * 4, 384, n, cudaMemcpyDeviceToDevice, st));
+  CK(cudaMemcpyAsync(S, P, n * 384, cudaMemcpyDeviceToDevice, st));
+  int rc = kgv_mu_scan(ctx, P, 96, n, false, tot, st);
+  if (rc) return rc;
+  rc = kgv_mu_scan(ctx, S, 96, n, true, tot, st);
+  if (rc) return rc;
+  CK(cudaMemcpyAsync(inv, P + 96 * (n - 1), 384, cudaMemcpyDeviceToDevice, st));
+  k_u3072_inverse_one<<<1, 32, 0, st>>>(inv);
+  CK(cudaGetLastError());
+  k_muhash_divide_all<<<nblk(n, KGV_COOP_GROUPS), 128, 0, st>>>(dnum, pitch_words, P, S, inv + 96, n, out);
+  CK(cudaGetLastError());
+  k_muhash_emit_hashes<<<nblk(n, 128), 128, 0, st>>>(out, n, dser, dhashes);
+  CK(cudaGetLastError());
+  ctx->launches += 3;
+  return KGV_OK;
+}
+
 extern "C" int kgv_muhash_finalize_batch(kgv_ctx* ctx, const uint8_t* numerators384, const uint8_t* denominators384, size_t n, size_t pitch_bytes, uint8_t* serialized384,
                                          uint8_t* hashes32) {
   if (!ctx) return KGV_ERR_ARG;
@@ -505,11 +531,9 @@ extern "C" int kgv_muhash_finalize_batch(kgv_ctx* ctx, const uint8_t* numerators
     ctx->err = "device numerators384 must be 16-byte aligned, hashes32 and serialized384 4-byte aligned";
     return KGV_ERR_ARG;
   }
-  const size_t n_chunks = (n + KGV_SCAN_CHUNK - 1) / KGV_SCAN_CHUNK;
-  // layout: [num in (host path only)] [P n] [S n] [out n] [tot chunks] [inverse scratch 3] [hashes n*32 (host path)] [serialized (host path)]
+  // layout: [num in (host path only)] [den in (host path only)] [finalize scratch] [hashes n*32 (host path)] [serialized (host path)]
   const size_t span = (n - 1) * pitch_bytes + 384;
-  size_t o_num = 0, o_den = al256(dev ? 0 : span), o_P = al256(o_den + (dev ? 0 : span)), o_S = al256(o_P + n * 384), o_out = al256(o_S + n * 384), o_tot = al256(o_out + n * 384),
-         o_inv = al256(o_tot + n_chunks * 384), o_h = al256(o_inv + 3 * 384), o_ser = al256(o_h + n * 32);
+  size_t o_num = 0, o_den = al256(dev ? 0 : span), o_fin = al256(o_den + (dev ? 0 : span)), o_h = o_fin + kgv_mu_finalize_scratch(n), o_ser = al256(o_h + n * 32);
   int rc = kgv_reserve(ctx, &ctx->d_mu, &ctx->d_mu_cap, al256(o_ser + (serialized384 ? n * 384 : 0)));
   if (rc) return rc;
   uint8_t* M = ctx->d_mu;
@@ -522,28 +546,33 @@ extern "C" int kgv_muhash_finalize_batch(kgv_ctx* ctx, const uint8_t* numerators
     CK(cudaMemcpyAsync(M + o_den, denominators384, span, cudaMemcpyHostToDevice, st));
     dnum = (const uint32_t*)(M + o_num); dden = (const uint32_t*)(M + o_den);
   }
-  uint32_t *P = (uint32_t*)(M + o_P), *S = (uint32_t*)(M + o_S), *out = (uint32_t*)(M + o_out), *tot = (uint32_t*)(M + o_tot), *inv = (uint32_t*)(M + o_inv);
-  CK(cudaMemcpy2DAsync(P, 384, dden, pitch_bytes, 384, n, cudaMemcpyDeviceToDevice, st));
-  CK(cudaMemcpyAsync(S, P, n * 384, cudaMemcpyDeviceToDevice, st));
-  rc = kgv_mu_scan(ctx, P, 96, n, false, tot, st);
-  if (rc) return rc;
-  rc = kgv_mu_scan(ctx, S, 96, n, true, tot, st);
-  if (rc) return rc;
-  CK(cudaMemcpyAsync(inv, P + 96 * (n - 1), 384, cudaMemcpyDeviceToDevice, st));
-  k_u3072_inverse_one<<<1, 32, 0, st>>>(inv);
-  CK(cudaGetLastError());
-  k_muhash_divide_all<<<nblk(n, KGV_COOP_GROUPS), 128, 0, st>>>(dnum, pitch_bytes / 4, P, S, inv + 96, n, out);
-  CK(cudaGetLastError());
   uint32_t* dh = dev ? (uint32_t*)hashes32 : (uint32_t*)(M + o_h);
   uint32_t* dser = !serialized384 ? nullptr : (dev ? (uint32_t*)serialized384 : (uint32_t*)(M + o_ser));
-  k_muhash_emit_hashes<<<nblk(n, 128), 128, 0, st>>>(out, n, dser, dh);
-  CK(cudaGetLastError());
-  ctx->launches += 3;
+  rc = kgv_mu_finalize_run(ctx, dnum, dden, n, pitch_bytes / 4, M + o_fin, dser, dh, st);
+  if (rc) return rc;
   if (!dev) {
     CK(cudaMemcpyAsync(hashes32, dh, n * 32, cudaMemcpyDeviceToHost, st));
     if (serialized384) CK(cudaMemcpyAsync(serialized384, dser, n * 384, cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
   }
+  return KGV_OK;
+}
+
+size_t kgv_mu_prefix_scratch(size_t n) { return al256((n + KGV_SCAN_CHUNK - 1) / KGV_SCAN_CHUNK * 384); }
+int kgv_mu_prefix_combine_run(kgv_ctx* ctx, const uint32_t* dinit, uint32_t* v, size_t n, uint32_t* tot, cudaStream_t st) {
+  if (n == 0) return KGV_OK;
+  if (dinit) {
+    k_u3072_mul_first<<<1, 32, 0, st>>>(v, dinit, 2, 96);
+    CK(cudaGetLastError());
+    ctx->launches++;
+  }
+  int rc = kgv_mu_scan(ctx, v, 192, n, false, tot, st);        // numerators
+  if (rc) return rc;
+  rc = kgv_mu_scan(ctx, v + 96, 192, n, false, tot, st);   // denominators
+  if (rc) return rc;
+  k_u3072_canonicalize<<<nblk(2 * n, 128), 128, 0, st>>>(v, 96, 2 * n);
+  CK(cudaGetLastError());
+  ctx->launches++;
   return KGV_OK;
 }
 
@@ -555,28 +584,16 @@ extern "C" int kgv_muhash_prefix_combine(kgv_ctx* ctx, const uint8_t* init768, u
   CK(cudaSetDevice(ctx->device));
   const bool dev = kgv_ptr_is_device(values768);
   if (dev && ((uintptr_t)values768 & 15)) { ctx->err = "device values768 must be 16-byte aligned"; return KGV_ERR_ARG; }  // scanned in place with 16-byte loads
-  const size_t n_chunks = (n + KGV_SCAN_CHUNK - 1) / KGV_SCAN_CHUNK;
-  size_t o_v = 0, o_tot = al256(dev ? 0 : n * 768), o_init = al256(o_tot + n_chunks * 384);
+  size_t o_v = 0, o_tot = al256(dev ? 0 : n * 768), o_init = o_tot + kgv_mu_prefix_scratch(n);
   int rc = kgv_reserve(ctx, &ctx->d_mu, &ctx->d_mu_cap, al256(o_init + 768));
   if (rc) return rc;
   uint8_t* M = ctx->d_mu;
   cudaStream_t st = ctx->stream;
   uint32_t* v = (uint32_t*)values768;
   if (!dev) { CK(cudaMemcpyAsync(M + o_v, values768, n * 768, cudaMemcpyHostToDevice, st)); v = (uint32_t*)(M + o_v); }
-  if (init768) {
-    CK(cudaMemcpyAsync(M + o_init, init768, 768, kgv_ptr_is_device(init768) ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, st));
-    k_u3072_mul_first<<<1, 32, 0, st>>>(v, (const uint32_t*)(M + o_init), 2, 96);
-    CK(cudaGetLastError());
-    ctx->launches++;
-  }
-  uint32_t* tot = (uint32_t*)(M + o_tot);
-  rc = kgv_mu_scan(ctx, v, 192, n, false, tot, st);        // numerators
+  if (init768) CK(cudaMemcpyAsync(M + o_init, init768, 768, kgv_ptr_is_device(init768) ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, st));
+  rc = kgv_mu_prefix_combine_run(ctx, init768 ? (const uint32_t*)(M + o_init) : nullptr, v, n, (uint32_t*)(M + o_tot), st);
   if (rc) return rc;
-  rc = kgv_mu_scan(ctx, v + 96, 192, n, false, tot, st);   // denominators
-  if (rc) return rc;
-  k_u3072_canonicalize<<<nblk(2 * n, 128), 128, 0, st>>>(v, 96, 2 * n);
-  CK(cudaGetLastError());
-  ctx->launches++;
   if (!dev) {
     CK(cudaMemcpyAsync(values768, v, n * 768, cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));

@@ -808,6 +808,9 @@ extern "C" int kgv_replay_window(kgv_ctx* ctx, kgv_utxo_table* table, const kgv_
   ctx->last_replay.o_ids = o_ids; ctx->last_replay.o_itx = o_itx; ctx->last_replay.o_otx = o_otx; ctx->last_replay.o_ent = o_ent; ctx->last_replay.o_acc = o_acc;
   ctx->last_replay.o_txb = o_txb; ctx->last_replay.o_rng = o_rng;
   ctx->last_replay.o_src = o_src; ctx->last_replay.o_inf = o_inf; ctx->last_replay.o_apv = o_apv;
+  ctx->last_replay.o_blk = o_blk; ctx->last_replay.o_res = o_res;
+  ctx->last_replay.block_flags.resize(n_blocks); ctx->last_replay.block_n_txs.resize(n_blocks);
+  for (size_t i = 0; i < n_blocks; i++) { ctx->last_replay.block_flags[i] = blocks[i].flags; ctx->last_replay.block_n_txs[i] = blocks[i].n_txs; }
   if (stats) {
     stats->n_accepted = n_acc; stats->n_sig_checks = n_items; stats->n_host_vm = n_vm;
     CK(cudaEventElapsedTime(&stats->pre_check_ms, ctx->ev_time[0], ctx->ev_time[1]));
@@ -874,6 +877,40 @@ __global__ void k_replay_group_ranges(const ReplayRange* __restrict__ ranges, co
   ilo[g] = i0; ihi[g] = any ? i1 : i0; olo[g] = o0; ohi[g] = any ? o1 : o0;
 }
 
+// scratch: [pov nt] [first nt] [ilo] [ihi] [olo] [ohi]
+size_t kgv_replay_muhash_scratch(kgv_ctx* ctx, size_t n_groups) { return al256(ctx->last_replay.nt * 8) + al256(ctx->last_replay.nt) + 4 * al256(n_groups * 4); }
+int kgv_replay_muhash_run(kgv_ctx* ctx, const uint32_t* dgf, size_t n_groups, uint8_t* scratch, uint32_t* vals, cudaStream_t st) {
+  const auto& L = ctx->last_replay;
+  uint8_t* R = ctx->d_replay;
+  const size_t nt = L.nt, ni = L.ni, no = L.no;
+  const size_t o_pov = 0, o_first = al256(nt * 8), o_ilo = o_first + al256(nt), o_ihi = o_ilo + al256(n_groups * 4), o_olo = o_ihi + al256(n_groups * 4),
+               o_ohi = o_olo + al256(n_groups * 4);
+  uint8_t* Wk = scratch;
+  uint32_t *e_den = nullptr, *e_num = nullptr;
+  int rc = kgv_mu_reserve(ctx, ni, no, &e_den, &e_num);
+  if (rc) return rc;
+  const ReplayRange* ranges = (const ReplayRange*)(R + L.o_rng);
+  const uint32_t *itx = (const uint32_t*)(R + L.o_itx), *otx = (const uint32_t*)(R + L.o_otx), *txb = (const uint32_t*)(R + L.o_txb);
+  const uint8_t* acc = R + L.o_acc;
+  k_replay_tx_pov<<<nblk(nt, 256), 256, 0, st>>>(ranges, txb, (uint32_t)nt, (uint64_t*)(Wk + o_pov), Wk + o_first);
+  CK(cudaGetLastError());
+  BatchView v{(const kgv_tx*)L.txs, (const kgv_input*)L.inputs, (const kgv_output*)L.outputs, (const DevEntry*)(R + L.o_ent), (const uint8_t*)L.bytes};
+  if (ni + no) {
+    k_muhash_replay_elements<<<nblk(ni + no, 128), 128, 0, st>>>(v, ni, no, itx, otx, acc, (const uint64_t*)(R + L.o_ids), (const uint64_t*)(Wk + o_pov), Wk + o_first, e_den, e_num);
+    CK(cudaGetLastError());
+  }
+  k_replay_group_ranges<<<nblk(n_groups, 128), 128, 0, st>>>(ranges, dgf, (uint32_t)n_groups, (uint32_t*)(Wk + o_ilo), (uint32_t*)(Wk + o_ihi),
+                                                            (uint32_t*)(Wk + o_olo), (uint32_t*)(Wk + o_ohi));
+  CK(cudaGetLastError());
+  ctx->launches += 3;
+  // an input of an accepted transaction is always found (the context rules saw it), so accept[itx[j]] alone selects the denominators
+  rc = kgv_mu_range_products(ctx, e_num, no, acc, otx, (const uint32_t*)(Wk + o_olo), (const uint32_t*)(Wk + o_ohi), (uint32_t)n_groups, vals, 192, st);
+  if (rc) return rc;
+  rc = kgv_mu_range_products(ctx, e_den, ni, acc, itx, (const uint32_t*)(Wk + o_ilo), (const uint32_t*)(Wk + o_ihi), (uint32_t)n_groups, vals + 96, 192, st);
+  if (rc) return rc;
+  return kgv_mu_canonicalize(ctx, vals, 96, 2 * n_groups, st);
+}
+
 extern "C" int kgv_replay_muhash(kgv_ctx* ctx, const uint32_t* group_first_block, size_t n_groups, uint8_t* values768) {
   if (!ctx) return KGV_ERR_ARG;
   std::lock_guard<std::recursive_mutex> g(ctx->mu);
@@ -885,39 +922,14 @@ extern "C" int kgv_replay_muhash(kgv_ctx* ctx, const uint32_t* group_first_block
   for (size_t i = 0; i < n_groups; i++) if (group_first_block[i] > group_first_block[i + 1]) { ctx->err = "group offsets not monotone"; return KGV_ERR_ARG; }
   CK(cudaSetDevice(ctx->device));
   cudaStream_t st = ctx->stream;
-  uint8_t* R = ctx->d_replay;
-  const size_t nt = L.nt, ni = L.ni, no = L.no;
   // scratch (d_work is free between validation calls)
-  size_t o_pov = 0, o_first = al256(nt * 8), o_gf = al256(o_first + nt), o_ilo = al256(o_gf + (n_groups + 1) * 4), o_ihi = al256(o_ilo + n_groups * 4), o_olo = al256(o_ihi + n_groups * 4),
-         o_ohi = al256(o_olo + n_groups * 4), o_val = al256(o_ohi + n_groups * 4);
+  const size_t o_gf = 0, o_mu = al256((n_groups + 1) * 4), o_val = o_mu + kgv_replay_muhash_scratch(ctx, n_groups);
   int rc = kgv_reserve(ctx, &ctx->d_work, &ctx->d_work_cap, al256(o_val + n_groups * 768));
   if (rc) return rc;
   uint8_t* Wk = ctx->d_work;
-  uint32_t *e_den = nullptr, *e_num = nullptr;
-  rc = kgv_mu_reserve(ctx, ni, no, &e_den, &e_num);
-  if (rc) return rc;
-  const ReplayRange* ranges = (const ReplayRange*)(R + L.o_rng);
-  const uint32_t *itx = (const uint32_t*)(R + L.o_itx), *otx = (const uint32_t*)(R + L.o_otx), *txb = (const uint32_t*)(R + L.o_txb);
-  const uint8_t* acc = R + L.o_acc;
-  CK(cudaMemcpyAsync(Wk + o_gf, group_first_block, (n_groups + 1) * 4, cudaMemcpyHostToDevice, st));
-  k_replay_tx_pov<<<nblk(nt, 256), 256, 0, st>>>(ranges, txb, (uint32_t)nt, (uint64_t*)(Wk + o_pov), Wk + o_first);
-  CK(cudaGetLastError());
-  BatchView v{(const kgv_tx*)L.txs, (const kgv_input*)L.inputs, (const kgv_output*)L.outputs, (const DevEntry*)(R + L.o_ent), (const uint8_t*)L.bytes};
-  if (ni + no) {
-    k_muhash_replay_elements<<<nblk(ni + no, 128), 128, 0, st>>>(v, ni, no, itx, otx, acc, (const uint64_t*)(R + L.o_ids), (const uint64_t*)(Wk + o_pov), Wk + o_first, e_den, e_num);
-    CK(cudaGetLastError());
-  }
-  k_replay_group_ranges<<<nblk(n_groups, 128), 128, 0, st>>>(ranges, (const uint32_t*)(Wk + o_gf), (uint32_t)n_groups, (uint32_t*)(Wk + o_ilo), (uint32_t*)(Wk + o_ihi),
-                                                            (uint32_t*)(Wk + o_olo), (uint32_t*)(Wk + o_ohi));
-  CK(cudaGetLastError());
-  ctx->launches += 3;
   uint32_t* vals = (uint32_t*)(Wk + o_val);
-  // an input of an accepted transaction is always found (the context rules saw it), so accept[itx[j]] alone selects the denominators
-  rc = kgv_mu_range_products(ctx, e_num, no, acc, otx, (const uint32_t*)(Wk + o_olo), (const uint32_t*)(Wk + o_ohi), (uint32_t)n_groups, vals, 192, st);
-  if (rc) return rc;
-  rc = kgv_mu_range_products(ctx, e_den, ni, acc, itx, (const uint32_t*)(Wk + o_ilo), (const uint32_t*)(Wk + o_ihi), (uint32_t)n_groups, vals + 96, 192, st);
-  if (rc) return rc;
-  rc = kgv_mu_canonicalize(ctx, vals, 96, 2 * n_groups, st);
+  CK(cudaMemcpyAsync(Wk + o_gf, group_first_block, (n_groups + 1) * 4, cudaMemcpyHostToDevice, st));
+  rc = kgv_replay_muhash_run(ctx, (const uint32_t*)(Wk + o_gf), n_groups, Wk + o_mu, vals, st);
   if (rc) return rc;
   const bool dev = kgv_ptr_is_device(values768);
   CK(cudaMemcpyAsync(values768, vals, n_groups * 768, dev ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, st));

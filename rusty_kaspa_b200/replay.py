@@ -26,6 +26,16 @@ REPLAY_BLOCK_DTYPE = np.dtype([("first_tx", "<u4"), ("n_txs", "<u4"), ("pov_daa_
 assert REPLAY_BLOCK_DTYPE.itemsize == 24
 REPLAY_ACCEPT_COINBASE, REPLAY_SKIP_SCRIPTS, REPLAY_VERIFY_ONLY = 1, 2, 4
 
+# kgv_replay_verify_chain (include/kgv.h)
+CHAIN_HEADER_DTYPE = np.dtype([("utxo_commitment", "u1", 32), ("accepted_id_merkle_root", "u1", 32), ("selected_parent_accepted_id_merkle_root", "u1", 32),
+                               ("blue_score", "<u8"), ("expected_subsidy", "<u8")])
+assert CHAIN_HEADER_DTYPE.itemsize == 112
+CHAIN_RESULT_DTYPE = np.dtype([("status", "<u4"), ("n_invalid_txs", "<u4"), ("n_txs", "<u4"), ("pad_", "<u4"), ("utxo_commitment", "u1", 32),
+                               ("accepted_id_merkle_root", "u1", 32), ("coinbase_hash", "u1", 32)])
+assert CHAIN_RESULT_DTYPE.itemsize == 112
+CHAIN_STATUS = {"Ok": 0, "BadUTXOCommitment": 1, "BadAcceptedIDMerkleRoot": 2, "BadCoinbaseTransaction": 3, "RewardOverflow": 4, "CoinbasePayloadUnparsable": 5}
+MERGED_RED, MERGED_NON_DAA = 1, 2
+
 
 class ReplayStats(ctypes.Structure):
     _fields_ = [("n_accepted", ctypes.c_uint64), ("n_sig_checks", ctypes.c_uint64), ("n_host_vm", ctypes.c_uint64), ("pre_check_ms", ctypes.c_float),
@@ -175,6 +185,31 @@ class DagReplayer:
         self.ctx._check(lib.kgv_replay_diffs(h, gf.ctypes.data, n_groups, ranges.ctypes.data, rk.ctypes.data, re.ctypes.data, ak.ctypes.data, ae.ctypes.data,
                                              by.ctypes.data, nr.value, na.value, nb.value, ctypes.byref(nr), ctypes.byref(na), ctypes.byref(nb)))
         return ReplayDiffs(ranges[:n_groups], rk[:nr.value], re[:nr.value], ak[:na.value], ae[:na.value], by[:nb.value])
+
+    def verify_chain(self, group_first, headers, merged_flags, init768, rules=None, body_rules=None):
+        """kgv_replay_verify_chain for the window just replayed: verify_expected_utxo_state of every chain block (utxo_validation.rs:182-228).
+        group_first: n_groups + 1 block offsets; group g is the chain block's selected parent (ACCEPT_COINBASE), the rest of its mergeset in
+        consensus order, then its own body (VERIFY_ONLY).  headers: CHAIN_HEADER_DTYPE per group; merged_flags: MERGED_* per window block;
+        init768: the multiset of the window's first selected parent (a MuHash, or 768 bytes numerator || denominator).
+        Returns (CHAIN_RESULT_DTYPE[n_groups], block_fees uint64[n_blocks], (n_groups, 768) uint8 running multisets)."""
+        from .validator import BodyRules, TxRules
+        gf = np.ascontiguousarray(group_first, dtype=np.uint32)
+        h = np.ascontiguousarray(headers, dtype=CHAIN_HEADER_DTYPE)
+        mf = np.ascontiguousarray(merged_flags, dtype=np.uint8)
+        if hasattr(init768, "numerator"):  # a MuHash
+            init768 = init768.numerator + init768.denominator
+        init = np.frombuffer(bytes(init768), dtype=np.uint8).copy() if isinstance(init768, (bytes, bytearray)) else np.ascontiguousarray(init768, dtype=np.uint8)
+        n_groups = len(gf) - 1
+        # the call reads one merged-flags byte and writes one fee per window block (group_first[-1] of them), and reads one header per group
+        if n_groups < 1 or len(h) != n_groups or len(mf) != int(gf[-1]) or init.size != 768:
+            raise ValueError("one header per group, one merged-flags byte per window block and a 768-byte init multiset")
+        rules, body_rules = rules or TxRules(), body_rules or BodyRules()
+        res = np.zeros(max(n_groups, 1), dtype=CHAIN_RESULT_DTYPE)
+        fees = np.zeros(max(len(mf), 1), dtype=np.uint64)
+        ms = np.zeros((max(n_groups, 1), 768), dtype=np.uint8)
+        self.ctx._check(self.ctx._lib.kgv_replay_verify_chain(self.ctx._h, gf.ctypes.data, n_groups, h.ctypes.data, mf.ctypes.data, init.ctypes.data,
+                                                              ctypes.byref(rules), ctypes.byref(body_rules), res.ctypes.data, fees.ctypes.data, ms.ctypes.data))
+        return res[:n_groups], fees[:len(mf)], ms[:n_groups]
 
     def replay_windowed(self, blocks):
         """blocks: list of (txs, pov[, flags]) forming ONE window. Returns per-block RESULT arrays (same values as blockwise)."""
