@@ -877,6 +877,81 @@ int kgv_utxo_rows_encode(const uint8_t* keys36, const kgv_utxo_entry* entries, c
 int kgv_utxo_rows_decode(const uint8_t* key_rows, const uint64_t* key_off, const uint8_t* value_rows, const uint64_t* value_off, size_t n, uint8_t* keys36,
                          kgv_utxo_entry* entries, uint8_t* bytes_out, size_t bytes_cap, size_t* bytes_used);
 
+/* ------------------------------------------------------------------------------------------------
+ * Block headers in isolation: the block hash, kHeavyHash proof of work and block level of a batch of headers
+ * (HeaderProcessor::validate_header_in_isolation, consensus/src/pipeline/header_processor/pre_ghostdag_validation.rs:17-24).
+ * Each header is independent and needs no store.  Ordering (GHOSTDAG, DAA / difficulty, parent existence and relations) stays
+ * with the caller.
+ * Header k's expanded parents_by_level (ParentsByLevel::expanded_iter, consensus/core/src/header.rs:45-47) is given by
+ * level_len[levels_off .. levels_off + n_levels), the number of parents at each level, and the parent hashes of all its levels
+ * in order at parents32 + 32 * parents_off.  Headers may share or reorder arena ranges.  An arena range that leaves level_len
+ * (n_level_entries entries) or parents32 (n_parents hashes) gives KGV_ERR_ARG, and so does a device headers / parents32 pointer
+ * that is not 8-byte aligned.  The pointers of one call are all host or all device.  Both calls end with a synchronise of the
+ * context's stream, also on device pointers: the arena ranges are checked by the kernels, and the call reports what they found.
+ * ------------------------------------------------------------------------------------------------ */
+typedef struct {
+  uint8_t hash_merkle_root[32];
+  uint8_t accepted_id_merkle_root[32];
+  uint8_t utxo_commitment[32];
+  uint8_t pruning_point[32];
+  uint8_t blue_work[24];   /* BlueWorkType (Uint192), big-endian                          */
+  uint64_t timestamp;      /* milliseconds                                                */
+  uint64_t nonce;
+  uint64_t daa_score;
+  uint64_t blue_score;
+  uint64_t parents_off;    /* first parent hash of level 0, in hashes from parents32      */
+  uint32_t levels_off;     /* first entry of the level sizes in level_len                */
+  uint32_t n_levels;       /* expanded_len(); 0 = genesis-shaped (no parents)            */
+  uint32_t bits;
+  uint16_t version;
+  uint16_t pad_;
+} kgv_header; /* 208 bytes */
+
+#define KGV_HEADER_SKIP_POW 1 /* kgv_header_rules.flags: skip_proof_of_work (pre_ghostdag_validation.rs:105) */
+typedef struct {
+  uint64_t timestamp_deviation_tolerance; /* seconds                                                              */
+  uint64_t now_ms;                        /* the clock unix_now() reads in the reference, given so results repeat */
+  uint32_t block_version;                 /* constants::BLOCK_VERSION                                             */
+  uint32_t max_block_parents;
+  uint32_t max_block_level;               /* params.max_block_level (BlockLevel, at most 255)                     */
+  uint32_t flags;                         /* KGV_HEADER_*                                                         */
+} kgv_header_rules; /* 32 bytes */
+
+/* the first failing rule, in the order validate_header_in_isolation checks them; a and b carry the error's numbers */
+#define KGV_HEADER_OK 0
+#define KGV_HEADER_WRONG_BLOCK_VERSION 1            /* WrongBlockVersion(a = version)                              */
+#define KGV_HEADER_TIME_TOO_FAR_INTO_THE_FUTURE 2   /* TimeTooFarIntoTheFuture(a = timestamp, b = max block time)  */
+#define KGV_HEADER_NO_PARENTS 3                     /* NoParents                                                   */
+#define KGV_HEADER_TOO_MANY_PARENTS 4               /* TooManyParents(a = level-0 parents, b = max_block_parents)  */
+#define KGV_HEADER_ORIGIN_PARENT 5                  /* OriginParent                                                */
+#define KGV_HEADER_INVALID_POW 6                    /* InvalidPoW                                                  */
+typedef struct {
+  uint32_t status;      /* KGV_HEADER_*                                                                       */
+  uint8_t level;        /* calc_level_from_pow (consensus/pow/src/lib.rs:72-75); max_block_level for genesis   */
+  uint8_t pow_passed;   /* pow <= target (lib.rs:47-52); 1 for genesis (lib.rs:62-64)                        */
+  uint16_t pad_;
+  uint64_t a, b;
+} kgv_header_result; /* 24 bytes, written for every header whatever its status */
+
+/* hashing::header::hash (consensus/core/src/hashing/header.rs:33-35) into hash32 and hash_override_nonce_time(h, 0, 0) (:7-30), the
+ * pre-PoW hash, into pre_pow32; either output may be NULL. */
+int kgv_hash_headers(kgv_ctx* ctx, const kgv_header* headers, size_t n, const uint8_t* parents32, size_t n_parents, const uint32_t* level_len,
+                     size_t n_level_entries, uint8_t* hash32, uint8_t* pre_pow32);
+/* validate_header_in_isolation (pre_ghostdag_validation.rs:17-24,30-68,102-106) of every header: version, timestamp against now_ms +
+ * tolerance, level-0 parent count, origin parent, then the proof of work (kaspa_pow::State::check_pow, consensus/pow/src/lib.rs:23-53:
+ * pre-PoW hash, matrix from xoshiro256++ redrawn until its rank is 64, cSHAKE256 "ProofOfWorkHash", kHeavyHash, pow <= the compact
+ * target).  With KGV_HEADER_SKIP_POW an insufficient proof of work is not an error; the level is still computed.  results: one record
+ * per header.  hash32 (the block hash) and pow32 (the PoW value, 32 bytes little-endian) may be NULL. */
+int kgv_validate_headers_in_isolation(kgv_ctx* ctx, const kgv_header* headers, size_t n, const uint8_t* parents32, size_t n_parents, const uint32_t* level_len,
+                                      size_t n_level_entries, const kgv_header_rules* rules, kgv_header_result* results, uint8_t* hash32, uint8_t* pow32);
+
+/* Test / audit hook: the proof-of-work matrix code on the device.  Host pointers only.
+ *   op 0: Matrix::compute_rank (consensus/pow/src/matrix.rs:141-174) of n caller matrices: in = n x 64 x 64 u16 (row-major), each
+ *         element converted to f64 as convert_to_float does; out = n u32 ranks.
+ *   op 1: Matrix::generate (matrix.rs:103-111) from n 32-byte seeds: out = n records of 4096 u8 elements (row-major) followed by a u32
+ *         count of the matrices drawn (4100 bytes each). */
+int kgv_debug_pow_matrix(kgv_ctx* ctx, int op, const uint8_t* in, size_t n, uint8_t* out);
+
 /* Test / audit hook: affine coordinates (x||y, 32-byte big-endian each) of entry v (1..65535) of
  * generator table `which` (0: v*G, 1: v*2^128*G) as built on the device. */
 int kgv_gtable_entry(kgv_ctx* ctx, int which, uint32_t v, uint8_t out_xy[64]);

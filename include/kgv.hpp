@@ -797,4 +797,75 @@ class BlockBodyProcessor {
   BodyRules body_;
 };
 
+// ---- HeaderProcessor: header validation in isolation for a batch of headers (kgv_validate_headers_in_isolation) ----
+struct Header {  // consensus/core/src/header.rs: the fields the header hash covers
+  uint16_t version = 1;
+  std::vector<std::vector<Hash>> parents_by_level;  // expanded: one entry per level
+  Hash hash_merkle_root{}, accepted_id_merkle_root{}, utxo_commitment{}, pruning_point{};
+  uint64_t timestamp = 0, nonce = 0, daa_score = 0, blue_score = 0;
+  uint32_t bits = 0;
+  std::array<uint8_t, 24> blue_work{};  // Uint192, big-endian
+};
+struct HeaderRules : kgv_header_rules {
+  // constants::BLOCK_VERSION and MAINNET_PARAMS: timestamp_deviation_tolerance 132 s, max_block_parents 16, max_block_level 225
+  HeaderRules() : kgv_header_rules{132, 0, 1, 16, 225, 0} {}
+};
+struct HeaderVerdicts {
+  std::vector<kgv_header_result> results;  // the first failing rule (KGV_HEADER_*), the level and the PoW pass bit of every header
+  std::vector<Hash> hashes;                // hashing::header::hash of every header
+};
+class HeaderProcessor {
+ public:
+  explicit HeaderProcessor(Context& c, const HeaderRules& rules = HeaderRules()) : c_(c), rules_(rules) {}
+  // validate_header_in_isolation (pre_ghostdag_validation.rs:17-24) of every header; the caller maps the statuses to RuleError and keeps
+  // the level for parents_by_level and its stores.  now_ms stands for unix_now().
+  HeaderVerdicts validate_headers_in_isolation(const std::vector<Header>& headers, uint64_t now_ms) {
+    Packed p(headers);
+    kgv_header_rules r = rules_;
+    r.now_ms = now_ms;
+    HeaderVerdicts v{std::vector<kgv_header_result>(headers.size()), std::vector<Hash>(headers.size())};
+    c_.check(kgv_validate_headers_in_isolation(c_.get(), p.recs.data(), p.recs.size(), p.parents.empty() ? nullptr : p.parents[0].data(), p.parents.size(),
+                                               p.lens.empty() ? nullptr : p.lens.data(), p.lens.size(), &r, v.results.data(),
+                                               headers.empty() ? nullptr : v.hashes[0].data(), nullptr));
+    return v;
+  }
+  // hashing::header::hash of every header (kgv_hash_headers)
+  std::vector<Hash> hash_headers(const std::vector<Header>& headers) {
+    Packed p(headers);
+    std::vector<Hash> out(headers.size());
+    c_.check(kgv_hash_headers(c_.get(), p.recs.data(), p.recs.size(), p.parents.empty() ? nullptr : p.parents[0].data(), p.parents.size(),
+                              p.lens.empty() ? nullptr : p.lens.data(), p.lens.size(), headers.empty() ? nullptr : out[0].data(), nullptr));
+    return out;
+  }
+
+ private:
+  struct Packed {  // the C records and the parents arena
+    std::vector<kgv_header> recs;
+    std::vector<Hash> parents;
+    std::vector<uint32_t> lens;
+    explicit Packed(const std::vector<Header>& hs) : recs(hs.size()) {
+      for (size_t k = 0; k < hs.size(); k++) {
+        const Header& h = hs[k];
+        kgv_header& r = recs[k];
+        std::memset(&r, 0, sizeof r);
+        std::memcpy(r.hash_merkle_root, h.hash_merkle_root.data(), 32);
+        std::memcpy(r.accepted_id_merkle_root, h.accepted_id_merkle_root.data(), 32);
+        std::memcpy(r.utxo_commitment, h.utxo_commitment.data(), 32);
+        std::memcpy(r.pruning_point, h.pruning_point.data(), 32);
+        std::memcpy(r.blue_work, h.blue_work.data(), 24);
+        r.timestamp = h.timestamp; r.nonce = h.nonce; r.daa_score = h.daa_score; r.blue_score = h.blue_score; r.bits = h.bits; r.version = h.version;
+        r.parents_off = parents.size();
+        r.levels_off = (uint32_t)lens.size();
+        r.n_levels = (uint32_t)h.parents_by_level.size();
+        for (const auto& lvl : h.parents_by_level) {
+          lens.push_back((uint32_t)lvl.size());
+          parents.insert(parents.end(), lvl.begin(), lvl.end());
+        }
+      }
+    }
+  };
+  Context& c_;
+  HeaderRules rules_;
+};
+
 }  // namespace kgv

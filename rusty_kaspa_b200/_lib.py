@@ -90,6 +90,8 @@ SYMBOLS = [
                                     _c.POINTER(_c.c_size_t), _c.POINTER(_c.c_size_t), _c.POINTER(_c.c_size_t)]),
     ("kgv_replay_verify_chain", _c.c_int, [_c.c_void_p, _u8p, _c.c_size_t, _u8p, _u8p, _u8p, _c.c_void_p, _c.c_void_p, _u8p, _u8p, _u8p]),
     ("kgv_utxo_muhash", _c.c_int, [_c.c_void_p, _c.c_void_p, _u8p]),
+    ("kgv_hash_headers", _c.c_int, [_c.c_void_p, _u8p, _c.c_size_t, _u8p, _c.c_size_t, _u8p, _c.c_size_t, _u8p, _u8p]),
+    ("kgv_validate_headers_in_isolation", _c.c_int, [_c.c_void_p, _u8p, _c.c_size_t, _u8p, _c.c_size_t, _u8p, _c.c_size_t, _c.c_void_p, _u8p, _u8p, _u8p]),
     ("kgv_script_execute", _c.c_int, [_c.c_void_p, _c.c_uint32, _c.c_uint32, _c.c_void_p, _c.c_void_p, _u8p]),
     ("kgv_check_scripts_host", _c.c_int, [_c.c_void_p, _c.c_void_p, _u8p, _c.c_size_t, _u8p]),
     ("kgv_check_scripts", _c.c_int, [_c.c_void_p, _c.c_void_p, _u8p, _c.c_size_t, _u8p]),
@@ -98,6 +100,7 @@ SYMBOLS = [
     ("kgv_gtable_entry", _c.c_int, [_c.c_void_p, _c.c_int, _c.c_uint32, _u8p]),
     ("kgv_debug_selftest", _c.c_int, [_c.c_void_p, _c.c_int, _u8p, _u8p, _c.c_size_t]),
     ("kgv_debug_u3072_level", _c.c_int, [_c.c_void_p, _c.c_int, _u8p, _c.c_size_t, _u8p]),
+    ("kgv_debug_pow_matrix", _c.c_int, [_c.c_void_p, _c.c_int, _u8p, _c.c_size_t, _u8p]),
     ("kgv_debug_schnorr_trace", _c.c_int, [_c.c_void_p, _u8p, _u8p, _u8p, _u8p, _u8p]),
     ("kgv_debug_key_form", _c.c_int, [_c.c_void_p, _c.c_int, _c.c_void_p]),
     ("kgv_debug_script_rounds", _c.c_int, [_c.c_void_p, _c.POINTER(_c.c_uint32)]),

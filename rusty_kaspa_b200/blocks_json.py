@@ -17,6 +17,26 @@ def _tx(t):
             "payload": bytes.fromhex(t["payload"]), "mass": t.get("mass", 0)}
 
 
+def header_from_json(h):
+    """One JSON header (simpa/src/blocks_json.rs field names) -> the header dict of headers.HeaderBatch: every field the header hash
+    covers, parents_by_level expanded (one list of 32-byte hashes per level), blue_work as an int, plus its stored "hash"."""
+    return {"hash": bytes.fromhex(h["hash"]), "version": h["version"],
+            "parents_by_level": [[bytes.fromhex(p) for p in lvl] for lvl in h["parentsByLevel"]],
+            "hash_merkle_root": bytes.fromhex(h["hashMerkleRoot"]), "accepted_id_merkle_root": bytes.fromhex(h["acceptedIdMerkleRoot"]),
+            "utxo_commitment": bytes.fromhex(h["utxoCommitment"]), "timestamp": h["timestamp"], "bits": h["bits"], "nonce": h["nonce"],
+            "daa_score": h["daaScore"], "blue_work": int(h["blueWork"] or "0", 16), "blue_score": h["blueScore"],
+            "pruning_point": bytes.fromhex(h["pruningPoint"])}
+
+
+def load_headers_json(path):
+    """Returns (params dict, list of header dicts (header_from_json)) in file order, from a blocks.json(.gz) dump or a headers-only
+    file of the same line format (first line params, then one {"header": ...} per line)."""
+    opener = gzip.open if str(path).endswith(".gz") else open
+    with opener(path, "rt") as f:
+        lines = [l for l in f.read().splitlines() if l.strip()]
+    return json.loads(lines[0]), [header_from_json(json.loads(l)["header"]) for l in lines[1:]]
+
+
 def load_blocks_json(path):
     """Returns (params dict, list of blocks); a block = {"hash", "daa_score", "blue_score", "hash_merkle_root",
     "accepted_id_merkle_root", "utxo_commitment", "parents" (level 0), "transactions" (tx dicts)} in file (topological) order."""
