@@ -15,11 +15,16 @@
  *   - plain pointers and sizes only; caller owns every buffer; the library never keeps a host
  *     pointer past the call.
  *   - every data pointer may be a HOST pointer (pageable or pinned) or a DEVICE pointer on the
- *     context's device; the library detects which (cudaPointerGetAttributes).  All data
- *     pointers of one call must be of the same kind.  With host pointers the call copies in,
- *     computes, copies out and returns after the results are in the caller's memory.  With
- *     device pointers the work is enqueued on the context's stream and the call returns
- *     without synchronising (use kgv_synchronize or your own stream sync).
+ *     context's device; the library detects which (cudaPointerGetAttributes), array by array.
+ *     A host input is copied in; a device input is read where it is.  A host output is
+ *     written through a device copy that comes back before the call returns; a device output
+ *     is written in place.  The call synchronises once at its end when some output is host
+ *     memory; with device outputs only, the work is enqueued on the context's stream and the
+ *     call returns without synchronising (use kgv_synchronize or your own stream sync).
+ *     The arrays of a kgv_tx_batch are all host or all device pointers (KGV_ERR_ARG
+ *     otherwise).  Each call states which of its other arrays must share one kind
+ *     (KGV_ERR_ARG otherwise), which may each be of either kind, and which must be host
+ *     memory or device memory.
  *   - return value: 0 = ok, negative = argument / CUDA / NCCL failure (kgv_last_error explains).
  *     An invalid signature is NEVER an error return: verdicts are per-item status bytes.
  *   - there is no CPU fallback: without a usable CUDA device kgv_create fails.
@@ -127,7 +132,7 @@ typedef struct {
   const kgv_output* outputs; size_t n_outputs;
   const kgv_utxo_entry* entries; /* one populated entry per input (PopulatedTransaction), or NULL */
   const uint8_t* bytes; size_t n_bytes;
-} kgv_tx_batch; /* the arrays are all host pointers or all device pointers */
+} kgv_tx_batch; /* the arrays are all host pointers or all device pointers (KGV_ERR_ARG otherwise) */
 
 /* Transaction ids / hashes of every tx of the batch: out32 = n_txs * 32 bytes.
  * Replaces consensus/core/src/hashing/tx.rs:16-42 (`hash`, `id`; keyed BLAKE2b). */

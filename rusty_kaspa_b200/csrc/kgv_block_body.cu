@@ -22,18 +22,6 @@ static_assert(sizeof(kgv_body_rules) == 16, "kgv_body_rules is 16 bytes");
 static_assert(sizeof(kgv_body_result) == 32, "kgv_body_result is 32 bytes");
 static_assert(sizeof(kgv_block_masses) == 24, "kgv_block_masses is 24 bytes");
 
-#define CK(call)                                                                                  \
-  do {                                                                                            \
-    cudaError_t e_ = (call);                                                                      \
-    if (e_ != cudaSuccess) {                                                                      \
-      char b_[256];                                                                               \
-      snprintf(b_, sizeof b_, "%s failed: %s (%s:%d)", #call, cudaGetErrorString(e_), __FILE__, __LINE__); \
-      ctx->err = b_;                                                                              \
-      return KGV_ERR_CUDA;                                                                        \
-    }                                                                                             \
-  } while (0)
-
-static inline size_t al256(size_t x) { return (x + 255) & ~(size_t)255; }
 
 constexpr int BODY_SET_THREADS = 256;
 constexpr uint32_t BODY_SET_SMEM_SLOTS = 8192;  // 32 KiB: a body of up to 4096 transactions + inputs keeps both of its sets in shared memory
@@ -214,9 +202,8 @@ extern "C" int kgv_validate_block_bodies(kgv_ctx* ctx, const kgv_tx_batch* batch
   for (uint32_t b = 0; b < n_blocks; b++)
     if (block_first_tx[b + 1] < block_first_tx[b]) { ctx->err = "block offsets not monotone"; return KGV_ERR_ARG; }
   CK(cudaSetDevice(ctx->device));
-  const bool dev = kgv_ptr_is_device(results) != 0;
-  for (const void* p : {(const void*)batch->txs, (const void*)headers, (const void*)masses, (const void*)roots32})
-    if (p && (kgv_ptr_is_device(p) != 0) != dev) { ctx->err = "kgv_validate_block_bodies: the batch, headers and outputs must all be host or all be device pointers"; return KGV_ERR_ARG; }
+  kgv_io io(ctx);
+  if (int rc = io.one_side("kgv_validate_block_bodies", {results, batch->txs, headers, masses, roots32})) return rc;
   kgv_dev_batch d{};
   if (batch->n_txs) {
     int rc = kgv_batch_to_device(ctx, batch, &d, false);
@@ -226,8 +213,7 @@ extern "C" int kgv_validate_block_bodies(kgv_ctx* ctx, const kgv_tx_batch* batch
   // tx hashes (consumed by the merkle tree) and the roots: d_in; everything else: d_work (the merkle tree owns d_scratch)
   int rc = kgv_reserve(ctx, &ctx->d_in, &ctx->d_in_cap, al256(nt * 32 + 32) + nb * 32);
   if (rc) return rc;
-  const size_t o_res = 0, o_bm = al256(o_res + nb * sizeof(kgv_body_result)), o_hdr = al256(o_bm + nb * sizeof(kgv_block_masses)),
-               o_first = al256(o_hdr + nb * sizeof(kgv_block_header_ctx)), o_txb = al256(o_first + (nb + 1) * 4), o_txr = al256(o_txb + nt * 4),
+  const size_t o_first = 0, o_txb = al256(o_first + (nb + 1) * 4), o_txr = al256(o_txb + nt * 4),
                o_txm = al256(o_txr + nt * sizeof(kgv_tx_result)), o_list = al256(o_txm + nt * sizeof(kgv_tx_masses)), o_ids = al256(o_list + (nt + 1) * 4),
                o_acc = al256(o_ids + nt * 32), o_tab = al256(o_acc + nb * sizeof(kgv_block_check_acc));
   rc = kgv_reserve(ctx, &ctx->d_work, &ctx->d_work_cap, o_tab + kgv_body_sets_scratch(nt, d.n_inputs));
@@ -236,13 +222,13 @@ extern "C" int kgv_validate_block_bodies(kgv_ctx* ctx, const kgv_tx_batch* batch
   cudaStream_t st = ctx->stream;
   uint64_t* dhash = (uint64_t*)ctx->d_in;
   uint64_t* droots = (uint64_t*)(ctx->d_in + al256(nt * 32 + 32));  // copied out below: roots32 is a byte array of any alignment
-  kgv_body_result* dres = dev ? results : (kgv_body_result*)(S + o_res);
-  kgv_block_masses* dbm = (dev || !masses) ? masses : (kgv_block_masses*)(S + o_bm);
-  const kgv_block_header_ctx* dhdr = headers;
-  if (!dev) {
-    CK(cudaMemcpyAsync(S + o_hdr, headers, nb * sizeof(kgv_block_header_ctx), cudaMemcpyHostToDevice, st));
-    dhdr = (const kgv_block_header_ctx*)(S + o_hdr);
-  }
+  const kgv_block_header_ctx* dhdr;
+  kgv_body_result* dres;
+  kgv_block_masses* dbm;
+  io.in(headers, nb * sizeof(kgv_block_header_ctx), &dhdr);
+  io.out(results, nb * sizeof(kgv_body_result), &dres);
+  io.out(masses, nb * sizeof(kgv_block_masses), &dbm);
+  if ((rc = io.stage())) return rc;
   uint32_t* dfirst = (uint32_t*)(S + o_first);
   uint32_t* dtxb = (uint32_t*)(S + o_txb);
   kgv_tx_result* dtxr = (kgv_tx_result*)(S + o_txr);
@@ -267,11 +253,6 @@ extern "C" int kgv_validate_block_bodies(kgv_ctx* ctx, const kgv_tx_batch* batch
   k_body_rules<<<grid, BODY_RULE_THREADS, 0, st>>>(a, dres, dbm);
   CK(cudaGetLastError());
   ctx->launches++;
-  if (roots32) CK(cudaMemcpyAsync(roots32, droots, nb * 32, dev ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, st));
-  if (!dev) {
-    CK(cudaMemcpyAsync(results, dres, nb * sizeof(kgv_body_result), cudaMemcpyDeviceToHost, st));
-    if (masses) CK(cudaMemcpyAsync(masses, dbm, nb * sizeof(kgv_block_masses), cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
-  }
-  return KGV_OK;
+  if (roots32 && (rc = io.copy_out(roots32, droots, nb * 32))) return rc;
+  return io.finish();
 }

@@ -20,19 +20,6 @@ using namespace kgv;
 static_assert(sizeof(kgv_chain_header) == 112, "kgv_chain_header is 112 bytes");
 static_assert(sizeof(kgv_chain_result) == 112, "kgv_chain_result is 112 bytes");
 
-#define CK(call)                                                                                  \
-  do {                                                                                            \
-    cudaError_t e_ = (call);                                                                      \
-    if (e_ != cudaSuccess) {                                                                      \
-      char b_[256];                                                                               \
-      snprintf(b_, sizeof b_, "%s failed: %s (%s:%d)", #call, cudaGetErrorString(e_), __FILE__, __LINE__); \
-      ctx->err = b_;                                                                              \
-      return KGV_ERR_CUDA;                                                                        \
-    }                                                                                             \
-  } while (0)
-
-static inline size_t al256(size_t x) { return (x + 255) & ~(size_t)255; }
-static inline unsigned nblk(size_t n, unsigned b) { return (unsigned)((n + b - 1) / b); }
 
 constexpr int CHAIN_BLOCK_WARPS = 4;
 
@@ -256,12 +243,12 @@ extern "C" int kgv_replay_verify_chain(kgv_ctx* ctx, const uint32_t* group_first
     }
     if (n > max_ids) max_ids = (uint32_t)n;
   }
-  const bool dev = kgv_ptr_is_device(results) != 0;
-  for (const void* p : {(const void*)headers, (const void*)merged_flags, (const void*)init768, (const void*)block_fees, (const void*)multisets768})
-    if (p && (kgv_ptr_is_device(p) != 0) != dev) { ctx->err = "all data arrays of one call must be host pointers or all device pointers"; return KGV_ERR_ARG; }
+  kgv_io io(ctx);
+  bool dev;
+  if (int rc = io.one_side("kgv_replay_verify_chain", {results, headers, merged_flags, init768, block_fees, multisets768}, &dev)) return rc;
   CK(cudaSetDevice(ctx->device));
   cudaStream_t st = ctx->stream;
-  const cudaMemcpyKind in_kind = dev ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, out_kind = dev ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost;
+  const cudaMemcpyKind in_kind = dev ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
   const size_t nt = L.nt, nb = L.n_blocks;
   // scratch (d_work is free between validation calls); inputs are copied in, outputs copied out, so the caller's arrays need no alignment
   const size_t o_gf = 0, o_hdr = o_gf + al256((n_groups + 1) * 4), o_mf = o_hdr + al256(n_groups * sizeof(kgv_chain_header)), o_init = o_mf + al256(nb),
@@ -310,9 +297,8 @@ extern "C" int kgv_replay_verify_chain(kgv_ctx* ctx, const uint32_t* group_first
   k_chain_verdict<<<nblk(n_groups * 32, 128), 128, 0, st>>>(a);
   CK(cudaGetLastError());
   ctx->launches++;
-  CK(cudaMemcpyAsync(results, a.out, n_groups * sizeof(kgv_chain_result), out_kind, st));
-  if (block_fees) CK(cudaMemcpyAsync(block_fees, a.fee, nb * 8, out_kind, st));
-  if (multisets768) CK(cudaMemcpyAsync(multisets768, vals, n_groups * 768, out_kind, st));
-  if (!dev) CK(cudaStreamSynchronize(st));
-  return KGV_OK;
+  if ((rc = io.copy_out(results, a.out, n_groups * sizeof(kgv_chain_result)))) return rc;
+  if (block_fees && (rc = io.copy_out(block_fees, a.fee, nb * 8))) return rc;
+  if (multisets768 && (rc = io.copy_out(multisets768, vals, n_groups * 768))) return rc;
+  return io.finish();
 }

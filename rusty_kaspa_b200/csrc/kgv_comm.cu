@@ -21,17 +21,6 @@
 #include <cstring>
 #include <vector>
 
-#define CK(call)                                                                                  \
-  do {                                                                                            \
-    cudaError_t e_ = (call);                                                                      \
-    if (e_ != cudaSuccess) {                                                                      \
-      char b_[256];                                                                               \
-      snprintf(b_, sizeof b_, "%s failed: %s (%s:%d)", #call, cudaGetErrorString(e_), __FILE__, __LINE__); \
-      ctx->err = b_;                                                                              \
-      return KGV_ERR_CUDA;                                                                        \
-    }                                                                                             \
-  } while (0)
-
 // ---------------------------------------------------------------------------------------------
 // NCCL through dlopen (the five entry points used; signatures as in nccl.h 2.x)
 // ---------------------------------------------------------------------------------------------

@@ -10,18 +10,6 @@
 
 using namespace kgv;
 
-#define CK(call)                                                                                  \
-  do {                                                                                            \
-    cudaError_t e_ = (call);                                                                      \
-    if (e_ != cudaSuccess) {                                                                      \
-      char b_[256];                                                                               \
-      snprintf(b_, sizeof b_, "%s failed: %s (%s:%d)", #call, cudaGetErrorString(e_), __FILE__, __LINE__); \
-      ctx->err = b_;                                                                              \
-      return KGV_ERR_CUDA;                                                                        \
-    }                                                                                             \
-  } while (0)
-
-static inline size_t al256(size_t x) { return (x + 255) & ~(size_t)255; }
 
 // range checks of a HOST batch (a device-resident batch is trusted: its producer is device code of the same process)
 static int kgv_check_host_batch(std::string& err_out, const kgv_tx_batch* b) {
@@ -159,9 +147,11 @@ int kgv_batch_to_device(kgv_ctx* ctx, const kgv_tx_batch* b, kgv_dev_batch* out,
     ctx->err = "batch array missing";
     return KGV_ERR_ARG;
   }
+  bool dev;
+  kgv_io io(ctx);
+  if (int rc = io.one_side("kgv_tx_batch", {b->txs, b->inputs, b->outputs, b->entries, b->bytes}, &dev)) return rc;
   out->n_txs = b->n_txs; out->n_inputs = b->n_inputs; out->n_outputs = b->n_outputs; out->n_bytes = b->n_bytes;
-  const void* probe = b->n_txs ? (const void*)b->txs : (const void*)b->bytes;
-  if (probe && kgv_ptr_is_device(probe)) {
+  if (dev) {
     out->txs = b->txs; out->inputs = b->inputs; out->outputs = b->outputs; out->entries = b->entries; out->bytes = b->bytes;
     return KGV_OK;
   }
@@ -257,20 +247,12 @@ static int digest_common(kgv_ctx* ctx, const kgv_tx_batch* batch, uint8_t* out32
   kgv_dev_batch d;
   int rc = kgv_batch_to_device(ctx, batch, &d, false);
   if (rc) return rc;
-  bool out_dev = kgv_ptr_is_device(out32);
-  uint8_t* dout = out32;
-  if (!out_dev) {
-    rc = kgv_reserve(ctx, &ctx->d_out, &ctx->d_out_cap, d.n_txs * 32);
-    if (rc) return rc;
-    dout = ctx->d_out;
-  }
-  rc = kgv_tx_digests_run(ctx, d, d.n_txs, (uint64_t*)dout, hash);
-  if (rc) return rc;
-  if (!out_dev) {
-    CK(cudaMemcpyAsync(out32, dout, d.n_txs * 32, cudaMemcpyDeviceToHost, ctx->stream));
-    CK(cudaStreamSynchronize(ctx->stream));
-  }
-  return KGV_OK;
+  kgv_io io(ctx);
+  uint8_t* dout;
+  io.out(out32, d.n_txs * 32, &dout);
+  if ((rc = io.stage())) return rc;
+  if ((rc = kgv_tx_digests_run(ctx, d, d.n_txs, (uint64_t*)dout, hash))) return rc;
+  return io.finish();
 }
 extern "C" int kgv_tx_ids(kgv_ctx* ctx, const kgv_tx_batch* batch, uint8_t* out32) { return digest_common(ctx, batch, out32, false); }
 extern "C" int kgv_tx_hashes(kgv_ctx* ctx, const kgv_tx_batch* batch, uint8_t* out32) { return digest_common(ctx, batch, out32, true); }
@@ -284,21 +266,17 @@ extern "C" int kgv_sighash(kgv_ctx* ctx, const kgv_tx_batch* batch, const kgv_si
   kgv_dev_batch d;
   int rc = kgv_batch_to_device(ctx, batch, &d, true);
   if (rc) return rc;
-  bool io_dev = kgv_ptr_is_device(items);
-  if ((bool)kgv_ptr_is_device(out32) != io_dev) { ctx->err = "items and out32 must both be host or both be device pointers"; return KGV_ERR_ARG; }
-  size_t o_reused = 0, o_ent = al256(d.n_txs * sizeof(SigHashReused)), o_items = al256(o_ent + d.n_inputs * sizeof(DevEntry));
-  rc = kgv_reserve(ctx, &ctx->d_scratch, &ctx->d_scratch_cap, o_items + (io_dev ? 0 : n_items * sizeof(kgv_sighash_item)) + 256);
+  kgv_io io(ctx);
+  if ((rc = io.one_side("kgv_sighash", {items, out32}))) return rc;
+  size_t o_reused = 0, o_ent = al256(d.n_txs * sizeof(SigHashReused));
+  rc = kgv_reserve(ctx, &ctx->d_scratch, &ctx->d_scratch_cap, al256(o_ent + d.n_inputs * sizeof(DevEntry)) + 256);
   if (rc) return rc;
   SigHashReused* dre = (SigHashReused*)(ctx->d_scratch + o_reused);
-  const kgv_sighash_item* ditems = items;
-  uint8_t* dout = out32;
-  if (!io_dev) {
-    CK(cudaMemcpyAsync(ctx->d_scratch + o_items, items, n_items * sizeof(kgv_sighash_item), cudaMemcpyHostToDevice, ctx->stream));
-    ditems = (const kgv_sighash_item*)(ctx->d_scratch + o_items);
-    rc = kgv_reserve(ctx, &ctx->d_out, &ctx->d_out_cap, n_items * 32);
-    if (rc) return rc;
-    dout = ctx->d_out;
-  }
+  const kgv_sighash_item* ditems;
+  uint8_t* dout;
+  io.in(items, n_items * sizeof(kgv_sighash_item), &ditems);
+  io.out(out32, n_items * 32, &dout);
+  if ((rc = io.stage())) return rc;
   DevEntry* dent = (DevEntry*)(ctx->d_scratch + o_ent);
   if (d.n_inputs) {
     k_entries_to_dev<<<(unsigned)((d.n_inputs + 127) / 128), 128, 0, ctx->stream>>>(d.entries, d.bytes, d.n_inputs, dent);
@@ -311,11 +289,7 @@ extern "C" int kgv_sighash(kgv_ctx* ctx, const kgv_tx_batch* batch, const kgv_si
   k_sighash_items<<<(unsigned)((n_items + 127) / 128), 128, 0, ctx->stream>>>(v, dre, ditems, n_items, (uint32_t)d.n_txs, (uint32_t)d.n_inputs, (uint32_t*)dout);
   CK(cudaGetLastError());
   ctx->launches += 2;
-  if (!io_dev) {
-    CK(cudaMemcpyAsync(out32, dout, n_items * 32, cudaMemcpyDeviceToHost, ctx->stream));
-    CK(cudaStreamSynchronize(ctx->stream));
-  }
-  return KGV_OK;
+  return io.finish();
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -418,19 +392,18 @@ extern "C" int kgv_merkle_roots(kgv_ctx* ctx, const uint8_t* hashes32, const uin
   const size_t n_total = first[n_groups];
   if (n_total && !hashes32) { ctx->err = "null argument"; return KGV_ERR_ARG; }
   CK(cudaSetDevice(ctx->device));
-  const bool dev = n_total ? kgv_ptr_is_device(hashes32) != 0 : kgv_ptr_is_device(roots32) != 0;
-  if ((kgv_ptr_is_device(roots32) != 0) != dev) { ctx->err = "hashes and roots must both be host or both be device pointers"; return KGV_ERR_ARG; }
+  kgv_io io(ctx);
+  int rc = io.one_side("kgv_merkle_roots", {n_total ? hashes32 : nullptr, roots32});
+  if (rc) return rc;
   // working copy of the hashes (the tree overwrites its input buffer) + device roots
-  int rc = kgv_reserve(ctx, &ctx->d_in, &ctx->d_in_cap, al256(n_total * 32 + 32) + (size_t)n_groups * 32);
+  rc = kgv_reserve(ctx, &ctx->d_in, &ctx->d_in_cap, al256(n_total * 32 + 32) + (size_t)n_groups * 32);
   if (rc) return rc;
   uint64_t* dh = (uint64_t*)ctx->d_in;
   uint64_t* dr = (uint64_t*)(ctx->d_in + al256(n_total * 32 + 32));
-  if (n_total) CK(cudaMemcpyAsync(dh, hashes32, n_total * 32, dev ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, ctx->stream));
-  rc = kgv_merkle_run(ctx, dh, n_total, first, n_groups, dr);
-  if (rc) return rc;
-  CK(cudaMemcpyAsync(roots32, dr, (size_t)n_groups * 32, dev ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, ctx->stream));
-  if (!dev) CK(cudaStreamSynchronize(ctx->stream));
-  return KGV_OK;
+  if (n_total) CK(cudaMemcpyAsync(dh, hashes32, n_total * 32, cudaMemcpyDefault, ctx->stream));
+  if ((rc = kgv_merkle_run(ctx, dh, n_total, first, n_groups, dr))) return rc;
+  if ((rc = io.copy_out(roots32, dr, (size_t)n_groups * 32))) return rc;
+  return io.finish();
 }
 
 // calc_hash_merkle_root (consensus/core/src/merkle.rs:5-7) for every block of a batch: block b = transactions
@@ -458,10 +431,9 @@ extern "C" int kgv_block_hash_merkle_roots(kgv_ctx* ctx, const kgv_tx_batch* bat
   if (rc) return rc;
   rc = kgv_merkle_run(ctx, dh, nt, block_first_tx, n_blocks, dr);
   if (rc) return rc;
-  const bool dev = kgv_ptr_is_device(roots32) != 0;
-  CK(cudaMemcpyAsync(roots32, dr, (size_t)n_blocks * 32, dev ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, ctx->stream));
-  if (!dev) CK(cudaStreamSynchronize(ctx->stream));
-  return KGV_OK;
+  kgv_io io(ctx);
+  if ((rc = io.copy_out(roots32, dr, (size_t)n_blocks * 32))) return rc;
+  return io.finish();
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -517,8 +489,7 @@ extern "C" int kgv_block_set_checks(kgv_ctx* ctx, const kgv_tx_batch* batch, con
   k_block_set_checks_final<<<(n_blocks + 127) / 128, 128, 0, st>>>((const BlockCheckAcc*)(S + o_acc), n_blocks, (kgv_block_check*)(S + o_out));
   CK(cudaGetLastError());
   ctx->launches++;
-  const bool dev = kgv_ptr_is_device(out) != 0;
-  CK(cudaMemcpyAsync(out, S + o_out, (size_t)n_blocks * sizeof(kgv_block_check), dev ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, st));
-  if (!dev) CK(cudaStreamSynchronize(st));
-  return KGV_OK;
+  kgv_io io(ctx);
+  if ((rc = io.copy_out(out, S + o_out, (size_t)n_blocks * sizeof(kgv_block_check)))) return rc;
+  return io.finish();
 }

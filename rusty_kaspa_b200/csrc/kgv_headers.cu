@@ -19,18 +19,6 @@ static_assert(sizeof(kgv_header) == 208, "kgv_header is 208 bytes");
 static_assert(sizeof(kgv_header_rules) == 32, "kgv_header_rules is 32 bytes");
 static_assert(sizeof(kgv_header_result) == 24, "kgv_header_result is 24 bytes");
 
-#define CK(call)                                                                                  \
-  do {                                                                                            \
-    cudaError_t e_ = (call);                                                                      \
-    if (e_ != cudaSuccess) {                                                                      \
-      char b_[256];                                                                               \
-      snprintf(b_, sizeof b_, "%s failed: %s (%s:%d)", #call, cudaGetErrorString(e_), __FILE__, __LINE__); \
-      ctx->err = b_;                                                                              \
-      return KGV_ERR_CUDA;                                                                        \
-    }                                                                                             \
-  } while (0)
-
-static inline size_t al256(size_t x) { return (x + 255) & ~(size_t)255; }
 
 constexpr int HDR_HASH_THREADS = 128;
 constexpr int HDR_CTA = 64;
@@ -192,43 +180,29 @@ __global__ void __launch_bounds__(HDR_CTA) k_pow_matrix_debug(int op, const uint
 
 // ---- C ABI ------------------------------------------------------------------------------------------------------------------------
 
-static int fail_arg(kgv_ctx* ctx, const char* m) {
-  ctx->err = m;
-  return KGV_ERR_ARG;
+// Declares the header arrays and the arena-range flag of a call; its HeaderArena is complete after io.stage() (ar->bad: clear it)
+static void declare_headers(kgv_io& io, const kgv_header* headers, size_t n, const uint8_t* parents32, size_t n_parents, const uint32_t* level_len,
+                            size_t n_level_entries, unsigned int* bad, HeaderArena* ar) {
+  ar->n = n; ar->n_parents = n_parents; ar->n_level_entries = n_level_entries;
+  io.in(headers, n * sizeof(kgv_header), &ar->h);
+  io.in(n_parents ? parents32 : nullptr, n_parents * 32, &ar->parents);
+  io.in(n_level_entries ? level_len : nullptr, n_level_entries * 4, &ar->level_len);
+  io.out(bad, 4, &ar->bad);  // a host scalar: finish() always waits for the call
 }
 
-// Makes the header arrays device resident (host arrays are staged in d_in); returns the arena and whether the call is on device pointers
-static int stage_headers(kgv_ctx* ctx, const kgv_header* headers, size_t n, const uint8_t* parents32, size_t n_parents, const uint32_t* level_len,
-                         size_t n_level_entries, bool* dev, HeaderArena* ar) {
-  *dev = kgv_ptr_is_device(headers) != 0;
+// the refusals shared by the two calls: null or mixed arrays, device arrays not 8-byte aligned
+static int check_headers(kgv_ctx* ctx, kgv_io& io, const char* call, const kgv_header* headers, const uint8_t* parents32, size_t n_parents,
+                         const uint32_t* level_len, size_t n_level_entries, const void* o0, const void* o1, const void* o2) {
   if ((n_parents && !parents32) || (n_level_entries && !level_len)) return fail_arg(ctx, "null argument");
-  if ((n_parents && (kgv_ptr_is_device(parents32) != 0) != *dev) || (n_level_entries && (kgv_ptr_is_device(level_len) != 0) != *dev))
-    return fail_arg(ctx, "all buffers of one call must be host pointers or all device pointers");
-  const size_t o_par = al256(n * sizeof(kgv_header)), o_len = o_par + al256(n_parents * 32);
-  // the flag that reports an arena range outside the arena, then (host calls) the staged arrays
-  int rc = kgv_reserve(ctx, &ctx->d_in, &ctx->d_in_cap, 256 + (*dev ? 0 : o_len + n_level_entries * 4));
-  if (rc) return rc;
-  ar->bad = (unsigned int*)ctx->d_in;
-  CK(cudaMemsetAsync(ar->bad, 0, 4, ctx->stream));
-  ar->n = n; ar->n_parents = n_parents; ar->n_level_entries = n_level_entries;
-  if (*dev) {
-    if (((uintptr_t)headers & 7) || ((uintptr_t)parents32 & 7)) return fail_arg(ctx, "device headers and parents32 must be 8-byte aligned");
-    ar->h = headers; ar->parents = parents32; ar->level_len = level_len;
-    return KGV_OK;
-  }
-  uint8_t* base = ctx->d_in + 256;
-  CK(cudaMemcpyAsync(base, headers, n * sizeof(kgv_header), cudaMemcpyHostToDevice, ctx->stream));
-  if (n_parents) CK(cudaMemcpyAsync(base + o_par, parents32, n_parents * 32, cudaMemcpyHostToDevice, ctx->stream));
-  if (n_level_entries) CK(cudaMemcpyAsync(base + o_len, level_len, n_level_entries * 4, cudaMemcpyHostToDevice, ctx->stream));
-  ar->h = (const kgv_header*)base; ar->parents = base + o_par; ar->level_len = (const uint32_t*)(base + o_len);
-  return KGV_OK;
+  bool dev;
+  if (int rc = io.one_side(call, {headers, n_parents ? parents32 : nullptr, n_level_entries ? level_len : nullptr, o0, o1, o2}, &dev)) return rc;
+  const uintptr_t a = (uintptr_t)headers | (uintptr_t)parents32 | (uintptr_t)o0 | (uintptr_t)o1 | (uintptr_t)o2;
+  return dev && (a & 7) ? fail_arg(ctx, "device headers, parents32 and outputs must be 8-byte aligned") : KGV_OK;
 }
 
 // waits for the call and reports an arena range outside the arena
-static int finish_headers(kgv_ctx* ctx, const HeaderArena& ar) {
-  unsigned int bad = 0;
-  CK(cudaMemcpyAsync(&bad, ar.bad, 4, cudaMemcpyDeviceToHost, ctx->stream));
-  CK(cudaStreamSynchronize(ctx->stream));
+static int finish_headers(kgv_ctx* ctx, kgv_io& io, const unsigned int& bad) {
+  if (int rc = io.finish()) return rc;
   return bad ? fail_arg(ctx, "a header's levels_off / parents_off range leaves the arena") : KGV_OK;
 }
 
@@ -240,28 +214,21 @@ extern "C" int kgv_hash_headers(kgv_ctx* ctx, const kgv_header* headers, size_t 
   if (n == 0) return KGV_OK;
   if (!headers || (!hash32 && !pre_pow32)) return fail_arg(ctx, "null argument");
   CK(cudaSetDevice(ctx->device));
-  bool dev;
-  HeaderArena ar;
-  int rc = stage_headers(ctx, headers, n, parents32, n_parents, level_len, n_level_entries, &dev, &ar);
+  kgv_io io(ctx);
+  int rc = check_headers(ctx, io, "kgv_hash_headers", headers, parents32, n_parents, level_len, n_level_entries, hash32, pre_pow32, nullptr);
   if (rc) return rc;
-  for (uint8_t* o : {hash32, pre_pow32})
-    if (o && (kgv_ptr_is_device(o) != 0) != dev) return fail_arg(ctx, "all buffers of one call must be host pointers or all device pointers");
-  if (dev && (((uintptr_t)hash32 & 7) || ((uintptr_t)pre_pow32 & 7))) return fail_arg(ctx, "device outputs must be 8-byte aligned");
-  uint64_t *dh = (uint64_t*)hash32, *dp = (uint64_t*)pre_pow32;
-  if (!dev) {
-    rc = kgv_reserve(ctx, &ctx->d_out, &ctx->d_out_cap, 64 * n);
-    if (rc) return rc;
-    dh = hash32 ? (uint64_t*)ctx->d_out : nullptr;
-    dp = pre_pow32 ? (uint64_t*)(ctx->d_out + 32 * n) : nullptr;
-  }
+  HeaderArena ar;
+  unsigned int bad = 0;
+  uint64_t *dh, *dp;
+  declare_headers(io, headers, n, parents32, n_parents, level_len, n_level_entries, &bad, &ar);
+  io.out((uint64_t*)hash32, 32 * n, &dh);
+  io.out((uint64_t*)pre_pow32, 32 * n, &dp);
+  if ((rc = io.stage())) return rc;
+  CK(cudaMemsetAsync(ar.bad, 0, 4, ctx->stream));
   k_header_hash<<<(unsigned)((n + HDR_HASH_THREADS - 1) / HDR_HASH_THREADS), HDR_HASH_THREADS, 0, ctx->stream>>>(ar, dh, dp);
   CK(cudaGetLastError());
   ctx->launches++;
-  if (!dev) {
-    if (hash32) CK(cudaMemcpyAsync(hash32, dh, 32 * n, cudaMemcpyDeviceToHost, ctx->stream));
-    if (pre_pow32) CK(cudaMemcpyAsync(pre_pow32, dp, 32 * n, cudaMemcpyDeviceToHost, ctx->stream));
-  }
-  return finish_headers(ctx, ar);
+  return finish_headers(ctx, io, bad);
 }
 
 // validate_header_in_isolation (pre_ghostdag_validation.rs:17-24) with check_pow_and_calc_block_level (:102-106) for every header
@@ -276,32 +243,22 @@ extern "C" int kgv_validate_headers_in_isolation(kgv_ctx* ctx, const kgv_header*
   if (rules->max_block_level > 255) return fail_arg(ctx, "max_block_level is a BlockLevel (u8)");
   if (n > 0x7FFFFFFFull) return fail_arg(ctx, "at most 2^31 - 1 headers per call");
   CK(cudaSetDevice(ctx->device));
-  bool dev;
-  ValidateArgs a;
-  int rc = stage_headers(ctx, headers, n, parents32, n_parents, level_len, n_level_entries, &dev, &a.ar);
+  kgv_io io(ctx);
+  int rc = check_headers(ctx, io, "kgv_validate_headers_in_isolation", headers, parents32, n_parents, level_len, n_level_entries, results, hash32, pow32);
   if (rc) return rc;
-  for (void* o : {(void*)results, (void*)hash32, (void*)pow32})
-    if (o && (kgv_ptr_is_device(o) != 0) != dev) return fail_arg(ctx, "all buffers of one call must be host pointers or all device pointers");
-  if (dev && (((uintptr_t)results & 7) || ((uintptr_t)hash32 & 7) || ((uintptr_t)pow32 & 7))) return fail_arg(ctx, "device outputs must be 8-byte aligned");
+  ValidateArgs a;
+  unsigned int bad = 0;
+  declare_headers(io, headers, n, parents32, n_parents, level_len, n_level_entries, &bad, &a.ar);
+  io.out(results, n * sizeof(kgv_header_result), &a.res);
+  io.out((uint64_t*)hash32, 32 * n, &a.hash);
+  io.out((uint64_t*)pow32, 32 * n, &a.pow);
+  if ((rc = io.stage())) return rc;
+  CK(cudaMemsetAsync(a.ar.bad, 0, 4, ctx->stream));
   a.r = *rules;
-  a.res = results; a.hash = (uint64_t*)hash32; a.pow = (uint64_t*)pow32;
-  const size_t o_hash = al256(n * sizeof(kgv_header_result)), o_pow = o_hash + al256(32 * n);
-  if (!dev) {
-    rc = kgv_reserve(ctx, &ctx->d_out, &ctx->d_out_cap, o_pow + 32 * n);
-    if (rc) return rc;
-    a.res = (kgv_header_result*)ctx->d_out;
-    a.hash = hash32 ? (uint64_t*)(ctx->d_out + o_hash) : nullptr;
-    a.pow = pow32 ? (uint64_t*)(ctx->d_out + o_pow) : nullptr;
-  }
   k_header_validate<<<(unsigned)n, HDR_CTA, 0, ctx->stream>>>(a);
   CK(cudaGetLastError());
   ctx->launches++;
-  if (!dev) {
-    CK(cudaMemcpyAsync(results, a.res, n * sizeof(kgv_header_result), cudaMemcpyDeviceToHost, ctx->stream));
-    if (hash32) CK(cudaMemcpyAsync(hash32, a.hash, 32 * n, cudaMemcpyDeviceToHost, ctx->stream));
-    if (pow32) CK(cudaMemcpyAsync(pow32, a.pow, 32 * n, cudaMemcpyDeviceToHost, ctx->stream));
-  }
-  return finish_headers(ctx, a.ar);
+  return finish_headers(ctx, io, bad);
 }
 
 extern "C" int kgv_debug_pow_matrix(kgv_ctx* ctx, int op, const uint8_t* in, size_t n, uint8_t* out) {

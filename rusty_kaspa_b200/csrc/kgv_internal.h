@@ -2,6 +2,8 @@
 #pragma once
 #include <cuda_runtime.h>
 #include <cstdint>
+#include <cstdio>
+#include <initializer_list>
 #include <mutex>
 #include <string>
 #include <thread>
@@ -27,9 +29,11 @@ struct kgv_ctx {
   cudaEvent_t ev_chunk[32] = {};                  // upload-complete events of the chunked host-pointer verify path
   cudaStream_t stream = nullptr;
   uint32_t* gtab = nullptr;     // [8][65536][16] u32: v*2^(32j)*G in table j, affine
-  uint8_t* d_in = nullptr;      // staging for host-pointer calls
+  uint8_t* d_io = nullptr;      // device stand-ins of a call's host arrays (kgv_io only)
+  size_t d_io_cap = 0;
+  uint8_t* d_in = nullptr;      // per-call device scratch (verify uploads, signature items, script rounds, merkle trees)
   size_t d_in_cap = 0;
-  uint8_t* d_out = nullptr;
+  uint8_t* d_out = nullptr;     // per-call device scratch (verify statuses, the script engine's phase 1)
   size_t d_out_cap = 0;
   uint8_t* d_batch = nullptr;   // staging for host-resident transaction batches
   size_t d_batch_cap = 0;
@@ -92,8 +96,93 @@ int kgv_ptr_is_device(const void* p);
 int kgv_malloc(kgv_ctx* ctx, void** p, size_t bytes);
 int kgv_reserve(kgv_ctx* ctx, uint8_t** buf, size_t* cap, size_t need);
 
-// ---- transaction batches on the device (kgv_hash.cu) ----
 #include "../../include/kgv.h"
+
+// returns KGV_ERR_CUDA from the enclosing function (which has `ctx` in scope) when a CUDA call fails
+#define CK(call)                                                                                  \
+  do {                                                                                            \
+    cudaError_t e_ = (call);                                                                      \
+    if (e_ != cudaSuccess) {                                                                      \
+      char b_[256];                                                                               \
+      snprintf(b_, sizeof b_, "%s failed: %s (%s:%d)", #call, cudaGetErrorString(e_), __FILE__, __LINE__); \
+      ctx->err = b_;                                                                              \
+      return KGV_ERR_CUDA;                                                                        \
+    }                                                                                             \
+  } while (0)
+
+static inline size_t al256(size_t x) { return (x + 255) & ~(size_t)255; }
+static inline unsigned nblk(size_t n, unsigned b) { return (unsigned)((n + b - 1) / b); }
+static inline int fail_arg(kgv_ctx* ctx, const char* m) {
+  if (ctx) ctx->err = m;
+  return KGV_ERR_ARG;
+}
+
+// ---- where a call's caller-owned arrays live (include/kgv.h, Conventions) ----
+// A call declares every array it reads (in) or writes (out) before it stages anything.  stage() gives each host array a device stand-in
+// in ctx->d_io (one kgv_reserve per call) and uploads the host inputs on ctx->stream; a device array is used where it is.  copy_out()
+// enqueues a copy of a device result into a caller's array of either kind.  finish() copies the host outputs back and synchronises
+// ctx->stream once, only when some output (of out or copy_out) is host memory; device outputs leave the call enqueued.
+//
+// Which arrays of a call must share a side (one_side), which are fixed to one, and which are each on their own side (the rest):
+//   kgv_schnorr_verify, kgv_ecdsa_verify     pk, msg, sig, status together (large host batches upload in chunks on the side stream)
+//   kgv_status_to_bitmap                     status, bitmap together
+//   kgv_tx_ids, kgv_tx_hashes                out32 on its own side
+//   kgv_sighash                              items and out32 together, independent of the batch
+//   kgv_merkle_roots                         hashes32 and roots32 together; first on the host
+//   kgv_block_hash_merkle_roots,
+//   kgv_block_set_checks                     the output on its own side; block_first_tx on the host
+//   kgv_muhash_elements                      numerator384 and denominator384 together; data and remove staged with host offsets
+//   kgv_muhash_combine, kgv_muhash_finalize  the inputs copied into the workspace from the side of the first; each output on its own side
+//   kgv_muhash_finalize_batch                numerators384, denominators384, hashes32 together; device arrays aligned
+//   kgv_muhash_prefix_combine                values768 (updated in place, 16-byte aligned on the device) and init768 each on their own side
+//   kgv_muhash_txs                           numerator384 and denominator384 together; accept on its own side
+//   kgv_utxo_lookup / _apply_diff / _export  each array on its own side
+//   kgv_utxo_import_chunk                    numerator384 on the host; keys36, entries, bytes each on their own side
+//   kgv_utxo_apply_accepted                  accept on its own side (a host accept: the call waits for the table)
+//   kgv_validate_txs, kgv_validate_populated results on its own side, independent of the batch
+//   kgv_validate_mempool_txs*                results, batch->txs, args, storage_mass, entries_out, scripts_out, masses, detail together
+//   kgv_validate_txs_in_isolation            results, batch->txs, masses together; rules on the host
+//   kgv_check_txs_standard_in_isolation      results, batch->txs, masses, detail together; the policy on the host
+//   kgv_check_txs_standard_in_context        results, batch->txs, masses, storage_mass, fee, detail together; the policy on the host
+//   kgv_outputs_dust                         is_dust and batch->outputs together
+//   kgv_validate_block_bodies                results, batch->txs, headers, masses, roots32 together; block_first_tx and the rules on the host
+//   kgv_hash_headers, kgv_validate_headers_in_isolation
+//                                            headers, parents32, level_len and the outputs together, device arrays 8-byte aligned; rules on the host
+//   kgv_replay_window                        blocks on the host; results and accept each on their own side
+//   kgv_replay_muhash                        values768 on its own side; group_first_block on the host
+//   kgv_replay_diffs                         the output arrays together (ranges alone when counting); group_first_block on the host
+//   kgv_replay_verify_chain                  results, headers, merged_flags, init768, block_fees, multisets768 together (inputs are copied into
+//                                            the call's own workspace from either side); group_first_block on the host
+//   kgv_check_scripts                        tx_indices and results each on their own side
+//   the kgv_comm.cu calls                    device arrays only
+// The arrays of a transaction batch are staged by kgv_batch_to_device (d_batch, or a prefetch slot) and must all be of one kind.
+class kgv_io {
+ public:
+  explicit kgv_io(kgv_ctx* c) : ctx(c) {}
+  // KGV_ERR_ARG, with a message naming `call`, unless the non-null pointers are all host or all device memory; *dev (may be null): their side
+  int one_side(const char* call, std::initializer_list<const void*> ps, bool* dev = nullptr);
+  bool is_device(const void* p);  // queried once per pointer and call
+  // *d = the array's device address: p itself for device memory (or null p), its stand-in after stage() for host memory
+  template <class T> void in(const T* p, size_t bytes, const T** d) { add(p, bytes, (const void**)d, true, false); }
+  template <class T> void out(T* p, size_t bytes, T** d) { add(p, bytes, (const void**)d, false, true); }
+  template <class T> void inout(T* p, size_t bytes, T** d) { add(p, bytes, (const void**)d, true, true); }  // updated in place
+  int stage();
+  int copy_out(void* p, const void* d, size_t bytes);
+  void trim(const void* p, size_t bytes);  // a declared output comes back only up to `bytes` (sizes known after the kernels)
+  int finish();
+
+ private:
+  void add(const void* p, size_t bytes, const void** d, bool in, bool out);
+  kgv_ctx* ctx;
+  struct Arr { const void* p; size_t bytes; const void** d; bool in, out; };
+  Arr arr[10];          // the host arrays of the call
+  int n_arr = 0;
+  struct Side { const void* p; bool dev; } side[16];
+  int n_side = 0;
+  bool host_out = false;
+};
+
+// ---- transaction batches on the device (kgv_hash.cu) ----
 struct kgv_dev_batch {
   const kgv_tx* txs;
   const kgv_input* inputs;
@@ -116,7 +205,7 @@ int kgv_launch_verify(kgv_ctx* ctx, const uint8_t* dpk, const uint8_t* dmsg, con
 int kgv_mu_reserve(kgv_ctx* ctx, size_t n_den, size_t n_num, uint32_t** e_den, uint32_t** e_num);
 // Multiply each tree down to one value (denominator on ctx->stream, numerator on the side stream) and write the two
 // canonical residues (384 little-endian bytes each) to host or device memory.
-int kgv_mu_reduce(kgv_ctx* ctx, size_t n_den, size_t n_num, uint8_t* out_num384, uint8_t* out_den384);
+int kgv_mu_reduce(kgv_ctx* ctx, kgv_io& io, size_t n_den, size_t n_num, uint8_t* out_num384, uint8_t* out_den384);
 // out + g * out_pitch_words = product of the level-0 elements E[lo[g] .. hi[g]) with flags[flag_index[j]] != 0 (one 16-lane group per range)
 int kgv_mu_range_products(kgv_ctx* ctx, const uint32_t* E, size_t stride, const uint8_t* flags, const uint32_t* flag_index, const uint32_t* lo, const uint32_t* hi, uint32_t n_segs,
                           uint32_t* out, size_t out_pitch_words, cudaStream_t st);

@@ -17,18 +17,6 @@ using namespace kgv;
 static_assert(sizeof(kgv_tx_rules) == 72, "kgv_tx_rules is 72 bytes");
 static_assert(sizeof(kgv_tx_masses) == 16, "kgv_tx_masses is 16 bytes");
 
-#define CK(call)                                                                                  \
-  do {                                                                                            \
-    cudaError_t e_ = (call);                                                                      \
-    if (e_ != cudaSuccess) {                                                                      \
-      char b_[256];                                                                               \
-      snprintf(b_, sizeof b_, "%s failed: %s (%s:%d)", #call, cudaGetErrorString(e_), __FILE__, __LINE__); \
-      ctx->err = b_;                                                                              \
-      return KGV_ERR_CUDA;                                                                        \
-    }                                                                                             \
-  } while (0)
-
-static inline size_t al256(size_t x) { return (x + 255) & ~(size_t)255; }
 
 constexpr int ISO_WARPS = 4;            // transactions per block of k_tx_isolation
 constexpr int ISO_LARGE_THREADS = 256;  // k_tx_isolation_large
@@ -171,27 +159,20 @@ extern "C" int kgv_validate_txs_in_isolation(kgv_ctx* ctx, const kgv_tx_batch* b
   if (batch->n_txs == 0) return KGV_OK;
   if (batch->n_txs > 0xFFFFFFFFull) { ctx->err = "kgv_validate_txs_in_isolation: more than 2^32 - 1 transactions"; return KGV_ERR_ARG; }
   CK(cudaSetDevice(ctx->device));
-  const bool dev = kgv_ptr_is_device(results) != 0;
-  for (const void* p : {(const void*)batch->txs, (const void*)masses})
-    if (p && (kgv_ptr_is_device(p) != 0) != dev) { ctx->err = "kgv_validate_txs_in_isolation: the batch and outputs must all be host or all be device pointers"; return KGV_ERR_ARG; }
+  kgv_io io(ctx);
+  if (int rc = io.one_side("kgv_validate_txs_in_isolation", {results, batch->txs, masses})) return rc;
   kgv_dev_batch d;
   int rc = kgv_batch_to_device(ctx, batch, &d, false);
   if (rc) return rc;
   const size_t nt = d.n_txs;
-  const size_t o_res = 0, o_mass = al256(nt * sizeof(kgv_tx_result)), o_list = al256(o_mass + nt * sizeof(kgv_tx_masses));
-  rc = kgv_reserve(ctx, &ctx->d_work, &ctx->d_work_cap, al256(o_list + (nt + 1) * 4));
-  if (rc) return rc;
-  uint8_t* S = ctx->d_work;
-  kgv_tx_result* dres = dev ? results : (kgv_tx_result*)(S + o_res);
-  kgv_tx_masses* dm = (dev || !masses) ? masses : (kgv_tx_masses*)(S + o_mass);
-  cudaStream_t st = ctx->stream;
+  kgv_tx_result* dres;
+  kgv_tx_masses* dm;
+  io.out(results, nt * sizeof(kgv_tx_result), &dres);
+  io.out(masses, nt * sizeof(kgv_tx_masses), &dm);
+  if ((rc = io.stage())) return rc;
+  if ((rc = kgv_reserve(ctx, &ctx->d_work, &ctx->d_work_cap, (nt + 1) * 4))) return rc;
   rc = kgv_isolation_run(ctx, d, *rules, ctx_daa_score, ctx_past_median_time, !(flags & KGV_ISOLATION_SKIP_FINALITY), dres, dm, nullptr,
-                         (uint32_t*)(S + o_list), st);
+                         (uint32_t*)ctx->d_work, ctx->stream);
   if (rc) return rc;
-  if (!dev) {
-    CK(cudaMemcpyAsync(results, dres, nt * sizeof(kgv_tx_result), cudaMemcpyDeviceToHost, st));
-    if (masses) CK(cudaMemcpyAsync(masses, dm, nt * sizeof(kgv_tx_masses), cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
-  }
-  return KGV_OK;
+  return io.finish();
 }

@@ -419,28 +419,76 @@ __global__ void k_status_to_bitmap(const uint8_t* __restrict__ status, size_t n,
 // ---------------------------------------------------------------------------------------------
 // context
 // ---------------------------------------------------------------------------------------------
-#define CK(call)                                                                                  \
-  do {                                                                                            \
-    cudaError_t e_ = (call);                                                                      \
-    if (e_ != cudaSuccess) {                                                                      \
-      char b_[256];                                                                               \
-      snprintf(b_, sizeof b_, "%s failed: %s (%s:%d)", #call, cudaGetErrorString(e_), __FILE__, __LINE__); \
-      ctx->err = b_;                                                                              \
-      return KGV_ERR_CUDA;                                                                        \
-    }                                                                                             \
-  } while (0)
-
-static int fail_arg(kgv_ctx* ctx, const char* msg) {
-  if (ctx) ctx->err = msg;
-  return KGV_ERR_ARG;
-}
-
 // 1 = device-accessible pointer, 0 = host pointer
 int kgv_ptr_is_device(const void* p) {
   cudaPointerAttributes a;
   cudaError_t e = cudaPointerGetAttributes(&a, p);
   if (e != cudaSuccess) { (void)cudaGetLastError(); return 0; }
   return a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged;
+}
+
+bool kgv_io::is_device(const void* p) {
+  for (int i = 0; i < n_side; i++)
+    if (side[i].p == p) return side[i].dev;
+  const bool dev = kgv_ptr_is_device(p) != 0;
+  if (n_side < 16) side[n_side++] = {p, dev};
+  return dev;
+}
+
+int kgv_io::one_side(const char* call, std::initializer_list<const void*> ps, bool* dev) {
+  int first = -1;  // side of the first non-null pointer
+  for (const void* p : ps) {
+    if (!p) continue;
+    const int d = is_device(p);
+    if (first < 0) first = d;
+    else if (d != first) {
+      ctx->err = std::string(call) + ": the arrays of one call must be all host pointers or all device pointers";
+      return KGV_ERR_ARG;
+    }
+  }
+  if (dev) *dev = first == 1;
+  return KGV_OK;
+}
+
+void kgv_io::add(const void* p, size_t bytes, const void** d, bool in, bool out) {
+  *d = p;
+  if (!p || is_device(p)) return;
+  arr[n_arr++] = {p, bytes, d, in, out};
+  host_out |= out;
+}
+
+int kgv_io::stage() {
+  size_t total = 0;
+  for (int i = 0; i < n_arr; i++) total += al256(arr[i].bytes);
+  if (total == 0) return KGV_OK;
+  int rc = kgv_reserve(ctx, &ctx->d_io, &ctx->d_io_cap, total);
+  if (rc) return rc;
+  size_t o = 0;
+  for (int i = 0; i < n_arr; i++) {
+    *arr[i].d = ctx->d_io + o;
+    if (arr[i].in && arr[i].bytes) CK(cudaMemcpyAsync(ctx->d_io + o, arr[i].p, arr[i].bytes, cudaMemcpyHostToDevice, ctx->stream));
+    o += al256(arr[i].bytes);
+  }
+  return KGV_OK;
+}
+
+int kgv_io::copy_out(void* p, const void* d, size_t bytes) {
+  const bool dev = is_device(p);
+  host_out |= !dev;
+  CK(cudaMemcpyAsync(p, d, bytes, dev ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, ctx->stream));
+  return KGV_OK;
+}
+
+void kgv_io::trim(const void* p, size_t bytes) {
+  for (int i = 0; i < n_arr; i++)
+    if (arr[i].p == p && bytes < arr[i].bytes) arr[i].bytes = bytes;
+}
+
+int kgv_io::finish() {
+  for (int i = 0; i < n_arr; i++)
+    if (arr[i].out && arr[i].bytes) CK(cudaMemcpyAsync((void*)arr[i].p, *arr[i].d, arr[i].bytes, cudaMemcpyDeviceToHost, ctx->stream));
+  if (host_out) CK(cudaStreamSynchronize(ctx->stream));
+  return KGV_OK;
 }
 
 // Per-call device buffers only ever grow.  The outgrown allocation is NOT freed on the spot: cudaFree synchronises the whole device, which
@@ -523,7 +571,7 @@ extern "C" void kgv_destroy(kgv_ctx* ctx) {
   if (ctx->copy_stream) cudaStreamSynchronize(ctx->copy_stream);
   cudaStreamSynchronize(ctx->stream);
   if (ctx->gtab) cudaFree(ctx->gtab);
-  for (uint8_t* b : {ctx->d_in, ctx->d_out, ctx->d_batch, ctx->prefetch[0].buf, ctx->prefetch[1].buf, ctx->d_scratch, ctx->d_mu, ctx->d_work, ctx->d_replay, ctx->d_keys[0], ctx->d_keys[1]})
+  for (uint8_t* b : {ctx->d_io, ctx->d_in, ctx->d_out, ctx->d_batch, ctx->prefetch[0].buf, ctx->prefetch[1].buf, ctx->d_scratch, ctx->d_mu, ctx->d_work, ctx->d_replay, ctx->d_keys[0], ctx->d_keys[1]})
     if (b) cudaFree(b);
   for (uint8_t* b : ctx->parked) cudaFree(b);
   for (cudaEvent_t e : ctx->ev_chunk) if (e) cudaEventDestroy(e);
@@ -643,54 +691,47 @@ static int verify_common(kgv_ctx* ctx, const uint8_t* pk, size_t pk_stride, cons
   if (n == 0) return KGV_OK;
   if (!pk || !msg || !sig || !status) return fail_arg(ctx, "null buffer");
   CK(cudaSetDevice(ctx->device));
-  int dev = kgv_ptr_is_device(pk);
-  if (kgv_ptr_is_device(msg) != dev || kgv_ptr_is_device(sig) != dev || kgv_ptr_is_device(status) != dev)
-    return fail_arg(ctx, "all buffers of one call must be host pointers or all device pointers");
-  const uint8_t *dpk = pk, *dmsg = msg, *dsig = sig;
-  uint8_t* dst = status;
-  if (!dev) {
+  kgv_io io(ctx);
+  bool dev;
+  if (int rc = io.one_side(ecdsa ? "kgv_ecdsa_verify" : "kgv_schnorr_verify", {pk, msg, sig, status}, &dev)) return rc;
+  // Large host batches are uploaded in chunks of one full persistent wave (resident threads x KGV_ITEMS signatures) on the
+  // side stream while the previous chunk is being verified: only the first chunk's upload is exposed.
+  const size_t chunk = (size_t)ctx->resident_blocks * KGV_BLOCK * KGV_ITEMS;
+  if (!dev && n >= 2 * chunk && (n + chunk - 1) / chunk <= 32) {
     size_t off_msg = (pk_stride * n + 255) & ~(size_t)255;
     size_t off_sig = off_msg + 32 * n;
     int rc = kgv_reserve(ctx, &ctx->d_in, &ctx->d_in_cap, off_sig + 64 * n);
     if (rc) return rc;
     rc = kgv_reserve(ctx, &ctx->d_out, &ctx->d_out_cap, n);
     if (rc) return rc;
-    dpk = ctx->d_in; dmsg = ctx->d_in + off_msg; dsig = ctx->d_in + off_sig; dst = ctx->d_out;
-    // Large host batches are uploaded in chunks of one full persistent wave (resident threads x KGV_ITEMS signatures) on the
-    // side stream while the previous chunk is being verified: only the first chunk's upload is exposed.
-    const size_t chunk = (size_t)ctx->resident_blocks * KGV_BLOCK * KGV_ITEMS;
-    if (n >= 2 * chunk && (n + chunk - 1) / chunk <= 32) {
-      CK(cudaEventRecord(ctx->ev_fork, ctx->stream));          // the staging buffers may still be read by earlier work of this stream
-      CK(cudaStreamWaitEvent(ctx->aux_stream, ctx->ev_fork, 0));
-      size_t c = 0;
-      for (size_t a = 0; a < n; a += chunk, c++) {
-        const size_t m = n - a < chunk ? n - a : chunk;
-        if (!ctx->ev_chunk[c]) CK(cudaEventCreateWithFlags(&ctx->ev_chunk[c], cudaEventDisableTiming));
-        CK(cudaMemcpyAsync(ctx->d_in + pk_stride * a, pk + pk_stride * a, pk_stride * m, cudaMemcpyHostToDevice, ctx->aux_stream));
-        CK(cudaMemcpyAsync(ctx->d_in + off_msg + 32 * a, msg + 32 * a, 32 * m, cudaMemcpyHostToDevice, ctx->aux_stream));
-        CK(cudaMemcpyAsync(ctx->d_in + off_sig + 64 * a, sig + 64 * a, 64 * m, cudaMemcpyHostToDevice, ctx->aux_stream));
-        CK(cudaEventRecord(ctx->ev_chunk[c], ctx->aux_stream));
-        CK(cudaStreamWaitEvent(ctx->stream, ctx->ev_chunk[c], 0));
-        int rc2 = kgv_launch_verify(ctx, dpk + pk_stride * a, dmsg + 32 * a, dsig + 64 * a, m, dst + a, ecdsa, ctx->stream);
-        if (rc2) return rc2;
-      }
-      CK(cudaMemcpyAsync(status, dst, n, cudaMemcpyDeviceToHost, ctx->stream));
-      CK(cudaStreamSynchronize(ctx->stream));
-      return KGV_OK;
+    const uint8_t *dpk = ctx->d_in, *dmsg = ctx->d_in + off_msg, *dsig = ctx->d_in + off_sig;
+    uint8_t* dst = ctx->d_out;
+    CK(cudaEventRecord(ctx->ev_fork, ctx->stream));          // the staging buffers may still be read by earlier work of this stream
+    CK(cudaStreamWaitEvent(ctx->aux_stream, ctx->ev_fork, 0));
+    size_t c = 0;
+    for (size_t a = 0; a < n; a += chunk, c++) {
+      const size_t m = n - a < chunk ? n - a : chunk;
+      if (!ctx->ev_chunk[c]) CK(cudaEventCreateWithFlags(&ctx->ev_chunk[c], cudaEventDisableTiming));
+      CK(cudaMemcpyAsync(ctx->d_in + pk_stride * a, pk + pk_stride * a, pk_stride * m, cudaMemcpyHostToDevice, ctx->aux_stream));
+      CK(cudaMemcpyAsync(ctx->d_in + off_msg + 32 * a, msg + 32 * a, 32 * m, cudaMemcpyHostToDevice, ctx->aux_stream));
+      CK(cudaMemcpyAsync(ctx->d_in + off_sig + 64 * a, sig + 64 * a, 64 * m, cudaMemcpyHostToDevice, ctx->aux_stream));
+      CK(cudaEventRecord(ctx->ev_chunk[c], ctx->aux_stream));
+      CK(cudaStreamWaitEvent(ctx->stream, ctx->ev_chunk[c], 0));
+      int rc2 = kgv_launch_verify(ctx, dpk + pk_stride * a, dmsg + 32 * a, dsig + 64 * a, m, dst + a, ecdsa, ctx->stream);
+      if (rc2) return rc2;
     }
-    CK(cudaMemcpyAsync(ctx->d_in, pk, pk_stride * n, cudaMemcpyHostToDevice, ctx->stream));
-    CK(cudaMemcpyAsync(ctx->d_in + off_msg, msg, 32 * n, cudaMemcpyHostToDevice, ctx->stream));
-    CK(cudaMemcpyAsync(ctx->d_in + off_sig, sig, 64 * n, cudaMemcpyHostToDevice, ctx->stream));
+    if ((rc = io.copy_out(status, dst, n))) return rc;
+    return io.finish();
   }
-  {
-    int rc = kgv_launch_verify(ctx, dpk, dmsg, dsig, n, dst, ecdsa, ctx->stream);
-    if (rc) return rc;
-  }
-  if (!dev) {
-    CK(cudaMemcpyAsync(status, dst, n, cudaMemcpyDeviceToHost, ctx->stream));
-    CK(cudaStreamSynchronize(ctx->stream));
-  }
-  return KGV_OK;
+  const uint8_t *dpk, *dmsg, *dsig;
+  uint8_t* dst;
+  io.in(pk, pk_stride * n, &dpk);
+  io.in(msg, 32 * n, &dmsg);
+  io.in(sig, 64 * n, &dsig);
+  io.out(status, n, &dst);
+  if (int rc = io.stage()) return rc;
+  if (int rc = kgv_launch_verify(ctx, dpk, dmsg, dsig, n, dst, ecdsa, ctx->stream)) return rc;
+  return io.finish();
 }
 
 extern "C" int kgv_schnorr_verify(kgv_ctx* ctx, const uint8_t* pk32, const uint8_t* msg32, const uint8_t* sig64, size_t n, uint8_t* status) {
@@ -706,27 +747,18 @@ extern "C" int kgv_status_to_bitmap(kgv_ctx* ctx, const uint8_t* status, size_t 
   if (n == 0) return KGV_OK;
   if (!status || !bitmap) return fail_arg(ctx, "null buffer");
   CK(cudaSetDevice(ctx->device));
-  int dev = kgv_ptr_is_device(status);
-  if (kgv_ptr_is_device(bitmap) != dev) return fail_arg(ctx, "all buffers of one call must be host pointers or all device pointers");
+  kgv_io io(ctx);
+  if (int rc = io.one_side("kgv_status_to_bitmap", {status, bitmap})) return rc;
   size_t nbytes = (n + 7) / 8;
-  const uint8_t* dsrc = status;
-  uint8_t* ddst = bitmap;
-  if (!dev) {
-    int rc = kgv_reserve(ctx, &ctx->d_in, &ctx->d_in_cap, n);
-    if (rc) return rc;
-    rc = kgv_reserve(ctx, &ctx->d_out, &ctx->d_out_cap, nbytes);
-    if (rc) return rc;
-    CK(cudaMemcpyAsync(ctx->d_in, status, n, cudaMemcpyHostToDevice, ctx->stream));
-    dsrc = ctx->d_in; ddst = ctx->d_out;
-  }
+  const uint8_t* dsrc;
+  uint8_t* ddst;
+  io.in(status, n, &dsrc);
+  io.out(bitmap, nbytes, &ddst);
+  if (int rc = io.stage()) return rc;
   k_status_to_bitmap<<<(unsigned)((nbytes + 255) / 256), 256, 0, ctx->stream>>>(dsrc, n, ddst);
   CK(cudaGetLastError());
   ctx->launches++;
-  if (!dev) {
-    CK(cudaMemcpyAsync(bitmap, ddst, nbytes, cudaMemcpyDeviceToHost, ctx->stream));
-    CK(cudaStreamSynchronize(ctx->stream));
-  }
-  return KGV_OK;
+  return io.finish();
 }
 
 extern "C" int kgv_debug_schnorr_trace(kgv_ctx* ctx, const uint8_t* pk32, const uint8_t* msg32, const uint8_t* sig64, uint32_t* trace_words,

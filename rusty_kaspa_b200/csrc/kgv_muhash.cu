@@ -13,19 +13,6 @@
 
 using namespace kgv;
 
-#define CK(call)                                                                                  \
-  do {                                                                                            \
-    cudaError_t e_ = (call);                                                                      \
-    if (e_ != cudaSuccess) {                                                                      \
-      char b_[256];                                                                               \
-      snprintf(b_, sizeof b_, "%s failed: %s (%s:%d)", #call, cudaGetErrorString(e_), __FILE__, __LINE__); \
-      ctx->err = b_;                                                                              \
-      return KGV_ERR_CUDA;                                                                        \
-    }                                                                                             \
-  } while (0)
-
-static inline size_t al256(size_t x) { return (x + 255) & ~(size_t)255; }
-static inline unsigned nblk(size_t n, unsigned b) { return (unsigned)((n + b - 1) / b); }
 
 // one level of a product tree: out[t] = in[2t] * in[2t+1] (the odd element out is copied)
 __global__ void __launch_bounds__(128) k_u3072_tree_level(const uint32_t* __restrict__ in, size_t n_in, uint32_t* __restrict__ out, uint32_t* __restrict__ wide) {
@@ -134,7 +121,7 @@ static int reduce_one(kgv_ctx* ctx, uint8_t* base, size_t n, cudaStream_t st) {
   return KGV_OK;
 }
 
-int kgv_mu_reduce(kgv_ctx* ctx, size_t n_den, size_t n_num, uint8_t* out_num384, uint8_t* out_den384) {
+int kgv_mu_reduce(kgv_ctx* ctx, kgv_io& io, size_t n_den, size_t n_num, uint8_t* out_num384, uint8_t* out_den384) {
   cudaStream_t st = ctx->stream, sx = ctx->aux_stream;
   uint8_t* b_den = ctx->d_mu;
   uint8_t* b_num = ctx->d_mu + tree_bytes(n_den);
@@ -146,11 +133,9 @@ int kgv_mu_reduce(kgv_ctx* ctx, size_t n_den, size_t n_num, uint8_t* out_num384,
   if (rc) return rc;
   CK(cudaEventRecord(ctx->ev_join, sx));
   CK(cudaStreamWaitEvent(st, ctx->ev_join, 0));
-  const bool dev = kgv_ptr_is_device(out_num384);
-  CK(cudaMemcpyAsync(out_den384, tree_out(b_den, n_den), 384, dev ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, st));
-  CK(cudaMemcpyAsync(out_num384, tree_out(b_num, n_num), 384, dev ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, st));
-  if (!dev) CK(cudaStreamSynchronize(st));
-  return KGV_OK;
+  if ((rc = io.copy_out(out_den384, tree_out(b_den, n_den), 384))) return rc;
+  if ((rc = io.copy_out(out_num384, tree_out(b_num, n_num), 384))) return rc;
+  return io.finish();
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -161,30 +146,26 @@ extern "C" int kgv_muhash_elements(kgv_ctx* ctx, const uint8_t* data, const uint
   if (!ctx) return KGV_ERR_ARG;
   std::lock_guard<std::recursive_mutex> g(ctx->mu);
   if (!numerator384 || !denominator384 || (n && (!offsets || !data))) { ctx->err = "null argument"; return KGV_ERR_ARG; }
-  if (kgv_ptr_is_device(numerator384) != kgv_ptr_is_device(denominator384)) { ctx->err = "outputs must both be host or both be device pointers"; return KGV_ERR_ARG; }
+  kgv_io io(ctx);
+  int rc = io.one_side("kgv_muhash_elements", {numerator384, denominator384});
+  if (rc) return rc;
   CK(cudaSetDevice(ctx->device));
   uint32_t *e_den = nullptr, *e_num = nullptr;
-  int rc = kgv_mu_reserve(ctx, n, n, &e_den, &e_num);
-  if (rc) return rc;
+  if ((rc = kgv_mu_reserve(ctx, n, n, &e_den, &e_num))) return rc;
   if (n) {
-    const uint8_t* ddata = data;
+    const uint8_t *ddata = data, *drem = remove;
     const uint64_t* doff = offsets;
-    const uint8_t* drem = remove;
-    if (!kgv_ptr_is_device(offsets)) {
-      uint64_t total = offsets[n];
-      size_t o_off = al256(total + 8), o_rem = al256(o_off + (n + 1) * 8);
-      rc = kgv_reserve(ctx, &ctx->d_in, &ctx->d_in_cap, al256(o_rem + n));
-      if (rc) return rc;
-      CK(cudaMemcpyAsync(ctx->d_in, data, total, cudaMemcpyHostToDevice, ctx->stream));
-      CK(cudaMemcpyAsync(ctx->d_in + o_off, offsets, (n + 1) * 8, cudaMemcpyHostToDevice, ctx->stream));
-      if (remove) CK(cudaMemcpyAsync(ctx->d_in + o_rem, remove, n, cudaMemcpyHostToDevice, ctx->stream));
-      ddata = ctx->d_in; doff = (const uint64_t*)(ctx->d_in + o_off); drem = remove ? ctx->d_in + o_rem : nullptr;
+    if (!io.is_device(offsets)) {  // the data's size is the end of the offsets, readable only in host memory
+      io.in(data, offsets[n], &ddata);
+      io.in(offsets, (n + 1) * 8, &doff);
+      io.in(remove, n, &drem);
+      if ((rc = io.stage())) return rc;
     }
     k_muhash_raw_elements<<<nblk(n, 128), 128, 0, ctx->stream>>>(ddata, doff, drem, n, e_den, e_num);
     CK(cudaGetLastError());
     ctx->launches++;
   }
-  return kgv_mu_reduce(ctx, n, n, numerator384, denominator384);
+  return kgv_mu_reduce(ctx, io, n, n, numerator384, denominator384);
 }
 
 // Test / audit hook: one product-tree level on caller values, by the same two level kernels reduce_one launches
@@ -234,8 +215,8 @@ extern "C" int kgv_muhash_combine(kgv_ctx* ctx, uint8_t* num_a, uint8_t* den_a, 
   int rc = kgv_reserve(ctx, &ctx->d_mu, &ctx->d_mu_cap, 4096);
   if (rc) return rc;
   uint8_t* w = ctx->d_mu;
-  const cudaMemcpyKind in = kgv_ptr_is_device(num_a) ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
-  const cudaMemcpyKind out = kgv_ptr_is_device(num_a) ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost;
+  kgv_io io(ctx);
+  const cudaMemcpyKind in = io.is_device(num_a) ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
   CK(cudaMemcpyAsync(w, num_a, 384, in, ctx->stream));
   CK(cudaMemcpyAsync(w + 384, den_a, 384, in, ctx->stream));
   CK(cudaMemcpyAsync(w + 768, num_b, 384, in, ctx->stream));
@@ -243,10 +224,8 @@ extern "C" int kgv_muhash_combine(kgv_ctx* ctx, uint8_t* num_a, uint8_t* den_a, 
   k_muhash_combine<<<1, 32, 0, ctx->stream>>>((uint32_t*)w);
   CK(cudaGetLastError());
   ctx->launches++;
-  CK(cudaMemcpyAsync(num_a, w, 384, out, ctx->stream));
-  CK(cudaMemcpyAsync(den_a, w + 384, 384, out, ctx->stream));
-  if (out == cudaMemcpyDeviceToHost) CK(cudaStreamSynchronize(ctx->stream));
-  return KGV_OK;
+  if ((rc = io.copy_out(num_a, w, 384)) || (rc = io.copy_out(den_a, w + 384, 384))) return rc;
+  return io.finish();
 }
 
 // finalize (lib.rs:98-115): serialized = numerator / denominator mod p (canonical), hash = BLAKE2b-256 keyed "MuHashFinalize".
@@ -302,17 +281,16 @@ extern "C" int kgv_muhash_finalize(kgv_ctx* ctx, const uint8_t* numerator384, co
   if (rc) return rc;
   uint8_t* w = ctx->d_mu;
   uint8_t* o = w + 4096;
-  const bool dev = kgv_ptr_is_device(numerator384);
+  kgv_io io(ctx);
+  const bool dev = io.is_device(numerator384);
   CK(cudaMemcpyAsync(w, numerator384, 384, dev ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, ctx->stream));
   CK(cudaMemcpyAsync(w + 384, denominator384, 384, dev ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, ctx->stream));
   k_muhash_finalize<<<1, 32, 0, ctx->stream>>>((uint32_t*)w, (uint32_t*)o);
   CK(cudaGetLastError());
   ctx->launches++;
-  const bool odev = kgv_ptr_is_device(hash32);
-  if (serialized384) CK(cudaMemcpyAsync(serialized384, o, 384, odev ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, ctx->stream));
-  CK(cudaMemcpyAsync(hash32, o + 384, 32, odev ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, ctx->stream));
-  if (!odev) CK(cudaStreamSynchronize(ctx->stream));
-  return KGV_OK;
+  if (serialized384 && (rc = io.copy_out(serialized384, o, 384))) return rc;
+  if ((rc = io.copy_out(hash32, o + 384, 32))) return rc;
+  return io.finish();
 }
 
 
@@ -525,37 +503,26 @@ extern "C" int kgv_muhash_finalize_batch(kgv_ctx* ctx, const uint8_t* numerators
   // k_muhash_divide_all reads numerator k with 16-byte loads at numerators384 + k * pitch_bytes; the hash / serialize kernel stores words
   if (!numerators384 || !denominators384 || !hashes32 || pitch_bytes < 384 || (pitch_bytes & 15)) { ctx->err = "bad argument (pitch_bytes must be >= 384 and a multiple of 16)"; return KGV_ERR_ARG; }
   CK(cudaSetDevice(ctx->device));
-  const bool dev = kgv_ptr_is_device(numerators384);
-  if (kgv_ptr_is_device(denominators384) != dev || kgv_ptr_is_device(hashes32) != dev) { ctx->err = "all buffers of one call must be host pointers or all device pointers"; return KGV_ERR_ARG; }
+  kgv_io io(ctx);
+  bool dev;
+  if (int rc = io.one_side("kgv_muhash_finalize_batch", {numerators384, denominators384, hashes32}, &dev)) return rc;
   if (dev && (((uintptr_t)numerators384 & 15) || ((uintptr_t)hashes32 & 3) || ((uintptr_t)serialized384 & 3))) {
     ctx->err = "device numerators384 must be 16-byte aligned, hashes32 and serialized384 4-byte aligned";
     return KGV_ERR_ARG;
   }
-  // layout: [num in (host path only)] [den in (host path only)] [finalize scratch] [hashes n*32 (host path)] [serialized (host path)]
+  // a strided host array is one contiguous span (the pitch interleaves numerators and denominators of MuHash records)
   const size_t span = (n - 1) * pitch_bytes + 384;
-  size_t o_num = 0, o_den = al256(dev ? 0 : span), o_fin = al256(o_den + (dev ? 0 : span)), o_h = o_fin + kgv_mu_finalize_scratch(n), o_ser = al256(o_h + n * 32);
-  int rc = kgv_reserve(ctx, &ctx->d_mu, &ctx->d_mu_cap, al256(o_ser + (serialized384 ? n * 384 : 0)));
+  int rc = kgv_reserve(ctx, &ctx->d_mu, &ctx->d_mu_cap, kgv_mu_finalize_scratch(n));
   if (rc) return rc;
-  uint8_t* M = ctx->d_mu;
-  cudaStream_t st = ctx->stream;
-  const uint32_t* dnum = (const uint32_t*)numerators384;
-  const uint32_t* dden = (const uint32_t*)denominators384;
-  if (!dev) {
-    // a strided host array is one contiguous span (the pitch interleaves numerators and denominators of MuHash records)
-    CK(cudaMemcpyAsync(M + o_num, numerators384, span, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(M + o_den, denominators384, span, cudaMemcpyHostToDevice, st));
-    dnum = (const uint32_t*)(M + o_num); dden = (const uint32_t*)(M + o_den);
-  }
-  uint32_t* dh = dev ? (uint32_t*)hashes32 : (uint32_t*)(M + o_h);
-  uint32_t* dser = !serialized384 ? nullptr : (dev ? (uint32_t*)serialized384 : (uint32_t*)(M + o_ser));
-  rc = kgv_mu_finalize_run(ctx, dnum, dden, n, pitch_bytes / 4, M + o_fin, dser, dh, st);
-  if (rc) return rc;
-  if (!dev) {
-    CK(cudaMemcpyAsync(hashes32, dh, n * 32, cudaMemcpyDeviceToHost, st));
-    if (serialized384) CK(cudaMemcpyAsync(serialized384, dser, n * 384, cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
-  }
-  return KGV_OK;
+  const uint32_t *dnum, *dden;
+  uint32_t *dh, *dser;
+  io.in((const uint32_t*)numerators384, span, &dnum);
+  io.in((const uint32_t*)denominators384, span, &dden);
+  io.out((uint32_t*)hashes32, n * 32, &dh);
+  io.out((uint32_t*)serialized384, n * 384, &dser);
+  if ((rc = io.stage())) return rc;
+  if ((rc = kgv_mu_finalize_run(ctx, dnum, dden, n, pitch_bytes / 4, ctx->d_mu, dser, dh, ctx->stream))) return rc;
+  return io.finish();
 }
 
 size_t kgv_mu_prefix_scratch(size_t n) { return al256((n + KGV_SCAN_CHUNK - 1) / KGV_SCAN_CHUNK * 384); }
@@ -582,23 +549,20 @@ extern "C" int kgv_muhash_prefix_combine(kgv_ctx* ctx, const uint8_t* init768, u
   if (n == 0) return KGV_OK;
   if (!values768) { ctx->err = "null argument"; return KGV_ERR_ARG; }
   CK(cudaSetDevice(ctx->device));
-  const bool dev = kgv_ptr_is_device(values768);
-  if (dev && ((uintptr_t)values768 & 15)) { ctx->err = "device values768 must be 16-byte aligned"; return KGV_ERR_ARG; }  // scanned in place with 16-byte loads
-  size_t o_v = 0, o_tot = al256(dev ? 0 : n * 768), o_init = o_tot + kgv_mu_prefix_scratch(n);
+  kgv_io io(ctx);
+  if (io.is_device(values768) && ((uintptr_t)values768 & 15)) { ctx->err = "device values768 must be 16-byte aligned"; return KGV_ERR_ARG; }  // scanned in place with 16-byte loads
+  const size_t o_init = kgv_mu_prefix_scratch(n);
   int rc = kgv_reserve(ctx, &ctx->d_mu, &ctx->d_mu_cap, al256(o_init + 768));
   if (rc) return rc;
   uint8_t* M = ctx->d_mu;
   cudaStream_t st = ctx->stream;
-  uint32_t* v = (uint32_t*)values768;
-  if (!dev) { CK(cudaMemcpyAsync(M + o_v, values768, n * 768, cudaMemcpyHostToDevice, st)); v = (uint32_t*)(M + o_v); }
-  if (init768) CK(cudaMemcpyAsync(M + o_init, init768, 768, kgv_ptr_is_device(init768) ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, st));
-  rc = kgv_mu_prefix_combine_run(ctx, init768 ? (const uint32_t*)(M + o_init) : nullptr, v, n, (uint32_t*)(M + o_tot), st);
+  uint32_t* v;
+  io.inout((uint32_t*)values768, n * 768, &v);
+  if ((rc = io.stage())) return rc;
+  if (init768) CK(cudaMemcpyAsync(M + o_init, init768, 768, io.is_device(init768) ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, st));
+  rc = kgv_mu_prefix_combine_run(ctx, init768 ? (const uint32_t*)(M + o_init) : nullptr, v, n, (uint32_t*)M, st);
   if (rc) return rc;
-  if (!dev) {
-    CK(cudaMemcpyAsync(values768, v, n * 768, cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
-  }
-  return KGV_OK;
+  return io.finish();
 }
 
 // products of ranges of level-0 elements (kgv_replay_muhash): E has `stride` elements; flags[flag_index[j]] != 0 selects element j

@@ -668,9 +668,7 @@ extern "C" int kgv_replay_window(kgv_ctx* ctx, kgv_utxo_table* table, const kgv_
   CK(cudaMemcpyAsync(dblk, blocks, n_blocks * sizeof(kgv_replay_block), cudaMemcpyHostToDevice, st));
   CK(cudaMemsetAsync(wm, 0, wm_cap * 4, st));
   CK(cudaMemsetAsync(cnt, 0, 64, st));
-  BatchView v0{d.txs, d.inputs, d.outputs, nullptr, d.bytes};
-  k_tx_ids_dev<<<nblk(nt, 128), 128, 0, st>>>(v0, (uint32_t)nt, ids);
-  CK(cudaGetLastError());
+  if ((rc = kgv_tx_digests_run(ctx, d, nt, ids, false))) return rc;
   CK(cudaMemsetAsync(R + o_sib, 0, nt, st));
   k_wm_insert<<<nblk(nt, 128), 128, 0, st>>>(ids, (uint32_t)nt, wm, wm_cap - 1, R + o_sib);
   CK(cudaGetLastError());
@@ -682,7 +680,7 @@ extern "C" int kgv_replay_window(kgv_ctx* ctx, kgv_utxo_table* table, const kgv_
   CK(cudaGetLastError());
   k_replay_ranges<<<nblk(n_blocks, 128), 128, 0, st>>>(dblk, (uint32_t)n_blocks, d.txs, (ReplayRange*)(R + o_rng));
   CK(cudaGetLastError());
-  ctx->launches += 6;
+  ctx->launches += 5;
   // ---- pre-check of every script of the window
   BatchView v{d.txs, d.inputs, d.outputs, dent, d.bytes};
   ReplaySrc* src = (ReplaySrc*)(R + o_src);
@@ -794,14 +792,12 @@ extern "C" int kgv_replay_window(kgv_ctx* ctx, kgv_utxo_table* table, const kgv_
     fprintf(stderr, "\n");
     for (auto& m : marks) cudaEventDestroy(m.second);
   }
-  const bool dev_out = kgv_ptr_is_device(results);
-  CK(cudaMemcpyAsync(results, res, nt * sizeof(kgv_tx_result), dev_out ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, st));
-  if (accept) CK(cudaMemcpyAsync(accept, dacc, nt, kgv_ptr_is_device(accept) ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, st));
+  kgv_io io(ctx);
   unsigned long long n_acc = 0;
-  if (stats || !dev_out) {
-    CK(cudaMemcpyAsync(&n_acc, cnt, 8, cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
-  }
+  if ((rc = io.copy_out(results, res, nt * sizeof(kgv_tx_result)))) return rc;
+  if (accept && (rc = io.copy_out(accept, dacc, nt))) return rc;
+  if (stats && (rc = io.copy_out(&n_acc, cnt, 8))) return rc;
+  if ((rc = io.finish())) return rc;
   ctx->last_replay.valid = true;
   ctx->last_replay.txs = d.txs; ctx->last_replay.inputs = d.inputs; ctx->last_replay.outputs = d.outputs; ctx->last_replay.bytes = d.bytes;
   ctx->last_replay.nt = nt; ctx->last_replay.ni = ni; ctx->last_replay.no = no; ctx->last_replay.n_blocks = n_blocks;
@@ -931,10 +927,9 @@ extern "C" int kgv_replay_muhash(kgv_ctx* ctx, const uint32_t* group_first_block
   CK(cudaMemcpyAsync(Wk + o_gf, group_first_block, (n_groups + 1) * 4, cudaMemcpyHostToDevice, st));
   rc = kgv_replay_muhash_run(ctx, (const uint32_t*)(Wk + o_gf), n_groups, Wk + o_mu, vals, st);
   if (rc) return rc;
-  const bool dev = kgv_ptr_is_device(values768);
-  CK(cudaMemcpyAsync(values768, vals, n_groups * 768, dev ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, st));
-  if (!dev) CK(cudaStreamSynchronize(st));
-  return KGV_OK;
+  kgv_io io(ctx);
+  if ((rc = io.copy_out(values768, vals, n_groups * 768))) return rc;
+  return io.finish();
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -1118,12 +1113,11 @@ extern "C" int kgv_replay_diffs(kgv_ctx* ctx, const uint32_t* group_first_block,
   if (group_first_block[0] != 0 || group_first_block[n_groups] != L.n_blocks) { ctx->err = "groups must tile the blocks of the window"; return KGV_ERR_ARG; }
   for (size_t i = 0; i < n_groups; i++) if (group_first_block[i] > group_first_block[i + 1]) { ctx->err = "group offsets not monotone"; return KGV_ERR_ARG; }
   const bool counting = !rem_keys36;
-  bool dev = ranges ? kgv_ptr_is_device(ranges) != 0 : false;
+  kgv_io io(ctx);
   if (!counting) {
     if (!rem_entries || !add_keys36 || !add_entries || (bytes_cap && !bytes)) { ctx->err = "null buffer"; return KGV_ERR_ARG; }
-    dev = kgv_ptr_is_device(rem_keys36) != 0;
-    for (const void* p : {(const void*)rem_entries, (const void*)add_keys36, (const void*)add_entries, (const void*)bytes, (const void*)ranges})
-      if (p && (kgv_ptr_is_device(p) != 0) != dev) { ctx->err = "all output arrays of one call must be host pointers or all device pointers"; return KGV_ERR_ARG; }
+    bool dev;
+    if (int rc = io.one_side("kgv_replay_diffs", {rem_keys36, rem_entries, add_keys36, add_entries, bytes, ranges}, &dev)) return rc;
     if (dev && (((uintptr_t)rem_entries | (uintptr_t)add_entries) & 7)) { ctx->err = "entry arrays must be 8-byte aligned"; return KGV_ERR_ARG; }
   }
   CK(cudaSetDevice(ctx->device));
@@ -1138,6 +1132,17 @@ extern "C" int kgv_replay_diffs(kgv_ctx* ctx, const uint32_t* group_first_block,
   int rc = kgv_reserve(ctx, &ctx->d_work, &ctx->d_work_cap, o_tot + 64);
   if (rc) return rc;
   uint8_t* Wk = ctx->d_work;
+  // the diffs come back up to their sizes, known after the scan
+  uint8_t *rk = nullptr, *ak = nullptr, *db = nullptr;
+  kgv_utxo_entry *re = nullptr, *ae = nullptr;
+  if (!counting) {
+    io.out(rem_keys36, max_rem * 36, &rk);
+    io.out(rem_entries, max_rem * sizeof(kgv_utxo_entry), &re);
+    io.out(add_keys36, max_add * 36, &ak);
+    io.out(add_entries, max_add * sizeof(kgv_utxo_entry), &ae);
+    io.out(bytes, bytes_cap, &db);
+    if ((rc = io.stage())) return rc;
+  }
   DiffArgs a;
   a.txs = (const kgv_tx*)L.txs; a.inputs = (const kgv_input*)L.inputs; a.outputs = (const kgv_output*)L.outputs; a.bytes = (const uint8_t*)L.bytes;
   a.dent = (const DevEntry*)(R + L.o_ent); a.ids = (const uint64_t*)(R + L.o_ids);
@@ -1166,7 +1171,7 @@ extern "C" int kgv_replay_diffs(kgv_ctx* ctx, const uint32_t* group_first_block,
   ctx->launches += 6 + (ni ? 1 : 0) + (ni + no ? 1 : 0);
   unsigned long long tot[4];
   CK(cudaMemcpyAsync(tot, dtot, sizeof tot, cudaMemcpyDeviceToHost, st));
-  if (ranges) CK(cudaMemcpyAsync(ranges, drg, n_groups * sizeof(kgv_diff_range), dev ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, st));
+  if (ranges && (rc = io.copy_out(ranges, drg, n_groups * sizeof(kgv_diff_range)))) return rc;
   CK(cudaStreamSynchronize(st));
   const size_t n_rem = (size_t)tot[0], n_add = (size_t)tot[2], n_bytes = (size_t)(tot[1] + tot[3]);
   if (n_rem_out) *n_rem_out = n_rem;
@@ -1176,28 +1181,13 @@ extern "C" int kgv_replay_diffs(kgv_ctx* ctx, const uint32_t* group_first_block,
   if (counting) return KGV_OK;
   if (n_rem > max_rem || n_add > max_add || n_bytes > bytes_cap) { ctx->err = "kgv_replay_diffs: the caller's arrays are too small (sizes returned)"; return KGV_ERR_NOMEM; }
   if (ni + no == 0) return KGV_OK;
-  uint8_t *rk = rem_keys36, *ak = add_keys36, *db = bytes;
-  kgv_utxo_entry *re = rem_entries, *ae = add_entries;
-  size_t s_re = al256(n_rem * 36), s_ak = al256(s_re + n_rem * sizeof(kgv_utxo_entry)), s_ae = al256(s_ak + n_add * 36), s_b = al256(s_ae + n_add * sizeof(kgv_utxo_entry));
-  if (!dev) {
-    rc = kgv_reserve(ctx, &ctx->d_out, &ctx->d_out_cap, s_b + n_bytes + 16);
-    if (rc) return rc;
-    rk = ctx->d_out; re = (kgv_utxo_entry*)(ctx->d_out + s_re); ak = ctx->d_out + s_ak; ae = (kgv_utxo_entry*)(ctx->d_out + s_ae); db = ctx->d_out + s_b;
-  }
   k_diff_gather<<<nblk(ni + no, 128), 128, 0, st>>>(a, rk, re, ak, ae, db);
   CK(cudaGetLastError());
   ctx->launches++;
-  if (!dev) {
-    if (n_rem) {
-      CK(cudaMemcpyAsync(rem_keys36, rk, n_rem * 36, cudaMemcpyDeviceToHost, st));
-      CK(cudaMemcpyAsync(rem_entries, re, n_rem * sizeof(kgv_utxo_entry), cudaMemcpyDeviceToHost, st));
-    }
-    if (n_add) {
-      CK(cudaMemcpyAsync(add_keys36, ak, n_add * 36, cudaMemcpyDeviceToHost, st));
-      CK(cudaMemcpyAsync(add_entries, ae, n_add * sizeof(kgv_utxo_entry), cudaMemcpyDeviceToHost, st));
-    }
-    if (n_bytes) CK(cudaMemcpyAsync(bytes, db, n_bytes, cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
-  }
-  return KGV_OK;
+  io.trim(rem_keys36, n_rem * 36);
+  io.trim(rem_entries, n_rem * sizeof(kgv_utxo_entry));
+  io.trim(add_keys36, n_add * 36);
+  io.trim(add_entries, n_add * sizeof(kgv_utxo_entry));
+  io.trim(bytes, n_bytes);
+  return io.finish();
 }

@@ -21,19 +21,6 @@
 
 using namespace kgv;
 
-#define CK(call)                                                                                  \
-  do {                                                                                            \
-    cudaError_t e_ = (call);                                                                      \
-    if (e_ != cudaSuccess) {                                                                      \
-      char b_[256];                                                                               \
-      snprintf(b_, sizeof b_, "%s failed: %s (%s:%d)", #call, cudaGetErrorString(e_), __FILE__, __LINE__); \
-      ctx->err = b_;                                                                              \
-      return KGV_ERR_CUDA;                                                                        \
-    }                                                                                             \
-  } while (0)
-
-static inline size_t al256(size_t x) { return (x + 255) & ~(size_t)255; }
-static inline unsigned nblk(size_t n, unsigned b) { return (unsigned)((n + b - 1) / b); }
 
 static const size_t kSlotBytes = 64ull << 20;  // ScriptSlots of one call, whatever the batch size
 
@@ -321,26 +308,24 @@ extern "C" int kgv_check_scripts(kgv_ctx* ctx, const kgv_tx_batch* batch, const 
   if (!batch || !batch->entries || (n && (!tx_indices || !results))) { ctx->err = "null argument"; return KGV_ERR_ARG; }
   if (n == 0) return KGV_OK;
   CK(cudaSetDevice(ctx->device));
-  const bool idx_dev = kgv_ptr_is_device(tx_indices) != 0, res_dev = kgv_ptr_is_device(results) != 0;
-  if (!idx_dev)
+  kgv_io io(ctx);
+  if (!io.is_device(tx_indices))
     for (size_t i = 0; i < n; i++)
       if (tx_indices[i] >= batch->n_txs) { ctx->err = "kgv_check_scripts: a transaction index is out of range"; return KGV_ERR_ARG; }
   kgv_dev_batch d;
   int rc = kgv_batch_to_device(ctx, batch, &d, true);
   if (rc) return rc;
   const size_t ni = d.n_inputs;
-  size_t o_ent = 0, o_list = al256(ni * sizeof(DevEntry)), o_res = al256(o_list + n * 4);
+  size_t o_ent = 0, o_res = al256(ni * sizeof(DevEntry));
   rc = kgv_reserve(ctx, &ctx->d_work, &ctx->d_work_cap, al256(o_res + n * sizeof(kgv_tx_result)));
   if (rc) return rc;
   uint8_t* W = ctx->d_work;
   DevEntry* dent = (DevEntry*)(W + o_ent);
   kgv_tx_result* dres = (kgv_tx_result*)(W + o_res);
   cudaStream_t st = ctx->stream;
-  const uint32_t* dlist = tx_indices;
-  if (!idx_dev) {
-    CK(cudaMemcpyAsync(W + o_list, tx_indices, n * 4, cudaMemcpyHostToDevice, st));
-    dlist = (const uint32_t*)(W + o_list);
-  }
+  const uint32_t* dlist;
+  io.in(tx_indices, n * 4, &dlist);
+  if ((rc = io.stage())) return rc;
   if (ni) {
     k_se_entries<<<nblk(ni, 128), 128, 0, st>>>(d.entries, d.bytes, ni, dent);
     CK(cudaGetLastError());
@@ -349,7 +334,6 @@ extern "C" int kgv_check_scripts(kgv_ctx* ctx, const kgv_tx_batch* batch, const 
   BatchView v{d.txs, d.inputs, d.outputs, dent, d.bytes};
   rc = kgv_script_engine_run(ctx, v, d.n_txs, dlist, n, dres, false, nullptr);
   if (rc) return rc;
-  CK(cudaMemcpyAsync(results, dres, n * sizeof(kgv_tx_result), res_dev ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, st));
-  if (!res_dev) CK(cudaStreamSynchronize(st));
-  return KGV_OK;
+  if ((rc = io.copy_out(results, dres, n * sizeof(kgv_tx_result)))) return rc;
+  return io.finish();
 }

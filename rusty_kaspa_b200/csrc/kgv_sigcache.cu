@@ -22,17 +22,6 @@
 
 using namespace kgv;
 
-#define CK(call)                                                                                  \
-  do {                                                                                            \
-    cudaError_t e_ = (call);                                                                      \
-    if (e_ != cudaSuccess) {                                                                      \
-      char b_[256];                                                                               \
-      snprintf(b_, sizeof b_, "%s failed: %s (%s:%d)", #call, cudaGetErrorString(e_), __FILE__, __LINE__); \
-      ctx->err = b_;                                                                              \
-      return KGV_ERR_CUDA;                                                                        \
-    }                                                                                             \
-  } while (0)
-
 #define SC_PROBE 8
 #define SC_EMPTY 0u
 #define SC_BUSY 0xFFu  // verdicts are stored as 1 (invalid) / 2 (valid)

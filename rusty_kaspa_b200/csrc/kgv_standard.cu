@@ -20,18 +20,6 @@ using namespace kgv;
 
 static_assert(sizeof(kgv_mempool_policy) == 16, "kgv_mempool_policy is 16 bytes");
 
-#define CK(call)                                                                                  \
-  do {                                                                                            \
-    cudaError_t e_ = (call);                                                                      \
-    if (e_ != cudaSuccess) {                                                                      \
-      char b_[256];                                                                               \
-      snprintf(b_, sizeof b_, "%s failed: %s (%s:%d)", #call, cudaGetErrorString(e_), __FILE__, __LINE__); \
-      ctx->err = b_;                                                                              \
-      return KGV_ERR_CUDA;                                                                        \
-    }                                                                                             \
-  } while (0)
-
-static inline size_t al256(size_t x) { return (x + 255) & ~(size_t)255; }
 
 constexpr int STD_WARPS = 4;  // transactions per block of the two transaction kernels
 
@@ -210,13 +198,6 @@ int kgv_standard_context_run(kgv_ctx* ctx, const kgv_dev_batch& d, const DevEntr
   return KGV_OK;
 }
 
-// every non-null pointer host when dev is false, device when it is true
-static bool same_side(bool dev, std::initializer_list<const void*> ps) {
-  for (const void* p : ps)
-    if (p && (kgv_ptr_is_device(p) != 0) != dev) return false;
-  return true;
-}
-
 extern "C" int kgv_check_txs_standard_in_isolation(kgv_ctx* ctx, const kgv_tx_batch* batch, const kgv_mempool_policy* policy, const kgv_tx_masses* masses,
                                                     kgv_tx_result* results, uint64_t* detail) {
   if (!ctx) return KGV_ERR_ARG;
@@ -225,34 +206,21 @@ extern "C" int kgv_check_txs_standard_in_isolation(kgv_ctx* ctx, const kgv_tx_ba
   if (batch->n_txs == 0) return KGV_OK;
   if (batch->n_txs > 0xFFFFFFFFull) { ctx->err = "kgv_check_txs_standard_in_isolation: more than 2^32 - 1 transactions"; return KGV_ERR_ARG; }
   CK(cudaSetDevice(ctx->device));
-  const bool dev = kgv_ptr_is_device(results) != 0;
-  if (!same_side(dev, {batch->txs, masses, detail})) {
-    ctx->err = "kgv_check_txs_standard_in_isolation: the batch, masses and outputs must all be host or all be device pointers";
-    return KGV_ERR_ARG;
-  }
+  kgv_io io(ctx);
+  if (int rc = io.one_side("kgv_check_txs_standard_in_isolation", {results, batch->txs, masses, detail})) return rc;
   kgv_dev_batch d;
   int rc = kgv_batch_to_device(ctx, batch, &d, false);
   if (rc) return rc;
   const size_t nt = d.n_txs;
-  const size_t o_res = 0, o_mass = al256(nt * sizeof(kgv_tx_result)), o_det = al256(o_mass + nt * sizeof(kgv_tx_masses));
-  rc = kgv_reserve(ctx, &ctx->d_work, &ctx->d_work_cap, al256(o_det + nt * 8));
-  if (rc) return rc;
-  uint8_t* S = ctx->d_work;
-  cudaStream_t st = ctx->stream;
-  const kgv_tx_masses* dm = masses;
-  if (!dev) {
-    CK(cudaMemcpyAsync(S + o_mass, masses, nt * sizeof(kgv_tx_masses), cudaMemcpyHostToDevice, st));
-    dm = (const kgv_tx_masses*)(S + o_mass);
-  }
-  kgv_tx_result* dres = dev ? results : (kgv_tx_result*)(S + o_res);
-  uint64_t* ddet = dev || !detail ? detail : (uint64_t*)(S + o_det);
-  if ((rc = kgv_standard_isolation_run(ctx, d, *policy, dm, false, dres, ddet, st))) return rc;
-  if (!dev) {
-    CK(cudaMemcpyAsync(results, dres, nt * sizeof(kgv_tx_result), cudaMemcpyDeviceToHost, st));
-    if (detail) CK(cudaMemcpyAsync(detail, ddet, nt * 8, cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
-  }
-  return KGV_OK;
+  const kgv_tx_masses* dm;
+  kgv_tx_result* dres;
+  uint64_t* ddet;
+  io.in(masses, nt * sizeof(kgv_tx_masses), &dm);
+  io.out(results, nt * sizeof(kgv_tx_result), &dres);
+  io.out(detail, nt * 8, &ddet);
+  if ((rc = io.stage())) return rc;
+  if ((rc = kgv_standard_isolation_run(ctx, d, *policy, dm, false, dres, ddet, ctx->stream))) return rc;
+  return io.finish();
 }
 
 extern "C" int kgv_check_txs_standard_in_context(kgv_ctx* ctx, const kgv_tx_batch* batch, const kgv_mempool_policy* policy, const kgv_tx_masses* masses,
@@ -264,42 +232,27 @@ extern "C" int kgv_check_txs_standard_in_context(kgv_ctx* ctx, const kgv_tx_batc
   if (batch->n_inputs && !batch->entries) { ctx->err = "kgv_check_txs_standard_in_context: batch->entries is required"; return KGV_ERR_ARG; }
   if (batch->n_txs > 0xFFFFFFFFull) { ctx->err = "kgv_check_txs_standard_in_context: more than 2^32 - 1 transactions"; return KGV_ERR_ARG; }
   CK(cudaSetDevice(ctx->device));
-  const bool dev = kgv_ptr_is_device(results) != 0;
-  if (!same_side(dev, {batch->txs, masses, storage_mass, fee, detail})) {
-    ctx->err = "kgv_check_txs_standard_in_context: the batch, its inputs and outputs must all be host or all be device pointers";
-    return KGV_ERR_ARG;
-  }
+  kgv_io io(ctx);
+  if (int rc = io.one_side("kgv_check_txs_standard_in_context", {results, batch->txs, masses, storage_mass, fee, detail})) return rc;
   kgv_dev_batch d;
   int rc = kgv_batch_to_device(ctx, batch, &d, batch->n_inputs != 0);
   if (rc) return rc;
   const size_t nt = d.n_txs;
-  // d_work: verdicts, masses, storage masses, fees, details, the overflow flag
-  const size_t o_res = 0, o_mass = al256(nt * sizeof(kgv_tx_result)), o_sm = al256(o_mass + nt * sizeof(kgv_tx_masses)), o_fee = al256(o_sm + nt * 8),
-               o_det = al256(o_fee + nt * 8), o_flag = al256(o_det + nt * 8);
-  rc = kgv_reserve(ctx, &ctx->d_work, &ctx->d_work_cap, o_flag + 8);
-  if (rc) return rc;
-  uint8_t* S = ctx->d_work;
-  cudaStream_t st = ctx->stream;
-  const kgv_tx_masses* dm = masses;
-  const uint64_t *dsm = storage_mass, *dfee = fee;
-  if (!dev) {
-    CK(cudaMemcpyAsync(S + o_mass, masses, nt * sizeof(kgv_tx_masses), cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(S + o_sm, storage_mass, nt * 8, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(S + o_fee, fee, nt * 8, cudaMemcpyHostToDevice, st));
-    dm = (const kgv_tx_masses*)(S + o_mass); dsm = (const uint64_t*)(S + o_sm); dfee = (const uint64_t*)(S + o_fee);
-  }
-  kgv_tx_result* dres = dev ? results : (kgv_tx_result*)(S + o_res);
-  uint64_t* ddet = dev || !detail ? detail : (uint64_t*)(S + o_det);
-  unsigned long long* dflag = (unsigned long long*)(S + o_flag);
-  CK(cudaMemsetAsync(dflag, 0, 8, st));
-  if ((rc = kgv_standard_context_run(ctx, d, nullptr, *policy, dm, dsm, dfee, dres, ddet, dflag, st))) return rc;
-  unsigned long long flag = 0;
-  if (!dev) {
-    CK(cudaMemcpyAsync(results, dres, nt * sizeof(kgv_tx_result), cudaMemcpyDeviceToHost, st));
-    if (detail) CK(cudaMemcpyAsync(detail, ddet, nt * 8, cudaMemcpyDeviceToHost, st));
-  }
-  CK(cudaMemcpyAsync(&flag, dflag, 8, cudaMemcpyDeviceToHost, st));
-  CK(cudaStreamSynchronize(st));
+  const kgv_tx_masses* dm;
+  const uint64_t *dsm, *dfee;
+  kgv_tx_result* dres;
+  uint64_t* ddet;
+  unsigned long long flag = 0, *dflag;  // a host scalar: finish() always synchronises to read it
+  io.in(masses, nt * sizeof(kgv_tx_masses), &dm);
+  io.in(storage_mass, nt * 8, &dsm);
+  io.in(fee, nt * 8, &dfee);
+  io.out(results, nt * sizeof(kgv_tx_result), &dres);
+  io.out(detail, nt * 8, &ddet);
+  io.out(&flag, 8, &dflag);
+  if ((rc = io.stage())) return rc;
+  CK(cudaMemsetAsync(dflag, 0, 8, ctx->stream));
+  if ((rc = kgv_standard_context_run(ctx, d, nullptr, *policy, dm, dsm, dfee, dres, ddet, dflag, ctx->stream))) return rc;
+  if ((rc = io.finish())) return rc;
   if (flag) { ctx->err = "kgv_check_txs_standard_in_context: compute mass * minimum_relay_transaction_fee overflows u64"; return KGV_ERR_ARG; }
   return KGV_OK;
 }
@@ -310,25 +263,17 @@ extern "C" int kgv_outputs_dust(kgv_ctx* ctx, const kgv_tx_batch* batch, uint64_
   if (!batch || (batch->n_outputs && !is_dust)) { ctx->err = "null argument"; return KGV_ERR_ARG; }
   if (batch->n_outputs == 0) return KGV_OK;
   CK(cudaSetDevice(ctx->device));
-  const bool dev = kgv_ptr_is_device(is_dust) != 0;
-  if (!same_side(dev, {batch->outputs})) { ctx->err = "kgv_outputs_dust: the batch and is_dust must both be host or both be device pointers"; return KGV_ERR_ARG; }
+  kgv_io io(ctx);
+  if (int rc = io.one_side("kgv_outputs_dust", {is_dust, batch->outputs})) return rc;
   kgv_dev_batch d;
   int rc = kgv_batch_to_device(ctx, batch, &d, false);
   if (rc) return rc;
   const size_t no = d.n_outputs;
-  uint8_t* out = is_dust;
-  if (!dev) {
-    rc = kgv_reserve(ctx, &ctx->d_work, &ctx->d_work_cap, al256(no));
-    if (rc) return rc;
-    out = ctx->d_work;
-  }
-  cudaStream_t st = ctx->stream;
-  k_outputs_dust<<<(unsigned)((no + 255) / 256), 256, 0, st>>>(d.outputs, d.bytes, no, minimum_relay_transaction_fee, out);
+  uint8_t* out;
+  io.out(is_dust, no, &out);
+  if ((rc = io.stage())) return rc;
+  k_outputs_dust<<<(unsigned)((no + 255) / 256), 256, 0, ctx->stream>>>(d.outputs, d.bytes, no, minimum_relay_transaction_fee, out);
   CK(cudaGetLastError());
   ctx->launches++;
-  if (!dev) {
-    CK(cudaMemcpyAsync(is_dust, out, no, cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
-  }
-  return KGV_OK;
+  return io.finish();
 }

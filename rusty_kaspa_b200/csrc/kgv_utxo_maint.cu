@@ -10,18 +10,6 @@
 
 using namespace kgv;
 
-#define CK(call)                                                                                  \
-  do {                                                                                            \
-    cudaError_t e_ = (call);                                                                      \
-    if (e_ != cudaSuccess) {                                                                      \
-      char b_[256];                                                                               \
-      snprintf(b_, sizeof b_, "%s failed: %s (%s:%d)", #call, cudaGetErrorString(e_), __FILE__, __LINE__); \
-      ctx->err = b_;                                                                              \
-      return KGV_ERR_CUDA;                                                                        \
-    }                                                                                             \
-  } while (0)
-
-static inline unsigned nblk(size_t n, unsigned b) { return (unsigned)((n + b - 1) / b); }
 
 // ---------------------------------------------------------------------------------------------
 // kernels

@@ -26,18 +26,6 @@
 
 using namespace kgv;
 
-#define CK(call)                                                                                  \
-  do {                                                                                            \
-    cudaError_t e_ = (call);                                                                      \
-    if (e_ != cudaSuccess) {                                                                      \
-      char b_[256];                                                                               \
-      snprintf(b_, sizeof b_, "%s failed: %s (%s:%d)", #call, cudaGetErrorString(e_), __FILE__, __LINE__); \
-      ctx->err = b_;                                                                              \
-      return KGV_ERR_CUDA;                                                                        \
-    }                                                                                             \
-  } while (0)
-
-static inline size_t al256(size_t x) { return (x + 255) & ~(size_t)255; }
 
 // KGV_DEBUG=1: synchronise and report after every stage of the fused path (locates a faulting kernel)
 #include <cstdlib>
@@ -461,14 +449,6 @@ __global__ void k_apply_insert(TableView t, BatchView b, size_t n_outputs, const
   k[8] = (uint32_t)(o - tx.first_output);
   table_put(t, k, out.value, pov, out.spk_version, tx_is_coinbase(tx) ? 1u : 0u, b.bytes + out.script_off, out.script_len);
 }
-__global__ void __launch_bounds__(128) k_tx_ids_dev(BatchView b, uint32_t n_txs, uint64_t* __restrict__ out) {
-  uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n_txs) return;
-  uint64_t d[4];
-  tx_id(d, b, i);
-#pragma unroll
-  for (int k = 0; k < 4; k++) out[4 * (size_t)i + k] = d[k];
-}
 
 // ---------------------------------------------------------------------------------------------
 // K8 MuHash elements (consensus/core/src/muhash.rs:16-33): one element per thread, written straight into level 0
@@ -532,7 +512,6 @@ __global__ void k_u3072_scatter(const uint32_t* __restrict__ values, size_t n, u
 // ---------------------------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------------------------
-static inline unsigned nblk(size_t n, unsigned b) { return (unsigned)((n + b - 1) / b); }
 
 extern "C" int kgv_utxo_create(kgv_ctx* ctx, uint64_t capacity_slots, kgv_utxo_table** out) {
   if (!ctx || !out) return KGV_ERR_ARG;
@@ -655,29 +634,19 @@ extern "C" int kgv_utxo_lookup(kgv_ctx* ctx, kgv_utxo_table* t, const uint8_t* k
   if (n == 0) return KGV_OK;
   if (!keys36 || !entries || !found || (script_stride && !scripts_out)) { ctx->err = "null buffer"; return KGV_ERR_ARG; }
   CK(cudaSetDevice(ctx->device));
-  bool dev = kgv_ptr_is_device(keys36);
-  const uint8_t* dk = keys36;
-  kgv_utxo_entry* de = entries;
-  uint8_t *ds = scripts_out, *df = found;
-  size_t o_e = 0, o_s = al256(n * sizeof(kgv_utxo_entry)), o_f = al256(o_s + n * (size_t)script_stride);
-  if (!dev) {
-    int rc = kgv_reserve(ctx, &ctx->d_in, &ctx->d_in_cap, n * 36);
-    if (rc) return rc;
-    rc = kgv_reserve(ctx, &ctx->d_out, &ctx->d_out_cap, o_f + n);
-    if (rc) return rc;
-    CK(cudaMemcpyAsync(ctx->d_in, keys36, n * 36, cudaMemcpyHostToDevice, ctx->stream));
-    dk = ctx->d_in; de = (kgv_utxo_entry*)(ctx->d_out + o_e); ds = ctx->d_out + o_s; df = ctx->d_out + o_f;
-  }
+  kgv_io io(ctx);
+  const uint8_t* dk;
+  kgv_utxo_entry* de;
+  uint8_t *ds, *df;
+  io.in(keys36, n * 36, &dk);
+  io.out(entries, n * sizeof(kgv_utxo_entry), &de);
+  io.out(script_stride ? scripts_out : nullptr, n * (size_t)script_stride, &ds);
+  io.out(found, n, &df);
+  if (int rc = io.stage()) return rc;
   k_utxo_lookup<<<nblk(n, 128), 128, 0, ctx->stream>>>(view_of(t), dk, n, de, ds, script_stride, df);
   CK(cudaGetLastError());
   ctx->launches++;
-  if (!dev) {
-    CK(cudaMemcpyAsync(entries, de, n * sizeof(kgv_utxo_entry), cudaMemcpyDeviceToHost, ctx->stream));
-    if (script_stride) CK(cudaMemcpyAsync(scripts_out, ds, n * (size_t)script_stride, cudaMemcpyDeviceToHost, ctx->stream));
-    CK(cudaMemcpyAsync(found, df, n, cudaMemcpyDeviceToHost, ctx->stream));
-    CK(cudaStreamSynchronize(ctx->stream));
-  }
-  return KGV_OK;
+  return io.finish();
 }
 
 extern "C" int kgv_utxo_apply_diff(kgv_ctx* ctx, kgv_utxo_table* t, const uint8_t* rem_keys36, size_t n_rem, uint8_t* rem_status,
@@ -693,34 +662,20 @@ extern "C" int kgv_utxo_apply_diff(kgv_ctx* ctx, kgv_utxo_table* t, const uint8_
     int rc = utxo_reserve(ctx, t, n_add + (t->base ? n_rem : 0), n_add_bytes + 8 * (uint64_t)n_add);
     if (rc) return rc;
   }
-  bool dev = kgv_ptr_is_device(probe);
-  size_t o_rk = 0, o_ak = al256(n_rem * 36), o_ae = al256(o_ak + n_add * 36), o_ab = al256(o_ae + n_add * sizeof(kgv_utxo_entry));
-  size_t o_rs = 0, o_as = al256(n_rem);
-  const uint8_t *drk = rem_keys36, *dak = add_keys36, *dab = add_bytes;
-  const kgv_utxo_entry* dae = add_entries;
-  uint8_t *drs = rem_status, *das = add_status;
-  if (!dev) {
-    int rc = kgv_reserve(ctx, &ctx->d_in, &ctx->d_in_cap, o_ab + n_add_bytes + 16);
-    if (rc) return rc;
-    rc = kgv_reserve(ctx, &ctx->d_out, &ctx->d_out_cap, o_as + n_add + 16);
-    if (rc) return rc;
-    if (n_rem) CK(cudaMemcpyAsync(ctx->d_in + o_rk, rem_keys36, n_rem * 36, cudaMemcpyHostToDevice, ctx->stream));
-    if (n_add) {
-      CK(cudaMemcpyAsync(ctx->d_in + o_ak, add_keys36, n_add * 36, cudaMemcpyHostToDevice, ctx->stream));
-      CK(cudaMemcpyAsync(ctx->d_in + o_ae, add_entries, n_add * sizeof(kgv_utxo_entry), cudaMemcpyHostToDevice, ctx->stream));
-      if (n_add_bytes) CK(cudaMemcpyAsync(ctx->d_in + o_ab, add_bytes, n_add_bytes, cudaMemcpyHostToDevice, ctx->stream));
-    }
-    drk = ctx->d_in + o_rk; dak = ctx->d_in + o_ak; dae = (const kgv_utxo_entry*)(ctx->d_in + o_ae); dab = ctx->d_in + o_ab;
-    drs = ctx->d_out + o_rs; das = ctx->d_out + o_as;
-  }
+  kgv_io io(ctx);
+  const uint8_t *drk, *dak, *dab;
+  const kgv_utxo_entry* dae;
+  uint8_t *drs, *das;
+  io.in(n_rem ? rem_keys36 : nullptr, n_rem * 36, &drk);
+  io.out(n_rem ? rem_status : nullptr, n_rem, &drs);
+  io.in(n_add ? add_keys36 : nullptr, n_add * 36, &dak);
+  io.in(n_add ? add_entries : nullptr, n_add * sizeof(kgv_utxo_entry), &dae);
+  io.in(n_add && n_add_bytes ? add_bytes : nullptr, n_add_bytes, &dab);
+  io.out(n_add ? add_status : nullptr, n_add, &das);
+  if (int rc = io.stage()) return rc;
   if (n_rem) { k_utxo_erase<<<nblk(n_rem, 128), 128, 0, ctx->stream>>>(view_of(t), drk, n_rem, drs); CK(cudaGetLastError()); ctx->launches++; }
   if (n_add) { k_utxo_insert<<<nblk(n_add, 128), 128, 0, ctx->stream>>>(view_of(t), dak, dae, dab, n_add, das); CK(cudaGetLastError()); ctx->launches++; }
-  if (!dev) {
-    if (n_rem && rem_status) CK(cudaMemcpyAsync(rem_status, drs, n_rem, cudaMemcpyDeviceToHost, ctx->stream));
-    if (n_add && add_status) CK(cudaMemcpyAsync(add_status, das, n_add, cudaMemcpyDeviceToHost, ctx->stream));
-    CK(cudaStreamSynchronize(ctx->stream));
-  }
-  return KGV_OK;
+  return io.finish();
 }
 
 extern "C" int kgv_utxo_export(kgv_ctx* ctx, kgv_utxo_table* t, uint8_t* keys36, kgv_utxo_entry* entries, uint8_t* bytes, size_t max_n, size_t bytes_cap, size_t* n_out,
@@ -731,18 +686,18 @@ extern "C" int kgv_utxo_export(kgv_ctx* ctx, kgv_utxo_table* t, uint8_t* keys36,
   const bool counting = !keys36;
   if (!counting && (!entries || (bytes_cap && !bytes))) { ctx->err = "null buffer"; return KGV_ERR_ARG; }
   CK(cudaSetDevice(ctx->device));
-  const bool dev = counting ? true : kgv_ptr_is_device(keys36);
-  uint8_t *dk = keys36, *db = bytes;
+  kgv_io io(ctx);
+  uint8_t *dk = nullptr, *db = bytes;
   kgv_utxo_entry* de = entries;
-  size_t o_e = al256(max_n * 36), o_b = al256(o_e + max_n * sizeof(kgv_utxo_entry));
-  if (!counting && !dev) {
-    int rc = kgv_reserve(ctx, &ctx->d_out, &ctx->d_out_cap, o_b + bytes_cap + 16);
-    if (rc) return rc;
-    dk = ctx->d_out; de = (kgv_utxo_entry*)(ctx->d_out + o_e); db = ctx->d_out + o_b;
+  if (!counting) {
+    io.out(keys36, max_n * 36, &dk);
+    io.out(entries, max_n * sizeof(kgv_utxo_entry), &de);
+    io.out(bytes, bytes_cap, &db);
+    if (int rc = io.stage()) return rc;
   }
   unsigned long long* cnt = t->counters + 8;  // (the digest's scratch words)
   CK(cudaMemsetAsync(cnt, 0, 2 * sizeof(unsigned long long), ctx->stream));
-  k_utxo_export<<<nblk(t->mask + 1, 128), 128, 0, ctx->stream>>>(view_of(t), counting ? nullptr : dk, de, db, max_n, bytes_cap, cnt);
+  k_utxo_export<<<nblk(t->mask + 1, 128), 128, 0, ctx->stream>>>(view_of(t), dk, de, db, max_n, bytes_cap, cnt);
   CK(cudaGetLastError());
   ctx->launches++;
   unsigned long long c[2];
@@ -752,15 +707,11 @@ extern "C" int kgv_utxo_export(kgv_ctx* ctx, kgv_utxo_table* t, uint8_t* keys36,
   if (bytes_out) *bytes_out = (size_t)c[1];
   if (counting) return KGV_OK;
   if (c[0] > max_n || c[1] > bytes_cap) { ctx->err = "kgv_utxo_export: the caller's arrays are too small (sizes returned)"; return KGV_ERR_NOMEM; }
-  if (!dev) {
-    if (c[0]) {
-      CK(cudaMemcpyAsync(keys36, dk, (size_t)c[0] * 36, cudaMemcpyDeviceToHost, ctx->stream));
-      CK(cudaMemcpyAsync(entries, de, (size_t)c[0] * sizeof(kgv_utxo_entry), cudaMemcpyDeviceToHost, ctx->stream));
-    }
-    if (c[1]) CK(cudaMemcpyAsync(bytes, db, (size_t)c[1], cudaMemcpyDeviceToHost, ctx->stream));
-    CK(cudaStreamSynchronize(ctx->stream));
-  }
-  return KGV_OK;
+  // only what the table held comes back
+  io.trim(keys36, (size_t)c[0] * 36);
+  io.trim(entries, (size_t)c[0] * sizeof(kgv_utxo_entry));
+  io.trim(bytes, (size_t)c[1]);
+  return io.finish();
 }
 
 extern "C" int kgv_utxo_import_chunk(kgv_ctx* ctx, kgv_utxo_table* t, const uint8_t* keys36, const kgv_utxo_entry* entries, const uint8_t* bytes, size_t n_bytes, size_t n,
@@ -771,20 +722,17 @@ extern "C" int kgv_utxo_import_chunk(kgv_ctx* ctx, kgv_utxo_table* t, const uint
   if (n == 0) return KGV_OK;
   if (!keys36 || !entries || (n_bytes && !bytes)) { ctx->err = "null buffer"; return KGV_ERR_ARG; }
   if (kgv_ptr_is_device(numerator384)) { ctx->err = "numerator384 is a host value"; return KGV_ERR_ARG; }
-  for (size_t i = 0; !kgv_ptr_is_device(keys36) && i < n; i++)
+  kgv_io io(ctx);
+  for (size_t i = 0; !io.is_device(keys36) && i < n; i++)
     if ((uint64_t)entries[i].script_off + entries[i].script_len > n_bytes) { ctx->err = "entry script outside the byte arena"; return KGV_ERR_ARG; }
   CK(cudaSetDevice(ctx->device));
-  const uint8_t *dk = keys36, *db = bytes;
-  const kgv_utxo_entry* de = entries;
-  if (!kgv_ptr_is_device(keys36)) {  // one upload serves the insert and the multiset
-    size_t o_e = al256(n * 36), o_b = al256(o_e + n * sizeof(kgv_utxo_entry));
-    int rc = kgv_reserve(ctx, &ctx->d_scratch, &ctx->d_scratch_cap, o_b + n_bytes + 16);
-    if (rc) return rc;
-    CK(cudaMemcpyAsync(ctx->d_scratch, keys36, n * 36, cudaMemcpyHostToDevice, ctx->stream));
-    CK(cudaMemcpyAsync(ctx->d_scratch + o_e, entries, n * sizeof(kgv_utxo_entry), cudaMemcpyHostToDevice, ctx->stream));
-    if (n_bytes) CK(cudaMemcpyAsync(ctx->d_scratch + o_b, bytes, n_bytes, cudaMemcpyHostToDevice, ctx->stream));
-    dk = ctx->d_scratch; de = (const kgv_utxo_entry*)(ctx->d_scratch + o_e); db = ctx->d_scratch + o_b;
-  }
+  // one upload serves the insert and the multiset
+  const uint8_t *dk, *db;
+  const kgv_utxo_entry* de;
+  io.in(keys36, n * 36, &dk);
+  io.in(entries, n * sizeof(kgv_utxo_entry), &de);
+  io.in(n_bytes ? bytes : nullptr, n_bytes, &db);
+  if (int rc = io.stage()) return rc;
   // pruning_meta.utxo_set.write_many(chunk) (consensus/mod.rs:1072)
   int rc = kgv_utxo_apply_diff(ctx, t, nullptr, 0, nullptr, dk, de, db, n_bytes, n, nullptr);
   if (rc) return rc;
@@ -796,7 +744,7 @@ extern "C" int kgv_utxo_import_chunk(kgv_ctx* ctx, kgv_utxo_table* t, const uint
   CK(cudaGetLastError());
   ctx->launches++;
   uint8_t chunk_num[384], chunk_den[384], one[384];
-  rc = kgv_mu_reduce(ctx, 0, n, chunk_num, chunk_den);
+  rc = kgv_mu_reduce(ctx, io, 0, n, chunk_num, chunk_den);
   if (rc) return rc;
   memset(one, 0, sizeof one);
   one[0] = 1;
@@ -1037,13 +985,9 @@ static int validate_core(kgv_ctx* ctx, kgv_utxo_table* table, const kgv_tx_batch
     rc = table ? scripts_with_engine(ctx, table, d, v, itx, dres) : kgv_scripts_phase(ctx, v, nt, ni, itx, dres, nullptr);
     if (rc) return rc;
   }
-  if (kgv_ptr_is_device(results)) {
-    CK(cudaMemcpyAsync(results, dres, nt * sizeof(kgv_tx_result), cudaMemcpyDeviceToDevice, st));
-  } else {
-    CK(cudaMemcpyAsync(results, dres, nt * sizeof(kgv_tx_result), cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
-  }
-  return KGV_OK;
+  kgv_io io(ctx);
+  if ((rc = io.copy_out(results, dres, nt * sizeof(kgv_tx_result)))) return rc;
+  return io.finish();
 }
 
 extern "C" int kgv_validate_populated(kgv_ctx* ctx, const kgv_tx_batch* batch, uint64_t pov_daa_score, uint32_t flags, const kgv_params* params,
@@ -1085,15 +1029,16 @@ static int mempool_core(kgv_ctx* ctx, kgv_utxo_table* t, const kgv_tx_batch* bat
   if (batch->n_txs == 0) return KGV_OK;
   if (iso && batch->n_txs > 0xFFFFFFFFull) { ctx->err = "kgv_validate_mempool_txs_in_parallel: more than 2^32 - 1 transactions"; return KGV_ERR_ARG; }
   CK(cudaSetDevice(ctx->device));
-  const bool dev = kgv_ptr_is_device(results) != 0;
-  for (const void* p : {(const void*)batch->txs, (const void*)args, (const void*)storage_mass, (const void*)entries_out, (const void*)(scripts_cap ? scripts_out : nullptr),
-                        (const void*)(iso ? iso->masses : nullptr), (const void*)(iso ? iso->detail : nullptr)})
-    if (p && (kgv_ptr_is_device(p) != 0) != dev) { ctx->err = "kgv_validate_mempool_txs: the batch, args and outputs must all be host or all be device pointers"; return KGV_ERR_ARG; }
+  kgv_io io(ctx);
+  bool dev;
+  if (int rc = io.one_side("kgv_validate_mempool_txs", {results, batch->txs, args, storage_mass, entries_out, scripts_cap ? scripts_out : nullptr,
+                                                        iso ? iso->masses : nullptr, iso ? iso->detail : nullptr}, &dev))
+    return rc;
   kgv_dev_batch d;
   int rc = kgv_batch_to_device(ctx, batch, &d, false);
   if (rc) return rc;
   const size_t nt = d.n_txs, ni = d.n_inputs;
-  // d_work: populated entries, input -> tx, verdicts, masses, script lengths and their offsets, the uploaded thresholds,
+  // d_work: populated entries, input -> tx, verdicts, masses, script lengths and their offsets,
   // counters [script bytes (64-bit), zero divisors, the scan's 32-bit total, the relay-fee overflow flag of the standardness policy]
   size_t o_ent = 0;
   size_t o_itx = al256(o_ent + ni * sizeof(DevEntry));
@@ -1101,20 +1046,29 @@ static int mempool_core(kgv_ctx* ctx, kgv_utxo_table* t, const kgv_tx_batch* bat
   size_t o_mass = al256(o_res + nt * sizeof(kgv_tx_result));
   size_t o_len = al256(o_mass + nt * 8);
   size_t o_off = al256(o_len + ni * 4);
-  size_t o_args = al256(o_off + ni * 4);
-  size_t o_cnt = al256(o_args + (args ? nt * sizeof(kgv_mempool_tx_args) : 0));
-  // with iso: its verdicts, max(compute, transient) per tx, the masses (for a host caller, or for the policy when the caller takes none),
-  // the large-transaction list, the policy's details for a host caller
+  size_t o_cnt = al256(o_off + ni * 4);
+  // with iso: its verdicts, max(compute, transient) per tx, the masses (for the policy when the caller takes none), the large-transaction list
   const kgv_mempool_policy* pol = iso ? iso->policy : nullptr;
   uint64_t* detail = iso ? iso->detail : nullptr;
-  const bool own_masses = iso && (iso->masses || pol) && !(dev && iso->masses);
+  const bool own_masses = iso && !iso->masses && pol;
   size_t o_iso = al256(o_cnt + 32);
   size_t o_nc = al256(o_iso + (iso ? nt * sizeof(kgv_tx_result) : 0));
   size_t o_ism = al256(o_nc + (iso ? nt * 8 : 0));
   size_t o_lst = al256(o_ism + (own_masses ? nt * sizeof(kgv_tx_masses) : 0));
-  size_t o_det = al256(o_lst + (iso ? (nt + 1) * 4 : 0));
-  rc = kgv_reserve(ctx, &ctx->d_work, &ctx->d_work_cap, iso ? al256(o_det + (pol && detail && !dev ? nt * 8 : 0)) : al256(o_cnt + 32));
+  rc = kgv_reserve(ctx, &ctx->d_work, &ctx->d_work_cap, iso ? al256(o_lst + (nt + 1) * 4) : al256(o_cnt + 32));
   if (rc) return rc;
+  // the entries' scripts come back up to their size, known after the context rules
+  const kgv_mempool_tx_args* dargs;
+  kgv_tx_masses* dism = nullptr;
+  uint64_t* ddet;
+  kgv_utxo_entry* de;
+  uint8_t* ds;
+  io.in(args, nt * sizeof(kgv_mempool_tx_args), &dargs);
+  if (iso) io.out(iso->masses, nt * sizeof(kgv_tx_masses), &dism);
+  io.out(pol ? detail : nullptr, nt * 8, &ddet);
+  io.out(ni ? entries_out : nullptr, ni * sizeof(kgv_utxo_entry), &de);
+  io.out(ni && entries_out && scripts_cap ? scripts_out : nullptr, scripts_cap, &ds);
+  if ((rc = io.stage())) return rc;
   uint8_t* S = ctx->d_work;
   DevEntry* dent = (DevEntry*)(S + o_ent);
   uint32_t *itx = (uint32_t*)(S + o_itx), *len = (uint32_t*)(S + o_len), *off = (uint32_t*)(S + o_off);
@@ -1122,20 +1076,13 @@ static int mempool_core(kgv_ctx* ctx, kgv_utxo_table* t, const kgv_tx_batch* bat
   kgv_tx_result* dres = (kgv_tx_result*)(S + o_res);
   uint64_t* dmass = (uint64_t*)(S + o_mass);
   cudaStream_t st = ctx->stream;
-  const kgv_mempool_tx_args* dargs = args;
-  if (args && !dev) {
-    CK(cudaMemcpyAsync(S + o_args, args, nt * sizeof(kgv_mempool_tx_args), cudaMemcpyHostToDevice, st));
-    dargs = (const kgv_mempool_tx_args*)(S + o_args);
-  }
   CK(cudaMemsetAsync(cnt, 0, 32, st));
   kgv_tx_result* gate = nullptr;
   uint64_t* dnc = nullptr;
-  kgv_tx_masses* dism = nullptr;
-  uint64_t* ddet = pol && detail && !dev ? (uint64_t*)(S + o_det) : detail;
   if (iso) {
     gate = (kgv_tx_result*)(S + o_iso);
     dnc = (uint64_t*)(S + o_nc);
-    dism = own_masses ? (kgv_tx_masses*)(S + o_ism) : iso->masses;
+    if (own_masses) dism = (kgv_tx_masses*)(S + o_ism);
     rc = kgv_isolation_run(ctx, d, *iso->rules, virtual_daa_score, iso->past_median_time, true, gate, dism, dnc, (uint32_t*)(S + o_lst), st);
     if (rc) return rc;
     STAGE("isolation");
@@ -1172,23 +1119,10 @@ static int mempool_core(kgv_ctx* ctx, kgv_utxo_table* t, const kgv_tx_batch* bat
   if (entries_out && n_script > 0xFFFFFFFFull) { ctx->err = "kgv_validate_mempool_txs: the entries' scripts exceed the 32-bit script_off range"; return KGV_ERR_ARG; }
   if (entries_out && n_script > scripts_cap) { ctx->err = "kgv_validate_mempool_txs: scripts_out is too small (size returned)"; return KGV_ERR_NOMEM; }
   if (entries_out && ni) {
-    kgv_utxo_entry* de = entries_out;
-    uint8_t* ds = scripts_out;
-    if (!dev) {
-      const size_t o_s = al256(ni * sizeof(kgv_utxo_entry));
-      rc = kgv_reserve(ctx, &ctx->d_out, &ctx->d_out_cap, o_s + n_script + 16);
-      if (rc) return rc;
-      de = (kgv_utxo_entry*)ctx->d_out;
-      ds = ctx->d_out + o_s;
-    }
     k_mempool_entries_out<<<nblk(ni, 128), 128, 0, st>>>(dent, off, ni, de, ds);
     CK(cudaGetLastError());
     ctx->launches++;
-    if (!dev) {
-      CK(cudaMemcpyAsync(entries_out, de, ni * sizeof(kgv_utxo_entry), cudaMemcpyDeviceToHost, st));
-      if (n_script) CK(cudaMemcpyAsync(scripts_out, ds, n_script, cudaMemcpyDeviceToHost, st));
-      CK(cudaStreamSynchronize(st));  // the script phase may reuse d_out
-    }
+    io.trim(scripts_out, n_script);
   }
   if (ni) {
     rc = scripts_with_engine(ctx, t, d, v, itx, dres);
@@ -1199,17 +1133,12 @@ static int mempool_core(kgv_ctx* ctx, kgv_utxo_table* t, const kgv_tx_batch* bat
     if ((rc = kgv_standard_context_run(ctx, d, dent, *pol, dism, dmass, nullptr, dres, ddet, fee_overflow, st))) return rc;
     STAGE("standard in context");
   }
-  const cudaMemcpyKind k = dev ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost;
-  CK(cudaMemcpyAsync(results, dres, nt * sizeof(kgv_tx_result), k, st));
-  CK(cudaMemcpyAsync(storage_mass, dmass, nt * 8, k, st));
-  if (iso && iso->masses && !dev) CK(cudaMemcpyAsync(iso->masses, dism, nt * sizeof(kgv_tx_masses), k, st));
+  if ((rc = io.copy_out(results, dres, nt * sizeof(kgv_tx_result))) || (rc = io.copy_out(storage_mass, dmass, nt * 8))) return rc;
   // the compute mass of a tx that reaches the fee check is at most 100 000 (standardness in isolation), so only a relay fee above
   // u64::MAX / 100 000 can overflow: a device-pointer caller waits for the flag only then
   unsigned long long overflow = 0;
-  const bool read_flag = pol && (!dev || pol->minimum_relay_transaction_fee > ~0ull / kgv::STD_MAX_TRANSACTION_MASS);
-  if (pol && detail && !dev) CK(cudaMemcpyAsync(detail, ddet, nt * 8, k, st));
-  if (read_flag) CK(cudaMemcpyAsync(&overflow, fee_overflow, 8, cudaMemcpyDeviceToHost, st));
-  if (!dev || read_flag) CK(cudaStreamSynchronize(st));
+  if (pol && (!dev || pol->minimum_relay_transaction_fee > ~0ull / kgv::STD_MAX_TRANSACTION_MASS) && (rc = io.copy_out(&overflow, fee_overflow, 8))) return rc;
+  if ((rc = io.finish())) return rc;
   if (overflow) { ctx->err = "kgv_validate_mempool_txs_with_policy: compute mass * minimum_relay_transaction_fee overflows u64"; return KGV_ERR_ARG; }
   return KGV_OK;
 }
@@ -1257,27 +1186,25 @@ extern "C" int kgv_utxo_apply_accepted(kgv_ctx* ctx, kgv_utxo_table* t, const kg
   rc = kgv_batch_to_device(ctx, batch, &d, false);
   if (rc) return rc;
   size_t nt = d.n_txs, ni = d.n_inputs, no = d.n_outputs;
-  size_t o_itx = 0, o_otx = al256(ni * 4), o_ids = al256(o_otx + no * 4), o_acc = al256(o_ids + nt * 32);
-  rc = kgv_reserve(ctx, &ctx->d_scratch, &ctx->d_scratch_cap, al256(o_acc + nt));
+  size_t o_itx = 0, o_otx = al256(ni * 4), o_ids = al256(o_otx + no * 4);
+  rc = kgv_reserve(ctx, &ctx->d_scratch, &ctx->d_scratch_cap, al256(o_ids + nt * 32));
   if (rc) return rc;
   uint8_t* S = ctx->d_scratch;
-  const uint8_t* dacc = accept;
-  if (!kgv_ptr_is_device(accept)) {
-    CK(cudaMemcpyAsync(S + o_acc, accept, nt, cudaMemcpyHostToDevice, ctx->stream));
-    dacc = S + o_acc;
-  }
+  kgv_io io(ctx);
+  const uint8_t* dacc;
+  io.in(accept, nt, &dacc);
+  if ((rc = io.stage())) return rc;
   BatchView v{d.txs, d.inputs, d.outputs, nullptr, d.bytes};
   cudaStream_t st = ctx->stream;
-  k_tx_ids_dev<<<nblk(nt, 128), 128, 0, st>>>(v, (uint32_t)nt, (uint64_t*)(S + o_ids));
-  CK(cudaGetLastError());
+  if ((rc = kgv_tx_digests_run(ctx, d, nt, (uint64_t*)(S + o_ids), false))) return rc;
   k_input_tx_index<<<nblk(nt, 128), 128, 0, st>>>(d.txs, (uint32_t)nt, (uint32_t*)(S + o_itx));
   CK(cudaGetLastError());
   k_output_tx_index<<<nblk(nt, 128), 128, 0, st>>>(d.txs, (uint32_t)nt, (uint32_t*)(S + o_otx));
   CK(cudaGetLastError());
-  ctx->launches += 3;
+  ctx->launches += 2;
   if (ni) { k_apply_erase<<<nblk(ni, 128), 128, 0, st>>>(view_of(t), d.txs, d.inputs, ni, (const uint32_t*)(S + o_itx), dacc); CK(cudaGetLastError()); ctx->launches++; }
   if (no) { k_apply_insert<<<nblk(no, 128), 128, 0, st>>>(view_of(t), v, no, (const uint32_t*)(S + o_otx), dacc, (const uint64_t*)(S + o_ids), pov_daa_score); CK(cudaGetLastError()); ctx->launches++; }
-  if (!kgv_ptr_is_device(accept)) CK(cudaStreamSynchronize(st));
+  if (!io.is_device(accept)) CK(cudaStreamSynchronize(st));  // a host-pointer call returns with the table updated
   return KGV_OK;
 }
 
@@ -1289,7 +1216,8 @@ extern "C" int kgv_muhash_txs(kgv_ctx* ctx, kgv_utxo_table* table, const kgv_tx_
   if (!ctx) return KGV_ERR_ARG;
   std::lock_guard<std::recursive_mutex> g(ctx->mu);
   if (!batch || !numerator384 || !denominator384 || (batch->n_txs && !accept)) { ctx->err = "null argument"; return KGV_ERR_ARG; }
-  if (kgv_ptr_is_device(numerator384) != kgv_ptr_is_device(denominator384)) { ctx->err = "outputs must both be host or both be device pointers"; return KGV_ERR_ARG; }
+  kgv_io io(ctx);
+  if (int rc = io.one_side("kgv_muhash_txs", {numerator384, denominator384})) return rc;
   CK(cudaSetDevice(ctx->device));
   kgv_dev_batch d;
   d.n_txs = d.n_inputs = d.n_outputs = d.n_bytes = 0;
@@ -1302,16 +1230,14 @@ extern "C" int kgv_muhash_txs(kgv_ctx* ctx, kgv_utxo_table* table, const kgv_tx_
   int rc = kgv_mu_reserve(ctx, ni, no, &e_den, &e_num);
   if (rc) return rc;
   if (nt) {
-    size_t o_ent = 0, o_itx = al256(o_ent + ni * sizeof(DevEntry)), o_otx = al256(o_itx + ni * 4), o_ids = al256(o_otx + no * 4), o_acc = al256(o_ids + nt * 32);
-    rc = kgv_reserve(ctx, &ctx->d_scratch, &ctx->d_scratch_cap, al256(o_acc + nt));
+    size_t o_ent = 0, o_itx = al256(o_ent + ni * sizeof(DevEntry)), o_otx = al256(o_itx + ni * 4), o_ids = al256(o_otx + no * 4);
+    rc = kgv_reserve(ctx, &ctx->d_scratch, &ctx->d_scratch_cap, al256(o_ids + nt * 32));
     if (rc) return rc;
     uint8_t* S = ctx->d_scratch;
     cudaStream_t st = ctx->stream;
-    const uint8_t* dacc = accept;
-    if (!kgv_ptr_is_device(accept)) {
-      CK(cudaMemcpyAsync(S + o_acc, accept, nt, cudaMemcpyHostToDevice, st));
-      dacc = S + o_acc;
-    }
+    const uint8_t* dacc;
+    io.in(accept, nt, &dacc);
+    if ((rc = io.stage())) return rc;
     DevEntry* dent = (DevEntry*)(S + o_ent);
     if (ni) {
       if (table) k_populate<<<nblk(ni, 128), 128, 0, st>>>(view_of(table), d.inputs, ni, dent);
@@ -1320,8 +1246,7 @@ extern "C" int kgv_muhash_txs(kgv_ctx* ctx, kgv_utxo_table* table, const kgv_tx_
       ctx->launches++;
     }
     BatchView v{d.txs, d.inputs, d.outputs, dent, d.bytes};
-    k_tx_ids_dev<<<nblk(nt, 128), 128, 0, st>>>(v, (uint32_t)nt, (uint64_t*)(S + o_ids));
-    CK(cudaGetLastError());
+    if ((rc = kgv_tx_digests_run(ctx, d, nt, (uint64_t*)(S + o_ids), false))) return rc;
     k_input_tx_index<<<nblk(nt, 128), 128, 0, st>>>(d.txs, (uint32_t)nt, (uint32_t*)(S + o_itx));
     CK(cudaGetLastError());
     k_output_tx_index<<<nblk(nt, 128), 128, 0, st>>>(d.txs, (uint32_t)nt, (uint32_t*)(S + o_otx));
@@ -1331,9 +1256,9 @@ extern "C" int kgv_muhash_txs(kgv_ctx* ctx, kgv_utxo_table* table, const kgv_tx_
                                                                (const uint64_t*)(S + o_ids), pov_daa_score, e_den, e_num);
       CK(cudaGetLastError());
     }
-    ctx->launches += 4;
+    ctx->launches += 3;
   }
-  return kgv_mu_reduce(ctx, ni, no, numerator384, denominator384);
+  return kgv_mu_reduce(ctx, io, ni, no, numerator384, denominator384);
 }
 
 // MuHash of the whole UTXO set (the pruning-point / virtual UTXO commitment: MuHash::add_utxo for every entry,
@@ -1351,6 +1276,7 @@ extern "C" int kgv_utxo_muhash(kgv_ctx* ctx, kgv_utxo_table* t, uint8_t* numerat
   if (rc) return rc;
   uint8_t* prods = ctx->d_out;                    // n_chunks x 384 B, contiguous values
   uint8_t* dummy_den = ctx->d_out + n_chunks * 384;
+  kgv_io io(ctx);
   for (size_t c = 0; c < n_chunks; c++) {
     const uint64_t first = (uint64_t)c * chunk;
     const size_t n = (size_t)((slots - first) < chunk ? (slots - first) : chunk);
@@ -1360,24 +1286,18 @@ extern "C" int kgv_utxo_muhash(kgv_ctx* ctx, kgv_utxo_table* t, uint8_t* numerat
     k_muhash_table_elements<<<nblk(n, 128), 128, 0, ctx->stream>>>(view_of(t), first, n, e_num);
     CK(cudaGetLastError());
     ctx->launches++;
-    rc = kgv_mu_reduce(ctx, 0, n, prods + 384 * c, dummy_den);
+    rc = kgv_mu_reduce(ctx, io, 0, n, prods + 384 * c, dummy_den);
     if (rc) return rc;
   }
-  if (n_chunks == 1) {
-    const bool dev = kgv_ptr_is_device(numerator384);
-    CK(cudaMemcpyAsync(numerator384, prods, 384, dev ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, ctx->stream));
-    if (!dev) CK(cudaStreamSynchronize(ctx->stream));
-    return KGV_OK;
-  }
+  if (n_chunks == 1) return (rc = io.copy_out(numerator384, prods, 384)) ? rc : io.finish();
   uint32_t *e_den = nullptr, *e_num = nullptr;
   rc = kgv_mu_reserve(ctx, 0, n_chunks, &e_den, &e_num);
   if (rc) return rc;
   k_u3072_scatter<<<nblk(n_chunks, 128), 128, 0, ctx->stream>>>((const uint32_t*)prods, n_chunks, e_num);
   CK(cudaGetLastError());
   ctx->launches++;
-  if (kgv_ptr_is_device(numerator384)) return kgv_mu_reduce(ctx, 0, n_chunks, numerator384, dummy_den);
-  uint8_t den_host[384];
-  return kgv_mu_reduce(ctx, 0, n_chunks, numerator384, den_host);
+  uint8_t den_host[384];  // the denominator goes to the numerator's side
+  return kgv_mu_reduce(ctx, io, 0, n_chunks, numerator384, io.is_device(numerator384) ? dummy_den : den_host);
 }
 
 #include "kgv_replay_impl.cuh"
