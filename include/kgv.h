@@ -24,7 +24,10 @@
  *     The arrays of a kgv_tx_batch are all host or all device pointers (KGV_ERR_ARG
  *     otherwise).  Each call states which of its other arrays must share one kind
  *     (KGV_ERR_ARG otherwise), which may each be of either kind, and which must be host
- *     memory or device memory.
+ *     memory or device memory.  The parameter structs (kgv_params, kgv_tx_rules, kgv_body_rules,
+ *     kgv_mempool_policy, kgv_header_rules), the block and group offsets the library reads to
+ *     plan a call, and the scalar results (counts, stats, epochs) are host memory: a device
+ *     pointer there gives KGV_ERR_ARG, with kgv_last_error naming the call and the argument.
  *   - return value: 0 = ok, negative = argument / CUDA / NCCL failure (kgv_last_error explains).
  *     An invalid signature is NEVER an error return: verdicts are per-item status bytes.
  *   - there is no CPU fallback: without a usable CUDA device kgv_create fails.
@@ -256,7 +259,9 @@ typedef struct kgv_utxo_table kgv_utxo_table;
 int kgv_utxo_create(kgv_ctx* ctx, uint64_t capacity_slots /* rounded up to a power of two */, kgv_utxo_table** out);
 void kgv_utxo_destroy(kgv_ctx* ctx, kgv_utxo_table* t);
 /* UtxoView::get for n outpoints: found[i] in {0,1}; entries[i].script_off = i*script_stride into scripts_out
- * (scripts longer than script_stride are truncated there; script_len is always the true length). */
+ * (scripts longer than script_stride are truncated there; script_len is always the true length).  Only the script bytes are
+ * written: the rest of each script_stride row keeps what the caller put there, whichever side scripts_out is on (a host scripts_out
+ * is uploaded first for that).  Each array on its own side. */
 int kgv_utxo_lookup(kgv_ctx* ctx, kgv_utxo_table* t, const uint8_t* keys36, size_t n, kgv_utxo_entry* entries, uint8_t* scripts_out,
                     uint32_t script_stride, uint8_t* found);
 /* write_diff_batch (utxo_set.rs:107-112): delete the removed outpoints, then put the added ones.
@@ -279,7 +284,8 @@ int kgv_utxo_export(kgv_ctx* ctx, kgv_utxo_table* t, uint8_t* keys36, kgv_utxo_e
  * written into the table (write_many) and MuHash::from_utxo of every (outpoint, entry), reduced, is combined into the running multiset
  * numerator384 (host value, in / out, 384 little-endian bytes; start from 1).  The caller then compares kgv_muhash_finalize(numerator, 1)
  * with the new pruning point's header.utxo_commitment (processor.rs:1133-1139: ImportedMultisetHashMismatch) and validates the pruning
- * point's own transactions with kgv_validate_txs (:1162-1172). */
+ * point's own transactions with kgv_validate_txs (:1162-1172).  keys36, entries and bytes may each be host or device memory; an entry
+ * whose script range leaves the n_bytes arena is refused (KGV_ERR_ARG) on either side. */
 int kgv_utxo_import_chunk(kgv_ctx* ctx, kgv_utxo_table* t, const uint8_t* keys36, const kgv_utxo_entry* entries, const uint8_t* bytes, size_t n_bytes, size_t n,
                           uint8_t* numerator384);
 
@@ -549,7 +555,7 @@ typedef struct {
 } kgv_replay_stats;
 /* results: n_txs records (host or device memory): the UTXO-context verdict when the context rules fail, else the script
  * verdict (KGV_TX_SKIPPED_COINBASE for coinbases).  accept (may be NULL): n_txs bytes, 1 = folded into the table.
- * stats may be NULL. */
+ * stats may be NULL.  results and accept are each on their own side; blocks, params and stats are host memory. */
 int kgv_replay_window(kgv_ctx* ctx, kgv_utxo_table* t, const kgv_tx_batch* batch, const kgv_replay_block* blocks, size_t n_blocks,
                       const kgv_params* params, kgv_tx_result* results, uint8_t* accept, kgv_replay_stats* stats);
 
@@ -573,7 +579,7 @@ int kgv_replay_muhash(kgv_ctx* ctx, const uint32_t* group_first_block, size_t n_
  * add = its removal keys and entries) - on a plain table or on a view layer.
  * Output arrays (ranges included) are all host or all device memory; device entry arrays must be 8-byte aligned.  With rem_keys36 == NULL only
  * the sizes (*n_rem_out, *n_add_out, *bytes_out) and `ranges` (may be NULL) are returned; arrays smaller than that give KGV_ERR_NOMEM with the
- * sizes and ranges still set.  Valid under the same conditions as kgv_replay_muhash: either may come first and either may be repeated.  Without a
+ * sizes and ranges still set.  The three counts are host memory.  Valid under the same conditions as kgv_replay_muhash: either may come first and either may be repeated.  Without a
  * current window or with groups that do not tile it: KGV_ERR_ARG. */
 typedef struct {
   uint64_t first_remove, n_remove;  /* rows of rem_keys36 / rem_entries that belong to the group */
@@ -763,11 +769,13 @@ int kgv_replay_verify_chain(kgv_ctx* ctx, const uint32_t* group_first_block, siz
  * A MuHash is the pair (numerator, denominator) of residues modulo 2^3072 - 1103717 (lib.rs:32-35); every function
  * here reads / writes them as 384 little-endian bytes each, CANONICAL (in [0, p)) on output.  The reference's
  * transient non-canonical representations (u3072.rs:49-57) are unobservable through serialize()/finalize().
- * Pointers of one call are all host or all device.
+ * Sides of the arrays (Conventions): the two outputs of kgv_muhash_elements / kgv_muhash_txs share one; every other array of
+ * these calls is on its own side, except as stated below.
  * ------------------------------------------------------------------------------------------------ */
 /* MuHash::add_element / remove_element (lib.rs:61-74) for n byte strings data[offsets[i] .. offsets[i+1]):
  * remove[i] != 0 multiplies the element into the denominator, else into the numerator (remove may be NULL).
- * Starts from the empty MuHash (1, 1). */
+ * Starts from the empty MuHash (1, 1).  With host offsets, data and remove may each be host or device memory; with device
+ * offsets (whose end, the data's size, the library cannot read) data and remove must be device memory too (KGV_ERR_ARG otherwise). */
 int kgv_muhash_elements(kgv_ctx* ctx, const uint8_t* data, const uint64_t* offsets, const uint8_t* remove, size_t n, uint8_t* numerator384,
                         uint8_t* denominator384);
 /* The MuHash half of validate_transactions_with_muhash_in_parallel (utxo_validation.rs:282-309): MuHash::from_transaction
@@ -775,18 +783,19 @@ int kgv_muhash_elements(kgv_ctx* ctx, const uint8_t* data, const uint64_t* offse
  * from batch->entries, or from `table` when it is non-NULL (call BEFORE kgv_utxo_apply_accepted erases them). */
 int kgv_muhash_txs(kgv_ctx* ctx, kgv_utxo_table* table, const kgv_tx_batch* batch, const uint8_t* accept, uint64_t pov_daa_score,
                    uint8_t* numerator384, uint8_t* denominator384);
-/* MuHash::combine (lib.rs:91-96): a.numerator *= b.numerator, a.denominator *= b.denominator */
+/* MuHash::combine (lib.rs:91-96): a.numerator *= b.numerator, a.denominator *= b.denominator.  Each of the four arrays on its own side. */
 int kgv_muhash_combine(kgv_ctx* ctx, uint8_t* numerator_a, uint8_t* denominator_a, const uint8_t* numerator_b, const uint8_t* denominator_b);
 /* MuHash::serialize + finalize (lib.rs:98-115): serialized = numerator / denominator (0 has inverse 0, u3072.rs:163-165),
  * hash = BLAKE2b-256 keyed "MuHashFinalize".  Sequential by nature (one modular inversion: 3 072 dependent squarings);
- * the reference calls it once per chain block outside the parallel section.  serialized384 may be NULL. */
+ * the reference calls it once per chain block outside the parallel section.  serialized384 may be NULL.  Each array on its own side. */
 int kgv_muhash_finalize(kgv_ctx* ctx, const uint8_t* numerator384, const uint8_t* denominator384, uint8_t* serialized384, uint8_t* hash32);
 /* n finalizations at once: hashes32[i] = MuHash{numerator_i, denominator_i}.finalize() (lib.rs:98-115) for NONZERO denominators (every
  * denominator_i mod p != 0, which a product of hashed elements always is); value i sits pitch_bytes after value i - 1 (384 for plain
  * arrays, 768 for (numerator || denominator) records).  ONE modular inversion for the whole batch (Montgomery's trick over prefix /
  * suffix products built by parallel scans): a chain block's commitment costs five multiplications instead of 3 072 squarings.
- * serialized384 (n * 384 contiguous bytes) may be NULL.  KGV_ERR_ARG unless pitch_bytes >= 384 is a multiple of 16 and, for device
- * pointers, numerators384 is 16-byte aligned and hashes32 / serialized384 are 4-byte aligned. */
+ * serialized384 (n * 384 contiguous bytes) may be NULL.  numerators384, denominators384 and hashes32 share one side, serialized384 is on
+ * its own.  KGV_ERR_ARG unless pitch_bytes >= 384 is a multiple of 16 and, for device pointers, numerators384 is 16-byte aligned and
+ * hashes32 / serialized384 are 4-byte aligned. */
 int kgv_muhash_finalize_batch(kgv_ctx* ctx, const uint8_t* numerators384, const uint8_t* denominators384, size_t n, size_t pitch_bytes, uint8_t* serialized384,
                               uint8_t* hashes32);
 /* The MuHash::combine chain of a replay (utxo_validation.rs:144): values768 holds n (numerator || denominator) records; on return record i is
@@ -863,7 +872,7 @@ int kgv_check_scripts_host(kgv_ctx* ctx, const kgv_tx_batch* batch, const uint32
  * transaction runs on the GPU; the signature checks its scripts reach are hashed and verified in rounds (through the attached SigCache,
  * if any), one synchronisation per round, at most 256 rounds.  This is what a caller runs after kgv_validate_populated reports
  * KGV_TX_NEEDS_HOST_VM for a device-resident batch; the table-backed calls (kgv_validate_txs, kgv_validate_mempool_txs,
- * kgv_replay_window) run the same engine internally. */
+ * kgv_replay_window) run the same engine internally.  An index >= batch->n_txs is refused (KGV_ERR_ARG) whichever side tx_indices is on. */
 int kgv_check_scripts(kgv_ctx* ctx, const kgv_tx_batch* batch, const uint32_t* tx_indices, size_t n, kgv_tx_result* results);
 
 /* ------------------------------------------------------------------------------------------------
@@ -890,8 +899,9 @@ int kgv_utxo_rows_decode(const uint8_t* key_rows, const uint64_t* key_off, const
  * Header k's expanded parents_by_level (ParentsByLevel::expanded_iter, consensus/core/src/header.rs:45-47) is given by
  * level_len[levels_off .. levels_off + n_levels), the number of parents at each level, and the parent hashes of all its levels
  * in order at parents32 + 32 * parents_off.  Headers may share or reorder arena ranges.  An arena range that leaves level_len
- * (n_level_entries entries) or parents32 (n_parents hashes) gives KGV_ERR_ARG, and so does a device headers / parents32 pointer
- * that is not 8-byte aligned.  The pointers of one call are all host or all device.  Both calls end with a synchronise of the
+ * (n_level_entries entries) or parents32 (n_parents hashes) gives KGV_ERR_ARG whichever side the arrays are on.  The arrays of one
+ * call (headers, parents32, level_len and the outputs) are all host or all device; as device memory, headers, parents32 and the
+ * outputs must be 8-byte aligned and level_len 4-byte aligned (KGV_ERR_ARG otherwise).  The rules struct is host memory.  Both calls end with a synchronise of the
  * context's stream, also on device pointers: the arena ranges are checked by the kernels, and the call reports what they found.
  * ------------------------------------------------------------------------------------------------ */
 typedef struct {
@@ -939,14 +949,16 @@ typedef struct {
 } kgv_header_result; /* 24 bytes, written for every header whatever its status */
 
 /* hashing::header::hash (consensus/core/src/hashing/header.rs:33-35) into hash32 and hash_override_nonce_time(h, 0, 0) (:7-30), the
- * pre-PoW hash, into pre_pow32; either output may be NULL. */
+ * pre-PoW hash, into pre_pow32; either output may be NULL.  headers, parents32, level_len and the outputs share one side; as device
+ * memory, headers, parents32 and the outputs must be 8-byte aligned and level_len 4-byte aligned (KGV_ERR_ARG otherwise). */
 int kgv_hash_headers(kgv_ctx* ctx, const kgv_header* headers, size_t n, const uint8_t* parents32, size_t n_parents, const uint32_t* level_len,
                      size_t n_level_entries, uint8_t* hash32, uint8_t* pre_pow32);
 /* validate_header_in_isolation (pre_ghostdag_validation.rs:17-24,30-68,102-106) of every header: version, timestamp against now_ms +
  * tolerance, level-0 parent count, origin parent, then the proof of work (kaspa_pow::State::check_pow, consensus/pow/src/lib.rs:23-53:
  * pre-PoW hash, matrix from xoshiro256++ redrawn until its rank is 64, cSHAKE256 "ProofOfWorkHash", kHeavyHash, pow <= the compact
  * target).  With KGV_HEADER_SKIP_POW an insufficient proof of work is not an error; the level is still computed.  results: one record
- * per header.  hash32 (the block hash) and pow32 (the PoW value, 32 bytes little-endian) may be NULL. */
+ * per header.  hash32 (the block hash) and pow32 (the PoW value, 32 bytes little-endian) may be NULL.  Sides and alignment as for
+ * kgv_hash_headers; rules is host memory. */
 int kgv_validate_headers_in_isolation(kgv_ctx* ctx, const kgv_header* headers, size_t n, const uint8_t* parents32, size_t n_parents, const uint32_t* level_len,
                                       size_t n_level_entries, const kgv_header_rules* rules, kgv_header_result* results, uint8_t* hash32, uint8_t* pow32);
 

@@ -196,7 +196,8 @@ extern "C" int kgv_validate_block_bodies(kgv_ctx* ctx, const kgv_tx_batch* batch
   if (flags & ~KGV_BODY_ISOLATION_ONLY) { ctx->err = "kgv_validate_block_bodies: unknown flags"; return KGV_ERR_ARG; }
   if (n_blocks == 0) return KGV_OK;
   if (!batch || !block_first_tx || !headers || !rules || !body_rules || !results) { ctx->err = "null argument"; return KGV_ERR_ARG; }
-  if (kgv_ptr_is_device(block_first_tx)) { ctx->err = "block offsets must be a host array"; return KGV_ERR_ARG; }
+  for (const auto& [what, p] : {std::pair<const char*, const void*>{"block_first_tx", block_first_tx}, {"rules", rules}, {"body_rules", body_rules}})
+    if (int rc = kgv_host_only(ctx, "kgv_validate_block_bodies", what, p)) return rc;
   if (batch->n_txs > 0xFFFFFFFFull || batch->n_inputs > 0x7FFFFFFFull) { ctx->err = "kgv_validate_block_bodies: more than 2^32 - 1 transactions or 2^31 - 1 inputs"; return KGV_ERR_ARG; }
   if (block_first_tx[0] != 0 || block_first_tx[n_blocks] != batch->n_txs) { ctx->err = "block offsets must start at 0 and end at the number of transactions"; return KGV_ERR_ARG; }
   for (uint32_t b = 0; b < n_blocks; b++)

@@ -227,7 +227,8 @@ extern "C" int kgv_replay_verify_chain(kgv_ctx* ctx, const uint32_t* group_first
     return KGV_ERR_ARG;
   }
   const auto& L = ctx->last_replay;
-  if (kgv_ptr_is_device(group_first_block)) { ctx->err = "group offsets must be a host array"; return KGV_ERR_ARG; }
+  for (const auto& [what, p] : {std::pair<const char*, const void*>{"group_first_block", group_first_block}, {"rules", rules}, {"body_rules", body_rules}})
+    if (int rc = kgv_host_only(ctx, "kgv_replay_verify_chain", what, p)) return rc;
   if (group_first_block[0] != 0 || group_first_block[n_groups] != L.n_blocks) { ctx->err = "groups must tile the blocks of the window"; return KGV_ERR_ARG; }
   // group layout: the selected parent (ACCEPT_COINBASE), the rest of the mergeset, the chain block's body (VERIFY_ONLY) last and only there
   uint32_t max_ids = 0;

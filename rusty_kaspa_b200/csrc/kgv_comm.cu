@@ -283,6 +283,7 @@ extern "C" int kgv_shard_allgather(kgv_ctx* ctx, kgv_comm* c, const uint8_t* loc
   if (!ctx || !c || c->ctx != ctx) return KGV_ERR_ARG;
   std::lock_guard<std::recursive_mutex> g(ctx->mu);
   if (!local_shard || !all_shards) { ctx->err = "null buffer"; return KGV_ERR_ARG; }
+  if (!kgv_ptr_is_device(local_shard) || !kgv_ptr_is_device(all_shards)) { ctx->err = "kgv_shard_allgather: local_shard and all_shards must be device memory"; return KGV_ERR_ARG; }
   if (!c->nccl) { ctx->err = "communicator was created without the NCCL transport"; return KGV_ERR_NCCL; }
   CK(cudaSetDevice(ctx->device));
   int rc = nccl().AllGather(local_shard, all_shards, nbytes_per_rank, /*ncclUint8*/ 1, c->nccl, ctx->stream);
@@ -301,7 +302,8 @@ static int p2p_ready(kgv_ctx* ctx, kgv_comm* c, size_t nbytes) {
 extern "C" int kgv_shard_publish_bitmap(kgv_ctx* ctx, kgv_comm* c, const uint8_t* status, size_t n, uint64_t* epoch_out) {
   if (!ctx || !c || c->ctx != ctx) return KGV_ERR_ARG;
   std::lock_guard<std::recursive_mutex> g(ctx->mu);
-  if ((n && !status) || !kgv_ptr_is_device(status)) { ctx->err = "status must be a device array"; return KGV_ERR_ARG; }
+  if ((n && !status) || !kgv_ptr_is_device(status)) { ctx->err = "kgv_shard_publish_bitmap: status must be device memory"; return KGV_ERR_ARG; }
+  if (int rc = kgv_host_only(ctx, "kgv_shard_publish_bitmap", "epoch_out", epoch_out)) return rc;
   int rc = p2p_ready(ctx, c, 4 * ((n + 31) / 32));
   if (rc) return rc;
   CK(cudaSetDevice(ctx->device));
@@ -320,7 +322,8 @@ extern "C" int kgv_shard_publish_bitmap(kgv_ctx* ctx, kgv_comm* c, const uint8_t
 extern "C" int kgv_shard_publish_bytes(kgv_ctx* ctx, kgv_comm* c, const uint8_t* src, size_t nbytes, uint64_t* epoch_out) {
   if (!ctx || !c || c->ctx != ctx) return KGV_ERR_ARG;
   std::lock_guard<std::recursive_mutex> g(ctx->mu);
-  if ((nbytes && !src) || (nbytes && !kgv_ptr_is_device(src))) { ctx->err = "src must be a device array"; return KGV_ERR_ARG; }
+  if ((nbytes && !src) || (nbytes && !kgv_ptr_is_device(src))) { ctx->err = "kgv_shard_publish_bytes: src must be device memory"; return KGV_ERR_ARG; }
+  if (int rc = kgv_host_only(ctx, "kgv_shard_publish_bytes", "epoch_out", epoch_out)) return rc;
   int rc = p2p_ready(ctx, c, nbytes);
   if (rc) return rc;
   CK(cudaSetDevice(ctx->device));
@@ -340,7 +343,7 @@ extern "C" int kgv_shard_wait(kgv_ctx* ctx, kgv_comm* c, uint64_t epoch, size_t 
   std::lock_guard<std::recursive_mutex> g(ctx->mu);
   int rc = p2p_ready(ctx, c, nbytes_per_rank);
   if (rc) return rc;
-  if (all_shards && !kgv_ptr_is_device(all_shards)) { ctx->err = "all_shards must be a device array"; return KGV_ERR_ARG; }
+  if (all_shards && !kgv_ptr_is_device(all_shards)) { ctx->err = "kgv_shard_wait: all_shards must be device memory"; return KGV_ERR_ARG; }
   CK(cudaSetDevice(ctx->device));
   k_wait_epoch<<<1, 32, 0, ctx->stream>>>((const unsigned long long*)(c->local + p2p_flags_off(c)), c->n_ranks, epoch);
   CK(cudaGetLastError());

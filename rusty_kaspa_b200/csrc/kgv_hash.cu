@@ -388,7 +388,7 @@ extern "C" int kgv_merkle_roots(kgv_ctx* ctx, const uint8_t* hashes32, const uin
   std::lock_guard<std::recursive_mutex> g(ctx->mu);
   if (n_groups == 0) return KGV_OK;
   if (!first || !roots32) { ctx->err = "null argument"; return KGV_ERR_ARG; }
-  if (kgv_ptr_is_device(first)) { ctx->err = "merkle group offsets must be a host array"; return KGV_ERR_ARG; }
+  if (int rc = kgv_host_only(ctx, "kgv_merkle_roots", "first", first)) return rc;
   const size_t n_total = first[n_groups];
   if (n_total && !hashes32) { ctx->err = "null argument"; return KGV_ERR_ARG; }
   CK(cudaSetDevice(ctx->device));
@@ -413,7 +413,7 @@ extern "C" int kgv_block_hash_merkle_roots(kgv_ctx* ctx, const kgv_tx_batch* bat
   std::lock_guard<std::recursive_mutex> g(ctx->mu);
   if (n_blocks == 0) return KGV_OK;
   if (!batch || !block_first_tx || !roots32) { ctx->err = "null argument"; return KGV_ERR_ARG; }
-  if (kgv_ptr_is_device(block_first_tx)) { ctx->err = "block offsets must be a host array"; return KGV_ERR_ARG; }
+  if (int rc = kgv_host_only(ctx, "kgv_block_hash_merkle_roots", "block_first_tx", block_first_tx)) return rc;
   if (block_first_tx[n_blocks] > batch->n_txs) { ctx->err = "block offsets exceed the batch"; return KGV_ERR_ARG; }
   CK(cudaSetDevice(ctx->device));
   kgv_dev_batch d;
@@ -460,7 +460,7 @@ extern "C" int kgv_block_set_checks(kgv_ctx* ctx, const kgv_tx_batch* batch, con
   std::lock_guard<std::recursive_mutex> g(ctx->mu);
   if (n_blocks == 0) return KGV_OK;
   if (!batch || !block_first_tx || !out) { ctx->err = "null argument"; return KGV_ERR_ARG; }
-  if (kgv_ptr_is_device(block_first_tx)) { ctx->err = "block offsets must be a host array"; return KGV_ERR_ARG; }
+  if (int rc = kgv_host_only(ctx, "kgv_block_set_checks", "block_first_tx", block_first_tx)) return rc;
   if (batch->n_txs > 0x7FFFFFFFull || batch->n_inputs > 0x7FFFFFFFull) { ctx->err = "kgv_block_set_checks: more than 2^31 - 1 transactions or inputs"; return KGV_ERR_ARG; }
   for (uint32_t b = 0; b < n_blocks; b++)
     if (block_first_tx[b + 1] < block_first_tx[b] || block_first_tx[b + 1] > batch->n_txs) { ctx->err = "block offsets not monotone / out of range"; return KGV_ERR_ARG; }

@@ -197,13 +197,14 @@ static int check_headers(kgv_ctx* ctx, kgv_io& io, const char* call, const kgv_h
   bool dev;
   if (int rc = io.one_side(call, {headers, n_parents ? parents32 : nullptr, n_level_entries ? level_len : nullptr, o0, o1, o2}, &dev)) return rc;
   const uintptr_t a = (uintptr_t)headers | (uintptr_t)parents32 | (uintptr_t)o0 | (uintptr_t)o1 | (uintptr_t)o2;
-  return dev && (a & 7) ? fail_arg(ctx, "device headers, parents32 and outputs must be 8-byte aligned") : KGV_OK;
+  if (dev && ((a & 7) || (n_level_entries && ((uintptr_t)level_len & 3)))) return fail_arg(ctx, (std::string(call) + ": device headers, parents32 and outputs must be 8-byte aligned, level_len 4-byte aligned").c_str());
+  return KGV_OK;
 }
 
 // waits for the call and reports an arena range outside the arena
-static int finish_headers(kgv_ctx* ctx, kgv_io& io, const unsigned int& bad) {
+static int finish_headers(kgv_ctx* ctx, kgv_io& io, const char* call, const unsigned int& bad) {
   if (int rc = io.finish()) return rc;
-  return bad ? fail_arg(ctx, "a header's levels_off / parents_off range leaves the arena") : KGV_OK;
+  return bad ? fail_arg(ctx, (std::string(call) + ": a header's levels_off / parents_off range leaves the arena").c_str()) : KGV_OK;
 }
 
 // hashing::header::hash and hash_override_nonce_time(h, 0, 0) (consensus/core/src/hashing/header.rs:7-35)
@@ -228,7 +229,7 @@ extern "C" int kgv_hash_headers(kgv_ctx* ctx, const kgv_header* headers, size_t 
   k_header_hash<<<(unsigned)((n + HDR_HASH_THREADS - 1) / HDR_HASH_THREADS), HDR_HASH_THREADS, 0, ctx->stream>>>(ar, dh, dp);
   CK(cudaGetLastError());
   ctx->launches++;
-  return finish_headers(ctx, io, bad);
+  return finish_headers(ctx, io, "kgv_hash_headers", bad);
 }
 
 // validate_header_in_isolation (pre_ghostdag_validation.rs:17-24) with check_pow_and_calc_block_level (:102-106) for every header
@@ -239,7 +240,7 @@ extern "C" int kgv_validate_headers_in_isolation(kgv_ctx* ctx, const kgv_header*
   std::lock_guard<std::recursive_mutex> g(ctx->mu);
   if (n == 0) return KGV_OK;
   if (!headers || !rules || !results) return fail_arg(ctx, "null argument");
-  if (kgv_ptr_is_device(rules)) return fail_arg(ctx, "rules must be a host struct");
+  if (int rc = kgv_host_only(ctx, "kgv_validate_headers_in_isolation", "rules", rules)) return rc;
   if (rules->max_block_level > 255) return fail_arg(ctx, "max_block_level is a BlockLevel (u8)");
   if (n > 0x7FFFFFFFull) return fail_arg(ctx, "at most 2^31 - 1 headers per call");
   CK(cudaSetDevice(ctx->device));
@@ -258,7 +259,7 @@ extern "C" int kgv_validate_headers_in_isolation(kgv_ctx* ctx, const kgv_header*
   k_header_validate<<<(unsigned)n, HDR_CTA, 0, ctx->stream>>>(a);
   CK(cudaGetLastError());
   ctx->launches++;
-  return finish_headers(ctx, io, bad);
+  return finish_headers(ctx, io, "kgv_validate_headers_in_isolation", bad);
 }
 
 extern "C" int kgv_debug_pow_matrix(kgv_ctx* ctx, int op, const uint8_t* in, size_t n, uint8_t* out) {

@@ -92,6 +92,9 @@ struct kgv_ctx {
 };
 
 int kgv_ptr_is_device(const void* p);
+// KGV_ERR_ARG, with a message naming `call` and the argument `what`, when p is device memory (an argument the call reads on the host);
+// KGV_OK for host memory and for null
+int kgv_host_only(kgv_ctx* ctx, const char* call, const char* what, const void* p);
 // cudaMalloc; under memory pressure the parked buffers are given back (after synchronising the context's streams) and the allocation retried
 int kgv_malloc(kgv_ctx* ctx, void** p, size_t bytes);
 int kgv_reserve(kgv_ctx* ctx, uint8_t** buf, size_t* cap, size_t need);
@@ -123,7 +126,10 @@ static inline int fail_arg(kgv_ctx* ctx, const char* m) {
 // enqueues a copy of a device result into a caller's array of either kind.  finish() copies the host outputs back and synchronises
 // ctx->stream once, only when some output (of out or copy_out) is host memory; device outputs leave the call enqueued.
 //
-// Which arrays of a call must share a side (one_side), which are fixed to one, and which are each on their own side (the rest):
+// Which arrays of a call must share a side (one_side), which are fixed to one, and which are each on their own side (the rest).  A host-only
+// argument given as device memory, or a device-only one given as host memory, is refused (KGV_ERR_ARG, naming the call and the argument)
+// before it is first read.  tests/test_gpu_residency.py restates this table; its side matrix (every allowed and every forbidden
+// assignment) covers the calls listed in BUILDERS there, and the host-only / device-only refusals of the others.
 //   kgv_schnorr_verify, kgv_ecdsa_verify     pk, msg, sig, status together (large host batches upload in chunks on the side stream)
 //   kgv_status_to_bitmap                     status, bitmap together
 //   kgv_tx_ids, kgv_tx_hashes                out32 on its own side
@@ -131,30 +137,41 @@ static inline int fail_arg(kgv_ctx* ctx, const char* m) {
 //   kgv_merkle_roots                         hashes32 and roots32 together; first on the host
 //   kgv_block_hash_merkle_roots,
 //   kgv_block_set_checks                     the output on its own side; block_first_tx on the host
-//   kgv_muhash_elements                      numerator384 and denominator384 together; data and remove staged with host offsets
-//   kgv_muhash_combine, kgv_muhash_finalize  the inputs copied into the workspace from the side of the first; each output on its own side
-//   kgv_muhash_finalize_batch                numerators384, denominators384, hashes32 together; device arrays aligned
+//   kgv_muhash_elements                      numerator384 and denominator384 together; with host offsets data and remove each on their own
+//                                            side, with device offsets data and remove on the device too
+//   kgv_muhash_combine, kgv_muhash_finalize  every input and every output on its own side
+//   kgv_muhash_finalize_batch                numerators384, denominators384, hashes32 together, serialized384 on its own side; device
+//                                            numerators384 16-byte aligned, device hashes32 and serialized384 4-byte aligned
 //   kgv_muhash_prefix_combine                values768 (updated in place, 16-byte aligned on the device) and init768 each on their own side
 //   kgv_muhash_txs                           numerator384 and denominator384 together; accept on its own side
-//   kgv_utxo_lookup / _apply_diff / _export  each array on its own side
-//   kgv_utxo_import_chunk                    numerator384 on the host; keys36, entries, bytes each on their own side
+//   kgv_utxo_muhash                          numerator384 on its own side
+//   kgv_utxo_lookup / _apply_diff            each array on its own side
+//   kgv_utxo_export                          each array on its own side; n_out and bytes_out on the host
+//   kgv_utxo_count, kgv_utxo_digest,
+//   kgv_utxo_stats, kgv_sigcache_counters    the results on the host
+//   kgv_utxo_import_chunk                    numerator384 on the host; keys36, entries, bytes each on their own side (the script ranges of
+//                                            entries are checked on either side)
 //   kgv_utxo_apply_accepted                  accept on its own side (a host accept: the call waits for the table)
-//   kgv_validate_txs, kgv_validate_populated results on its own side, independent of the batch
-//   kgv_validate_mempool_txs*                results, batch->txs, args, storage_mass, entries_out, scripts_out, masses, detail together
+//   kgv_validate_txs, kgv_validate_populated results on its own side, independent of the batch; params on the host
+//   kgv_validate_mempool_txs*                results, batch->txs, args, storage_mass, entries_out, scripts_out, masses, detail together;
+//                                            params, rules, policy and scripts_used on the host
 //   kgv_validate_txs_in_isolation            results, batch->txs, masses together; rules on the host
 //   kgv_check_txs_standard_in_isolation      results, batch->txs, masses, detail together; the policy on the host
 //   kgv_check_txs_standard_in_context        results, batch->txs, masses, storage_mass, fee, detail together; the policy on the host
 //   kgv_outputs_dust                         is_dust and batch->outputs together
-//   kgv_validate_block_bodies                results, batch->txs, headers, masses, roots32 together; block_first_tx and the rules on the host
+//   kgv_validate_block_bodies                results, batch->txs, headers, masses, roots32 together; block_first_tx, rules and body_rules on
+//                                            the host
 //   kgv_hash_headers, kgv_validate_headers_in_isolation
-//                                            headers, parents32, level_len and the outputs together, device arrays 8-byte aligned; rules on the host
-//   kgv_replay_window                        blocks on the host; results and accept each on their own side
+//                                            headers, parents32, level_len and the outputs together, device arrays 8-byte aligned (level_len
+//                                            4-byte); rules on the host
+//   kgv_replay_window                        blocks, params and stats on the host; results and accept each on their own side
 //   kgv_replay_muhash                        values768 on its own side; group_first_block on the host
-//   kgv_replay_diffs                         the output arrays together (ranges alone when counting); group_first_block on the host
+//   kgv_replay_diffs                         the output arrays together (ranges alone when counting), device entry arrays 8-byte aligned;
+//                                            group_first_block and the counts on the host
 //   kgv_replay_verify_chain                  results, headers, merged_flags, init768, block_fees, multisets768 together (inputs are copied into
-//                                            the call's own workspace from either side); group_first_block on the host
-//   kgv_check_scripts                        tx_indices and results each on their own side
-//   the kgv_comm.cu calls                    device arrays only
+//                                            the call's own workspace from either side); group_first_block, rules and body_rules on the host
+//   kgv_check_scripts                        tx_indices and results each on their own side (the indices are range-checked on either side)
+//   the kgv_comm.cu calls                    device arrays only; epoch_out on the host
 // The arrays of a transaction batch are staged by kgv_batch_to_device (d_batch, or a prefetch slot) and must all be of one kind.
 class kgv_io {
  public:

@@ -156,6 +156,7 @@ extern "C" int kgv_validate_txs_in_isolation(kgv_ctx* ctx, const kgv_tx_batch* b
   std::lock_guard<std::recursive_mutex> g(ctx->mu);
   if (!batch || !rules || (batch->n_txs && !results)) { ctx->err = "null argument"; return KGV_ERR_ARG; }
   if (flags & ~KGV_ISOLATION_SKIP_FINALITY) { ctx->err = "kgv_validate_txs_in_isolation: unknown flags"; return KGV_ERR_ARG; }
+  if (int rc = kgv_host_only(ctx, "kgv_validate_txs_in_isolation", "rules", rules)) return rc;
   if (batch->n_txs == 0) return KGV_OK;
   if (batch->n_txs > 0xFFFFFFFFull) { ctx->err = "kgv_validate_txs_in_isolation: more than 2^32 - 1 transactions"; return KGV_ERR_ARG; }
   CK(cudaSetDevice(ctx->device));

@@ -427,6 +427,12 @@ int kgv_ptr_is_device(const void* p) {
   return a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged;
 }
 
+int kgv_host_only(kgv_ctx* ctx, const char* call, const char* what, const void* p) {
+  if (!p || !kgv_ptr_is_device(p)) return KGV_OK;
+  ctx->err = std::string(call) + ": " + what + " must be host memory";
+  return KGV_ERR_ARG;
+}
+
 bool kgv_io::is_device(const void* p) {
   for (int i = 0; i < n_side; i++)
     if (side[i].p == p) return side[i].dev;

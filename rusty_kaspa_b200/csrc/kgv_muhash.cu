@@ -149,6 +149,8 @@ extern "C" int kgv_muhash_elements(kgv_ctx* ctx, const uint8_t* data, const uint
   kgv_io io(ctx);
   int rc = io.one_side("kgv_muhash_elements", {numerator384, denominator384});
   if (rc) return rc;
+  // device offsets cannot be read here to size a host copy of the data: then data and remove are device arrays too
+  if (n && io.is_device(offsets) && (rc = io.one_side("kgv_muhash_elements", {offsets, data, remove}))) return rc;
   CK(cudaSetDevice(ctx->device));
   uint32_t *e_den = nullptr, *e_num = nullptr;
   if ((rc = kgv_mu_reserve(ctx, n, n, &e_den, &e_num))) return rc;
@@ -216,11 +218,9 @@ extern "C" int kgv_muhash_combine(kgv_ctx* ctx, uint8_t* num_a, uint8_t* den_a, 
   if (rc) return rc;
   uint8_t* w = ctx->d_mu;
   kgv_io io(ctx);
-  const cudaMemcpyKind in = io.is_device(num_a) ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
-  CK(cudaMemcpyAsync(w, num_a, 384, in, ctx->stream));
-  CK(cudaMemcpyAsync(w + 384, den_a, 384, in, ctx->stream));
-  CK(cudaMemcpyAsync(w + 768, num_b, 384, in, ctx->stream));
-  CK(cudaMemcpyAsync(w + 1152, den_b, 384, in, ctx->stream));
+  const uint8_t* ins[4] = {num_a, den_a, num_b, den_b};  // each copied in from its own side
+  for (int i = 0; i < 4; i++)
+    CK(cudaMemcpyAsync(w + 384 * i, ins[i], 384, io.is_device(ins[i]) ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, ctx->stream));
   k_muhash_combine<<<1, 32, 0, ctx->stream>>>((uint32_t*)w);
   CK(cudaGetLastError());
   ctx->launches++;
@@ -282,9 +282,9 @@ extern "C" int kgv_muhash_finalize(kgv_ctx* ctx, const uint8_t* numerator384, co
   uint8_t* w = ctx->d_mu;
   uint8_t* o = w + 4096;
   kgv_io io(ctx);
-  const bool dev = io.is_device(numerator384);
-  CK(cudaMemcpyAsync(w, numerator384, 384, dev ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, ctx->stream));
-  CK(cudaMemcpyAsync(w + 384, denominator384, 384, dev ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, ctx->stream));
+  const uint8_t* ins[2] = {numerator384, denominator384};  // each copied in from its own side
+  for (int i = 0; i < 2; i++)
+    CK(cudaMemcpyAsync(w + 384 * i, ins[i], 384, io.is_device(ins[i]) ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, ctx->stream));
   k_muhash_finalize<<<1, 32, 0, ctx->stream>>>((uint32_t*)w, (uint32_t*)o);
   CK(cudaGetLastError());
   ctx->launches++;
@@ -506,8 +506,9 @@ extern "C" int kgv_muhash_finalize_batch(kgv_ctx* ctx, const uint8_t* numerators
   kgv_io io(ctx);
   bool dev;
   if (int rc = io.one_side("kgv_muhash_finalize_batch", {numerators384, denominators384, hashes32}, &dev)) return rc;
-  if (dev && (((uintptr_t)numerators384 & 15) || ((uintptr_t)hashes32 & 3) || ((uintptr_t)serialized384 & 3))) {
-    ctx->err = "device numerators384 must be 16-byte aligned, hashes32 and serialized384 4-byte aligned";
+  // serialized384 is on its own side: its alignment is checked when it is device memory, whatever the side of the others
+  if ((dev && (((uintptr_t)numerators384 & 15) || ((uintptr_t)hashes32 & 3))) || (serialized384 && io.is_device(serialized384) && ((uintptr_t)serialized384 & 3))) {
+    ctx->err = "kgv_muhash_finalize_batch: device numerators384 must be 16-byte aligned, hashes32 and serialized384 4-byte aligned";
     return KGV_ERR_ARG;
   }
   // a strided host array is one contiguous span (the pitch interleaves numerators and denominators of MuHash records)
@@ -550,7 +551,7 @@ extern "C" int kgv_muhash_prefix_combine(kgv_ctx* ctx, const uint8_t* init768, u
   if (!values768) { ctx->err = "null argument"; return KGV_ERR_ARG; }
   CK(cudaSetDevice(ctx->device));
   kgv_io io(ctx);
-  if (io.is_device(values768) && ((uintptr_t)values768 & 15)) { ctx->err = "device values768 must be 16-byte aligned"; return KGV_ERR_ARG; }  // scanned in place with 16-byte loads
+  if (io.is_device(values768) && ((uintptr_t)values768 & 15)) { ctx->err = "kgv_muhash_prefix_combine: device values768 must be 16-byte aligned"; return KGV_ERR_ARG; }  // scanned in place with 16-byte loads
   const size_t o_init = kgv_mu_prefix_scratch(n);
   int rc = kgv_reserve(ctx, &ctx->d_mu, &ctx->d_mu_cap, al256(o_init + 768));
   if (rc) return rc;

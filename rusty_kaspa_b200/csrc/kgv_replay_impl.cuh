@@ -586,6 +586,8 @@ extern "C" int kgv_replay_window(kgv_ctx* ctx, kgv_utxo_table* table, const kgv_
   if (!ctx || !table) return KGV_ERR_ARG;
   std::lock_guard<std::recursive_mutex> g(ctx->mu);
   if (!batch || !prm || (n_blocks && !blocks) || (batch->n_txs && !results)) { ctx->err = "null argument"; return KGV_ERR_ARG; }
+  for (const auto& [what, p] : {std::pair<const char*, const void*>{"blocks", blocks}, {"params", prm}, {"stats", stats}})
+    if (int rc = kgv_host_only(ctx, "kgv_replay_window", what, p)) return rc;
   if (stats) { stats->n_accepted = 0; stats->n_sig_checks = 0; stats->n_host_vm = 0; stats->pre_check_ms = 0; stats->in_order_ms = 0; }
   if (batch->n_txs == 0 || n_blocks == 0) return KGV_OK;
   if (n_blocks > 0xFFFFFFFFull) { ctx->err = "too many blocks"; return KGV_ERR_ARG; }
@@ -594,10 +596,10 @@ extern "C" int kgv_replay_window(kgv_ctx* ctx, kgv_utxo_table* table, const kgv_
   {
     uint64_t at = 0;
     for (size_t i = 0; i < n_blocks; i++) {
-      if (blocks[i].first_tx != at || blocks[i].flags > 7u) { ctx->err = "replay blocks must tile the batch contiguously, in order, with known flags"; return KGV_ERR_ARG; }
+      if (blocks[i].first_tx != at || blocks[i].flags > 7u) { ctx->err = "kgv_replay_window: replay blocks must tile the batch contiguously, in order, with known flags"; return KGV_ERR_ARG; }
       at += blocks[i].n_txs;
     }
-    if (at != batch->n_txs) { ctx->err = "replay blocks do not cover the batch"; return KGV_ERR_ARG; }
+    if (at != batch->n_txs) { ctx->err = "kgv_replay_window: replay blocks do not cover the batch"; return KGV_ERR_ARG; }
   }
   CK(cudaSetDevice(ctx->device));
   int rc = utxo_reserve(ctx, table, batch->n_outputs + (table->base ? batch->n_inputs : 0), batch->n_bytes + 8 * (uint64_t)batch->n_outputs);
@@ -914,6 +916,7 @@ extern "C" int kgv_replay_muhash(kgv_ctx* ctx, const uint32_t* group_first_block
   if (!group_first_block || !values768) { ctx->err = "null argument"; return KGV_ERR_ARG; }
   if (!ctx->last_replay.valid) { ctx->err = "kgv_replay_muhash must directly follow the kgv_replay_window call it refers to"; return KGV_ERR_ARG; }
   const auto& L = ctx->last_replay;
+  if (int rc = kgv_host_only(ctx, "kgv_replay_muhash", "group_first_block", group_first_block)) return rc;
   if (group_first_block[0] != 0 || group_first_block[n_groups] != L.n_blocks) { ctx->err = "groups must tile the blocks of the window"; return KGV_ERR_ARG; }
   for (size_t i = 0; i < n_groups; i++) if (group_first_block[i] > group_first_block[i + 1]) { ctx->err = "group offsets not monotone"; return KGV_ERR_ARG; }
   CK(cudaSetDevice(ctx->device));
@@ -1109,7 +1112,9 @@ extern "C" int kgv_replay_diffs(kgv_ctx* ctx, const uint32_t* group_first_block,
   if (!group_first_block || n_groups == 0) { ctx->err = "kgv_replay_diffs: no groups"; return KGV_ERR_ARG; }
   if (!ctx->last_replay.valid) { ctx->err = "kgv_replay_diffs refers to the last kgv_replay_window call, and none is current (another batch was staged or the table rehashed since)"; return KGV_ERR_ARG; }
   const auto& L = ctx->last_replay;
-  if (kgv_ptr_is_device(group_first_block)) { ctx->err = "group offsets must be a host array"; return KGV_ERR_ARG; }
+  for (const auto& [what, p] : {std::pair<const char*, const void*>{"group_first_block", group_first_block}, {"n_rem_out", n_rem_out}, {"n_add_out", n_add_out},
+                                {"bytes_out", bytes_out}})
+    if (int rc = kgv_host_only(ctx, "kgv_replay_diffs", what, p)) return rc;
   if (group_first_block[0] != 0 || group_first_block[n_groups] != L.n_blocks) { ctx->err = "groups must tile the blocks of the window"; return KGV_ERR_ARG; }
   for (size_t i = 0; i < n_groups; i++) if (group_first_block[i] > group_first_block[i + 1]) { ctx->err = "group offsets not monotone"; return KGV_ERR_ARG; }
   const bool counting = !rem_keys36;
@@ -1118,7 +1123,7 @@ extern "C" int kgv_replay_diffs(kgv_ctx* ctx, const uint32_t* group_first_block,
     if (!rem_entries || !add_keys36 || !add_entries || (bytes_cap && !bytes)) { ctx->err = "null buffer"; return KGV_ERR_ARG; }
     bool dev;
     if (int rc = io.one_side("kgv_replay_diffs", {rem_keys36, rem_entries, add_keys36, add_entries, bytes, ranges}, &dev)) return rc;
-    if (dev && (((uintptr_t)rem_entries | (uintptr_t)add_entries) & 7)) { ctx->err = "entry arrays must be 8-byte aligned"; return KGV_ERR_ARG; }
+    if (dev && (((uintptr_t)rem_entries | (uintptr_t)add_entries) & 7)) { ctx->err = "kgv_replay_diffs: device entry arrays must be 8-byte aligned"; return KGV_ERR_ARG; }
   }
   CK(cudaSetDevice(ctx->device));
   cudaStream_t st = ctx->stream;

@@ -309,9 +309,17 @@ extern "C" int kgv_check_scripts(kgv_ctx* ctx, const kgv_tx_batch* batch, const 
   if (n == 0) return KGV_OK;
   CK(cudaSetDevice(ctx->device));
   kgv_io io(ctx);
-  if (!io.is_device(tx_indices))
-    for (size_t i = 0; i < n; i++)
-      if (tx_indices[i] >= batch->n_txs) { ctx->err = "kgv_check_scripts: a transaction index is out of range"; return KGV_ERR_ARG; }
+  // the indices are range-checked here whatever their side: device indices are read through a host copy
+  std::vector<uint32_t> idx_host;
+  const uint32_t* hidx = tx_indices;
+  if (io.is_device(tx_indices)) {
+    idx_host.resize(n);
+    CK(cudaMemcpyAsync(idx_host.data(), tx_indices, n * 4, cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+    hidx = idx_host.data();
+  }
+  for (size_t i = 0; i < n; i++)
+    if (hidx[i] >= batch->n_txs) { ctx->err = "kgv_check_scripts: a transaction index is out of range"; return KGV_ERR_ARG; }
   kgv_dev_batch d;
   int rc = kgv_batch_to_device(ctx, batch, &d, true);
   if (rc) return rc;

@@ -178,6 +178,8 @@ extern "C" int kgv_sigcache_clear(kgv_ctx* ctx, kgv_sigcache* c) {
 extern "C" int kgv_sigcache_counters(kgv_ctx* ctx, kgv_sigcache* c, uint64_t* hits, uint64_t* inserts, uint64_t* lookups, uint64_t* evictions) {
   if (!ctx || !c) return KGV_ERR_ARG;
   std::lock_guard<std::recursive_mutex> g(ctx->mu);
+  for (const auto& [what, p] : {std::pair<const char*, const void*>{"hits", hits}, {"inserts", inserts}, {"lookups", lookups}, {"evictions", evictions}})
+    if (int rc = kgv_host_only(ctx, "kgv_sigcache_counters", what, p)) return rc;
   CK(cudaSetDevice(ctx->device));
   unsigned long long h[4];
   CK(cudaMemcpyAsync(h, c->counters, sizeof h, cudaMemcpyDeviceToHost, ctx->stream));

@@ -203,6 +203,7 @@ extern "C" int kgv_check_txs_standard_in_isolation(kgv_ctx* ctx, const kgv_tx_ba
   if (!ctx) return KGV_ERR_ARG;
   std::lock_guard<std::recursive_mutex> g(ctx->mu);
   if (!batch || !policy || (batch->n_txs && (!results || !masses))) { ctx->err = "null argument"; return KGV_ERR_ARG; }
+  if (int rc = kgv_host_only(ctx, "kgv_check_txs_standard_in_isolation", "policy", policy)) return rc;
   if (batch->n_txs == 0) return KGV_OK;
   if (batch->n_txs > 0xFFFFFFFFull) { ctx->err = "kgv_check_txs_standard_in_isolation: more than 2^32 - 1 transactions"; return KGV_ERR_ARG; }
   CK(cudaSetDevice(ctx->device));
@@ -228,6 +229,7 @@ extern "C" int kgv_check_txs_standard_in_context(kgv_ctx* ctx, const kgv_tx_batc
   if (!ctx) return KGV_ERR_ARG;
   std::lock_guard<std::recursive_mutex> g(ctx->mu);
   if (!batch || !policy || (batch->n_txs && (!results || !masses || !storage_mass || !fee))) { ctx->err = "null argument"; return KGV_ERR_ARG; }
+  if (int rc = kgv_host_only(ctx, "kgv_check_txs_standard_in_context", "policy", policy)) return rc;
   if (batch->n_txs == 0) return KGV_OK;
   if (batch->n_inputs && !batch->entries) { ctx->err = "kgv_check_txs_standard_in_context: batch->entries is required"; return KGV_ERR_ARG; }
   if (batch->n_txs > 0xFFFFFFFFull) { ctx->err = "kgv_check_txs_standard_in_context: more than 2^32 - 1 transactions"; return KGV_ERR_ARG; }

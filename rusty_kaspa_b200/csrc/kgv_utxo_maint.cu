@@ -280,6 +280,7 @@ int utxo_reserve(kgv_ctx* ctx, kgv_utxo_table* t, uint64_t m, uint64_t b) {
 extern "C" int kgv_utxo_stats(kgv_ctx* ctx, kgv_utxo_table* t, kgv_utxo_table_stats* out) {
   if (!ctx || !t || !out) return KGV_ERR_ARG;
   std::lock_guard<std::recursive_mutex> g(ctx->mu);
+  if (int rc = kgv_host_only(ctx, "kgv_utxo_stats", "out", out)) return rc;
   CK(cudaSetDevice(ctx->device));
   return utxo_scan(ctx, t, out, nullptr);
 }

@@ -640,7 +640,7 @@ extern "C" int kgv_utxo_lookup(kgv_ctx* ctx, kgv_utxo_table* t, const uint8_t* k
   uint8_t *ds, *df;
   io.in(keys36, n * 36, &dk);
   io.out(entries, n * sizeof(kgv_utxo_entry), &de);
-  io.out(script_stride ? scripts_out : nullptr, n * (size_t)script_stride, &ds);
+  io.inout(script_stride ? scripts_out : nullptr, n * (size_t)script_stride, &ds);  // only each script's bytes are written: the rest stays the caller's
   io.out(found, n, &df);
   if (int rc = io.stage()) return rc;
   k_utxo_lookup<<<nblk(n, 128), 128, 0, ctx->stream>>>(view_of(t), dk, n, de, ds, script_stride, df);
@@ -685,6 +685,8 @@ extern "C" int kgv_utxo_export(kgv_ctx* ctx, kgv_utxo_table* t, uint8_t* keys36,
   if (t->base) { ctx->err = "export is defined on plain tables: commit the view first"; return KGV_ERR_ARG; }
   const bool counting = !keys36;
   if (!counting && (!entries || (bytes_cap && !bytes))) { ctx->err = "null buffer"; return KGV_ERR_ARG; }
+  for (const auto& [what, p] : {std::pair<const char*, const void*>{"n_out", n_out}, {"bytes_out", bytes_out}})
+    if (int rc = kgv_host_only(ctx, "kgv_utxo_export", what, p)) return rc;
   CK(cudaSetDevice(ctx->device));
   kgv_io io(ctx);
   uint8_t *dk = nullptr, *db = bytes;
@@ -721,11 +723,20 @@ extern "C" int kgv_utxo_import_chunk(kgv_ctx* ctx, kgv_utxo_table* t, const uint
   if (!numerator384) { ctx->err = "null argument"; return KGV_ERR_ARG; }
   if (n == 0) return KGV_OK;
   if (!keys36 || !entries || (n_bytes && !bytes)) { ctx->err = "null buffer"; return KGV_ERR_ARG; }
-  if (kgv_ptr_is_device(numerator384)) { ctx->err = "numerator384 is a host value"; return KGV_ERR_ARG; }
+  if (int rc = kgv_host_only(ctx, "kgv_utxo_import_chunk", "numerator384", numerator384)) return rc;
   kgv_io io(ctx);
-  for (size_t i = 0; !io.is_device(keys36) && i < n; i++)
-    if ((uint64_t)entries[i].script_off + entries[i].script_len > n_bytes) { ctx->err = "entry script outside the byte arena"; return KGV_ERR_ARG; }
   CK(cudaSetDevice(ctx->device));
+  // the script ranges are checked here whatever the side of entries: device entries are read through a host copy
+  std::vector<kgv_utxo_entry> entries_host;
+  const kgv_utxo_entry* he = entries;
+  if (io.is_device(entries)) {
+    entries_host.resize(n);
+    CK(cudaMemcpyAsync(entries_host.data(), entries, n * sizeof(kgv_utxo_entry), cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+    he = entries_host.data();
+  }
+  for (size_t i = 0; i < n; i++)
+    if ((uint64_t)he[i].script_off + he[i].script_len > n_bytes) { ctx->err = "kgv_utxo_import_chunk: entry script outside the byte arena"; return KGV_ERR_ARG; }
   // one upload serves the insert and the multiset
   const uint8_t *dk, *db;
   const kgv_utxo_entry* de;
@@ -756,6 +767,7 @@ extern "C" int kgv_utxo_import_chunk(kgv_ctx* ctx, kgv_utxo_table* t, const uint
 extern "C" int kgv_utxo_count(kgv_ctx* ctx, kgv_utxo_table* t, uint64_t* count) {
   if (!ctx || !t || !count) return KGV_ERR_ARG;
   std::lock_guard<std::recursive_mutex> g(ctx->mu);
+  if (int rc = kgv_host_only(ctx, "kgv_utxo_count", "count", count)) return rc;
   if (t->base) { ctx->err = "count / digest / MuHash are defined on plain tables: commit the view first"; return KGV_ERR_ARG; }
   CK(cudaSetDevice(ctx->device));
   unsigned long long c[4];
@@ -769,6 +781,7 @@ extern "C" int kgv_utxo_count(kgv_ctx* ctx, kgv_utxo_table* t, uint64_t* count) 
 extern "C" int kgv_utxo_digest(kgv_ctx* ctx, kgv_utxo_table* t, uint8_t out32[32]) {
   if (!ctx || !t || !out32) return KGV_ERR_ARG;
   std::lock_guard<std::recursive_mutex> g(ctx->mu);
+  if (int rc = kgv_host_only(ctx, "kgv_utxo_digest", "out32", out32)) return rc;
   if (t->base) { ctx->err = "count / digest / MuHash are defined on plain tables: commit the view first"; return KGV_ERR_ARG; }
   CK(cudaSetDevice(ctx->device));
   unsigned long long* acc = t->counters + 8;
@@ -950,6 +963,7 @@ static int validate_core(kgv_ctx* ctx, kgv_utxo_table* table, const kgv_tx_batch
                          kgv_tx_result* results) {
   if (!batch || !prm || (batch->n_txs && !results)) { ctx->err = "null argument"; return KGV_ERR_ARG; }
   if (flags > KGV_FLAGS_SCRIPTS_ONLY) { ctx->err = "unknown validation flags"; return KGV_ERR_ARG; }
+  if (int rc = kgv_host_only(ctx, table ? "kgv_validate_txs" : "kgv_validate_populated", "params", prm)) return rc;
   if (batch->n_txs == 0) return KGV_OK;
   CK(cudaSetDevice(ctx->device));
   kgv_dev_batch d;
@@ -1021,6 +1035,10 @@ struct MempoolIso {
 static int mempool_core(kgv_ctx* ctx, kgv_utxo_table* t, const kgv_tx_batch* batch, uint64_t virtual_daa_score, const kgv_params* prm,
                         const kgv_mempool_tx_args* args, kgv_tx_result* results, uint64_t* storage_mass, kgv_utxo_entry* entries_out,
                         uint8_t* scripts_out, size_t scripts_cap, size_t* scripts_used, const MempoolIso* iso) {
+  const char* call = !iso ? "kgv_validate_mempool_txs" : iso->policy ? "kgv_validate_mempool_txs_with_policy" : "kgv_validate_mempool_txs_in_parallel";
+  for (const auto& [what, p] : {std::pair<const char*, const void*>{"params", prm}, {"rules", iso ? iso->rules : nullptr},
+                                {"policy", iso ? iso->policy : nullptr}, {"scripts_used", scripts_used}})
+    if (int rc = kgv_host_only(ctx, call, what, p)) return rc;
   if (scripts_used) *scripts_used = 0;
   if (!batch || !prm || (batch->n_txs && (!results || !storage_mass)) || (entries_out && scripts_cap && !scripts_out) || (iso && !iso->rules)) {
     ctx->err = "null argument";
@@ -1031,7 +1049,7 @@ static int mempool_core(kgv_ctx* ctx, kgv_utxo_table* t, const kgv_tx_batch* bat
   CK(cudaSetDevice(ctx->device));
   kgv_io io(ctx);
   bool dev;
-  if (int rc = io.one_side("kgv_validate_mempool_txs", {results, batch->txs, args, storage_mass, entries_out, scripts_cap ? scripts_out : nullptr,
+  if (int rc = io.one_side(call, {results, batch->txs, args, storage_mass, entries_out, scripts_cap ? scripts_out : nullptr,
                                                         iso ? iso->masses : nullptr, iso ? iso->detail : nullptr}, &dev))
     return rc;
   kgv_dev_batch d;
