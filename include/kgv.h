@@ -484,6 +484,39 @@ int kgv_sigcache_counters(kgv_ctx* ctx, kgv_sigcache* cache, uint64_t* hits, uin
 int kgv_set_sigcache(kgv_ctx* ctx, kgv_sigcache* cache /* NULL: detach */);
 
 /* ------------------------------------------------------------------------------------------------
+ * Key cache: prepared public keys kept across verify launches.  The reference has no counterpart: libsecp256k1 lifts the key and builds
+ * its tables on every secp256k1_schnorrsig_verify / secp256k1_ecdsa_verify, and so does every verify launch here without it (per-launch
+ * records only in launches of more items than the device's resident threads whose keys repeat).
+ * An opt-in, device-resident table of comb-form key records (8 320 bytes each, about 8.4 KB per key with its slot: 2^16 keys take about
+ * 550 MB), owned by one context and off by default.  While it is on, every verify launch of that context (the verify entry points,
+ * validation, mempool validation, replay windows, the device script engine, the SigCache's misses) looks its keys up: a stored key's
+ * signatures run the 30-doubling joint comb ladder from the stored record whatever the launch's size, the other keys are verified as
+ * without the cache and stored for the next launch (a launch of at most one item per resident thread stores them after its verification,
+ * off the call's path; a larger one stores them first when the per-launch rule would prepare records and the cache holds them all, else it
+ * runs as without the cache).  Verdicts never depend on it.  Where it loses: a launch that stores many new keys (cold large launches build
+ * a full record per key, even for keys used a few times), and the call right after one that stored keys (it waits for that insert);
+ * DESIGN.md §5 has the numbers.
+ * - kgv_keycache_create gives the context its cache, on: one partition per item kind with its own capacity in keys (0: that kind is not
+ *   cached), Schnorr keyed by x, ECDSA by tag || x (02 and 03 of one x are two keys).  Both 0, one above KGV_KEYCACHE_MAX_KEYS, or a context
+ *   that has a cache is KGV_ERR_ARG; memory that cannot be allocated KGV_ERR_NOMEM.  The cache belongs to the context alone (another
+ *   context's inserts could replace a record one of its launches reads); under sharding each rank's context has its own.
+ * - Eight-way sets; a full set replaces its least recently used key, never one that the current launch of the kind reads.
+ * - kgv_set_keycache turns the lookups off (0) and on again, keeping the records; kgv_keycache_clear empties both partitions and zeroes
+ *   their counters; kgv_keycache_destroy waits for the cache's work and frees it (KGV_OK without one; kgv_destroy does the same).
+ * - kgv_keycache_counter: a counter of the partition ecdsa selects (0 without a cache, that partition, or with a bad argument; UINT64_MAX
+ *   when the device fails): KGV_KEYCACHE_LOOKUPS items looked up, KGV_KEYCACHE_HITS items verified from a stored record (a large launch
+ *   the cache does not take counts its lookups, no hits), KGV_KEYCACHE_INSERTS keys stored, KGV_KEYCACHE_EVICTIONS stored keys replaced;
+ *   stored keys = inserts - evictions.
+ * ------------------------------------------------------------------------------------------------ */
+#define KGV_KEYCACHE_MAX_KEYS (1ull << 20) /* per kind: about 8.8 GB of records */
+enum { KGV_KEYCACHE_LOOKUPS = 0, KGV_KEYCACHE_HITS = 1, KGV_KEYCACHE_INSERTS = 2, KGV_KEYCACHE_EVICTIONS = 3 };
+int kgv_keycache_create(kgv_ctx* ctx, uint64_t schnorr_keys, uint64_t ecdsa_keys);
+int kgv_keycache_destroy(kgv_ctx* ctx);
+int kgv_keycache_clear(kgv_ctx* ctx);
+uint64_t kgv_keycache_counter(kgv_ctx* ctx, int ecdsa, int which);
+int kgv_set_keycache(kgv_ctx* ctx, int enabled);
+
+/* ------------------------------------------------------------------------------------------------
  * Multi-GPU (SURVEY.md §8b kgv_shard_allgather, §8e): signature batches shard across GPUs as contiguous ranges, one context (and
  * normally one process) per GPU; the only exchange step of the path is "every rank ends up with every shard's verdicts".
  * The reference has no counterpart (rayon on one host, utxo_validation.rs:269-277).

@@ -440,6 +440,27 @@ class SigCache {
   kgv_sigcache* h_ = nullptr;
 };
 
+// ---- prepared public keys kept across verify launches (kgv_keycache; no counterpart in the reference): the context's own ----
+class KeyCache {
+ public:
+  KeyCache(Context& c, uint64_t schnorr_keys, uint64_t ecdsa_keys) : c_(c) { c_.check(kgv_keycache_create(c_.get(), schnorr_keys, ecdsa_keys)); }
+  ~KeyCache() { kgv_keycache_destroy(c_.get()); }
+  KeyCache(const KeyCache&) = delete;
+  KeyCache& operator=(const KeyCache&) = delete;
+  void enable(bool on) { c_.check(kgv_set_keycache(c_.get(), on)); }
+  void clear() { c_.check(kgv_keycache_clear(c_.get())); }
+  struct Counters { uint64_t lookups, hits, inserts, evictions; };
+  Counters counters(bool ecdsa) {
+    Counters k{kgv_keycache_counter(c_.get(), ecdsa, KGV_KEYCACHE_LOOKUPS), kgv_keycache_counter(c_.get(), ecdsa, KGV_KEYCACHE_HITS),
+               kgv_keycache_counter(c_.get(), ecdsa, KGV_KEYCACHE_INSERTS), kgv_keycache_counter(c_.get(), ecdsa, KGV_KEYCACHE_EVICTIONS)};
+    if (k.lookups == UINT64_MAX || k.hits == UINT64_MAX || k.inserts == UINT64_MAX || k.evictions == UINT64_MAX) c_.check(KGV_ERR_CUDA);
+    return k;
+  }
+
+ private:
+  Context& c_;
+};
+
 // ---- transaction validation in UTXO context ----
 struct Params {
   uint64_t coinbase_maturity = 100, storage_mass_parameter = 1000000000000ull, max_sompi = 2900000000000000000ull;  // consensus/core/src/config/params.rs, constants.rs

@@ -63,6 +63,11 @@ SYMBOLS = [
     ("kgv_sigcache_clear", _c.c_int, [_c.c_void_p, _c.c_void_p]),
     ("kgv_sigcache_counters", _c.c_int, [_c.c_void_p, _c.c_void_p, _c.POINTER(_c.c_uint64), _c.POINTER(_c.c_uint64), _c.POINTER(_c.c_uint64), _c.POINTER(_c.c_uint64)]),
     ("kgv_set_sigcache", _c.c_int, [_c.c_void_p, _c.c_void_p]),
+    ("kgv_keycache_create", _c.c_int, [_c.c_void_p, _c.c_uint64, _c.c_uint64]),
+    ("kgv_keycache_destroy", _c.c_int, [_c.c_void_p]),
+    ("kgv_keycache_clear", _c.c_int, [_c.c_void_p]),
+    ("kgv_keycache_counter", _c.c_uint64, [_c.c_void_p, _c.c_int, _c.c_int]),
+    ("kgv_set_keycache", _c.c_int, [_c.c_void_p, _c.c_int]),
     ("kgv_comm_unique_id", _c.c_int, [_u8p]),
     ("kgv_comm_create", _c.c_int, [_c.c_void_p, _c.c_int, _c.c_int, _u8p, _c.c_size_t, _c.POINTER(_c.c_void_p)]),
     ("kgv_comm_destroy", None, [_c.c_void_p]),

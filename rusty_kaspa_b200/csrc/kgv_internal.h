@@ -75,6 +75,7 @@ struct kgv_ctx {
     std::vector<uint32_t> block_flags, block_n_txs;  // host copy of the blocks' flags and sizes
   } last_replay;
   struct kgv_sigcache* sigcache = nullptr;  // kgv_set_sigcache: verdicts of the validation calls are looked up / remembered here
+  struct kgv_keycache* keycache = nullptr;  // kgv_set_keycache: comb key records kept across the verify launches (kgv_lib.cu)
   struct kgv_comm* shard_comm = nullptr;  // kgv_set_sharding: signature checks of the validation calls are split over its ranks
   std::vector<uint8_t*> parked;  // outgrown per-call buffers, released when the caller synchronises / destroys the context (kgv_reserve)
   uint64_t launches = 0;

@@ -132,8 +132,11 @@ struct KeyCacheView {
   const uint32_t* item_slot;  // item -> table slot (only the items the launch verifies are set)
   const uint32_t* recs;       // records, KGV_KR_WORDS or KGV_JR_WORDS words each
   const uint32_t* n_rec;      // distinct keys of the launch; nullptr: no key cache
-  // the key source of item i: its record and the launch's form, or no record (the launch makes none)
+  const uint32_t* item_rec;   // a launch over stored keys only (kgv_keycache): item -> its stored comb record + 1; nullptr: not such a launch
+  const uint32_t* kc_recs;    // that cache's records, KGV_JR_WORDS words each
+  // the key source of item i: its stored record, else its record and the launch's form, or no record (the launch makes none)
   __device__ __forceinline__ KeySrc key_of(size_t i, size_t n) const {
+    if (item_rec) return KeySrc{kc_recs + (size_t)(item_rec[i] - 1) * KGV_JR_WORDS, true};
     const int f = n_rec ? key_form(*n_rec, n) : KGV_KEYS_INLINE;
     if (f == KGV_KEYS_INLINE) return KeySrc{nullptr, false};
     const bool comb = f == KGV_KEYS_COMB;
@@ -164,14 +167,17 @@ __device__ __forceinline__ uint64_t key_hash(const uint32_t* w, int nw) {
 
 // One thread per item: find or claim the key's slot; a claimed slot gets the next record index.  Whichever item's atomicCAS claims the
 // slot becomes its representative: the record depends on the key bytes alone.  Once the launch has more keys than records allow (key_form),
-// the remaining items stop (the verify kernels then take the inline key path for every item).
-template <bool ALIGNED, bool ECDSA>
+// the remaining items stop (the verify kernels then take the inline key path for every item).  ALL: every distinct key gets a
+// representative until there are more than `limit` (the device key cache's misses, kgv_keycache below).
+template <bool ALIGNED, bool ECDSA, bool ALL = false>
 __global__ void __launch_bounds__(256) k_key_dedup(const uint8_t* __restrict__ pk, size_t n_arg, const uint32_t* __restrict__ index,
                                                    const uint32_t* __restrict__ n_dev, KeySlot* __restrict__ table, uint32_t mask,
-                                                   uint32_t* __restrict__ item_slot, uint32_t* __restrict__ rec_rep, uint32_t* n_rec) {
+                                                   uint32_t* __restrict__ item_slot, uint32_t* __restrict__ rec_rep, uint32_t* n_rec,
+                                                   uint32_t limit) {
   const size_t n = n_dev ? (size_t)*n_dev : n_arg;
   const size_t t = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (t >= n || key_form(*(volatile uint32_t*)n_rec, n) == KGV_KEYS_INLINE) return;
+  if (t >= n) return;
+  if (ALL ? *(volatile uint32_t*)n_rec > limit : key_form(*(volatile uint32_t*)n_rec, n) == KGV_KEYS_INLINE) return;
   const size_t i = index ? index[t] : t;
   const int nw = ECDSA ? 9 : 8;
   uint32_t w[9];
@@ -200,7 +206,7 @@ __global__ void __launch_bounds__(256) k_key_dedup(const uint8_t* __restrict__ p
   base = __shfl_sync(act, base, leader);
   if (won) {
     const uint32_t r = base + __popc(ball & ((1u << lane) - 1));
-    if (key_form(r + 1, n) != KGV_KEYS_INLINE) {  // (r < the host's bound of the rec_rep / record arrays)
+    if (ALL || key_form(r + 1, n) != KGV_KEYS_INLINE) {  // (r < the host's bound of the rec_rep / record arrays)
       rec_rep[r] = (uint32_t)i;
       table[s].rec = r + 1;
     }
@@ -227,6 +233,151 @@ __global__ void __launch_bounds__(KGV_BLOCK, KGV_PREP_BLOCKS_PER_SM) k_key_prepa
   key_words<false, ECDSA>(w, pk, rec_rep[r]);
   if (f == KGV_KEYS_COMB) key_joint_record_build(recs + (size_t)r * KGV_JR_WORDS, ECDSA ? w[8] : 2u, w);
   else key_rec_build(recs + (size_t)r * KGV_KR_WORDS, ECDSA ? w[8] : 2u, w);
+}
+
+// ---- device key cache (kgv_keycache, include/kgv.h): comb-form key records kept across the verify launches of one context ----
+// One partition per item kind.  Set-associative: a key's set is its key_hash modulo the number of sets; slot s of the partition owns
+// record s (KGV_JR_WORDS words), so there is no allocator and a lookup reads one set.  stamp: the partition launch that last used the
+// slot (0: empty).  A launch stamps the slots it reads, and an insert only takes a slot stamped by an earlier launch (the empty one first,
+// then the least recently used), so no launch evicts a record it reads.
+#define KGV_KC_WAYS 8
+struct KcSet {
+  uint32_t stamp[KGV_KC_WAYS];
+  uint32_t fp[KGV_KC_WAYS];           // high half of the key's hash
+  uint32_t key[KGV_KC_WAYS][9];       // key_words: x, and the tag for ECDSA
+};
+struct KcPart {
+  KcSet* sets;
+  uint32_t* recs;
+  uint32_t n_sets;                     // 0: the kind has no partition
+  unsigned long long* ctr;             // [0] lookups, [1] hits, [2] inserts, [3] evictions
+};
+// per-launch words of a partition's scratch
+enum { KC_N = 0, KC_ORD_HIT = 1, KC_N_MISS = 2, KC_DIST_HIT = 3, KC_TAKE = 4, KC_N_REC = 5, KC_ORD_MISS = 6 };
+enum { KC_COUNT = 1, KC_ORDER = 2, KC_GATED = 4 };
+
+// position of this lane among the active lanes with pred, after the earlier warps' (one atomic per warp)
+__device__ __forceinline__ uint32_t warp_claim(uint32_t* ctr, bool pred) {
+  const uint32_t act = __activemask(), ball = __ballot_sync(act, pred);
+  const int lane = threadIdx.x & 31, leader = __ffs(act) - 1;
+  uint32_t base = 0;
+  if (lane == leader && ball) base = atomicAdd(ctr, (uint32_t)__popc(ball));
+  return __shfl_sync(act, base, leader) + __popc(ball & ((1u << lane) - 1));
+}
+__device__ __forceinline__ void warp_count(unsigned long long* ctr, bool pred) {
+  const uint32_t act = __activemask(), ball = __ballot_sync(act, pred);
+  if ((threadIdx.x & 31) == __ffs(act) - 1 && ball) atomicAdd(ctr, (unsigned long long)__popc(ball));
+}
+
+// One thread per item the launch verifies (index and n_dev honoured): probes the key's set.
+//   KC_COUNT  counts lookups, stamps the hit slots (KC_DIST_HIT: distinct slots hit), and appends each miss's key bytes to miss_keys
+//             (KC_N_MISS of them), the input of the insert
+//   KC_ORDER  counts the hits (items the stored-record launch verifies); item_rec[i] = slot + 1 of a hit; the hits listed in order
+//             (KC_ORD_HIT of them), the misses in miss_order (KC_ORD_MISS):
+//             two verify launches, each of one key form.  (A block never mixes forms: ecmult_joint's staging and the inline path's
+//             odd-multiples table lay the threads' shared memory out differently, so a thread of one form overwrites its neighbours'.)
+//   KC_GATED  the launch's insert did not take it (KC_TAKE == 0): every item in miss_order, as given
+template <bool ALIGNED, bool ECDSA>
+__global__ void __launch_bounds__(256) k_kc_lookup(const uint8_t* __restrict__ pk, size_t n_arg, const uint32_t* __restrict__ index,
+                                                   const uint32_t* __restrict__ n_dev, KcPart p, uint32_t stamp, int mode, uint32_t* hdr,
+                                                   uint32_t* __restrict__ item_rec, uint32_t* __restrict__ order, uint32_t* __restrict__ miss_order,
+                                                   uint8_t* __restrict__ miss_keys) {
+  const size_t n = n_dev ? (size_t)*n_dev : n_arg;
+  const size_t t = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (t == 0 && (mode & KC_COUNT)) hdr[KC_N] = (uint32_t)n;
+  const bool taken = !(mode & KC_GATED) || *(volatile uint32_t*)(hdr + KC_TAKE);
+  if (t == 0 && !taken) hdr[KC_ORD_MISS] = (uint32_t)n;
+  if (t >= n) return;
+  const size_t i = index ? index[t] : t;
+  if (!taken) {
+    miss_order[t] = (uint32_t)i;
+    return;
+  }
+  const int nw = ECDSA ? 9 : 8;
+  uint32_t w[9];
+  key_words<ALIGNED, ECDSA>(w, pk, i);
+  const uint64_t h = key_hash(w, nw);
+  const uint32_t set = (uint32_t)(h % p.n_sets), fp = (uint32_t)(h >> 32);
+  KcSet* s = p.sets + set;
+  int way = -1;
+  for (int k = 0; k < KGV_KC_WAYS && way < 0; k++) {
+    if (!s->stamp[k] || s->fp[k] != fp) continue;
+    bool eq = true;
+    for (int q = 0; q < nw; q++) eq = eq && s->key[k][q] == w[q];
+    if (eq) way = k;
+  }
+  const bool hit = way >= 0;
+  if (mode & KC_COUNT) {
+    if (hit && atomicExch(&s->stamp[way], stamp) != stamp) atomicAdd(&hdr[KC_DIST_HIT], 1u);
+    const uint32_t k = warp_claim(&hdr[KC_N_MISS], !hit);
+    if (!hit) {
+      const int len = ECDSA ? 33 : 32;
+      for (int b = 0; b < len; b++) miss_keys[(size_t)len * k + b] = pk[(size_t)len * i + b];
+    }
+    warp_count(&p.ctr[0], true);
+  }
+  if (mode & KC_ORDER) {
+    warp_count(&p.ctr[1], hit);
+    if (hit) item_rec[i] = set * KGV_KC_WAYS + way + 1;
+    const uint32_t h_pos = warp_claim(&hdr[KC_ORD_HIT], hit), m_pos = warp_claim(&hdr[KC_ORD_MISS], !hit);
+    if (hit) order[h_pos] = (uint32_t)i;
+    else miss_order[m_pos] = (uint32_t)i;
+  }
+}
+
+// One thread per distinct miss (k_key_dedup<.., true> over miss_keys): takes a slot of the key's set stamped by an earlier launch (empty
+// first, then the least recently used), writes the key and builds its comb-form record there (key_joint_record_build).  A set whose every
+// slot this launch uses keeps its records; the key is then not stored.  gate (launches of more items than resident threads): insert only
+// when today's rule would make records for the launch's keys (key_form over the distinct hits and misses) or nothing is missing, and the
+// partition holds them all; KC_TAKE = 1 then, and the verify reads every record from the partition.
+template <bool ECDSA>
+__global__ void __launch_bounds__(KGV_BLOCK, KGV_PREP_BLOCKS_PER_SM) k_kc_insert(KcPart p, const uint8_t* __restrict__ miss_keys,
+                                                                            const uint32_t* __restrict__ rec_rep, uint32_t* hdr, uint32_t stamp, bool gate) {
+  const uint32_t n_rec = hdr[KC_N_REC];
+  if (gate) {
+    const uint32_t keys = hdr[KC_DIST_HIT] + n_rec;
+    const bool take = keys <= p.n_sets * KGV_KC_WAYS && (n_rec == 0 || key_form(keys, hdr[KC_N]) != KGV_KEYS_INLINE);
+    if (!take) return;
+    if (blockIdx.x == 0 && threadIdx.x == 0) hdr[KC_TAKE] = 1;
+  }
+  const uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
+  if (r >= n_rec) return;
+  const int nw = ECDSA ? 9 : 8;
+  uint32_t w[9];
+  key_words<false, ECDSA>(w, miss_keys, rec_rep[r]);
+  const uint64_t h = key_hash(w, nw);
+  const uint32_t set = (uint32_t)(h % p.n_sets);
+  KcSet* s = p.sets + set;
+  int way;
+  uint32_t old;
+  for (;;) {
+    way = -1;
+    old = stamp;
+    for (int k = 0; k < KGV_KC_WAYS; k++) {
+      const uint32_t v = *(volatile uint32_t*)&s->stamp[k];
+      if (v < old) { old = v; way = k; }
+    }
+    if (way < 0) return;
+    if (atomicCAS(&s->stamp[way], old, stamp) == old) break;
+  }
+  s->fp[way] = (uint32_t)(h >> 32);
+  for (int q = 0; q < nw; q++) s->key[way][q] = w[q];
+  atomicAdd(&p.ctr[2], 1ull);
+  if (old) atomicAdd(&p.ctr[3], 1ull);
+  key_joint_record_build(p.recs + (size_t)(set * KGV_KC_WAYS + way) * KGV_JR_WORDS, ECDSA ? w[8] : 2u, w);
+}
+
+// a launch the device key cache took makes no per-launch records: its n_rec is set past every bound, so k_key_dedup and k_key_prepare
+// return at once and key_of finds no per-launch record
+__global__ void k_kc_stand_down(const uint32_t* hdr, uint32_t* n_rec) {
+  if (hdr[KC_TAKE]) *n_rec = 0xFFFFFFFFu;
+}
+// stamps wrap after 2^32 launches of a partition: every used slot restarts at 1
+__global__ void k_kc_restamp(KcSet* sets, uint32_t n_sets) {
+  const uint32_t s = blockIdx.x * blockDim.x + threadIdx.x;
+  if (s >= n_sets) return;
+  for (int k = 0; k < KGV_KC_WAYS; k++)
+    if (sets[s].stamp[k]) sets[s].stamp[k] = 1;
 }
 
 // Each thread verifies KGV_ITEMS consecutive-stride items (i = tid + j * total_threads: coalesced) and shares
@@ -497,6 +648,9 @@ int kgv_io::finish() {
   return KGV_OK;
 }
 
+static void keycache_quiesce(kgv_keycache* kc);
+static void keycache_free(kgv_ctx* ctx);
+
 // Per-call device buffers only ever grow.  The outgrown allocation is NOT freed on the spot: cudaFree synchronises the whole device, which
 // stalls every other stream and deadlocks a process that drives several contexts of one device whose kernels wait for each other (the
 // peer-exchange wait kernels of kgv_comm.cu); cudaMallocAsync was tried and blocks in the same situation (measured).  Outgrown buffers are
@@ -509,6 +663,7 @@ int kgv_malloc(kgv_ctx* ctx, void** p, size_t bytes) {
     (void)cudaGetLastError();
     cudaStreamSynchronize(ctx->stream);
     cudaStreamSynchronize(ctx->aux_stream);
+    if (ctx->keycache) keycache_quiesce(ctx->keycache);  // a deferred key insert may still read a parked scratch
     for (uint8_t* q : ctx->parked) cudaFree(q);
     ctx->parked.clear();
     e = cudaMalloc(p, bytes);
@@ -576,6 +731,7 @@ extern "C" void kgv_destroy(kgv_ctx* ctx) {
   for (auto& P : ctx->prefetch) if (P.worker.joinable()) P.worker.join();
   if (ctx->copy_stream) cudaStreamSynchronize(ctx->copy_stream);
   cudaStreamSynchronize(ctx->stream);
+  keycache_free(ctx);
   if (ctx->gtab) cudaFree(ctx->gtab);
   for (uint8_t* b : {ctx->d_io, ctx->d_in, ctx->d_out, ctx->d_batch, ctx->prefetch[0].buf, ctx->prefetch[1].buf, ctx->d_scratch, ctx->d_mu, ctx->d_work, ctx->d_replay, ctx->d_keys[0], ctx->d_keys[1]})
     if (b) cudaFree(b);
@@ -614,6 +770,7 @@ extern "C" int kgv_synchronize(kgv_ctx* ctx) {
   if (!ctx->parked.empty()) {  // the caller declared the context idle: outgrown buffers can go
     CK(cudaStreamSynchronize(ctx->aux_stream));
     if (ctx->copy_stream) CK(cudaStreamSynchronize(ctx->copy_stream));
+    if (ctx->keycache) keycache_quiesce(ctx->keycache);
     for (uint8_t* p : ctx->parked) cudaFree(p);
     ctx->parked.clear();
   }
@@ -629,8 +786,9 @@ extern "C" uint64_t kgv_launch_count(const kgv_ctx* ctx) { return ctx ? ctx->lau
 // Enqueues the per-launch key cache of a verify launch on st: table cleared, k_key_dedup, k_key_prepare.  Sized from the host's n (an
 // upper bound of *n_dev when given); the scratch belongs to the item kind (Schnorr and ECDSA launches of one validation call run
 // side by side on two streams) and lives until the next launch of that kind, which the stream order puts after this one.
+// stand_down (may be null): the device key cache's launch words; when its insert took the launch, no per-launch record is made.
 static int key_cache_launch(kgv_ctx* ctx, const uint8_t* dpk, size_t n, bool ecdsa, bool aligned, cudaStream_t st, const uint32_t* index,
-                            const uint32_t* n_dev, KeyCacheView* kc) {
+                            const uint32_t* n_dev, KeyCacheView* kc, const uint32_t* stand_down = nullptr) {
   uint32_t slots = 64;
   while (slots < 2 * n) slots <<= 1;                       // load factor <= 1/2
   const uint32_t cap = (uint32_t)(n / 2 < KGV_KEY_RECORDS_MAX ? n / 2 : KGV_KEY_RECORDS_MAX);  // key_form's bounds
@@ -645,10 +803,15 @@ static int key_cache_launch(kgv_ctx* ctx, const uint8_t* dpk, size_t n, bool ecd
   KeySlot* table = (KeySlot*)(K + o_tab);
   uint32_t *item_slot = (uint32_t*)(K + o_item), *rec_rep = (uint32_t*)(K + o_rep), *recs = (uint32_t*)(K + o_rec);
   CK(cudaMemsetAsync(K, 0, o_item, st));
+  if (stand_down) {
+    k_kc_stand_down<<<1, 1, 0, st>>>(stand_down, n_rec);
+    CK(cudaGetLastError());
+    ctx->launches++;
+  }
   const unsigned gd = (unsigned)((n + 255) / 256);
   // (ECDSA keys, at a 33-byte stride, are never word aligned)
   const auto dedup = ecdsa ? k_key_dedup<false, true> : aligned ? k_key_dedup<true, false> : k_key_dedup<false, false>;
-  dedup<<<gd, 256, 0, st>>>(dpk, n, index, n_dev, table, slots - 1, item_slot, rec_rep, n_rec);
+  dedup<<<gd, 256, 0, st>>>(dpk, n, index, n_dev, table, slots - 1, item_slot, rec_rep, n_rec, 0u);
   CK(cudaGetLastError());
   ctx->launches++;
   if (cap) {
@@ -659,6 +822,88 @@ static int key_cache_launch(kgv_ctx* ctx, const uint8_t* dpk, size_t n, bool ecd
     ctx->launches++;
   }
   *kc = KeyCacheView{table, item_slot, recs, n_rec};
+  return KGV_OK;
+}
+
+// ---- device key cache, host side ----
+struct kgv_keycache {
+  bool enabled = true;                  // kgv_set_keycache
+  struct Part {
+    KcPart v{};
+    uint32_t stamp = 0;                 // launches of the kind so far (the stamp of the last one)
+    cudaStream_t side = nullptr;        // the second verify launch, and the deferred inserts of small launches
+    cudaEvent_t ev_looked_up = nullptr, ev_verified = nullptr, ev_inserted = nullptr;
+    cudaEvent_t ev_done = nullptr;      // the end of the last launch of the kind on its caller's stream
+    bool pending = false;               // an insert on side that the next launch of the kind waits for
+    uint8_t* scratch = nullptr;         // per-launch words, item records, order, miss keys, dedup table
+    size_t scratch_cap = 0;
+  } part[2];
+};
+
+// waits for every launch and insert of the cache (events, not streams: a caller's stream may be gone by then)
+static void keycache_quiesce(kgv_keycache* kc) {
+  for (auto& P : kc->part) {
+    if (P.ev_done) cudaEventSynchronize(P.ev_done);
+    if (P.side) cudaStreamSynchronize(P.side);
+  }
+}
+static void keycache_free(kgv_ctx* ctx) {
+  kgv_keycache* kc = ctx->keycache;
+  if (!kc) return;
+  keycache_quiesce(kc);
+  ctx->keycache = nullptr;
+  for (auto& P : kc->part) {
+    for (void* p : {(void*)P.v.sets, (void*)P.v.recs, (void*)P.v.ctr, (void*)P.scratch}) if (p) cudaFree(p);
+    for (cudaEvent_t e : {P.ev_looked_up, P.ev_verified, P.ev_inserted, P.ev_done}) if (e) cudaEventDestroy(e);
+    if (P.side) cudaStreamDestroy(P.side);
+  }
+  delete kc;
+}
+
+struct KcScratch {
+  uint32_t *hdr, *item_rec, *order, *miss_order, *item_slot, *rec_rep;
+  uint8_t* miss_keys;
+  KeySlot* table;
+  uint32_t slots;
+};
+// Starts a launch of partition P on st: after the kind's previous insert, with this launch's stamp and cleared launch words.  The scratch
+// is sized from the host's n (an upper bound of *n_dev when given) and, like the per-launch key cache's, belongs to the kind.
+static int kc_begin(kgv_ctx* ctx, kgv_keycache::Part& P, size_t n, bool ecdsa, cudaStream_t st, KcScratch* s) {
+  if (P.pending) CK(cudaStreamWaitEvent(st, P.ev_inserted, 0));
+  P.pending = false;
+  uint32_t slots = 64;
+  while (slots < 2 * n) slots <<= 1;
+  const size_t o_irec = 256, o_ord = al256(o_irec + 4 * n), o_mord = al256(o_ord + 4 * n), o_mk = al256(o_mord + 4 * n);
+  const size_t o_tab = al256(o_mk + (ecdsa ? 33 : 32) * n);
+  const size_t o_islot = al256(o_tab + (size_t)slots * sizeof(KeySlot)), o_rep = al256(o_islot + 4 * n);
+  if (int rc = kgv_reserve(ctx, &P.scratch, &P.scratch_cap, o_rep + 4 * n)) return rc;
+  uint8_t* S = P.scratch;
+  *s = KcScratch{(uint32_t*)S, (uint32_t*)(S + o_irec), (uint32_t*)(S + o_ord), (uint32_t*)(S + o_mord), (uint32_t*)(S + o_islot), (uint32_t*)(S + o_rep), S + o_mk,
+                 (KeySlot*)(S + o_tab), slots};
+  if (++P.stamp == 0xFFFFFFFFu) {
+    k_kc_restamp<<<nblk(P.v.n_sets, 256), 256, 0, st>>>(P.v.sets, P.v.n_sets);
+    CK(cudaGetLastError());
+    ctx->launches++;
+    P.stamp = 2;
+  }
+  CK(cudaMemsetAsync(S, 0, 256, st));
+  return KGV_OK;
+}
+// the insert of a launch's misses on st: k_key_dedup over the miss keys, then k_kc_insert
+static int kc_insert(kgv_ctx* ctx, kgv_keycache::Part& P, const KcScratch& s, size_t n, bool ecdsa, cudaStream_t st, bool gate) {
+  CK(cudaMemsetAsync(s.table, 0, (size_t)s.slots * sizeof(KeySlot), st));
+  // (the miss keys are packed from a 256-byte aligned base: Schnorr's are word aligned)
+  // a large launch's insert takes at most the partition's slots and KGV_KEY_RECORDS_MAX keys (k_kc_insert's gate): past that many the
+  // dedup stops, the gate refuses the launch
+  const uint32_t slots = P.v.n_sets * KGV_KC_WAYS, limit = gate ? std::min(slots, (uint32_t)KGV_KEY_RECORDS_MAX) : 0xFFFFFFFFu;
+  const auto dedup = ecdsa ? k_key_dedup<false, true, true> : k_key_dedup<true, false, true>;
+  dedup<<<nblk(n, 256), 256, 0, st>>>(s.miss_keys, n, nullptr, s.hdr + KC_N_MISS, s.table, s.slots - 1, s.item_slot, s.rec_rep, s.hdr + KC_N_REC,
+                                      limit);
+  CK(cudaGetLastError());
+  const auto insert = ecdsa ? k_kc_insert<true> : k_kc_insert<false>;
+  insert<<<nblk(n, KGV_BLOCK), KGV_BLOCK, 0, st>>>(P.v, s.miss_keys, s.rec_rep, s.hdr, P.stamp, gate);
+  CK(cudaGetLastError());
+  ctx->launches += 2;
   return KGV_OK;
 }
 
@@ -676,17 +921,146 @@ int kgv_launch_verify(kgv_ctx* ctx, const uint8_t* dpk, const uint8_t* dmsg, con
   // comes on top of a verify that shortens by the same latency (small batches measured 10 % slower with it).
   KeyCacheView kc{};
   const bool key_cache = n > (size_t)ctx->resident_blocks * KGV_BLOCK;
-  if (key_cache) {
-    int rc = key_cache_launch(ctx, dpk, n, ecdsa, aligned, st, index, n_dev, &kc);
-    if (rc) return rc;
-  }
+  // With a device key cache (kgv_keycache) the items whose keys are stored are verified from their comb records by one launch on st, the
+  // others by a second launch, of the form they take without the cache, on the partition's side stream at the same time; st waits for
+  // it.  A small launch stores its misses afterwards on the side stream, off the call's path; a large one stores them first when its insert
+  // takes the launch (k_kc_insert), else every item goes to the second launch, which then runs as without the cache.
+  kgv_keycache::Part* kp = ctx->keycache && ctx->keycache->enabled && ctx->keycache->part[ecdsa].v.n_sets ? &ctx->keycache->part[ecdsa] : nullptr;
   if (!index) {
     auto& lv = ctx->last_verify[ecdsa];
-    lv.n = n; lv.blocks = blocks; lv.key_cache = key_cache; lv.stream = st;
+    lv.n = n; lv.blocks = blocks; lv.key_cache = key_cache && !kp; lv.stream = st;
   }
-  k_verify[ecdsa][index != nullptr][aligned]<<<blocks, KGV_BLOCK, smem, st>>>(dpk, dmsg, dsig, n, dst, ctx->gtab, index, n_dev, kc);
+  if (!kp) {
+    if (key_cache) {
+      int rc = key_cache_launch(ctx, dpk, n, ecdsa, aligned, st, index, n_dev, &kc);
+      if (rc) return rc;
+    }
+    k_verify[ecdsa][index != nullptr][aligned]<<<blocks, KGV_BLOCK, smem, st>>>(dpk, dmsg, dsig, n, dst, ctx->gtab, index, n_dev, kc);
+    CK(cudaGetLastError());
+    ctx->launches++;
+    return KGV_OK;
+  }
+  KcScratch ks{};
+  if (int rc = kc_begin(ctx, *kp, n, ecdsa, st, &ks)) return rc;
+  const auto lookup = ecdsa ? k_kc_lookup<false, true> : aligned ? k_kc_lookup<true, false> : k_kc_lookup<false, false>;
+  lookup<<<nblk(n, 256), 256, 0, st>>>(dpk, n, index, n_dev, kp->v, kp->stamp, key_cache ? KC_COUNT : KC_COUNT | KC_ORDER, ks.hdr, ks.item_rec,
+                                       ks.order, ks.miss_order, ks.miss_keys);
   CK(cudaGetLastError());
   ctx->launches++;
+  if (key_cache) {
+    if (int rc = kc_insert(ctx, *kp, ks, n, ecdsa, st, true)) return rc;
+    if (int rc = key_cache_launch(ctx, dpk, n, ecdsa, aligned, st, index, n_dev, &kc, ks.hdr)) return rc;
+    lookup<<<nblk(n, 256), 256, 0, st>>>(dpk, n, index, n_dev, kp->v, kp->stamp, KC_ORDER | KC_GATED, ks.hdr, ks.item_rec, ks.order, ks.miss_order,
+                                         ks.miss_keys);
+    CK(cudaGetLastError());
+    ctx->launches++;
+  }
+  CK(cudaEventRecord(kp->ev_looked_up, st));
+  CK(cudaStreamWaitEvent(kp->side, kp->ev_looked_up, 0));
+  KeyCacheView stored{};
+  stored.item_rec = ks.item_rec;
+  stored.kc_recs = kp->v.recs;
+  k_verify[ecdsa][1][aligned]<<<blocks, KGV_BLOCK, smem, st>>>(dpk, dmsg, dsig, n, dst, ctx->gtab, ks.order, ks.hdr + KC_ORD_HIT, stored);
+  CK(cudaGetLastError());
+  k_verify[ecdsa][1][aligned]<<<blocks, KGV_BLOCK, smem, kp->side>>>(dpk, dmsg, dsig, n, dst, ctx->gtab, ks.miss_order, ks.hdr + KC_ORD_MISS, kc);
+  CK(cudaGetLastError());
+  ctx->launches += 2;
+  CK(cudaEventRecord(kp->ev_verified, kp->side));
+  CK(cudaStreamWaitEvent(st, kp->ev_verified, 0));
+  CK(cudaEventRecord(kp->ev_done, st));
+  if (!key_cache) {
+    if (int rc = kc_insert(ctx, *kp, ks, n, ecdsa, kp->side, false)) return rc;
+    CK(cudaEventRecord(kp->ev_inserted, kp->side));
+    kp->pending = true;
+  }
+  return KGV_OK;
+}
+
+extern "C" int kgv_keycache_create(kgv_ctx* ctx, uint64_t schnorr_keys, uint64_t ecdsa_keys) {
+  if (!ctx) return KGV_ERR_ARG;
+  std::lock_guard<std::recursive_mutex> g(ctx->mu);
+  if (ctx->keycache) return fail_arg(ctx, "kgv_keycache_create: the context has a key cache");
+  if (schnorr_keys == 0 && ecdsa_keys == 0) return fail_arg(ctx, "kgv_keycache_create: both capacities are 0");
+  if (schnorr_keys > KGV_KEYCACHE_MAX_KEYS || ecdsa_keys > KGV_KEYCACHE_MAX_KEYS)
+    return fail_arg(ctx, "kgv_keycache_create: a capacity above KGV_KEYCACHE_MAX_KEYS");
+  CK(cudaSetDevice(ctx->device));
+  ctx->keycache = new kgv_keycache();
+  auto body = [&]() -> int {
+    for (int k = 0; k < 2; k++) {
+      auto& P = ctx->keycache->part[k];
+      CK(cudaStreamCreateWithFlags(&P.side, cudaStreamNonBlocking));
+      for (cudaEvent_t* e : {&P.ev_looked_up, &P.ev_verified, &P.ev_inserted, &P.ev_done}) CK(cudaEventCreateWithFlags(e, cudaEventDisableTiming));
+      const uint64_t keys = k ? ecdsa_keys : schnorr_keys;
+      if (!keys) continue;
+      const uint32_t n_sets = (uint32_t)((keys + KGV_KC_WAYS - 1) / KGV_KC_WAYS);
+      if (int rc = kgv_malloc(ctx, (void**)&P.v.sets, (size_t)n_sets * sizeof(KcSet))) return rc;
+      if (int rc = kgv_malloc(ctx, (void**)&P.v.recs, (size_t)n_sets * KGV_KC_WAYS * KGV_JR_WORDS * 4)) return rc;
+      if (int rc = kgv_malloc(ctx, (void**)&P.v.ctr, 4 * sizeof(unsigned long long))) return rc;
+      P.v.n_sets = n_sets;
+      CK(cudaMemsetAsync(P.v.sets, 0, (size_t)n_sets * sizeof(KcSet), ctx->stream));
+      CK(cudaMemsetAsync(P.v.ctr, 0, 4 * sizeof(unsigned long long), ctx->stream));
+    }
+    CK(cudaStreamSynchronize(ctx->stream));
+    return KGV_OK;
+  };
+  if (int rc = body()) {
+    keycache_free(ctx);
+    return rc;
+  }
+  return KGV_OK;
+}
+
+extern "C" int kgv_keycache_destroy(kgv_ctx* ctx) {
+  if (!ctx) return KGV_ERR_ARG;
+  std::lock_guard<std::recursive_mutex> g(ctx->mu);
+  CK(cudaSetDevice(ctx->device));
+  keycache_free(ctx);
+  return KGV_OK;
+}
+
+extern "C" int kgv_keycache_clear(kgv_ctx* ctx) {
+  if (!ctx) return KGV_ERR_ARG;
+  std::lock_guard<std::recursive_mutex> g(ctx->mu);
+  kgv_keycache* kc = ctx->keycache;
+  if (!kc) return fail_arg(ctx, "kgv_keycache_clear: the context has no key cache");
+  CK(cudaSetDevice(ctx->device));
+  keycache_quiesce(kc);
+  for (auto& P : kc->part) {
+    if (!P.v.n_sets) continue;
+    CK(cudaMemsetAsync(P.v.sets, 0, (size_t)P.v.n_sets * sizeof(KcSet), ctx->stream));
+    CK(cudaMemsetAsync(P.v.ctr, 0, 4 * sizeof(unsigned long long), ctx->stream));
+  }
+  CK(cudaStreamSynchronize(ctx->stream));
+  return KGV_OK;
+}
+
+extern "C" uint64_t kgv_keycache_counter(kgv_ctx* ctx, int ecdsa, int which) {
+  if (!ctx) return 0;
+  std::lock_guard<std::recursive_mutex> g(ctx->mu);
+  kgv_keycache* kc = ctx->keycache;
+  if (!kc || which < 0 || which > 3) return 0;
+  const auto& P = kc->part[ecdsa ? 1 : 0];
+  if (!P.v.n_sets) return 0;
+  unsigned long long v = 0;
+  cudaError_t e = cudaSetDevice(ctx->device);
+  if (e == cudaSuccess) {
+    keycache_quiesce(kc);
+    e = cudaMemcpyAsync(&v, P.v.ctr + which, sizeof v, cudaMemcpyDeviceToHost, P.side);
+  }
+  if (e == cudaSuccess) e = cudaStreamSynchronize(P.side);
+  if (e != cudaSuccess) {
+    ctx->err = std::string("kgv_keycache_counter: ") + cudaGetErrorString(e);
+    (void)cudaGetLastError();
+    return UINT64_MAX;
+  }
+  return v;
+}
+
+extern "C" int kgv_set_keycache(kgv_ctx* ctx, int enabled) {
+  if (!ctx) return KGV_ERR_ARG;
+  std::lock_guard<std::recursive_mutex> g(ctx->mu);
+  if (!ctx->keycache) return fail_arg(ctx, "kgv_set_keycache: the context has no key cache");
+  ctx->keycache->enabled = enabled != 0;
   return KGV_OK;
 }
 

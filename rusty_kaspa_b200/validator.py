@@ -569,3 +569,36 @@ class SigCache:
             self.detach()
             self.ctx._lib.kgv_sigcache_destroy(self._h)
             self._h = None
+
+
+class KeyCache:
+    """The context's device cache of prepared public keys (kgv_keycache): comb-form key records kept across verify launches, so a key met
+    before runs the joint comb ladder in launches of any size.  Capacities are in keys per kind (about 8.4 KB each).  Created on; detach()
+    / attach() turn its lookups off and on (records kept); verdicts never change."""
+
+    _NAMES = ("lookups", "hits", "inserts", "evictions")
+
+    def __init__(self, ctx, schnorr_keys=1 << 12, ecdsa_keys=1 << 10):
+        self.ctx = ctx
+        ctx._check(ctx._lib.kgv_keycache_create(ctx._h, int(schnorr_keys), int(ecdsa_keys)))
+        self._open = True
+
+    def attach(self):
+        self.ctx._check(self.ctx._lib.kgv_set_keycache(self.ctx._h, 1))
+
+    def detach(self):
+        self.ctx._check(self.ctx._lib.kgv_set_keycache(self.ctx._h, 0))
+
+    def clear(self):
+        self.ctx._check(self.ctx._lib.kgv_keycache_clear(self.ctx._h))
+
+    def counters(self, ecdsa=False):
+        v = [int(self.ctx._lib.kgv_keycache_counter(self.ctx._h, int(bool(ecdsa)), k)) for k in range(4)]
+        if any(x == 2**64 - 1 for x in v):
+            self.ctx._check(-2)  # KGV_ERR_CUDA, with the context's message
+        return dict(zip(self._NAMES, v))
+
+    def close(self):
+        if self._open:
+            self._open = False
+            self.ctx._check(self.ctx._lib.kgv_keycache_destroy(self.ctx._h))
