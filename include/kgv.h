@@ -33,7 +33,8 @@
  *   - there is no CPU fallback: without a usable CUDA device kgv_create fails.
  *   - results are deterministic and independent of batch split or GPU count.
  *   - a context serialises its calls with an internal mutex; use one context per thread for
- *     concurrency.
+ *     concurrency.  A UTXO table (plain or a view) may be used from every context of its
+ *     device at once, under a reader/writer lock per table (Threading, next to the views).
  */
 #ifndef KGV_H
 #define KGV_H
@@ -297,7 +298,29 @@ int kgv_utxo_import_chunk(kgv_ctx* ctx, kgv_utxo_table* t, const uint8_t* keys36
  *   writes (kgv_utxo_apply_diff, kgv_utxo_apply_accepted, the in-order pass of kgv_replay_window) go to the layer only: removing an entry that
  *   lives below records a removal marker, removing the layer's own addition cancels it, re-adding a removed outpoint keeps the lower entry hidden.
  * `base` is never modified until kgv_utxo_view_commit folds the layer into it (write_diff_batch, utxo_set.rs:107-112); kgv_utxo_view_discard drops
- * the layer's content (a candidate chain that lost).  Count / digest / MuHash are defined on plain tables only. */
+ * the layer's content (a candidate chain that lost).  Count / digest / MuHash are defined on plain tables only.
+ *
+ * Threading: a table, plain or a view, may be used from any context of its device, at the same time (a table given to a context of another
+ * device: KGV_ERR_ARG with a kgv_last_error message).  Each table has a reader/writer lock, with the semantics of the reference's RwLock
+ * around the virtual UTXO set (processor.rs:270-272, 556-564, 853-858), ordered on the GPU by CUDA events:
+ *   - a call READS a table when it looks entries up in it: kgv_utxo_lookup, _count, _digest, _export, _stats, kgv_utxo_muhash,
+ *     kgv_muhash_txs, the populate step of kgv_validate_txs / kgv_validate_mempool_txs / _in_parallel / _with_policy / kgv_replay_window, and
+ *     the layer kgv_utxo_view_commit folds.  Reading a view reads every layer below it.  kgv_replay_muhash / _diffs / _verify_chain read the
+ *     layers of the last replay window's table (KGV_ERR_ARG when one was rehashed since);
+ *   - a call WRITES a table when it changes its slots, arena, counters, capacity or layout: kgv_utxo_apply_diff, _apply_accepted,
+ *     _import_chunk, the in-order pass of kgv_replay_window into it, kgv_utxo_view_commit (writes the base), _view_discard, _rehash,
+ *     _set_max_load, the growth inside any write, and kgv_utxo_destroy.  A write excludes the reads and writes of every context;
+ *   - a read sees the state the writes enqueued before it started left, never part of a write.  Writes to one table take effect in the order
+ *     their calls entered.  Writers are preferred: once a write waits, new reads wait behind it, so a steady stream of mempool calls cannot
+ *     starve a commit;
+ *   - a call that reads a view and writes its top layer (a replay into the layer) reads the layers below and writes the top, so mempool calls
+ *     on the base run beside a replay into a view over it.  Only the commit excludes them.
+ * A read does not block the host: its stream waits for the event that ends the last write.  A write waits on the host until the open reads of
+ * other contexts have finished enqueuing (the reference's upgrade()), then its stream waits for their events.  A call holds its tables from
+ * its first enqueued access to its last, host synchronisations inside it included; a call touching several tables takes them bottom layer
+ * first.  Arrays a write gives up (rehash, growth) are freed once that write has completed on the GPU, at the writing context's
+ * kgv_synchronize or kgv_destroy; kgv_utxo_destroy frees the rest.  With one context nothing changes but one event record and one stream wait
+ * per table and call.  A table must outlive every call on it, from every context. */
 int kgv_utxo_view_create(kgv_ctx* ctx, kgv_utxo_table* base, uint64_t capacity_slots, kgv_utxo_table** out);
 int kgv_utxo_view_commit(kgv_ctx* ctx, kgv_utxo_table* view);
 int kgv_utxo_view_discard(kgv_ctx* ctx, kgv_utxo_table* view);

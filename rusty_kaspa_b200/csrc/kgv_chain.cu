@@ -248,6 +248,8 @@ extern "C" int kgv_replay_verify_chain(kgv_ctx* ctx, const uint32_t* group_first
   bool dev;
   if (int rc = io.one_side("kgv_replay_verify_chain", {results, headers, merged_flags, init768, block_fees, multisets768}, &dev)) return rc;
   CK(cudaSetDevice(ctx->device));
+  kgv_table_access acc(ctx);
+  if (int rc = kgv_last_replay_read(ctx, acc, "kgv_replay_verify_chain")) return rc;
   cudaStream_t st = ctx->stream;
   const cudaMemcpyKind in_kind = dev ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
   const size_t nt = L.nt, nb = L.n_blocks;

@@ -2,8 +2,10 @@
 #pragma once
 #include <cuda_runtime.h>
 #include <cstdint>
+#include <condition_variable>
 #include <cstdio>
 #include <initializer_list>
+#include <memory>
 #include <mutex>
 #include <string>
 #include <thread>
@@ -73,11 +75,15 @@ struct kgv_ctx {
     size_t o_src = 0, o_inf = 0, o_apv = 0;
     size_t o_blk = 0, o_res = 0;                    // the kgv_replay_block records and the per-transaction results
     std::vector<uint32_t> block_flags, block_n_txs;  // host copy of the blocks' flags and sizes
+    struct kgv_utxo_table* table = nullptr;          // the table replayed into, and the rehashes of its layers then: the populated entries'
+    uint64_t rehashes = 0;                           // long scripts lie in those layers' arenas
   } last_replay;
   struct kgv_sigcache* sigcache = nullptr;  // kgv_set_sigcache: verdicts of the validation calls are looked up / remembered here
   struct kgv_keycache* keycache = nullptr;  // kgv_set_keycache: comb key records kept across the verify launches (kgv_lib.cu)
   struct kgv_comm* shard_comm = nullptr;  // kgv_set_sharding: signature checks of the validation calls are split over its ranks
   std::vector<uint8_t*> parked;  // outgrown per-call buffers, released when the caller synchronises / destroys the context (kgv_reserve)
+  // tables whose arrays a write of this context gave up (rehash, growth): released from the table's list at kgv_synchronize / kgv_destroy
+  std::vector<std::shared_ptr<struct kgv_table_sync>> retiring;
   uint64_t launches = 0;
   uint32_t last_script_rounds = 0;  // verification rounds of the last device script engine run (kgv_debug_script_rounds)
   // the last non-indexed verify launch of each kind ([0] Schnorr, [1] ECDSA), for kgv_debug_key_form
@@ -243,8 +249,62 @@ int kgv_mu_finalize_run(kgv_ctx* ctx, const uint32_t* dnum, const uint32_t* dden
 size_t kgv_replay_muhash_scratch(kgv_ctx* ctx, size_t n_groups);
 int kgv_replay_muhash_run(kgv_ctx* ctx, const uint32_t* dgf, size_t n_groups, uint8_t* scratch, uint32_t* vals, cudaStream_t st);
 
-// ---- shared pieces of the validation path (kgv_validate.cu) ----
+// ---- one UTXO table used from every context of its device (kgv_utxo_maint.cu; include/kgv.h, "Threading") ----
+// A reader/writer lock per table whose ordering lives on the GPU.  A call registers before it enqueues the first work that touches the
+// table and drops the registration after the last.  A read makes its stream wait for the event that ends the last write; the host does
+// not block unless a write is open or queued.  A write waits on the host until the reads of OTHER contexts have dropped (the reference's
+// upgrade()), makes its stream wait for their events and the last write's, and records the new last-write event when it drops.  Writers
+// enter in ticket order and readers wait while one is queued, so a steady stream of reads cannot starve a commit.  Registration is
+// reentrant per context (entry points call each other under the context's recursive mutex); a read inside the context's own write is part
+// of that write.
+struct kgv_table_sync {
+  int device = 0;
+  std::mutex m;
+  std::condition_variable cv;
+  struct Reader { const kgv_ctx* ctx; int depth; };
+  std::vector<Reader> readers;            // open read registrations
+  const void* writer = nullptr;           // the context whose write is open (write_depth > 0)
+  int write_depth = 0;
+  uint64_t next_ticket = 0, serving = 0;  // writers queued or open: next_ticket - serving
+  cudaEvent_t last_write = nullptr;       // ends the last write
+  std::vector<std::pair<cudaStream_t, cudaEvent_t>> reads;  // end the reads since that write: one event per stream, re-recorded
+  std::vector<cudaEvent_t> pool;          // cudaEventDisableTiming events not in use
+  uint64_t writes = 0;
+  std::vector<void*> retiring;            // arrays the open write gave up
+  cudaEvent_t retire_ev = nullptr;        // (reserved for them by kgv_table_retire)
+  struct Retired { cudaEvent_t done; std::vector<void*> ptrs; };
+  std::vector<Retired> retired;           // freed once `done` has completed
+};
 struct kgv_utxo_table;
+// The registrations of one call, dropped (events recorded on ctx->stream) when it goes out of scope.
+class kgv_table_access {
+ public:
+  explicit kgv_table_access(kgv_ctx* c) : ctx(c) {}
+  ~kgv_table_access() { release(); }
+  kgv_table_access(const kgv_table_access&) = delete;
+  kgv_table_access& operator=(const kgv_table_access&) = delete;
+  // A read on every layer of t's view chain, except `written` (a layer of it, or null) which gets a write; bottom layer first, so calls
+  // that touch several tables cannot deadlock.  KGV_ERR_ARG, naming `call`, when a layer belongs to another device than the context.
+  int acquire(const char* call, kgv_utxo_table* t, kgv_utxo_table* written = nullptr);
+  void release();
+
+ private:
+  enum Mode { kNone, kRead, kWrite };
+  int lock(kgv_table_sync* s, Mode m);
+  kgv_ctx* ctx;
+  struct Held { kgv_table_sync* s; Mode m; cudaEvent_t ev; };
+  std::vector<Held> held;
+};
+// Hands an array of t to the table's release list: freed after the open write of ctx (which gave it up) has completed on the GPU.
+int kgv_table_retire(kgv_ctx* ctx, kgv_utxo_table* t, void* p);
+// kgv_replay_muhash / _diffs / _verify_chain: a read of the layers of the last replay window's table, refused (KGV_ERR_ARG, naming `call`) when
+// one of them was rehashed since by any context.
+int kgv_last_replay_read(kgv_ctx* ctx, kgv_table_access& acc, const char* call);
+uint64_t kgv_chain_rehashes(const kgv_utxo_table* t);
+// Frees the retired arrays of the tables this context wrote whose writes have completed; wait: wait for the others and free them too.
+void kgv_release_retired(kgv_ctx* ctx, bool wait);
+
+// ---- shared pieces of the validation path (kgv_validate.cu) ----
 // Growth policy of a table (kgv_utxo_set_max_load, kgv_utxo_maint.cu): called by every table writer before it writes.  m bounds the slots the
 // call can newly occupy, b the long-script bytes it can append.  Returns at once when the policy is off; otherwise it may rehash the table
 // (KGV_ERR_NOMEM when that fails: the caller returns before writing anything).

@@ -666,6 +666,7 @@ int kgv_malloc(kgv_ctx* ctx, void** p, size_t bytes) {
     if (ctx->keycache) keycache_quiesce(ctx->keycache);  // a deferred key insert may still read a parked scratch
     for (uint8_t* q : ctx->parked) cudaFree(q);
     ctx->parked.clear();
+    kgv_release_retired(ctx, false);
     e = cudaMalloc(p, bytes);
   }
   if (e != cudaSuccess) { ctx->err = std::string("cudaMalloc failed: ") + cudaGetErrorString(e); (void)cudaGetLastError(); *p = nullptr; return KGV_ERR_NOMEM; }
@@ -736,6 +737,7 @@ extern "C" void kgv_destroy(kgv_ctx* ctx) {
   for (uint8_t* b : {ctx->d_io, ctx->d_in, ctx->d_out, ctx->d_batch, ctx->prefetch[0].buf, ctx->prefetch[1].buf, ctx->d_scratch, ctx->d_mu, ctx->d_work, ctx->d_replay, ctx->d_keys[0], ctx->d_keys[1]})
     if (b) cudaFree(b);
   for (uint8_t* b : ctx->parked) cudaFree(b);
+  kgv_release_retired(ctx, true);
   for (cudaEvent_t e : ctx->ev_chunk) if (e) cudaEventDestroy(e);
   for (cudaEvent_t e : ctx->ev_time) if (e) cudaEventDestroy(e);
   if (ctx->ev_prefetch) cudaEventDestroy(ctx->ev_prefetch);
@@ -774,6 +776,7 @@ extern "C" int kgv_synchronize(kgv_ctx* ctx) {
     for (uint8_t* p : ctx->parked) cudaFree(p);
     ctx->parked.clear();
   }
+  kgv_release_retired(ctx, false);  // table arrays given up by this context's writes, once those writes have completed
   return KGV_OK;
 }
 

@@ -602,6 +602,9 @@ extern "C" int kgv_replay_window(kgv_ctx* ctx, kgv_utxo_table* table, const kgv_
     if (at != batch->n_txs) { ctx->err = "kgv_replay_window: replay blocks do not cover the batch"; return KGV_ERR_ARG; }
   }
   CK(cudaSetDevice(ctx->device));
+  // a write on the table replayed into, a read on the layers below it: mempool calls on the base run beside a replay into a view over it
+  kgv_table_access acc(ctx);
+  if (int rc = acc.acquire("kgv_replay_window", table, table)) return rc;
   int rc = utxo_reserve(ctx, table, batch->n_outputs + (table->base ? batch->n_inputs : 0), batch->n_bytes + 8 * (uint64_t)batch->n_outputs);
   if (rc) return rc;
   kgv_dev_batch d;
@@ -807,6 +810,7 @@ extern "C" int kgv_replay_window(kgv_ctx* ctx, kgv_utxo_table* table, const kgv_
   ctx->last_replay.o_txb = o_txb; ctx->last_replay.o_rng = o_rng;
   ctx->last_replay.o_src = o_src; ctx->last_replay.o_inf = o_inf; ctx->last_replay.o_apv = o_apv;
   ctx->last_replay.o_blk = o_blk; ctx->last_replay.o_res = o_res;
+  ctx->last_replay.table = table; ctx->last_replay.rehashes = kgv_chain_rehashes(table);
   ctx->last_replay.block_flags.resize(n_blocks); ctx->last_replay.block_n_txs.resize(n_blocks);
   for (size_t i = 0; i < n_blocks; i++) { ctx->last_replay.block_flags[i] = blocks[i].flags; ctx->last_replay.block_n_txs[i] = blocks[i].n_txs; }
   if (stats) {
@@ -920,6 +924,8 @@ extern "C" int kgv_replay_muhash(kgv_ctx* ctx, const uint32_t* group_first_block
   if (group_first_block[0] != 0 || group_first_block[n_groups] != L.n_blocks) { ctx->err = "groups must tile the blocks of the window"; return KGV_ERR_ARG; }
   for (size_t i = 0; i < n_groups; i++) if (group_first_block[i] > group_first_block[i + 1]) { ctx->err = "group offsets not monotone"; return KGV_ERR_ARG; }
   CK(cudaSetDevice(ctx->device));
+  kgv_table_access acc(ctx);
+  if (int rc = kgv_last_replay_read(ctx, acc, "kgv_replay_muhash")) return rc;
   cudaStream_t st = ctx->stream;
   // scratch (d_work is free between validation calls)
   const size_t o_gf = 0, o_mu = al256((n_groups + 1) * 4), o_val = o_mu + kgv_replay_muhash_scratch(ctx, n_groups);
@@ -1126,6 +1132,8 @@ extern "C" int kgv_replay_diffs(kgv_ctx* ctx, const uint32_t* group_first_block,
     if (dev && (((uintptr_t)rem_entries | (uintptr_t)add_entries) & 7)) { ctx->err = "kgv_replay_diffs: device entry arrays must be 8-byte aligned"; return KGV_ERR_ARG; }
   }
   CK(cudaSetDevice(ctx->device));
+  kgv_table_access acc(ctx);
+  if (int rc = kgv_last_replay_read(ctx, acc, "kgv_replay_diffs")) return rc;
   cudaStream_t st = ctx->stream;
   uint8_t* R = ctx->d_replay;
   const size_t nt = L.nt, ni = L.ni, no = L.no;

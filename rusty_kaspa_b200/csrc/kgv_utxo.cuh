@@ -11,6 +11,8 @@
 // Slot loads are L2-coherent (ld.global.cg: the table is written by other SMs of the same launch), never L1 cached
 // (random 128-byte accesses have no L1 reuse).
 #pragma once
+#include <memory>
+
 #include "kgv_script_std.cuh"
 
 #define SLOT_EMPTY 0u
@@ -49,6 +51,9 @@ struct kgv_utxo_table {
   uint32_t max_load = 0;         // growth policy in permille of the capacity, 0 = off
   uint64_t occ_bound = 0;        // with the policy on: upper bounds of the non-EMPTY slots and of counters[2] (exact at the last read + every
   uint64_t arena_bound = 0;      // write's reservation since), so that most writes need no counter read
+  // the table's device and the order of the calls of every context on it (kgv_internal.h); shared with the contexts that still have
+  // arrays of this table to release
+  std::shared_ptr<struct kgv_table_sync> sync;
 };
 
 struct TableView {

@@ -163,7 +163,162 @@ __global__ void __launch_bounds__(256) k_utxo_rehash(TableView old, UtxoSlot* __
 }
 
 // ---------------------------------------------------------------------------------------------
-// host side
+// host side: the calls of several contexts on one table (kgv_internal.h)
+// ---------------------------------------------------------------------------------------------
+static int pooled_event(kgv_table_sync* s, cudaEvent_t* ev) {  // (s->m held)
+  if (!s->pool.empty()) { *ev = s->pool.back(); s->pool.pop_back(); return KGV_OK; }
+  return cudaEventCreateWithFlags(ev, cudaEventDisableTiming) == cudaSuccess ? KGV_OK : KGV_ERR_CUDA;
+}
+
+int kgv_table_access::lock(kgv_table_sync* s, Mode m) {
+  std::unique_lock<std::mutex> g(s->m);
+  cudaStream_t st = ctx->stream;
+  Held h{s, m, nullptr};
+  if (s->writer == ctx && s->write_depth > 0) {  // nested in this context's own write
+    if (m == kWrite) s->write_depth++;
+    else h.m = kNone;
+    held.push_back(h);
+    return KGV_OK;
+  }
+  cudaError_t e = cudaSuccess;
+  if (m == kRead) {
+    auto it = s->readers.begin();
+    while (it != s->readers.end() && it->ctx != ctx) ++it;
+    if (it != s->readers.end()) {  // nested in a read of this context: a queued writer waits for it, so this must not wait for the writer
+      it->depth++;
+      held.push_back(h);
+      return KGV_OK;
+    }
+    if (pooled_event(s, &h.ev)) { ctx->err = "cudaEventCreate failed for a table read"; return KGV_ERR_CUDA; }
+    s->cv.wait(g, [&] { return s->write_depth == 0 && s->next_ticket == s->serving; });
+    s->readers.push_back({ctx, 1});
+    if (s->last_write) e = cudaStreamWaitEvent(st, s->last_write, 0);
+  } else {
+    if (!s->last_write && pooled_event(s, &s->last_write)) { ctx->err = "cudaEventCreate failed for a table write"; return KGV_ERR_CUDA; }
+    const uint64_t ticket = s->next_ticket++;
+    s->cv.wait(g, [&] {
+      if (s->serving != ticket || s->write_depth) return false;
+      for (const auto& r : s->readers) if (r.ctx != ctx) return false;
+      return true;
+    });
+    s->writer = ctx;
+    s->write_depth = 1;
+    for (const auto& r : s->reads) {
+      if (e == cudaSuccess) e = cudaStreamWaitEvent(st, r.second, 0);
+      s->pool.push_back(r.second);
+    }
+    s->reads.clear();
+    if (e == cudaSuccess) e = cudaStreamWaitEvent(st, s->last_write, 0);
+  }
+  held.push_back(h);  // held from here on, so that release() undoes it even when the wait failed
+  if (e != cudaSuccess) { ctx->err = std::string("ordering a table access: ") + cudaGetErrorString(e); return KGV_ERR_CUDA; }
+  return KGV_OK;
+}
+
+int kgv_table_access::acquire(const char* call, kgv_utxo_table* t, kgv_utxo_table* written) {
+  kgv_utxo_table* chain[64];
+  int n = 0;
+  for (kgv_utxo_table* L = t; L; L = L->base) {
+    if (n == 64) { ctx->err = std::string(call) + ": a view chain deeper than 64 layers"; return KGV_ERR_LIMIT; }
+    if (L->sync->device != ctx->device) {
+      ctx->err = std::string(call) + ": the UTXO table belongs to device " + std::to_string(L->sync->device) + ", the context to device " +
+                 std::to_string(ctx->device);
+      return KGV_ERR_ARG;
+    }
+    chain[n++] = L;
+  }
+  while (n--)
+    if (int rc = lock(chain[n]->sync.get(), chain[n] == written ? kWrite : kRead)) return rc;
+  return KGV_OK;
+}
+
+void kgv_table_access::release() {
+  cudaStream_t st = ctx->stream;
+  while (!held.empty()) {
+    Held h = held.back();
+    held.pop_back();
+    kgv_table_sync* s = h.s;
+    std::lock_guard<std::mutex> g(s->m);
+    if (h.m == kWrite) {
+      if (--s->write_depth) continue;
+      cudaEventRecord(s->last_write, st);
+      s->writes++;
+      if (!s->retiring.empty()) {
+        cudaEventRecord(s->retire_ev, st);
+        s->retired.push_back({s->retire_ev, std::move(s->retiring)});
+        s->retiring.clear();
+        s->retire_ev = nullptr;
+      }
+      s->writer = nullptr;
+      s->serving++;
+    } else if (h.m == kRead) {
+      auto it = s->readers.begin();
+      while (it != s->readers.end() && it->ctx != ctx) ++it;
+      if (it == s->readers.end() || --it->depth) continue;
+      s->readers.erase(it);
+      cudaEvent_t ev = h.ev;
+      for (auto& r : s->reads)  // a later record on the same stream supersedes the earlier one
+        if (r.first == st) { s->pool.push_back(ev); ev = r.second; break; }
+      if (ev == h.ev) s->reads.push_back({st, ev});
+      cudaEventRecord(ev, st);
+    } else {
+      continue;
+    }
+    s->cv.notify_all();
+  }
+}
+
+int kgv_table_retire(kgv_ctx* ctx, kgv_utxo_table* t, void* p) {
+  kgv_table_sync* s = t->sync.get();
+  std::lock_guard<std::mutex> g(s->m);
+  if (!s->retire_ev && pooled_event(s, &s->retire_ev)) {
+    ctx->err = "cudaEventCreate failed for a released table array";
+    return KGV_ERR_CUDA;
+  }
+  s->retiring.push_back(p);
+  for (const auto& r : ctx->retiring) if (r.get() == s) return KGV_OK;
+  ctx->retiring.push_back(t->sync);
+  return KGV_OK;
+}
+
+void kgv_release_retired(kgv_ctx* ctx, bool wait) {
+  auto& v = ctx->retiring;
+  for (size_t i = 0; i < v.size();) {
+    kgv_table_sync* s = v[i].get();
+    bool empty;
+    {
+      std::lock_guard<std::mutex> g(s->m);
+      auto& R = s->retired;
+      for (size_t j = 0; j < R.size();) {
+        if (wait) cudaEventSynchronize(R[j].done);
+        if (cudaEventQuery(R[j].done) != cudaSuccess) { (void)cudaGetLastError(); j++; continue; }
+        for (void* p : R[j].ptrs) cudaFree(p);
+        s->pool.push_back(R[j].done);
+        R.erase(R.begin() + j);
+      }
+      empty = R.empty() && s->retiring.empty();
+    }
+    if (empty) v.erase(v.begin() + i);
+    else i++;
+  }
+}
+
+uint64_t kgv_chain_rehashes(const kgv_utxo_table* t) {
+  uint64_t n = 0;
+  for (; t; t = t->base) n += t->rehashes;
+  return n;
+}
+
+int kgv_last_replay_read(kgv_ctx* ctx, kgv_table_access& acc, const char* call) {
+  if (int rc = acc.acquire(call, ctx->last_replay.table)) return rc;
+  if (kgv_chain_rehashes(ctx->last_replay.table) == ctx->last_replay.rehashes) return KGV_OK;
+  ctx->last_replay.valid = false;
+  ctx->err = std::string(call) + " refers to the last kgv_replay_window call, and its table was rehashed since";
+  return KGV_ERR_ARG;
+}
+
+// ---------------------------------------------------------------------------------------------
+// host side: maintenance
 // ---------------------------------------------------------------------------------------------
 // counters + one stats pass; synchronises
 static int utxo_scan(kgv_ctx* ctx, kgv_utxo_table* t, kgv_utxo_table_stats* out, uint64_t* n_entries) {
@@ -229,9 +384,8 @@ static int utxo_rehash(kgv_ctx* ctx, kgv_utxo_table* t, uint64_t capacity_slots,
   k_utxo_rehash<<<nblk(t->mask + 1, 256), 256, 0, st>>>(view_of(t), slots, cap - 1, overflow, arena, t->counters);
   CK(cudaGetLastError());
   ctx->launches++;
-  // the old arrays may still be read by work queued before this call on other layers' behalf: parked, released when the context is idle
-  ctx->parked.push_back((uint8_t*)t->slots);
-  ctx->parked.push_back(t->overflow);
+  // the old arrays may still be read by work queued before this write, of any context: released once the write has completed
+  if ((rc = kgv_table_retire(ctx, t, t->slots)) || (rc = kgv_table_retire(ctx, t, t->overflow))) return rc;
   t->slots = slots;
   t->mask = cap - 1;
   t->overflow = overflow;
@@ -282,6 +436,8 @@ extern "C" int kgv_utxo_stats(kgv_ctx* ctx, kgv_utxo_table* t, kgv_utxo_table_st
   std::lock_guard<std::recursive_mutex> g(ctx->mu);
   if (int rc = kgv_host_only(ctx, "kgv_utxo_stats", "out", out)) return rc;
   CK(cudaSetDevice(ctx->device));
+  kgv_table_access acc(ctx);
+  if (int rc = acc.acquire("kgv_utxo_stats", t)) return rc;
   return utxo_scan(ctx, t, out, nullptr);
 }
 
@@ -289,6 +445,8 @@ extern "C" int kgv_utxo_rehash(kgv_ctx* ctx, kgv_utxo_table* t, uint64_t capacit
   if (!ctx || !t) return KGV_ERR_ARG;
   std::lock_guard<std::recursive_mutex> g(ctx->mu);
   CK(cudaSetDevice(ctx->device));
+  kgv_table_access acc(ctx);
+  if (int rc = acc.acquire("kgv_utxo_rehash", t, t)) return rc;
   return utxo_rehash(ctx, t, capacity_slots, 0);
 }
 
@@ -297,6 +455,8 @@ extern "C" int kgv_utxo_set_max_load(kgv_ctx* ctx, kgv_utxo_table* t, uint32_t m
   std::lock_guard<std::recursive_mutex> g(ctx->mu);
   if (max_load_permille > 900) { ctx->err = "max_load_permille: 0 (off) or 1..900"; return KGV_ERR_ARG; }
   CK(cudaSetDevice(ctx->device));
+  kgv_table_access acc(ctx);
+  if (int rc = acc.acquire("kgv_utxo_set_max_load", t, t)) return rc;
   t->max_load = max_load_permille;
   if (max_load_permille) {  // start the host-side bounds from the exact values
     unsigned long long c[3];

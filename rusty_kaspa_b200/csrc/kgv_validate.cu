@@ -521,6 +521,8 @@ extern "C" int kgv_utxo_create(kgv_ctx* ctx, uint64_t capacity_slots, kgv_utxo_t
   uint64_t cap = 1024;
   while (cap < capacity_slots) cap <<= 1;
   kgv_utxo_table* t = new kgv_utxo_table();
+  t->sync = std::make_shared<kgv_table_sync>();
+  t->sync->device = ctx->device;
   t->mask = cap - 1;
   t->overflow_cap = cap * 8 < (64ull << 20) ? (64ull << 20) : cap * 8;
   cudaError_t e = cudaMalloc((void**)&t->slots, cap * sizeof(UtxoSlot));
@@ -549,6 +551,11 @@ extern "C" int kgv_utxo_create(kgv_ctx* ctx, uint64_t capacity_slots, kgv_utxo_t
 // ---------------------------------------------------------------------------------------------
 extern "C" int kgv_utxo_view_create(kgv_ctx* ctx, kgv_utxo_table* base, uint64_t capacity_slots, kgv_utxo_table** out) {
   if (!ctx || !base || !out) return KGV_ERR_ARG;
+  if (base->sync->device != ctx->device) {
+    std::lock_guard<std::recursive_mutex> g(ctx->mu);
+    ctx->err = "kgv_utxo_view_create: the base table belongs to device " + std::to_string(base->sync->device) + ", the context to device " + std::to_string(ctx->device);
+    return KGV_ERR_ARG;
+  }
   int rc = kgv_utxo_create(ctx, capacity_slots, out);
   if (rc) return rc;
   std::lock_guard<std::recursive_mutex> g(ctx->mu);
@@ -598,6 +605,8 @@ extern "C" int kgv_utxo_view_commit(kgv_ctx* ctx, kgv_utxo_table* view) {
   if (!ctx || !view || !view->base) return KGV_ERR_ARG;
   std::lock_guard<std::recursive_mutex> g(ctx->mu);
   CK(cudaSetDevice(ctx->device));
+  kgv_table_access acc(ctx);  // reads the layer, writes the base
+  if (int rc = acc.acquire("kgv_utxo_view_commit", view, view->base)) return rc;
   if (view->base->max_load) {  // the base takes at most the layer's entries and its long scripts
     unsigned long long c[3];
     CK(cudaMemcpyAsync(c, view->counters, sizeof c, cudaMemcpyDeviceToHost, ctx->stream));
@@ -617,11 +626,37 @@ extern "C" int kgv_utxo_view_discard(kgv_ctx* ctx, kgv_utxo_table* view) {
   if (!ctx || !view || !view->base) return KGV_ERR_ARG;
   std::lock_guard<std::recursive_mutex> g(ctx->mu);
   CK(cudaSetDevice(ctx->device));
+  kgv_table_access acc(ctx);
+  if (int rc = acc.acquire("kgv_utxo_view_discard", view, view)) return rc;
   return view_clear(ctx, view);
 }
+// A write like any other: it waits for the open reads and writes of every context, then for their work on the GPU, and frees the table's
+// arrays, those retired by earlier rehashes included.
 extern "C" void kgv_utxo_destroy(kgv_ctx* ctx, kgv_utxo_table* t) {
   if (!t) return;
-  if (ctx) { cudaSetDevice(ctx->device); cudaStreamSynchronize(ctx->stream); }
+  kgv_table_sync* s = t->sync.get();
+  cudaSetDevice(s->device);
+  if (ctx) cudaStreamSynchronize(ctx->stream);
+  {
+    std::unique_lock<std::mutex> g(s->m);
+    const uint64_t ticket = s->next_ticket++;
+    s->cv.wait(g, [&] { return s->serving == ticket && s->write_depth == 0 && s->readers.empty(); });
+    for (const auto& r : s->reads) cudaEventSynchronize(r.second);
+    if (s->last_write) cudaEventSynchronize(s->last_write);
+    for (const auto& r : s->retired) {
+      cudaEventSynchronize(r.done);
+      for (void* p : r.ptrs) cudaFree(p);
+      s->pool.push_back(r.done);
+    }
+    s->retired.clear();
+    for (const auto& r : s->reads) s->pool.push_back(r.second);
+    s->reads.clear();
+    if (s->last_write) s->pool.push_back(s->last_write);
+    s->last_write = nullptr;
+    for (cudaEvent_t e : s->pool) cudaEventDestroy(e);
+    s->pool.clear();
+    s->serving++;
+  }
   cudaFree(t->slots); cudaFree(t->overflow); cudaFree(t->counters);
   if (t->d_view) cudaFree(t->d_view);
   delete t;
@@ -634,6 +669,8 @@ extern "C" int kgv_utxo_lookup(kgv_ctx* ctx, kgv_utxo_table* t, const uint8_t* k
   if (n == 0) return KGV_OK;
   if (!keys36 || !entries || !found || (script_stride && !scripts_out)) { ctx->err = "null buffer"; return KGV_ERR_ARG; }
   CK(cudaSetDevice(ctx->device));
+  kgv_table_access acc(ctx);
+  if (int rc = acc.acquire("kgv_utxo_lookup", t)) return rc;
   kgv_io io(ctx);
   const uint8_t* dk;
   kgv_utxo_entry* de;
@@ -658,6 +695,8 @@ extern "C" int kgv_utxo_apply_diff(kgv_ctx* ctx, kgv_utxo_table* t, const uint8_
   CK(cudaSetDevice(ctx->device));
   const void* probe = n_rem ? (const void*)rem_keys36 : (const void*)add_keys36;
   if (!probe) return KGV_OK;
+  kgv_table_access acc(ctx);
+  if (int rc = acc.acquire("kgv_utxo_apply_diff", t, t)) return rc;
   {  // a view layer records a removal marker for an entry that lives below
     int rc = utxo_reserve(ctx, t, n_add + (t->base ? n_rem : 0), n_add_bytes + 8 * (uint64_t)n_add);
     if (rc) return rc;
@@ -688,6 +727,8 @@ extern "C" int kgv_utxo_export(kgv_ctx* ctx, kgv_utxo_table* t, uint8_t* keys36,
   for (const auto& [what, p] : {std::pair<const char*, const void*>{"n_out", n_out}, {"bytes_out", bytes_out}})
     if (int rc = kgv_host_only(ctx, "kgv_utxo_export", what, p)) return rc;
   CK(cudaSetDevice(ctx->device));
+  kgv_table_access acc(ctx);
+  if (int rc = acc.acquire("kgv_utxo_export", t)) return rc;
   kgv_io io(ctx);
   uint8_t *dk = nullptr, *db = bytes;
   kgv_utxo_entry* de = entries;
@@ -697,7 +738,9 @@ extern "C" int kgv_utxo_export(kgv_ctx* ctx, kgv_utxo_table* t, uint8_t* keys36,
     io.out(bytes, bytes_cap, &db);
     if (int rc = io.stage()) return rc;
   }
-  unsigned long long* cnt = t->counters + 8;  // (the digest's scratch words)
+  // the counts live in the context's scratch: other contexts may export the table at the same time
+  if (int rc = kgv_reserve(ctx, &ctx->d_work, &ctx->d_work_cap, 2 * sizeof(unsigned long long))) return rc;
+  unsigned long long* cnt = (unsigned long long*)ctx->d_work;
   CK(cudaMemsetAsync(cnt, 0, 2 * sizeof(unsigned long long), ctx->stream));
   k_utxo_export<<<nblk(t->mask + 1, 128), 128, 0, ctx->stream>>>(view_of(t), dk, de, db, max_n, bytes_cap, cnt);
   CK(cudaGetLastError());
@@ -726,6 +769,8 @@ extern "C" int kgv_utxo_import_chunk(kgv_ctx* ctx, kgv_utxo_table* t, const uint
   if (int rc = kgv_host_only(ctx, "kgv_utxo_import_chunk", "numerator384", numerator384)) return rc;
   kgv_io io(ctx);
   CK(cudaSetDevice(ctx->device));
+  kgv_table_access acc(ctx);
+  if (int rc = acc.acquire("kgv_utxo_import_chunk", t, t)) return rc;
   // the script ranges are checked here whatever the side of entries: device entries are read through a host copy
   std::vector<kgv_utxo_entry> entries_host;
   const kgv_utxo_entry* he = entries;
@@ -770,6 +815,8 @@ extern "C" int kgv_utxo_count(kgv_ctx* ctx, kgv_utxo_table* t, uint64_t* count) 
   if (int rc = kgv_host_only(ctx, "kgv_utxo_count", "count", count)) return rc;
   if (t->base) { ctx->err = "count / digest / MuHash are defined on plain tables: commit the view first"; return KGV_ERR_ARG; }
   CK(cudaSetDevice(ctx->device));
+  kgv_table_access acc(ctx);
+  if (int rc = acc.acquire("kgv_utxo_count", t)) return rc;
   unsigned long long c[4];
   CK(cudaMemcpyAsync(c, t->counters, sizeof c, cudaMemcpyDeviceToHost, ctx->stream));
   CK(cudaStreamSynchronize(ctx->stream));
@@ -784,7 +831,11 @@ extern "C" int kgv_utxo_digest(kgv_ctx* ctx, kgv_utxo_table* t, uint8_t out32[32
   if (int rc = kgv_host_only(ctx, "kgv_utxo_digest", "out32", out32)) return rc;
   if (t->base) { ctx->err = "count / digest / MuHash are defined on plain tables: commit the view first"; return KGV_ERR_ARG; }
   CK(cudaSetDevice(ctx->device));
-  unsigned long long* acc = t->counters + 8;
+  kgv_table_access access(ctx);
+  if (int rc = access.acquire("kgv_utxo_digest", t)) return rc;
+  // the sums live in the context's scratch: other contexts may digest the table at the same time
+  if (int rc = kgv_reserve(ctx, &ctx->d_work, &ctx->d_work_cap, 8 * sizeof(unsigned long long))) return rc;
+  unsigned long long* acc = (unsigned long long*)ctx->d_work;
   CK(cudaMemsetAsync(acc, 0, 8 * sizeof(unsigned long long), ctx->stream));
   k_utxo_digest<<<nblk(t->mask + 1, 128), 128, 0, ctx->stream>>>(view_of(t), acc);
   CK(cudaGetLastError());
@@ -942,12 +993,12 @@ __global__ void k_count_status(const kgv_tx_result* __restrict__ res, uint32_t n
 // The script phase of a validation call against a table (kgv_validate_txs, kgv_validate_mempool_txs), then the device script engine for what
 // it declined: utxo_validation.rs:282-309 accepts ANY transaction whose scripts execute successfully, so a non-standard spend must not leave
 // the call undecided.  The engine runs on the entries the call populated (v.entries), long scripts in the table's overflow arena included.
-static int scripts_with_engine(kgv_ctx* ctx, kgv_utxo_table* table, const kgv_dev_batch& d, const BatchView& v, const uint32_t* itx, kgv_tx_result* dres) {
+// cnt: one u64 of device scratch of the call (not of the table, which other contexts may be reading at the same time).
+static int scripts_with_engine(kgv_ctx* ctx, unsigned long long* cnt, const kgv_dev_batch& d, const BatchView& v, const uint32_t* itx, kgv_tx_result* dres) {
   const size_t nt = d.n_txs;
   int rc = kgv_scripts_phase(ctx, v, nt, d.n_inputs, itx, dres, nullptr);
   if (rc) return rc;
   cudaStream_t st = ctx->stream;
-  unsigned long long* cnt = table->counters + 4;
   unsigned long long n_vm = 0;
   CK(cudaMemsetAsync(cnt, 0, 8, st));
   k_count_status<<<nblk(nt, 256), 256, 0, st>>>(dres, (uint32_t)nt, KGV_TX_NEEDS_HOST_VM, cnt);
@@ -966,6 +1017,9 @@ static int validate_core(kgv_ctx* ctx, kgv_utxo_table* table, const kgv_tx_batch
   if (int rc = kgv_host_only(ctx, table ? "kgv_validate_txs" : "kgv_validate_populated", "params", prm)) return rc;
   if (batch->n_txs == 0) return KGV_OK;
   CK(cudaSetDevice(ctx->device));
+  kgv_table_access acc(ctx);
+  if (table)
+    if (int rc = acc.acquire("kgv_validate_txs", table)) return rc;
   kgv_dev_batch d;
   int rc = kgv_batch_to_device(ctx, batch, &d, table == nullptr);
   if (rc) return rc;
@@ -973,7 +1027,8 @@ static int validate_core(kgv_ctx* ctx, kgv_utxo_table* table, const kgv_tx_batch
   size_t o_ent = 0;
   size_t o_itx = al256(o_ent + ni * sizeof(DevEntry));
   size_t o_res = al256(o_itx + ni * 4);
-  rc = kgv_reserve(ctx, &ctx->d_work, &ctx->d_work_cap, al256(o_res + nt * sizeof(kgv_tx_result)));
+  size_t o_cnt = al256(o_res + nt * sizeof(kgv_tx_result));
+  rc = kgv_reserve(ctx, &ctx->d_work, &ctx->d_work_cap, o_cnt + 8);
   if (rc) return rc;
   uint8_t* S = ctx->d_work;
   DevEntry* dent = (DevEntry*)(S + o_ent);
@@ -996,7 +1051,7 @@ static int validate_core(kgv_ctx* ctx, kgv_utxo_table* table, const kgv_tx_batch
   ctx->launches++;
   STAGE("tx_context");
   if (flags != KGV_FLAGS_SKIP_SCRIPT_CHECKS && ni) {
-    rc = table ? scripts_with_engine(ctx, table, d, v, itx, dres) : kgv_scripts_phase(ctx, v, nt, ni, itx, dres, nullptr);
+    rc = table ? scripts_with_engine(ctx, (unsigned long long*)(S + o_cnt), d, v, itx, dres) : kgv_scripts_phase(ctx, v, nt, ni, itx, dres, nullptr);
     if (rc) return rc;
   }
   kgv_io io(ctx);
@@ -1047,6 +1102,9 @@ static int mempool_core(kgv_ctx* ctx, kgv_utxo_table* t, const kgv_tx_batch* bat
   if (batch->n_txs == 0) return KGV_OK;
   if (iso && batch->n_txs > 0xFFFFFFFFull) { ctx->err = "kgv_validate_mempool_txs_in_parallel: more than 2^32 - 1 transactions"; return KGV_ERR_ARG; }
   CK(cudaSetDevice(ctx->device));
+  // one read of the table for the three mempool calls, over the whole call: kernels enqueued after its host synchronisations still read it
+  kgv_table_access acc(ctx);
+  if (int rc = acc.acquire(call, t)) return rc;
   kgv_io io(ctx);
   bool dev;
   if (int rc = io.one_side(call, {results, batch->txs, args, storage_mass, entries_out, scripts_cap ? scripts_out : nullptr,
@@ -1057,7 +1115,8 @@ static int mempool_core(kgv_ctx* ctx, kgv_utxo_table* t, const kgv_tx_batch* bat
   if (rc) return rc;
   const size_t nt = d.n_txs, ni = d.n_inputs;
   // d_work: populated entries, input -> tx, verdicts, masses, script lengths and their offsets,
-  // counters [script bytes (64-bit), zero divisors, the scan's 32-bit total, the relay-fee overflow flag of the standardness policy]
+  // counters [script bytes (64-bit), zero divisors, the scan's 32-bit total, the relay-fee overflow flag of the standardness policy, the
+  // script engine's count]
   size_t o_ent = 0;
   size_t o_itx = al256(o_ent + ni * sizeof(DevEntry));
   size_t o_res = al256(o_itx + ni * 4);
@@ -1069,11 +1128,11 @@ static int mempool_core(kgv_ctx* ctx, kgv_utxo_table* t, const kgv_tx_batch* bat
   const kgv_mempool_policy* pol = iso ? iso->policy : nullptr;
   uint64_t* detail = iso ? iso->detail : nullptr;
   const bool own_masses = iso && !iso->masses && pol;
-  size_t o_iso = al256(o_cnt + 32);
+  size_t o_iso = al256(o_cnt + 40);
   size_t o_nc = al256(o_iso + (iso ? nt * sizeof(kgv_tx_result) : 0));
   size_t o_ism = al256(o_nc + (iso ? nt * 8 : 0));
   size_t o_lst = al256(o_ism + (own_masses ? nt * sizeof(kgv_tx_masses) : 0));
-  rc = kgv_reserve(ctx, &ctx->d_work, &ctx->d_work_cap, iso ? al256(o_lst + (nt + 1) * 4) : al256(o_cnt + 32));
+  rc = kgv_reserve(ctx, &ctx->d_work, &ctx->d_work_cap, iso ? al256(o_lst + (nt + 1) * 4) : al256(o_cnt + 40));
   if (rc) return rc;
   // the entries' scripts come back up to their size, known after the context rules
   const kgv_mempool_tx_args* dargs;
@@ -1143,7 +1202,7 @@ static int mempool_core(kgv_ctx* ctx, kgv_utxo_table* t, const kgv_tx_batch* bat
     io.trim(scripts_out, n_script);
   }
   if (ni) {
-    rc = scripts_with_engine(ctx, t, d, v, itx, dres);
+    rc = scripts_with_engine(ctx, cnt + 4, d, v, itx, dres);
     if (rc) return rc;
   }
   unsigned long long* fee_overflow = cnt + 3;
@@ -1198,6 +1257,8 @@ extern "C" int kgv_utxo_apply_accepted(kgv_ctx* ctx, kgv_utxo_table* t, const kg
   if (!batch || (batch->n_txs && !accept)) { ctx->err = "null argument"; return KGV_ERR_ARG; }
   if (batch->n_txs == 0) return KGV_OK;
   CK(cudaSetDevice(ctx->device));
+  kgv_table_access acc(ctx);
+  if (int rc = acc.acquire("kgv_utxo_apply_accepted", t, t)) return rc;
   int rc = utxo_reserve(ctx, t, batch->n_outputs + (t->base ? batch->n_inputs : 0), batch->n_bytes + 8 * (uint64_t)batch->n_outputs);
   if (rc) return rc;
   kgv_dev_batch d;
@@ -1237,6 +1298,9 @@ extern "C" int kgv_muhash_txs(kgv_ctx* ctx, kgv_utxo_table* table, const kgv_tx_
   kgv_io io(ctx);
   if (int rc = io.one_side("kgv_muhash_txs", {numerator384, denominator384})) return rc;
   CK(cudaSetDevice(ctx->device));
+  kgv_table_access acc(ctx);
+  if (table)
+    if (int rc = acc.acquire("kgv_muhash_txs", table)) return rc;
   kgv_dev_batch d;
   d.n_txs = d.n_inputs = d.n_outputs = d.n_bytes = 0;
   if (batch->n_txs) {
@@ -1287,6 +1351,8 @@ extern "C" int kgv_utxo_muhash(kgv_ctx* ctx, kgv_utxo_table* t, uint8_t* numerat
   if (!numerator384) { ctx->err = "null argument"; return KGV_ERR_ARG; }
   if (t->base) { ctx->err = "count / digest / MuHash are defined on plain tables: commit the view first"; return KGV_ERR_ARG; }
   CK(cudaSetDevice(ctx->device));
+  kgv_table_access acc(ctx);
+  if (int rc = acc.acquire("kgv_utxo_muhash", t)) return rc;
   const uint64_t slots = t->mask + 1;
   const size_t chunk = slots < ((uint64_t)1 << 17) ? (size_t)slots : ((size_t)1 << 17);
   const size_t n_chunks = (size_t)((slots + chunk - 1) / chunk);

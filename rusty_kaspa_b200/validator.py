@@ -158,9 +158,17 @@ class GpuUtxoSet:
         self._h = h
 
     def close(self):
-        if self._h:
+        if self._h and getattr(self, "_owner", True):
             self._lib.kgv_utxo_destroy(self.ctx._h, self._h)
-            self._h = None
+        self._h = None
+
+    def on(self, ctx):
+        """This same table with its calls issued on `ctx`, another context of its device (include/kgv.h, Threading).  The returned object
+        does not own the table: close() on it only drops the handle."""
+        v = GpuUtxoSet.__new__(GpuUtxoSet)
+        v.__dict__.update(self.__dict__)
+        v.ctx, v._owner = ctx, False
+        return v
 
     # ---- composed views (utxo_view.rs:22-35): a diff layer over this set
     def compose(self, capacity_slots=1 << 16):
