@@ -320,7 +320,8 @@ int kgv_utxo_import_chunk(kgv_ctx* ctx, kgv_utxo_table* t, const uint8_t* keys36
  * its first enqueued access to its last, host synchronisations inside it included; a call touching several tables takes them bottom layer
  * first.  Arrays a write gives up (rehash, growth) are freed once that write has completed on the GPU, at the writing context's
  * kgv_synchronize or kgv_destroy; kgv_utxo_destroy frees the rest.  With one context nothing changes but one event record and one stream wait
- * per table and call.  A table must outlive every call on it, from every context. */
+ * per table and call.  A table must outlive every call on it, from every context.  The partitions of a key cache shared by several contexts
+ * (kgv_keycache_share) take the same lock, per verify launch and always after a call's tables (Key cache, Threading). */
 int kgv_utxo_view_create(kgv_ctx* ctx, kgv_utxo_table* base, uint64_t capacity_slots, kgv_utxo_table** out);
 int kgv_utxo_view_commit(kgv_ctx* ctx, kgv_utxo_table* view);
 int kgv_utxo_view_discard(kgv_ctx* ctx, kgv_utxo_table* view);
@@ -511,29 +512,44 @@ int kgv_set_sigcache(kgv_ctx* ctx, kgv_sigcache* cache /* NULL: detach */);
  * its tables on every secp256k1_schnorrsig_verify / secp256k1_ecdsa_verify, and so does every verify launch here without it (per-launch
  * records only in launches of more items than the device's resident threads whose keys repeat).
  * An opt-in, device-resident table of comb-form key records (8 320 bytes each, about 8.4 KB per key with its slot: 2^16 keys take about
- * 550 MB), owned by one context and off by default.  While it is on, every verify launch of that context (the verify entry points,
- * validation, mempool validation, replay windows, the device script engine, the SigCache's misses) looks its keys up: a stored key's
- * signatures run the 30-doubling joint comb ladder from the stored record whatever the launch's size, the other keys are verified as
- * without the cache and stored for the next launch (a launch of at most one item per resident thread stores them after its verification,
- * off the call's path; a larger one stores them first when the per-launch rule would prepare records and the cache holds them all, else it
- * runs as without the cache).  Verdicts never depend on it.  Where it loses: a launch that stores many new keys (cold large launches build
- * a full record per key, even for keys used a few times), and the call right after one that stored keys (it waits for that insert);
- * DESIGN.md §5 has the numbers.
- * - kgv_keycache_create gives the context its cache, on: one partition per item kind with its own capacity in keys (0: that kind is not
- *   cached), Schnorr keyed by x, ECDSA by tag || x (02 and 03 of one x are two keys).  Both 0, one above KGV_KEYCACHE_MAX_KEYS, or a context
- *   that has a cache is KGV_ERR_ARG; memory that cannot be allocated KGV_ERR_NOMEM.  The cache belongs to the context alone (another
- *   context's inserts could replace a record one of its launches reads); under sharding each rank's context has its own.
- * - Eight-way sets; a full set replaces its least recently used key, never one that the current launch of the kind reads.
- * - kgv_set_keycache turns the lookups off (0) and on again, keeping the records; kgv_keycache_clear empties both partitions and zeroes
- *   their counters; kgv_keycache_destroy waits for the cache's work and frees it (KGV_OK without one; kgv_destroy does the same).
- * - kgv_keycache_counter: a counter of the partition ecdsa selects (0 without a cache, that partition, or with a bad argument; UINT64_MAX
- *   when the device fails): KGV_KEYCACHE_LOOKUPS items looked up, KGV_KEYCACHE_HITS items verified from a stored record (a large launch
- *   the cache does not take counts its lookups, no hits), KGV_KEYCACHE_INSERTS keys stored, KGV_KEYCACHE_EVICTIONS stored keys replaced;
- *   stored keys = inserts - evictions.
+ * 550 MB), off by default, that the contexts of one device can share.  While it is on for a context, every verify launch of that context
+ * (the verify entry points, validation, mempool validation, replay windows, the device script engine, the SigCache's misses) looks its
+ * keys up: a stored key's signatures run the 30-doubling joint comb ladder from the stored record whatever the launch's size, the other
+ * keys are verified as without the cache and stored for the next launch of any context sharing it (a launch of at most one item per
+ * resident thread stores them after its verification, off the call's path; a larger one stores them first when the per-launch rule would
+ * prepare records and the cache holds them all, else it runs as without the cache).  Verdicts never depend on it.  Where it loses: a
+ * launch that stores many new keys (cold large launches build a full record per key, even for keys used a few times), and the call right
+ * after one that stored keys (it waits for that insert); DESIGN.md §5 has the numbers.
+ * - kgv_keycache_create creates a cache and attaches it to the context, on: one partition per item kind with its own capacity in keys (0:
+ *   that kind is not cached), Schnorr keyed by x, ECDSA by tag || x (02 and 03 of one x are two keys).  Both 0, one above
+ *   KGV_KEYCACHE_MAX_KEYS, or a context that has a cache is KGV_ERR_ARG; memory that cannot be allocated KGV_ERR_NOMEM.
+ * - kgv_keycache_share attaches the cache `holder` has to `ctx` as well, on for ctx: one cache per device, so a key the mempool context met
+ *   is stored for the block and template contexts too, and the records exist once.  KGV_ERR_ARG (naming the call) when holder has no cache,
+ *   ctx already has one, ctx == holder, or the two contexts are on different devices.  Under sharding each rank's context has its own cache.
+ * - Eight-way sets; a full set replaces its least recently used key, never one that a launch still running reads.
+ * - kgv_set_keycache turns the context's lookups off (0) and on again, keeping the records; another context attached to the same cache
+ *   keeps its own setting (a mempool context keeps it on while an IBD context turns it off).
+ * - kgv_keycache_clear empties both partitions of the cache and zeroes their counters, for every context attached to it.
+ * - kgv_keycache_destroy detaches the context (KGV_OK without a cache; kgv_destroy does the same) after waiting for its own launches and
+ *   inserts; the records are freed when the last attached context detaches, the creator included, in any order.
+ * - kgv_keycache_counter: a counter of the partition ecdsa selects, shared by every attached context (0 without a cache, that partition, or
+ *   with a bad argument; UINT64_MAX when the device fails): KGV_KEYCACHE_LOOKUPS items looked up, KGV_KEYCACHE_HITS items verified from a
+ *   stored record (a large launch the cache does not take counts its lookups, no hits), KGV_KEYCACHE_INSERTS keys stored,
+ *   KGV_KEYCACHE_EVICTIONS stored keys replaced; stored keys = inserts - evictions.  It covers the launches of every attached context
+ *   enqueued before the call.
+ * Threading: the contexts attached to one cache may run at the same time, each from its own thread.  Each partition has the reader/writer
+ * lock of the UTXO tables (Threading, next to the views), ordered on the GPU by CUDA events: a verify launch READS the partition from its
+ * lookup to the end of its stored-record launch; storing keys, the clear and the counter reads WRITE it.  A launch's stamps and counters
+ * are atomics that concurrent readers share, so two contexts' lookups run side by side; an insert waits on the GPU for the reads enqueued
+ * before it and excludes every other access while it runs, so no launch of any context reads a record that is being rewritten.  A
+ * registration covers one launch's enqueue, taken after any UTXO table lock of its call and holding no other lock, so a write waits on the
+ * host only for other contexts to finish enqueuing a launch, never for a whole call or its host synchronisations.  With one context
+ * nothing changes but the lock's event records and stream waits: one of each per lookup, one record and two waits per insert.
  * ------------------------------------------------------------------------------------------------ */
 #define KGV_KEYCACHE_MAX_KEYS (1ull << 20) /* per kind: about 8.8 GB of records */
 enum { KGV_KEYCACHE_LOOKUPS = 0, KGV_KEYCACHE_HITS = 1, KGV_KEYCACHE_INSERTS = 2, KGV_KEYCACHE_EVICTIONS = 3 };
 int kgv_keycache_create(kgv_ctx* ctx, uint64_t schnorr_keys, uint64_t ecdsa_keys);
+int kgv_keycache_share(kgv_ctx* ctx, kgv_ctx* holder);
 int kgv_keycache_destroy(kgv_ctx* ctx);
 int kgv_keycache_clear(kgv_ctx* ctx);
 uint64_t kgv_keycache_counter(kgv_ctx* ctx, int ecdsa, int which);

@@ -440,10 +440,13 @@ class SigCache {
   kgv_sigcache* h_ = nullptr;
 };
 
-// ---- prepared public keys kept across verify launches (kgv_keycache; no counterpart in the reference): the context's own ----
+// ---- prepared public keys kept across verify launches (kgv_keycache; no counterpart in the reference), shared by contexts of one device ----
+// Each KeyCache attaches one context; the records live until the last one is destroyed, in any order.
 class KeyCache {
  public:
   KeyCache(Context& c, uint64_t schnorr_keys, uint64_t ecdsa_keys) : c_(c) { c_.check(kgv_keycache_create(c_.get(), schnorr_keys, ecdsa_keys)); }
+  // the cache of `holder`, attached to c as well (kgv_keycache_share): e.g. the block context's cache shared with the mempool's context
+  KeyCache(Context& c, KeyCache& holder) : c_(c) { c_.check(kgv_keycache_share(c_.get(), holder.c_.get())); }
   ~KeyCache() { kgv_keycache_destroy(c_.get()); }
   KeyCache(const KeyCache&) = delete;
   KeyCache& operator=(const KeyCache&) = delete;

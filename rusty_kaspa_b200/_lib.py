@@ -64,6 +64,7 @@ SYMBOLS = [
     ("kgv_sigcache_counters", _c.c_int, [_c.c_void_p, _c.c_void_p, _c.POINTER(_c.c_uint64), _c.POINTER(_c.c_uint64), _c.POINTER(_c.c_uint64), _c.POINTER(_c.c_uint64)]),
     ("kgv_set_sigcache", _c.c_int, [_c.c_void_p, _c.c_void_p]),
     ("kgv_keycache_create", _c.c_int, [_c.c_void_p, _c.c_uint64, _c.c_uint64]),
+    ("kgv_keycache_share", _c.c_int, [_c.c_void_p, _c.c_void_p]),
     ("kgv_keycache_destroy", _c.c_int, [_c.c_void_p]),
     ("kgv_keycache_clear", _c.c_int, [_c.c_void_p]),
     ("kgv_keycache_counter", _c.c_uint64, [_c.c_void_p, _c.c_int, _c.c_int]),

@@ -79,7 +79,7 @@ struct kgv_ctx {
     uint64_t rehashes = 0;                           // long scripts lie in those layers' arenas
   } last_replay;
   struct kgv_sigcache* sigcache = nullptr;  // kgv_set_sigcache: verdicts of the validation calls are looked up / remembered here
-  struct kgv_keycache* keycache = nullptr;  // kgv_set_keycache: comb key records kept across the verify launches (kgv_lib.cu)
+  struct kgv_keycache* keycache = nullptr;  // the context's attachment to a key cache (kgv_keycache_create / _share, kgv_lib.cu)
   struct kgv_comm* shard_comm = nullptr;  // kgv_set_sharding: signature checks of the validation calls are split over its ranks
   std::vector<uint8_t*> parked;  // outgrown per-call buffers, released when the caller synchronises / destroys the context (kgv_reserve)
   // tables whose arrays a write of this context gave up (rehash, growth): released from the table's list at kgv_synchronize / kgv_destroy
@@ -274,9 +274,10 @@ struct kgv_table_sync {
   cudaEvent_t retire_ev = nullptr;        // (reserved for them by kgv_table_retire)
   struct Retired { cudaEvent_t done; std::vector<void*> ptrs; };
   std::vector<Retired> retired;           // freed once `done` has completed
+  ~kgv_table_sync();                      // destroys the events left (the lock's users have finished on the GPU)
 };
 struct kgv_utxo_table;
-// The registrations of one call, dropped (events recorded on ctx->stream) when it goes out of scope.
+// The registrations of one call, dropped (events recorded on the stream each was taken for: ctx->stream for tables) when it goes out of scope.
 class kgv_table_access {
  public:
   explicit kgv_table_access(kgv_ctx* c) : ctx(c) {}
@@ -286,13 +287,15 @@ class kgv_table_access {
   // A read on every layer of t's view chain, except `written` (a layer of it, or null) which gets a write; bottom layer first, so calls
   // that touch several tables cannot deadlock.  KGV_ERR_ARG, naming `call`, when a layer belongs to another device than the context.
   int acquire(const char* call, kgv_utxo_table* t, kgv_utxo_table* written = nullptr);
+  // A read (or a write) of one bare lock for work enqueued on st, whose release event is recorded there (the key cache's partitions).
+  int acquire(kgv_table_sync* s, bool write, cudaStream_t st);
   void release();
 
  private:
   enum Mode { kNone, kRead, kWrite };
-  int lock(kgv_table_sync* s, Mode m);
+  int lock(kgv_table_sync* s, Mode m, cudaStream_t st);
   kgv_ctx* ctx;
-  struct Held { kgv_table_sync* s; Mode m; cudaEvent_t ev; };
+  struct Held { kgv_table_sync* s; Mode m; cudaEvent_t ev; cudaStream_t st; };
   std::vector<Held> held;
 };
 // Hands an array of t to the table's release list: freed after the open write of ctx (which gave it up) has completed on the GPU.

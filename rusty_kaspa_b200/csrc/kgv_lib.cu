@@ -235,7 +235,7 @@ __global__ void __launch_bounds__(KGV_BLOCK, KGV_PREP_BLOCKS_PER_SM) k_key_prepa
   else key_rec_build(recs + (size_t)r * KGV_KR_WORDS, ECDSA ? w[8] : 2u, w);
 }
 
-// ---- device key cache (kgv_keycache, include/kgv.h): comb-form key records kept across the verify launches of one context ----
+// ---- device key cache (kgv_keycache, include/kgv.h): comb-form key records kept across the verify launches of the contexts sharing it ----
 // One partition per item kind.  Set-associative: a key's set is its key_hash modulo the number of sets; slot s of the partition owns
 // record s (KGV_JR_WORDS words), so there is no allocator and a lookup reads one set.  stamp: the partition launch that last used the
 // slot (0: empty).  A launch stamps the slots it reads, and an insert only takes a slot stamped by an earlier launch (the empty one first,
@@ -829,11 +829,32 @@ static int key_cache_launch(kgv_ctx* ctx, const uint8_t* dpk, size_t n, bool ecd
 }
 
 // ---- device key cache, host side ----
-struct kgv_keycache {
-  bool enabled = true;                  // kgv_set_keycache
+// A cache is its records, shared by every context attached to it (kgv_keycache_share), and one attachment per context: the streams, events
+// and scratch of that context's launches, whose deferred inserts read the scratch of the launch that made them.
+//
+// Each partition has the UTXO tables' reader/writer lock (kgv_table_sync, ordered on the GPU).  A verify launch READS from its k_kc_lookup to
+// the end of its stored-record launch (the stamps and counters it updates are atomics that concurrent readers share); k_kc_insert, at the
+// end of a small launch or before a large one verifies (which then holds the write throughout), k_kc_restamp, kgv_keycache_clear and kgv_keycache_counter WRITE.
+// So while an insert runs, no launch of any context reads the partition but the inserting launch itself, whose hits carry its stamp: the
+// insert's rule (a slot stamped by an earlier launch) keeps what that launch reads, and takes nothing another context still reads.
+// Lock order: the partition is taken inside kgv_launch_verify, after any UTXO table the call holds, and no other lock is taken while it is
+// held; the Schnorr and ECDSA partitions are never held together.  A registration covers one launch's enqueue, never a whole call, so the
+// host synchronisations of a replay window never make another context's insert wait on the host.
+struct kgv_keycache_shared {
   struct Part {
     KcPart v{};
-    uint32_t stamp = 0;                 // launches of the kind so far (the stamp of the last one)
+    kgv_table_sync sync;                // the partition's lock; its mutex also guards stamp
+    uint32_t stamp = 0;                 // stamps handed out so far (the stamp of the last launch)
+  } part[2];
+  ~kgv_keycache_shared() {              // the last attached context detaches: every launch and insert on it has finished
+    for (auto& P : part)
+      for (void* p : {(void*)P.v.sets, (void*)P.v.recs, (void*)P.v.ctr}) if (p) cudaFree(p);
+  }
+};
+struct kgv_keycache {
+  std::shared_ptr<kgv_keycache_shared> shared;  // its reference count: the attached contexts
+  bool enabled = true;                  // kgv_set_keycache, for this context's launches
+  struct Part {
     cudaStream_t side = nullptr;        // the second verify launch, and the deferred inserts of small launches
     cudaEvent_t ev_looked_up = nullptr, ev_verified = nullptr, ev_inserted = nullptr;
     cudaEvent_t ev_done = nullptr;      // the end of the last launch of the kind on its caller's stream
@@ -843,24 +864,59 @@ struct kgv_keycache {
   } part[2];
 };
 
-// waits for every launch and insert of the cache (events, not streams: a caller's stream may be gone by then)
+// waits for every launch and insert of this context's attachment (events, not streams: a caller's stream may be gone by then)
 static void keycache_quiesce(kgv_keycache* kc) {
   for (auto& P : kc->part) {
     if (P.ev_done) cudaEventSynchronize(P.ev_done);
     if (P.side) cudaStreamSynchronize(P.side);
   }
 }
+// detaches the context; the records go with the last attached context
 static void keycache_free(kgv_ctx* ctx) {
   kgv_keycache* kc = ctx->keycache;
   if (!kc) return;
   keycache_quiesce(kc);
   ctx->keycache = nullptr;
   for (auto& P : kc->part) {
-    for (void* p : {(void*)P.v.sets, (void*)P.v.recs, (void*)P.v.ctr, (void*)P.scratch}) if (p) cudaFree(p);
+    if (P.scratch) cudaFree(P.scratch);
     for (cudaEvent_t e : {P.ev_looked_up, P.ev_verified, P.ev_inserted, P.ev_done}) if (e) cudaEventDestroy(e);
     if (P.side) cudaStreamDestroy(P.side);
   }
   delete kc;
+}
+static int keycache_attach(kgv_ctx* ctx, std::shared_ptr<kgv_keycache_shared> shared) {
+  ctx->keycache = new kgv_keycache();
+  ctx->keycache->shared = std::move(shared);
+  for (auto& P : ctx->keycache->part) {
+    CK(cudaStreamCreateWithFlags(&P.side, cudaStreamNonBlocking));
+    for (cudaEvent_t* e : {&P.ev_looked_up, &P.ev_verified, &P.ev_inserted, &P.ev_done}) CK(cudaEventCreateWithFlags(e, cudaEventDisableTiming));
+  }
+  return KGV_OK;
+}
+
+// Takes partition P's lock for work on st, a write when `write`.  A verify launch gets its stamp here; at the stamps' wrap every used slot
+// restarts at 1 (k_kc_restamp), which only a write may do, so a read that meets the wrap is taken again as a write.  A deferred insert
+// (insert) stamps with the last stamp handed out, its own launch's when one context uses the cache: no launch reads during an insert, so
+// the stamp only keeps the slots of the last launch, of any context, as the most recently used.
+static int kc_lock(kgv_ctx* ctx, kgv_table_access& acc, kgv_keycache_shared::Part& P, bool write, cudaStream_t st, bool insert, uint32_t* stamp) {
+  for (;;) {
+    if (int rc = acc.acquire(&P.sync, write, st)) return rc;
+    bool wrap;
+    {
+      std::lock_guard<std::mutex> g(P.sync.m);
+      wrap = !insert && P.stamp + 1 == 0xFFFFFFFFu;
+      if (write || !wrap) *stamp = insert ? P.stamp : wrap ? (P.stamp = 2) : ++P.stamp;
+    }
+    if (!wrap) return KGV_OK;
+    if (write) {
+      k_kc_restamp<<<nblk(P.v.n_sets, 256), 256, 0, st>>>(P.v.sets, P.v.n_sets);
+      CK(cudaGetLastError());
+      ctx->launches++;
+      return KGV_OK;
+    }
+    acc.release();
+    write = true;
+  }
 }
 
 struct KcScratch {
@@ -869,8 +925,8 @@ struct KcScratch {
   KeySlot* table;
   uint32_t slots;
 };
-// Starts a launch of partition P on st: after the kind's previous insert, with this launch's stamp and cleared launch words.  The scratch
-// is sized from the host's n (an upper bound of *n_dev when given) and, like the per-launch key cache's, belongs to the kind.
+// Starts a launch of the attachment's partition P on st: after the kind's previous insert of this context, with cleared launch words.
+// The scratch is sized from the host's n (an upper bound of *n_dev when given) and, like the per-launch key cache's, belongs to the kind.
 static int kc_begin(kgv_ctx* ctx, kgv_keycache::Part& P, size_t n, bool ecdsa, cudaStream_t st, KcScratch* s) {
   if (P.pending) CK(cudaStreamWaitEvent(st, P.ev_inserted, 0));
   P.pending = false;
@@ -883,28 +939,22 @@ static int kc_begin(kgv_ctx* ctx, kgv_keycache::Part& P, size_t n, bool ecdsa, c
   uint8_t* S = P.scratch;
   *s = KcScratch{(uint32_t*)S, (uint32_t*)(S + o_irec), (uint32_t*)(S + o_ord), (uint32_t*)(S + o_mord), (uint32_t*)(S + o_islot), (uint32_t*)(S + o_rep), S + o_mk,
                  (KeySlot*)(S + o_tab), slots};
-  if (++P.stamp == 0xFFFFFFFFu) {
-    k_kc_restamp<<<nblk(P.v.n_sets, 256), 256, 0, st>>>(P.v.sets, P.v.n_sets);
-    CK(cudaGetLastError());
-    ctx->launches++;
-    P.stamp = 2;
-  }
   CK(cudaMemsetAsync(S, 0, 256, st));
   return KGV_OK;
 }
-// the insert of a launch's misses on st: k_key_dedup over the miss keys, then k_kc_insert
-static int kc_insert(kgv_ctx* ctx, kgv_keycache::Part& P, const KcScratch& s, size_t n, bool ecdsa, cudaStream_t st, bool gate) {
+// the insert of a launch's misses into partition p on st: k_key_dedup over the miss keys, then k_kc_insert
+static int kc_insert(kgv_ctx* ctx, const KcPart& p, const KcScratch& s, size_t n, bool ecdsa, cudaStream_t st, uint32_t stamp, bool gate) {
   CK(cudaMemsetAsync(s.table, 0, (size_t)s.slots * sizeof(KeySlot), st));
   // (the miss keys are packed from a 256-byte aligned base: Schnorr's are word aligned)
   // a large launch's insert takes at most the partition's slots and KGV_KEY_RECORDS_MAX keys (k_kc_insert's gate): past that many the
   // dedup stops, the gate refuses the launch
-  const uint32_t slots = P.v.n_sets * KGV_KC_WAYS, limit = gate ? std::min(slots, (uint32_t)KGV_KEY_RECORDS_MAX) : 0xFFFFFFFFu;
+  const uint32_t slots = p.n_sets * KGV_KC_WAYS, limit = gate ? std::min(slots, (uint32_t)KGV_KEY_RECORDS_MAX) : 0xFFFFFFFFu;
   const auto dedup = ecdsa ? k_key_dedup<false, true, true> : k_key_dedup<true, false, true>;
   dedup<<<nblk(n, 256), 256, 0, st>>>(s.miss_keys, n, nullptr, s.hdr + KC_N_MISS, s.table, s.slots - 1, s.item_slot, s.rec_rep, s.hdr + KC_N_REC,
                                       limit);
   CK(cudaGetLastError());
   const auto insert = ecdsa ? k_kc_insert<true> : k_kc_insert<false>;
-  insert<<<nblk(n, KGV_BLOCK), KGV_BLOCK, 0, st>>>(P.v, s.miss_keys, s.rec_rep, s.hdr, P.stamp, gate);
+  insert<<<nblk(n, KGV_BLOCK), KGV_BLOCK, 0, st>>>(p, s.miss_keys, s.rec_rep, s.hdr, stamp, gate);
   CK(cudaGetLastError());
   ctx->launches += 2;
   return KGV_OK;
@@ -928,12 +978,13 @@ int kgv_launch_verify(kgv_ctx* ctx, const uint8_t* dpk, const uint8_t* dmsg, con
   // others by a second launch, of the form they take without the cache, on the partition's side stream at the same time; st waits for
   // it.  A small launch stores its misses afterwards on the side stream, off the call's path; a large one stores them first when its insert
   // takes the launch (k_kc_insert), else every item goes to the second launch, which then runs as without the cache.
-  kgv_keycache::Part* kp = ctx->keycache && ctx->keycache->enabled && ctx->keycache->part[ecdsa].v.n_sets ? &ctx->keycache->part[ecdsa] : nullptr;
+  kgv_keycache* cache = ctx->keycache;
+  kgv_keycache_shared::Part* sp = cache && cache->enabled && cache->shared->part[ecdsa].v.n_sets ? &cache->shared->part[ecdsa] : nullptr;
   if (!index) {
     auto& lv = ctx->last_verify[ecdsa];
-    lv.n = n; lv.blocks = blocks; lv.key_cache = key_cache && !kp; lv.stream = st;
+    lv.n = n; lv.blocks = blocks; lv.key_cache = key_cache && !sp; lv.stream = st;
   }
-  if (!kp) {
+  if (!sp) {
     if (key_cache) {
       int rc = key_cache_launch(ctx, dpk, n, ecdsa, aligned, st, index, n_dev, &kc);
       if (rc) return rc;
@@ -943,17 +994,21 @@ int kgv_launch_verify(kgv_ctx* ctx, const uint8_t* dpk, const uint8_t* dmsg, con
     ctx->launches++;
     return KGV_OK;
   }
+  kgv_keycache::Part* kp = &cache->part[ecdsa];
   KcScratch ks{};
   if (int rc = kc_begin(ctx, *kp, n, ecdsa, st, &ks)) return rc;
+  kgv_table_access acc(ctx);
+  uint32_t stamp;
+  if (int rc = kc_lock(ctx, acc, *sp, key_cache, st, false, &stamp)) return rc;
   const auto lookup = ecdsa ? k_kc_lookup<false, true> : aligned ? k_kc_lookup<true, false> : k_kc_lookup<false, false>;
-  lookup<<<nblk(n, 256), 256, 0, st>>>(dpk, n, index, n_dev, kp->v, kp->stamp, key_cache ? KC_COUNT : KC_COUNT | KC_ORDER, ks.hdr, ks.item_rec,
+  lookup<<<nblk(n, 256), 256, 0, st>>>(dpk, n, index, n_dev, sp->v, stamp, key_cache ? KC_COUNT : KC_COUNT | KC_ORDER, ks.hdr, ks.item_rec,
                                        ks.order, ks.miss_order, ks.miss_keys);
   CK(cudaGetLastError());
   ctx->launches++;
   if (key_cache) {
-    if (int rc = kc_insert(ctx, *kp, ks, n, ecdsa, st, true)) return rc;
+    if (int rc = kc_insert(ctx, sp->v, ks, n, ecdsa, st, stamp, true)) return rc;
     if (int rc = key_cache_launch(ctx, dpk, n, ecdsa, aligned, st, index, n_dev, &kc, ks.hdr)) return rc;
-    lookup<<<nblk(n, 256), 256, 0, st>>>(dpk, n, index, n_dev, kp->v, kp->stamp, KC_ORDER | KC_GATED, ks.hdr, ks.item_rec, ks.order, ks.miss_order,
+    lookup<<<nblk(n, 256), 256, 0, st>>>(dpk, n, index, n_dev, sp->v, stamp, KC_ORDER | KC_GATED, ks.hdr, ks.item_rec, ks.order, ks.miss_order,
                                          ks.miss_keys);
     CK(cudaGetLastError());
     ctx->launches++;
@@ -962,9 +1017,10 @@ int kgv_launch_verify(kgv_ctx* ctx, const uint8_t* dpk, const uint8_t* dmsg, con
   CK(cudaStreamWaitEvent(kp->side, kp->ev_looked_up, 0));
   KeyCacheView stored{};
   stored.item_rec = ks.item_rec;
-  stored.kc_recs = kp->v.recs;
+  stored.kc_recs = sp->v.recs;
   k_verify[ecdsa][1][aligned]<<<blocks, KGV_BLOCK, smem, st>>>(dpk, dmsg, dsig, n, dst, ctx->gtab, ks.order, ks.hdr + KC_ORD_HIT, stored);
   CK(cudaGetLastError());
+  acc.release();  // the last read of the partition's records
   k_verify[ecdsa][1][aligned]<<<blocks, KGV_BLOCK, smem, kp->side>>>(dpk, dmsg, dsig, n, dst, ctx->gtab, ks.miss_order, ks.hdr + KC_ORD_MISS, kc);
   CK(cudaGetLastError());
   ctx->launches += 2;
@@ -972,7 +1028,9 @@ int kgv_launch_verify(kgv_ctx* ctx, const uint8_t* dpk, const uint8_t* dmsg, con
   CK(cudaStreamWaitEvent(st, kp->ev_verified, 0));
   CK(cudaEventRecord(kp->ev_done, st));
   if (!key_cache) {
-    if (int rc = kc_insert(ctx, *kp, ks, n, ecdsa, kp->side, false)) return rc;
+    if (int rc = kc_lock(ctx, acc, *sp, true, kp->side, true, &stamp)) return rc;
+    if (int rc = kc_insert(ctx, sp->v, ks, n, ecdsa, kp->side, stamp, false)) return rc;
+    acc.release();
     CK(cudaEventRecord(kp->ev_inserted, kp->side));
     kp->pending = true;
   }
@@ -987,26 +1045,41 @@ extern "C" int kgv_keycache_create(kgv_ctx* ctx, uint64_t schnorr_keys, uint64_t
   if (schnorr_keys > KGV_KEYCACHE_MAX_KEYS || ecdsa_keys > KGV_KEYCACHE_MAX_KEYS)
     return fail_arg(ctx, "kgv_keycache_create: a capacity above KGV_KEYCACHE_MAX_KEYS");
   CK(cudaSetDevice(ctx->device));
-  ctx->keycache = new kgv_keycache();
-  auto body = [&]() -> int {
-    for (int k = 0; k < 2; k++) {
-      auto& P = ctx->keycache->part[k];
-      CK(cudaStreamCreateWithFlags(&P.side, cudaStreamNonBlocking));
-      for (cudaEvent_t* e : {&P.ev_looked_up, &P.ev_verified, &P.ev_inserted, &P.ev_done}) CK(cudaEventCreateWithFlags(e, cudaEventDisableTiming));
-      const uint64_t keys = k ? ecdsa_keys : schnorr_keys;
-      if (!keys) continue;
-      const uint32_t n_sets = (uint32_t)((keys + KGV_KC_WAYS - 1) / KGV_KC_WAYS);
-      if (int rc = kgv_malloc(ctx, (void**)&P.v.sets, (size_t)n_sets * sizeof(KcSet))) return rc;
-      if (int rc = kgv_malloc(ctx, (void**)&P.v.recs, (size_t)n_sets * KGV_KC_WAYS * KGV_JR_WORDS * 4)) return rc;
-      if (int rc = kgv_malloc(ctx, (void**)&P.v.ctr, 4 * sizeof(unsigned long long))) return rc;
-      P.v.n_sets = n_sets;
-      CK(cudaMemsetAsync(P.v.sets, 0, (size_t)n_sets * sizeof(KcSet), ctx->stream));
-      CK(cudaMemsetAsync(P.v.ctr, 0, 4 * sizeof(unsigned long long), ctx->stream));
-    }
-    CK(cudaStreamSynchronize(ctx->stream));
-    return KGV_OK;
-  };
-  if (int rc = body()) {
+  auto shared = std::make_shared<kgv_keycache_shared>();
+  for (int k = 0; k < 2; k++) {
+    auto& P = shared->part[k];
+    P.sync.device = ctx->device;
+    const uint64_t keys = k ? ecdsa_keys : schnorr_keys;
+    if (!keys) continue;
+    const uint32_t n_sets = (uint32_t)((keys + KGV_KC_WAYS - 1) / KGV_KC_WAYS);
+    if (int rc = kgv_malloc(ctx, (void**)&P.v.sets, (size_t)n_sets * sizeof(KcSet))) return rc;
+    if (int rc = kgv_malloc(ctx, (void**)&P.v.recs, (size_t)n_sets * KGV_KC_WAYS * KGV_JR_WORDS * 4)) return rc;
+    if (int rc = kgv_malloc(ctx, (void**)&P.v.ctr, 4 * sizeof(unsigned long long))) return rc;
+    P.v.n_sets = n_sets;
+    CK(cudaMemsetAsync(P.v.sets, 0, (size_t)n_sets * sizeof(KcSet), ctx->stream));
+    CK(cudaMemsetAsync(P.v.ctr, 0, 4 * sizeof(unsigned long long), ctx->stream));
+  }
+  CK(cudaStreamSynchronize(ctx->stream));
+  if (int rc = keycache_attach(ctx, std::move(shared))) {
+    keycache_free(ctx);
+    return rc;
+  }
+  return KGV_OK;
+}
+
+extern "C" int kgv_keycache_share(kgv_ctx* ctx, kgv_ctx* holder) {
+  if (!ctx || !holder) return KGV_ERR_ARG;
+  if (ctx == holder) return fail_arg(ctx, "kgv_keycache_share: ctx and holder are the same context");
+  std::scoped_lock g(ctx->mu, holder->mu);
+  if (!holder->keycache) return fail_arg(ctx, "kgv_keycache_share: the holder has no key cache");
+  if (ctx->keycache) return fail_arg(ctx, "kgv_keycache_share: the context has a key cache");
+  if (ctx->device != holder->device) {
+    ctx->err = "kgv_keycache_share: the holder's cache is on device " + std::to_string(holder->device) + ", the context on device " +
+               std::to_string(ctx->device);
+    return KGV_ERR_ARG;
+  }
+  CK(cudaSetDevice(ctx->device));
+  if (int rc = keycache_attach(ctx, holder->keycache->shared)) {
     keycache_free(ctx);
     return rc;
   }
@@ -1021,15 +1094,17 @@ extern "C" int kgv_keycache_destroy(kgv_ctx* ctx) {
   return KGV_OK;
 }
 
+// a write on each partition in turn: it waits for the launches and inserts of every attached context enqueued before it
 extern "C" int kgv_keycache_clear(kgv_ctx* ctx) {
   if (!ctx) return KGV_ERR_ARG;
   std::lock_guard<std::recursive_mutex> g(ctx->mu);
   kgv_keycache* kc = ctx->keycache;
   if (!kc) return fail_arg(ctx, "kgv_keycache_clear: the context has no key cache");
   CK(cudaSetDevice(ctx->device));
-  keycache_quiesce(kc);
-  for (auto& P : kc->part) {
+  for (auto& P : kc->shared->part) {
     if (!P.v.n_sets) continue;
+    kgv_table_access acc(ctx);
+    if (int rc = acc.acquire(&P.sync, true, ctx->stream)) return rc;
     CK(cudaMemsetAsync(P.v.sets, 0, (size_t)P.v.n_sets * sizeof(KcSet), ctx->stream));
     CK(cudaMemsetAsync(P.v.ctr, 0, 4 * sizeof(unsigned long long), ctx->stream));
   }
@@ -1037,20 +1112,24 @@ extern "C" int kgv_keycache_clear(kgv_ctx* ctx) {
   return KGV_OK;
 }
 
+// read under a write, so that the value covers the launches of every attached context enqueued before the call
 extern "C" uint64_t kgv_keycache_counter(kgv_ctx* ctx, int ecdsa, int which) {
   if (!ctx) return 0;
   std::lock_guard<std::recursive_mutex> g(ctx->mu);
   kgv_keycache* kc = ctx->keycache;
   if (!kc || which < 0 || which > 3) return 0;
-  const auto& P = kc->part[ecdsa ? 1 : 0];
+  const int k = ecdsa ? 1 : 0;
+  auto& P = kc->shared->part[k];
   if (!P.v.n_sets) return 0;
   unsigned long long v = 0;
+  const cudaStream_t side = kc->part[k].side;
   cudaError_t e = cudaSetDevice(ctx->device);
   if (e == cudaSuccess) {
-    keycache_quiesce(kc);
-    e = cudaMemcpyAsync(&v, P.v.ctr + which, sizeof v, cudaMemcpyDeviceToHost, P.side);
+    kgv_table_access acc(ctx);
+    if (acc.acquire(&P.sync, true, side)) return UINT64_MAX;
+    e = cudaMemcpyAsync(&v, P.v.ctr + which, sizeof v, cudaMemcpyDeviceToHost, side);
   }
-  if (e == cudaSuccess) e = cudaStreamSynchronize(P.side);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(side);
   if (e != cudaSuccess) {
     ctx->err = std::string("kgv_keycache_counter: ") + cudaGetErrorString(e);
     (void)cudaGetLastError();

@@ -170,10 +170,16 @@ static int pooled_event(kgv_table_sync* s, cudaEvent_t* ev) {  // (s->m held)
   return cudaEventCreateWithFlags(ev, cudaEventDisableTiming) == cudaSuccess ? KGV_OK : KGV_ERR_CUDA;
 }
 
-int kgv_table_access::lock(kgv_table_sync* s, Mode m) {
+kgv_table_sync::~kgv_table_sync() {
+  for (const auto& r : reads) cudaEventDestroy(r.second);
+  for (const auto& r : retired) cudaEventDestroy(r.done);
+  for (cudaEvent_t e : pool) cudaEventDestroy(e);
+  for (cudaEvent_t e : {last_write, retire_ev}) if (e) cudaEventDestroy(e);
+}
+
+int kgv_table_access::lock(kgv_table_sync* s, Mode m, cudaStream_t st) {
   std::unique_lock<std::mutex> g(s->m);
-  cudaStream_t st = ctx->stream;
-  Held h{s, m, nullptr};
+  Held h{s, m, nullptr, st};
   if (s->writer == ctx && s->write_depth > 0) {  // nested in this context's own write
     if (m == kWrite) s->write_depth++;
     else h.m = kNone;
@@ -228,16 +234,18 @@ int kgv_table_access::acquire(const char* call, kgv_utxo_table* t, kgv_utxo_tabl
     chain[n++] = L;
   }
   while (n--)
-    if (int rc = lock(chain[n]->sync.get(), chain[n] == written ? kWrite : kRead)) return rc;
+    if (int rc = lock(chain[n]->sync.get(), chain[n] == written ? kWrite : kRead, ctx->stream)) return rc;
   return KGV_OK;
 }
 
+int kgv_table_access::acquire(kgv_table_sync* s, bool write, cudaStream_t st) { return lock(s, write ? kWrite : kRead, st); }
+
 void kgv_table_access::release() {
-  cudaStream_t st = ctx->stream;
   while (!held.empty()) {
     Held h = held.back();
     held.pop_back();
     kgv_table_sync* s = h.s;
+    const cudaStream_t st = h.st;
     std::lock_guard<std::mutex> g(s->m);
     if (h.m == kWrite) {
       if (--s->write_depth) continue;

@@ -580,9 +580,10 @@ class SigCache:
 
 
 class KeyCache:
-    """The context's device cache of prepared public keys (kgv_keycache): comb-form key records kept across verify launches, so a key met
-    before runs the joint comb ladder in launches of any size.  Capacities are in keys per kind (about 8.4 KB each).  Created on; detach()
-    / attach() turn its lookups off and on (records kept); verdicts never change."""
+    """A device cache of prepared public keys (kgv_keycache): comb-form key records kept across verify launches, so a key met before runs
+    the joint comb ladder in launches of any size.  Capacities are in keys per kind (about 8.4 KB each).  Created on; detach() / attach()
+    turn this context's lookups off and on (records kept); verdicts never change.  on(ctx) shares the cache with another context of the
+    device."""
 
     _NAMES = ("lookups", "hits", "inserts", "evictions")
 
@@ -590,6 +591,15 @@ class KeyCache:
         self.ctx = ctx
         ctx._check(ctx._lib.kgv_keycache_create(ctx._h, int(schnorr_keys), int(ecdsa_keys)))
         self._open = True
+
+    def on(self, ctx):
+        """The same cache attached to `ctx`, another context of its device (kgv_keycache_share), as a handle of its own: its attach() /
+        detach() switch ctx's lookups, its close() detaches ctx.  The records live until every handle is closed (or its context destroyed),
+        in any order."""
+        ctx._check(ctx._lib.kgv_keycache_share(ctx._h, self.ctx._h))
+        v = KeyCache.__new__(KeyCache)
+        v.ctx, v._open = ctx, True
+        return v
 
     def attach(self):
         self.ctx._check(self.ctx._lib.kgv_set_keycache(self.ctx._h, 1))
