@@ -81,15 +81,19 @@ k_body_sets(const kgv_tx* __restrict__ txs, const kgv_input* __restrict__ inputs
   }
 }
 
-size_t kgv_body_sets_scratch(size_t n_txs, size_t n_inputs) { return al256(8 * (n_txs + n_inputs)); }
+void kgv_body_sets_work::carve(kgv_carve& c, size_t n_txs, size_t n_inputs) {
+  const size_t at = c.at;
+  tab = c.take<uint32_t>(2 * (n_txs + n_inputs));
+  bytes = c.at - at;
+}
 
 int kgv_body_sets_run(kgv_ctx* ctx, const kgv_dev_batch& d, size_t n_txs, const uint64_t* dids, const uint32_t* dfirst, uint32_t n_blocks,
-                      kgv_block_check_acc* dacc, uint32_t* dtab, cudaStream_t st) {
+                      kgv_block_check_acc* dacc, const kgv_body_sets_work& w, cudaStream_t st) {
   // the key of the sets' hashes (body_hash_id / body_hash_outpoint), drawn once per process; the verdicts do not depend on it
   static const uint64_t salt = [] { std::random_device r; return (uint64_t)r() << 32 | r(); }();
   if (n_blocks == 0 || n_txs == 0) return KGV_OK;
-  CK(cudaMemsetAsync(dtab, 0xFF, kgv_body_sets_scratch(n_txs, d.n_inputs), st));
-  k_body_sets<<<std::min(n_blocks, BODY_MAX_GRID), BODY_SET_THREADS, 0, st>>>(d.txs, d.inputs, dids, dfirst, n_blocks, (uint32_t)n_txs, salt, dacc, dtab);
+  CK(cudaMemsetAsync(w.tab, 0xFF, w.bytes, st));
+  k_body_sets<<<std::min(n_blocks, BODY_MAX_GRID), BODY_SET_THREADS, 0, st>>>(d.txs, d.inputs, dids, dfirst, n_blocks, (uint32_t)n_txs, salt, dacc, w.tab);
   CK(cudaGetLastError());
   ctx->launches++;
   return KGV_OK;
@@ -212,17 +216,21 @@ extern "C" int kgv_validate_block_bodies(kgv_ctx* ctx, const kgv_tx_batch* batch
   }
   const size_t nt = d.n_txs, nb = n_blocks;
   // tx hashes (consumed by the merkle tree) and the roots: d_in; everything else: d_work (the merkle tree owns d_scratch)
-  int rc = kgv_reserve(ctx, &ctx->d_in, &ctx->d_in_cap, al256(nt * 32 + 32) + nb * 32);
+  uint64_t *dhash, *droots;  // droots is copied out below: roots32 is a byte array of any alignment
+  int rc = kgv_reserve_carved(ctx, &ctx->d_in, &ctx->d_in_cap, [&](kgv_carve& c) { dhash = c.take<uint64_t>(nt * 4, 32); droots = c.take<uint64_t>(nb * 4); });
   if (rc) return rc;
-  const size_t o_first = 0, o_txb = al256(o_first + (nb + 1) * 4), o_txr = al256(o_txb + nt * 4),
-               o_txm = al256(o_txr + nt * sizeof(kgv_tx_result)), o_list = al256(o_txm + nt * sizeof(kgv_tx_masses)), o_ids = al256(o_list + (nt + 1) * 4),
-               o_acc = al256(o_ids + nt * 32), o_tab = al256(o_acc + nb * sizeof(kgv_block_check_acc));
-  rc = kgv_reserve(ctx, &ctx->d_work, &ctx->d_work_cap, o_tab + kgv_body_sets_scratch(nt, d.n_inputs));
+  uint32_t *dfirst, *dtxb, *dlist;
+  kgv_tx_result* dtxr;
+  kgv_tx_masses* dtxm;
+  uint64_t* dids;
+  kgv_block_check_acc* dacc;
+  kgv_body_sets_work sets;
+  rc = kgv_reserve_carved(ctx, &ctx->d_work, &ctx->d_work_cap, [&](kgv_carve& c) {
+    dfirst = c.take<uint32_t>(nb + 1); dtxb = c.take<uint32_t>(nt); dtxr = c.take<kgv_tx_result>(nt); dtxm = c.take<kgv_tx_masses>(nt);
+    dlist = c.take<uint32_t>(nt + 1); dids = c.take<uint64_t>(nt * 4); dacc = c.take<kgv_block_check_acc>(nb); sets.carve(c, nt, d.n_inputs);
+  });
   if (rc) return rc;
-  uint8_t* S = ctx->d_work;
   cudaStream_t st = ctx->stream;
-  uint64_t* dhash = (uint64_t*)ctx->d_in;
-  uint64_t* droots = (uint64_t*)(ctx->d_in + al256(nt * 32 + 32));  // copied out below: roots32 is a byte array of any alignment
   const kgv_block_header_ctx* dhdr;
   kgv_body_result* dres;
   kgv_block_masses* dbm;
@@ -230,11 +238,6 @@ extern "C" int kgv_validate_block_bodies(kgv_ctx* ctx, const kgv_tx_batch* batch
   io.out(results, nb * sizeof(kgv_body_result), &dres);
   io.out(masses, nb * sizeof(kgv_block_masses), &dbm);
   if ((rc = io.stage())) return rc;
-  uint32_t* dfirst = (uint32_t*)(S + o_first);
-  uint32_t* dtxb = (uint32_t*)(S + o_txb);
-  kgv_tx_result* dtxr = (kgv_tx_result*)(S + o_txr);
-  kgv_tx_masses* dtxm = (kgv_tx_masses*)(S + o_txm);
-  kgv_block_check_acc* dacc = (kgv_block_check_acc*)(S + o_acc);
   CK(cudaMemcpyAsync(dfirst, block_first_tx, (nb + 1) * 4, cudaMemcpyHostToDevice, st));
   CK(cudaMemsetAsync(dacc, 0xFF, nb * sizeof(kgv_block_check_acc), st));
   const unsigned grid = std::min(n_blocks, BODY_MAX_GRID);
@@ -246,9 +249,9 @@ extern "C" int kgv_validate_block_bodies(kgv_ctx* ctx, const kgv_tx_batch* batch
   }
   if ((rc = kgv_tx_digests_run(ctx, d, nt, dhash, true))) return rc;
   if ((rc = kgv_merkle_run(ctx, dhash, nt, block_first_tx, n_blocks, droots))) return rc;
-  if ((rc = kgv_tx_digests_run(ctx, d, nt, (uint64_t*)(S + o_ids), false))) return rc;
-  if ((rc = kgv_isolation_run(ctx, d, *rules, 0, 0, !isolation_only, dtxr, dtxm, nullptr, (uint32_t*)(S + o_list), st, dhdr, dtxb))) return rc;
-  if ((rc = kgv_body_sets_run(ctx, d, nt, (const uint64_t*)(S + o_ids), dfirst, n_blocks, dacc, (uint32_t*)(S + o_tab), st))) return rc;
+  if ((rc = kgv_tx_digests_run(ctx, d, nt, dids, false))) return rc;
+  if ((rc = kgv_isolation_run(ctx, d, *rules, 0, 0, !isolation_only, dtxr, dtxm, nullptr, dlist, st, dhdr, dtxb))) return rc;
+  if ((rc = kgv_body_sets_run(ctx, d, nt, dids, dfirst, n_blocks, dacc, sets, st))) return rc;
   const BodyArgs a{d.txs, d.bytes, dfirst, dhdr, droots, dtxr, dtxm, dacc, n_blocks, isolation_only, body_rules->max_block_mass,
                    body_rules->max_coinbase_payload_len, rules->coinbase_payload_script_public_key_max_len};
   k_body_rules<<<grid, BODY_RULE_THREADS, 0, st>>>(a, dres, dbm);

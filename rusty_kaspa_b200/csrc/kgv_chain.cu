@@ -254,48 +254,51 @@ extern "C" int kgv_replay_verify_chain(kgv_ctx* ctx, const uint32_t* group_first
   const cudaMemcpyKind in_kind = dev ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
   const size_t nt = L.nt, nb = L.n_blocks;
   // scratch (d_work is free between validation calls); inputs are copied in, outputs copied out, so the caller's arrays need no alignment
-  const size_t o_gf = 0, o_hdr = o_gf + al256((n_groups + 1) * 4), o_mf = o_hdr + al256(n_groups * sizeof(kgv_chain_header)), o_init = o_mf + al256(nb),
-               o_fee = o_init + al256(768), o_code = o_fee + al256(nb * 8), o_flag = o_code + al256(nb), o_scan = o_flag + al256(nt * 4),
-               o_tot = o_scan + al256(nt * 4), o_ids = o_tot + 256, o_idf = o_ids + al256(nt * 32 + 32), o_inner = o_idf + al256((n_groups + 1) * 4),
-               o_mk = o_inner + al256(n_groups * 32), o_mu = o_mk + al256(kgv_merkle_scratch(nt)), o_val = o_mu + al256(kgv_replay_muhash_scratch(ctx, n_groups)),
-               o_ptot = o_val + al256(n_groups * 768), o_fin = o_ptot + kgv_mu_prefix_scratch(n_groups), o_hash = o_fin + kgv_mu_finalize_scratch(n_groups),
-               o_res = o_hash + al256(n_groups * 32), total = o_res + al256(n_groups * sizeof(kgv_chain_result));
-  int rc = kgv_reserve(ctx, &ctx->d_work, &ctx->d_work_cap, total);
-  if (rc) return rc;
-  uint8_t* Wk = ctx->d_work;
-  uint8_t* R = ctx->d_replay;
-  CK(cudaMemcpyAsync(Wk + o_gf, group_first_block, (n_groups + 1) * 4, cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync(Wk + o_hdr, headers, n_groups * sizeof(kgv_chain_header), in_kind, st));
-  CK(cudaMemcpyAsync(Wk + o_mf, merged_flags, nb, in_kind, st));
-  CK(cudaMemcpyAsync(Wk + o_init, init768, 768, in_kind, st));
   ChainArgs a;
+  uint32_t *gf, *init, *scan, *n_ids, *vals, *commit;
+  uint64_t* inner;
+  kgv_chain_header* hdr;
+  uint8_t* mflags;
+  kgv_merkle_work mk;
+  kgv_replay_muhash_work mu;
+  kgv_mu_prefix_work ptot;
+  kgv_mu_finalize_work fin;
+  int rc = kgv_reserve_carved(ctx, &ctx->d_work, &ctx->d_work_cap, [&](kgv_carve& c) {
+    gf = c.take<uint32_t>(n_groups + 1); hdr = c.take<kgv_chain_header>(n_groups); mflags = c.take<uint8_t>(nb); init = c.take<uint32_t>(192);
+    a.fee = c.take<uint64_t>(nb); a.code = c.take<uint8_t>(nb); a.flag = c.take<uint32_t>(nt); scan = c.take<uint32_t>(nt); n_ids = c.take<uint32_t>(64);
+    a.comp = c.take<uint64_t>(nt * 4, 32); a.id_first = c.take<uint32_t>(n_groups + 1); inner = c.take<uint64_t>(n_groups * 4);
+    mk.carve(c, nt); mu.carve(c, nt, n_groups); vals = c.take<uint32_t>(n_groups * 192); ptot.carve(c, n_groups); fin.carve(c, n_groups);
+    commit = c.take<uint32_t>(n_groups * 8); a.out = c.take<kgv_chain_result>(n_groups);
+  });
+  if (rc) return rc;
+  CK(cudaMemcpyAsync(gf, group_first_block, (n_groups + 1) * 4, cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync(hdr, headers, n_groups * sizeof(kgv_chain_header), in_kind, st));
+  CK(cudaMemcpyAsync(mflags, merged_flags, nb, in_kind, st));
+  CK(cudaMemcpyAsync(init, init768, 768, in_kind, st));
   a.v = BatchView{(const kgv_tx*)L.txs, (const kgv_input*)L.inputs, (const kgv_output*)L.outputs, nullptr, (const uint8_t*)L.bytes};
-  a.blk = (const kgv_replay_block*)(R + L.o_blk); a.res = (const kgv_tx_result*)(R + L.o_res); a.accept = R + L.o_acc; a.ids = (const uint64_t*)(R + L.o_ids);
-  a.gf = (const uint32_t*)(Wk + o_gf); a.n_groups = (uint32_t)n_groups; a.nt = (uint32_t)nt;
-  a.hdr = (const kgv_chain_header*)(Wk + o_hdr); a.mflags = Wk + o_mf;
+  a.blk = L.blk; a.res = L.res; a.accept = L.acc; a.ids = L.ids;
+  a.gf = gf; a.n_groups = (uint32_t)n_groups; a.nt = (uint32_t)nt;
+  a.hdr = hdr; a.mflags = mflags;
   a.max_payload_len = body_rules->max_coinbase_payload_len; a.max_spk_len = rules->coinbase_payload_script_public_key_max_len;
-  a.fee = (uint64_t*)(Wk + o_fee); a.code = Wk + o_code; a.flag = (uint32_t*)(Wk + o_flag); a.scan = (const uint32_t*)(Wk + o_scan);
-  a.n_ids = (const uint32_t*)(Wk + o_tot); a.comp = (uint64_t*)(Wk + o_ids); a.id_first = (uint32_t*)(Wk + o_idf); a.inner = (const uint64_t*)(Wk + o_inner);
-  a.commit = (const uint32_t*)(Wk + o_hash); a.out = (kgv_chain_result*)(Wk + o_res);
+  a.scan = scan; a.n_ids = n_ids; a.inner = inner; a.commit = commit;
   // fees, payloads and accepted-id flags per block; the accepted ids, compacted; their merkle roots per group
   k_chain_blocks<<<(unsigned)n_groups, 32 * CHAIN_BLOCK_WARPS, 0, st>>>(a);
   CK(cudaGetLastError());
-  rc = kgv_scan_u32(ctx, a.flag, (uint32_t*)(Wk + o_scan), nullptr, nullptr, nt, (uint32_t*)(Wk + o_tot), st);
+  rc = kgv_scan_u32(ctx, a.flag, scan, nullptr, nullptr, nt, n_ids, st);
   if (rc) return rc;
   k_chain_compact<<<nblk(nt, 256), 256, 0, st>>>(a);
   CK(cudaGetLastError());
   k_chain_id_first<<<nblk(n_groups + 1, 128), 128, 0, st>>>(a);
   CK(cudaGetLastError());
   ctx->launches += 3;
-  rc = kgv_merkle_levels(ctx, a.comp, nt, a.id_first, (uint32_t)n_groups, max_ids, Wk + o_mk, (uint64_t*)(Wk + o_inner), st);
+  rc = kgv_merkle_levels(ctx, a.comp, nt, a.id_first, (uint32_t)n_groups, max_ids, mk, inner, st);
   if (rc) return rc;
   // the running multiset after every group, finalized in one batch
-  uint32_t* vals = (uint32_t*)(Wk + o_val);
-  rc = kgv_replay_muhash_run(ctx, a.gf, n_groups, Wk + o_mu, vals, st);
+  rc = kgv_replay_muhash_run(ctx, a.gf, n_groups, mu, vals, st);
   if (rc) return rc;
-  rc = kgv_mu_prefix_combine_run(ctx, (const uint32_t*)(Wk + o_init), vals, n_groups, (uint32_t*)(Wk + o_ptot), st);
+  rc = kgv_mu_prefix_combine_run(ctx, init, vals, n_groups, ptot, st);
   if (rc) return rc;
-  rc = kgv_mu_finalize_run(ctx, vals, vals + 96, n_groups, 192, Wk + o_fin, nullptr, (uint32_t*)(Wk + o_hash), st);
+  rc = kgv_mu_finalize_run(ctx, vals, vals + 96, n_groups, 192, fin, nullptr, commit, st);
   if (rc) return rc;
   k_chain_verdict<<<nblk(n_groups * 32, 128), 128, 0, st>>>(a);
   CK(cudaGetLastError());

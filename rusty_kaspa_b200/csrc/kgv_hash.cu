@@ -268,16 +268,16 @@ extern "C" int kgv_sighash(kgv_ctx* ctx, const kgv_tx_batch* batch, const kgv_si
   if (rc) return rc;
   kgv_io io(ctx);
   if ((rc = io.one_side("kgv_sighash", {items, out32}))) return rc;
-  size_t o_reused = 0, o_ent = al256(d.n_txs * sizeof(SigHashReused));
-  rc = kgv_reserve(ctx, &ctx->d_scratch, &ctx->d_scratch_cap, al256(o_ent + d.n_inputs * sizeof(DevEntry)) + 256);
+  SigHashReused* dre;
+  DevEntry* dent;
+  rc = kgv_reserve_carved(ctx, &ctx->d_scratch, &ctx->d_scratch_cap,
+                          [&](kgv_carve& c) { dre = c.take<SigHashReused>(d.n_txs); dent = c.take<DevEntry>(d.n_inputs, 256); });
   if (rc) return rc;
-  SigHashReused* dre = (SigHashReused*)(ctx->d_scratch + o_reused);
   const kgv_sighash_item* ditems;
   uint8_t* dout;
   io.in(items, n_items * sizeof(kgv_sighash_item), &ditems);
   io.out(out32, n_items * 32, &dout);
   if ((rc = io.stage())) return rc;
-  DevEntry* dent = (DevEntry*)(ctx->d_scratch + o_ent);
   if (d.n_inputs) {
     k_entries_to_dev<<<(unsigned)((d.n_inputs + 127) / 128), 128, 0, ctx->stream>>>(d.entries, d.bytes, d.n_inputs, dent);
     CK(cudaGetLastError());
@@ -341,20 +341,18 @@ __global__ void k_merkle_collect(const uint64_t* __restrict__ cur, const uint32_
 }
 
 // dh: device array of up to n_cap hashes (modified: used as one of the two ping-pong buffers); dfirst: n_groups + 1 DEVICE offsets
-size_t kgv_merkle_scratch(size_t n_cap) { return al256(n_cap * 4) + al256(n_cap * 32 + 32); }
-int kgv_merkle_levels(kgv_ctx* ctx, uint64_t* dh, size_t n_cap, const uint32_t* dfirst, uint32_t n_groups, uint32_t max_n, uint8_t* scratch, uint64_t* droots,
-                      cudaStream_t st) {
-  uint32_t* dgid = (uint32_t*)scratch;
-  uint64_t* other = (uint64_t*)(scratch + al256(n_cap * 4));
+void kgv_merkle_work::carve(kgv_carve& c, size_t n_cap) { gid = c.take<uint32_t>(n_cap); other = c.take<uint64_t>(n_cap * 4, 32); }
+int kgv_merkle_levels(kgv_ctx* ctx, uint64_t* dh, size_t n_cap, const uint32_t* dfirst, uint32_t n_groups, uint32_t max_n, const kgv_merkle_work& w,
+                      uint64_t* droots, cudaStream_t st) {
   if (n_cap) {
-    k_merkle_group_index<<<(n_groups + 127) / 128, 128, 0, st>>>(dfirst, n_groups, dgid);
+    k_merkle_group_index<<<(n_groups + 127) / 128, 128, 0, st>>>(dfirst, n_groups, w.gid);
     CK(cudaGetLastError());
     ctx->launches++;
   }
   uint64_t* cur = dh;
-  uint64_t* nxt = other;
+  uint64_t* nxt = w.other;
   for (uint32_t level = 0; ((uint64_t)1 << level) < max_n; level++) {
-    k_merkle_level<<<(unsigned)((n_cap + 127) / 128), 128, 0, st>>>(cur, nxt, dfirst, n_groups, dgid, n_cap, level);
+    k_merkle_level<<<(unsigned)((n_cap + 127) / 128), 128, 0, st>>>(cur, nxt, dfirst, n_groups, w.gid, n_cap, level);
     CK(cudaGetLastError());
     ctx->launches++;
     uint64_t* t = cur; cur = nxt; nxt = t;
@@ -374,13 +372,12 @@ int kgv_merkle_run(kgv_ctx* ctx, uint64_t* dh, size_t n_total, const uint32_t* f
     uint32_t n = first_host[g + 1] - first_host[g];
     if (n > max_n) max_n = n;
   }
-  const size_t o_first = 0, o_lv = al256((n_groups + 1) * 4);
-  int rc = kgv_reserve(ctx, &ctx->d_scratch, &ctx->d_scratch_cap, o_lv + kgv_merkle_scratch(n_total));
+  uint32_t* dfirst;
+  kgv_merkle_work w;
+  int rc = kgv_reserve_carved(ctx, &ctx->d_scratch, &ctx->d_scratch_cap, [&](kgv_carve& c) { dfirst = c.take<uint32_t>(n_groups + 1); w.carve(c, n_total); });
   if (rc) return rc;
-  uint8_t* S = ctx->d_scratch;
-  uint32_t* dfirst = (uint32_t*)(S + o_first);
   CK(cudaMemcpyAsync(dfirst, first_host, (n_groups + 1) * 4, cudaMemcpyHostToDevice, ctx->stream));
-  return kgv_merkle_levels(ctx, dh, n_total, dfirst, n_groups, max_n, S + o_lv, droots, ctx->stream);
+  return kgv_merkle_levels(ctx, dh, n_total, dfirst, n_groups, max_n, w, droots, ctx->stream);
 }
 
 extern "C" int kgv_merkle_roots(kgv_ctx* ctx, const uint8_t* hashes32, const uint32_t* first, uint32_t n_groups, uint8_t* roots32) {
@@ -396,10 +393,9 @@ extern "C" int kgv_merkle_roots(kgv_ctx* ctx, const uint8_t* hashes32, const uin
   int rc = io.one_side("kgv_merkle_roots", {n_total ? hashes32 : nullptr, roots32});
   if (rc) return rc;
   // working copy of the hashes (the tree overwrites its input buffer) + device roots
-  rc = kgv_reserve(ctx, &ctx->d_in, &ctx->d_in_cap, al256(n_total * 32 + 32) + (size_t)n_groups * 32);
+  uint64_t *dh, *dr;
+  rc = kgv_reserve_carved(ctx, &ctx->d_in, &ctx->d_in_cap, [&](kgv_carve& c) { dh = c.take<uint64_t>(n_total * 4, 32); dr = c.take<uint64_t>((size_t)n_groups * 4); });
   if (rc) return rc;
-  uint64_t* dh = (uint64_t*)ctx->d_in;
-  uint64_t* dr = (uint64_t*)(ctx->d_in + al256(n_total * 32 + 32));
   if (n_total) CK(cudaMemcpyAsync(dh, hashes32, n_total * 32, cudaMemcpyDefault, ctx->stream));
   if ((rc = kgv_merkle_run(ctx, dh, n_total, first, n_groups, dr))) return rc;
   if ((rc = io.copy_out(roots32, dr, (size_t)n_groups * 32))) return rc;
@@ -423,10 +419,9 @@ extern "C" int kgv_block_hash_merkle_roots(kgv_ctx* ctx, const kgv_tx_batch* bat
     if (rc) return rc;
   }
   const size_t nt = block_first_tx[n_blocks];
-  int rc = kgv_reserve(ctx, &ctx->d_in, &ctx->d_in_cap, al256(nt * 32 + 32) + (size_t)n_blocks * 32);
+  uint64_t *dh, *dr;
+  int rc = kgv_reserve_carved(ctx, &ctx->d_in, &ctx->d_in_cap, [&](kgv_carve& c) { dh = c.take<uint64_t>(nt * 4, 32); dr = c.take<uint64_t>((size_t)n_blocks * 4); });
   if (rc) return rc;
-  uint64_t* dh = (uint64_t*)ctx->d_in;
-  uint64_t* dr = (uint64_t*)(ctx->d_in + al256(nt * 32 + 32));
   rc = kgv_tx_digests_run(ctx, d, nt, dh, true);
   if (rc) return rc;
   rc = kgv_merkle_run(ctx, dh, nt, block_first_tx, n_blocks, dr);
@@ -472,24 +467,29 @@ extern "C" int kgv_block_set_checks(kgv_ctx* ctx, const kgv_tx_batch* batch, con
     if (rc) return rc;
   }
   const size_t nt = block_first_tx[n_blocks];
-  size_t o_ids = 0, o_first = al256(nt * 32 + 32), o_acc = al256(o_first + (n_blocks + 1) * 4), o_out = al256(o_acc + (size_t)n_blocks * sizeof(BlockCheckAcc));
-  const size_t o_tab = al256(o_out + (size_t)n_blocks * sizeof(kgv_block_check));
-  int rc = kgv_reserve(ctx, &ctx->d_scratch, &ctx->d_scratch_cap, al256(o_tab + kgv_body_sets_scratch(nt, d.n_inputs)));
+  uint64_t* ids;
+  uint32_t* first;
+  BlockCheckAcc* acc;
+  kgv_block_check* dout;
+  kgv_body_sets_work sets;
+  int rc = kgv_reserve_carved(ctx, &ctx->d_scratch, &ctx->d_scratch_cap, [&](kgv_carve& c) {
+    ids = c.take<uint64_t>(nt * 4, 32); first = c.take<uint32_t>(n_blocks + 1); acc = c.take<BlockCheckAcc>(n_blocks); dout = c.take<kgv_block_check>(n_blocks);
+    sets.carve(c, nt, d.n_inputs);
+  });
   if (rc) return rc;
-  uint8_t* S = ctx->d_scratch;
   cudaStream_t st = ctx->stream;
-  CK(cudaMemcpyAsync(S + o_first, block_first_tx, (n_blocks + 1) * 4, cudaMemcpyHostToDevice, st));
-  CK(cudaMemsetAsync(S + o_acc, 0xFF, (size_t)n_blocks * sizeof(BlockCheckAcc), st));
+  CK(cudaMemcpyAsync(first, block_first_tx, (n_blocks + 1) * 4, cudaMemcpyHostToDevice, st));
+  CK(cudaMemsetAsync(acc, 0xFF, (size_t)n_blocks * sizeof(BlockCheckAcc), st));
   if (nt) {
-    rc = kgv_tx_digests_run(ctx, d, nt, (uint64_t*)(S + o_ids), false);
+    rc = kgv_tx_digests_run(ctx, d, nt, ids, false);
     if (rc) return rc;
-    rc = kgv_body_sets_run(ctx, d, nt, (const uint64_t*)(S + o_ids), (const uint32_t*)(S + o_first), n_blocks, (BlockCheckAcc*)(S + o_acc), (uint32_t*)(S + o_tab), st);
+    rc = kgv_body_sets_run(ctx, d, nt, ids, first, n_blocks, acc, sets, st);
     if (rc) return rc;
   }
-  k_block_set_checks_final<<<(n_blocks + 127) / 128, 128, 0, st>>>((const BlockCheckAcc*)(S + o_acc), n_blocks, (kgv_block_check*)(S + o_out));
+  k_block_set_checks_final<<<(n_blocks + 127) / 128, 128, 0, st>>>(acc, n_blocks, dout);
   CK(cudaGetLastError());
   ctx->launches++;
   kgv_io io(ctx);
-  if ((rc = io.copy_out(out, S + o_out, (size_t)n_blocks * sizeof(kgv_block_check)))) return rc;
+  if ((rc = io.copy_out(out, dout, (size_t)n_blocks * sizeof(kgv_block_check)))) return rc;
   return io.finish();
 }

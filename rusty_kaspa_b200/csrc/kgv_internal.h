@@ -11,6 +11,8 @@
 #include <thread>
 #include <vector>
 
+#include "../../include/kgv.h"
+
 #ifndef KGV_BLOCK
 #define KGV_BLOCK 128         // threads per block of the verification kernels
 #endif
@@ -21,6 +23,11 @@
 #ifndef KGV_ITEMS
 #define KGV_ITEMS 4           // signatures per thread sharing one modular inversion (see k_schnorr_verify)
 #endif
+
+namespace kgv { struct DevEntry; }
+struct ReplayRange;
+struct ReplaySrc;
+struct ReplayTxInfo;
 
 struct kgv_ctx {
   int device = 0;
@@ -71,9 +78,18 @@ struct kgv_ctx {
     bool valid = false;
     const void *txs = nullptr, *inputs = nullptr, *outputs = nullptr, *bytes = nullptr;
     size_t nt = 0, ni = 0, no = 0, n_blocks = 0;
-    size_t o_ids = 0, o_itx = 0, o_otx = 0, o_ent = 0, o_acc = 0, o_txb = 0, o_rng = 0;  // offsets into d_replay
-    size_t o_src = 0, o_inf = 0, o_apv = 0;
-    size_t o_blk = 0, o_res = 0;                    // the kgv_replay_block records and the per-transaction results
+    // the window's arrays in d_replay (kgv_replay_impl.cuh).  Read only while `valid` is set: only kgv_replay_window reserves d_replay, and
+    // it clears `valid` first (kgv_batch_to_device), so these never outlive the buffer they point into.
+    const uint64_t* ids = nullptr;
+    const uint32_t *itx = nullptr, *otx = nullptr, *txb = nullptr;
+    const uint8_t* acc = nullptr;
+    const unsigned long long* apv = nullptr;
+    const kgv::DevEntry* ent = nullptr;
+    const ReplayRange* rng = nullptr;
+    const ReplaySrc* src = nullptr;
+    const ReplayTxInfo* inf = nullptr;
+    const kgv_replay_block* blk = nullptr;
+    const kgv_tx_result* res = nullptr;
     std::vector<uint32_t> block_flags, block_n_txs;  // host copy of the blocks' flags and sizes
     struct kgv_utxo_table* table = nullptr;          // the table replayed into, and the rehashes of its layers then: the populated entries'
     uint64_t rehashes = 0;                           // long scripts lie in those layers' arenas
@@ -106,8 +122,6 @@ int kgv_host_only(kgv_ctx* ctx, const char* call, const char* what, const void* 
 int kgv_malloc(kgv_ctx* ctx, void** p, size_t bytes);
 int kgv_reserve(kgv_ctx* ctx, uint8_t** buf, size_t* cap, size_t need);
 
-#include "../../include/kgv.h"
-
 // returns KGV_ERR_CUDA from the enclosing function (which has `ctx` in scope) when a CUDA call fails
 #define CK(call)                                                                                  \
   do {                                                                                            \
@@ -125,6 +139,29 @@ static inline unsigned nblk(size_t n, unsigned b) { return (unsigned)((n + b - 1
 static inline int fail_arg(kgv_ctx* ctx, const char* m) {
   if (ctx) ctx->err = m;
   return KGV_ERR_ARG;
+}
+
+// ---- a call's device scratch, declared once ----
+// A cursor over a buffer: take<T>(n, pad) hands out T[n] plus pad bytes at the cursor, and the next array starts 256-byte aligned after it.
+// With a null base it only measures (every pointer is null, `at` ends at the layout's size).  A layout is one function of a kgv_carve&
+// that takes its arrays in order; run once to measure and once on the buffer, it gives the size and the pointers from the same code.
+struct kgv_carve {
+  uint8_t* base = nullptr;  // null: measure only
+  size_t at = 0;
+  template <class T> T* take(size_t n, size_t pad_bytes = 0) {
+    T* p = base ? (T*)(base + at) : nullptr;
+    at = al256(at + n * sizeof(T) + pad_bytes);
+    return p;
+  }
+};
+// Runs lay(c) to measure, reserves *buf (kgv_reserve) to at least that size, and runs lay(c) again on the buffer.
+template <class F> int kgv_reserve_carved(kgv_ctx* ctx, uint8_t** buf, size_t* cap, F&& lay) {
+  kgv_carve m;
+  lay(m);
+  if (int rc = kgv_reserve(ctx, buf, cap, m.at)) return rc;
+  kgv_carve c{*buf};
+  lay(c);
+  return KGV_OK;
 }
 
 // ---- where a call's caller-owned arrays live (include/kgv.h, Conventions) ----
@@ -234,20 +271,26 @@ int kgv_mu_reduce(kgv_ctx* ctx, kgv_io& io, size_t n_den, size_t n_num, uint8_t*
 int kgv_mu_range_products(kgv_ctx* ctx, const uint32_t* E, size_t stride, const uint8_t* flags, const uint32_t* flag_index, const uint32_t* lo, const uint32_t* hi, uint32_t n_segs,
                           uint32_t* out, size_t out_pitch_words, cudaStream_t st);
 int kgv_mu_canonicalize(kgv_ctx* ctx, uint32_t* vals, size_t pitch_words, size_t n, cudaStream_t st);
-// kgv_muhash_prefix_combine on device records (v: n (numerator || denominator) records, 16-byte aligned; dinit: one record or null), in place;
-// tot: kgv_mu_prefix_scratch(n) bytes
-size_t kgv_mu_prefix_scratch(size_t n);
-int kgv_mu_prefix_combine_run(kgv_ctx* ctx, const uint32_t* dinit, uint32_t* v, size_t n, uint32_t* tot, cudaStream_t st);
+// kgv_muhash_prefix_combine on device records (v: n (numerator || denominator) records, 16-byte aligned; dinit: one record or null), in place
+struct kgv_mu_prefix_work { uint32_t* tot; void carve(kgv_carve& c, size_t n); };  // tot: the scan's chunk totals
+int kgv_mu_prefix_combine_run(kgv_ctx* ctx, const uint32_t* dinit, uint32_t* v, size_t n, const kgv_mu_prefix_work& w, cudaStream_t st);
 // kgv_muhash_finalize_batch on device values (numerator k at dnum + k * pitch_words, 16-byte aligned); dser (may be null) / dhashes: n values
-// of 384 / 32 bytes, 4-byte aligned; scratch: kgv_mu_finalize_scratch(n) bytes, 256-byte aligned
-size_t kgv_mu_finalize_scratch(size_t n);
-int kgv_mu_finalize_run(kgv_ctx* ctx, const uint32_t* dnum, const uint32_t* dden, size_t n, size_t pitch_words, uint8_t* scratch, uint32_t* dser,
-                        uint32_t* dhashes, cudaStream_t st);
+// of 384 / 32 bytes, 4-byte aligned
+struct kgv_mu_finalize_work {  // prefix and suffix products, the quotients, the scan's chunk totals, the inversion's operands
+  uint32_t *P, *S, *out, *tot, *inv;
+  void carve(kgv_carve& c, size_t n);
+};
+int kgv_mu_finalize_run(kgv_ctx* ctx, const uint32_t* dnum, const uint32_t* dden, size_t n, size_t pitch_words, const kgv_mu_finalize_work& w,
+                        uint32_t* dser, uint32_t* dhashes, cudaStream_t st);
 // kgv_replay_muhash on the last window's state (kgv_validate.cu): dgf = n_groups + 1 device block offsets; vals = n_groups canonical
-// (numerator || denominator) records, 768 bytes apart, 16-byte aligned; scratch: kgv_replay_muhash_scratch(n_groups) bytes, 256-byte aligned.
-// The element arrays live in d_mu.
-size_t kgv_replay_muhash_scratch(kgv_ctx* ctx, size_t n_groups);
-int kgv_replay_muhash_run(kgv_ctx* ctx, const uint32_t* dgf, size_t n_groups, uint8_t* scratch, uint32_t* vals, cudaStream_t st);
+// (numerator || denominator) records, 768 bytes apart, 16-byte aligned.  The element arrays live in d_mu.
+struct kgv_replay_muhash_work {  // per transaction its block's DAA score and whether it is the block's first; per group its input / output range
+  uint64_t* pov;
+  uint8_t* first;
+  uint32_t *ilo, *ihi, *olo, *ohi;
+  void carve(kgv_carve& c, size_t nt, size_t n_groups);
+};
+int kgv_replay_muhash_run(kgv_ctx* ctx, const uint32_t* dgf, size_t n_groups, const kgv_replay_muhash_work& w, uint32_t* vals, cudaStream_t st);
 
 // ---- one UTXO table used from every context of its device (kgv_utxo_maint.cu; include/kgv.h, "Threading") ----
 // A reader/writer lock per table whose ordering lives on the GPU.  A call registers before it enqueues the first work that touches the
@@ -343,7 +386,6 @@ int kgv_standard_isolation_run(kgv_ctx* ctx, const kgv_dev_batch& d, const kgv_m
 // check_transaction_standard_in_context on st.  dent: the populated entries of a validation call, or null to read d.entries.  dfee: the
 // fees, or null to check only the txs whose dres status is KGV_TX_OK with their dres fee (then only failures are written).  *dflag |= 1
 // when a reached fee check's mass * fee overflows u64.
-namespace kgv { struct DevEntry; }
 int kgv_standard_context_run(kgv_ctx* ctx, const kgv_dev_batch& d, const kgv::DevEntry* dent, const kgv_mempool_policy& p, const kgv_tx_masses* dmasses,
                              const uint64_t* dsmass, const uint64_t* dfee, kgv_tx_result* dres, uint64_t* ddetail, unsigned long long* dflag,
                              cudaStream_t st);
@@ -353,18 +395,21 @@ int kgv_standard_context_run(kgv_ctx* ctx, const kgv_dev_batch& d, const kgv::De
 int kgv_tx_digests_run(kgv_ctx* ctx, const kgv_dev_batch& d, size_t n, uint64_t* out, bool hash);
 // merkle roots of n_groups groups over the device hashes dh (overwritten); first_host: n_groups + 1 offsets on the host.  Uses d_scratch.
 int kgv_merkle_run(kgv_ctx* ctx, uint64_t* dh, size_t n_total, const uint32_t* first_host, uint32_t n_groups, uint64_t* droots);
-// the same with DEVICE offsets dfirst (n_groups + 1, from 0 to at most n_cap hashes) and max_n >= the largest group; scratch:
-// kgv_merkle_scratch(n_cap) bytes, 256-byte aligned.  Enqueued on st.
-size_t kgv_merkle_scratch(size_t n_cap);
-int kgv_merkle_levels(kgv_ctx* ctx, uint64_t* dh, size_t n_cap, const uint32_t* dfirst, uint32_t n_groups, uint32_t max_n, uint8_t* scratch, uint64_t* droots,
-                      cudaStream_t st);
+// the same with DEVICE offsets dfirst (n_groups + 1, from 0 to at most n_cap hashes) and max_n >= the largest group.  Enqueued on st.
+struct kgv_merkle_work { uint32_t* gid; uint64_t* other; void carve(kgv_carve& c, size_t n_cap); };  // every hash's group, the levels' second buffer
+int kgv_merkle_levels(kgv_ctx* ctx, uint64_t* dh, size_t n_cap, const uint32_t* dfirst, uint32_t n_groups, uint32_t max_n, const kgv_merkle_work& w,
+                      uint64_t* droots, cudaStream_t st);
 // check_duplicate_transactions / check_block_double_spends / check_no_chained_transactions of every block (kgv_block_body.cu): dacc[b] gets
 // the lowest offending tx / input / input index within the batch, 0xFFFFFFFF where a check passes.  dids: the tx ids; dfirst: the block
-// offsets on the device; dtab: scratch of kgv_body_sets_scratch(n_txs, n_inputs) bytes.
+// offsets on the device.
 struct kgv_block_check_acc { unsigned int dup_tx, double_spend, chained; };
-size_t kgv_body_sets_scratch(size_t n_txs, size_t n_inputs);
+struct kgv_body_sets_work {  // the blocks' hashed sets, cleared whole (up to the next 256-byte boundary)
+  uint32_t* tab;
+  size_t bytes;
+  void carve(kgv_carve& c, size_t n_txs, size_t n_inputs);
+};
 int kgv_body_sets_run(kgv_ctx* ctx, const kgv_dev_batch& d, size_t n_txs, const uint64_t* dids, const uint32_t* dfirst, uint32_t n_blocks,
-                      kgv_block_check_acc* dacc, uint32_t* dtab, cudaStream_t st);
+                      kgv_block_check_acc* dacc, const kgv_body_sets_work& w, cudaStream_t st);
 
 // ---- multi-GPU exchange used by the sharded script phase (kgv_comm.cu) ----
 // Every rank contributes `per` bytes at buf + rank * per (device memory, n_ranks * per bytes in all); on return (stream order)

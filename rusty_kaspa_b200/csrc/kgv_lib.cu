@@ -796,16 +796,15 @@ static int key_cache_launch(kgv_ctx* ctx, const uint8_t* dpk, size_t n, bool ecd
   while (slots < 2 * n) slots <<= 1;                       // load factor <= 1/2
   const uint32_t cap = (uint32_t)(n / 2 < KGV_KEY_RECORDS_MAX ? n / 2 : KGV_KEY_RECORDS_MAX);  // key_form's bounds
   const size_t cap_comb = n / KGV_COMB_USES < KGV_KEY_RECORDS_MAX ? n / KGV_COMB_USES : KGV_KEY_RECORDS_MAX;
-  const size_t rec_bytes = std::max((size_t)cap * KGV_KR_WORDS, cap_comb * KGV_JR_WORDS) * 4;
-  const size_t o_tab = 256, o_item = o_tab + (size_t)slots * sizeof(KeySlot);
-  const size_t o_rep = (o_item + n * 4 + 255) & ~(size_t)255, o_rec = (o_rep + (size_t)cap * 4 + 255) & ~(size_t)255;
-  int rc = kgv_reserve(ctx, &ctx->d_keys[ecdsa], &ctx->d_keys_cap[ecdsa], o_rec + rec_bytes);
+  const size_t rec_words = std::max((size_t)cap * KGV_KR_WORDS, cap_comb * KGV_JR_WORDS);
+  uint32_t *n_rec, *item_slot, *rec_rep, *recs;
+  KeySlot* table;
+  int rc = kgv_reserve_carved(ctx, &ctx->d_keys[ecdsa], &ctx->d_keys_cap[ecdsa], [&](kgv_carve& c) {
+    n_rec = c.take<uint32_t>(64);  // a 256-byte header: the record count
+    table = c.take<KeySlot>(slots); item_slot = c.take<uint32_t>(n); rec_rep = c.take<uint32_t>(cap); recs = c.take<uint32_t>(rec_words);
+  });
   if (rc) return rc;
-  uint8_t* K = ctx->d_keys[ecdsa];
-  uint32_t* n_rec = (uint32_t*)K;
-  KeySlot* table = (KeySlot*)(K + o_tab);
-  uint32_t *item_slot = (uint32_t*)(K + o_item), *rec_rep = (uint32_t*)(K + o_rep), *recs = (uint32_t*)(K + o_rec);
-  CK(cudaMemsetAsync(K, 0, o_item, st));
+  CK(cudaMemsetAsync(n_rec, 0, (uint8_t*)item_slot - (uint8_t*)n_rec, st));  // the header and the slot table
   if (stand_down) {
     k_kc_stand_down<<<1, 1, 0, st>>>(stand_down, n_rec);
     CK(cudaGetLastError());
@@ -932,14 +931,14 @@ static int kc_begin(kgv_ctx* ctx, kgv_keycache::Part& P, size_t n, bool ecdsa, c
   P.pending = false;
   uint32_t slots = 64;
   while (slots < 2 * n) slots <<= 1;
-  const size_t o_irec = 256, o_ord = al256(o_irec + 4 * n), o_mord = al256(o_ord + 4 * n), o_mk = al256(o_mord + 4 * n);
-  const size_t o_tab = al256(o_mk + (ecdsa ? 33 : 32) * n);
-  const size_t o_islot = al256(o_tab + (size_t)slots * sizeof(KeySlot)), o_rep = al256(o_islot + 4 * n);
-  if (int rc = kgv_reserve(ctx, &P.scratch, &P.scratch_cap, o_rep + 4 * n)) return rc;
-  uint8_t* S = P.scratch;
-  *s = KcScratch{(uint32_t*)S, (uint32_t*)(S + o_irec), (uint32_t*)(S + o_ord), (uint32_t*)(S + o_mord), (uint32_t*)(S + o_islot), (uint32_t*)(S + o_rep), S + o_mk,
-                 (KeySlot*)(S + o_tab), slots};
-  CK(cudaMemsetAsync(S, 0, 256, st));
+  int rc = kgv_reserve_carved(ctx, &P.scratch, &P.scratch_cap, [&](kgv_carve& c) {
+    s->hdr = c.take<uint32_t>(64);  // the 256-byte header of launch words
+    s->item_rec = c.take<uint32_t>(n); s->order = c.take<uint32_t>(n); s->miss_order = c.take<uint32_t>(n); s->miss_keys = c.take<uint8_t>((ecdsa ? 33 : 32) * n);
+    s->table = c.take<KeySlot>(slots); s->item_slot = c.take<uint32_t>(n); s->rec_rep = c.take<uint32_t>(n);
+  });
+  if (rc) return rc;
+  s->slots = slots;
+  CK(cudaMemsetAsync(s->hdr, 0, 256, st));
   return KGV_OK;
 }
 // the insert of a launch's misses into partition p on st: k_key_dedup over the miss keys, then k_kc_insert
@@ -1160,13 +1159,13 @@ static int verify_common(kgv_ctx* ctx, const uint8_t* pk, size_t pk_stride, cons
   // side stream while the previous chunk is being verified: only the first chunk's upload is exposed.
   const size_t chunk = (size_t)ctx->resident_blocks * KGV_BLOCK * KGV_ITEMS;
   if (!dev && n >= 2 * chunk && (n + chunk - 1) / chunk <= 32) {
-    size_t off_msg = (pk_stride * n + 255) & ~(size_t)255;
-    size_t off_sig = off_msg + 32 * n;
-    int rc = kgv_reserve(ctx, &ctx->d_in, &ctx->d_in_cap, off_sig + 64 * n);
+    uint8_t *dpk, *dmsg;
+    // the messages, and the signatures straight after them
+    int rc = kgv_reserve_carved(ctx, &ctx->d_in, &ctx->d_in_cap, [&](kgv_carve& c) { dpk = c.take<uint8_t>(pk_stride * n); dmsg = c.take<uint8_t>(96 * n); });
     if (rc) return rc;
+    uint8_t* dsig = dmsg + 32 * n;
     rc = kgv_reserve(ctx, &ctx->d_out, &ctx->d_out_cap, n);
     if (rc) return rc;
-    const uint8_t *dpk = ctx->d_in, *dmsg = ctx->d_in + off_msg, *dsig = ctx->d_in + off_sig;
     uint8_t* dst = ctx->d_out;
     CK(cudaEventRecord(ctx->ev_fork, ctx->stream));          // the staging buffers may still be read by earlier work of this stream
     CK(cudaStreamWaitEvent(ctx->aux_stream, ctx->ev_fork, 0));
@@ -1174,9 +1173,9 @@ static int verify_common(kgv_ctx* ctx, const uint8_t* pk, size_t pk_stride, cons
     for (size_t a = 0; a < n; a += chunk, c++) {
       const size_t m = n - a < chunk ? n - a : chunk;
       if (!ctx->ev_chunk[c]) CK(cudaEventCreateWithFlags(&ctx->ev_chunk[c], cudaEventDisableTiming));
-      CK(cudaMemcpyAsync(ctx->d_in + pk_stride * a, pk + pk_stride * a, pk_stride * m, cudaMemcpyHostToDevice, ctx->aux_stream));
-      CK(cudaMemcpyAsync(ctx->d_in + off_msg + 32 * a, msg + 32 * a, 32 * m, cudaMemcpyHostToDevice, ctx->aux_stream));
-      CK(cudaMemcpyAsync(ctx->d_in + off_sig + 64 * a, sig + 64 * a, 64 * m, cudaMemcpyHostToDevice, ctx->aux_stream));
+      CK(cudaMemcpyAsync(dpk + pk_stride * a, pk + pk_stride * a, pk_stride * m, cudaMemcpyHostToDevice, ctx->aux_stream));
+      CK(cudaMemcpyAsync(dmsg + 32 * a, msg + 32 * a, 32 * m, cudaMemcpyHostToDevice, ctx->aux_stream));
+      CK(cudaMemcpyAsync(dsig + 64 * a, sig + 64 * a, 64 * m, cudaMemcpyHostToDevice, ctx->aux_stream));
       CK(cudaEventRecord(ctx->ev_chunk[c], ctx->aux_stream));
       CK(cudaStreamWaitEvent(ctx->stream, ctx->ev_chunk[c], 0));
       int rc2 = kgv_launch_verify(ctx, dpk + pk_stride * a, dmsg + 32 * a, dsig + 64 * a, m, dst + a, ecdsa, ctx->stream);

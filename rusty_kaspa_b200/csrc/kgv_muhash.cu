@@ -80,29 +80,31 @@ __global__ void __launch_bounds__(128) k_muhash_raw_elements(const uint8_t* __re
 // ---------------------------------------------------------------------------------------------
 // tree driver
 // ---------------------------------------------------------------------------------------------
-struct MuTreeMem { uint32_t *lvl0, *lvl1, *wide; };
-static size_t tree_bytes(size_t n) { size_t h = (n + 1) / 2; return al256(n * 384) + al256(h * 384) + al256(h * 768) + 512; }
-static MuTreeMem tree_mem(uint8_t* base, size_t n) {
-  size_t h = (n + 1) / 2;
-  MuTreeMem m;
-  m.lvl0 = (uint32_t*)base;
-  m.lvl1 = (uint32_t*)(base + al256(n * 384));
-  m.wide = (uint32_t*)(base + al256(n * 384) + al256(h * 384));
-  return m;
-}
-static uint32_t* tree_out(uint8_t* base, size_t n) { size_t h = (n + 1) / 2; return (uint32_t*)(base + al256(n * 384) + al256(h * 384) + al256(h * 768)); }
+// one product tree of n elements in d_mu: level 0, level 1, the wide-product rows and the result (384 bytes in a 512-byte slot)
+struct MuTree {
+  size_t n;
+  uint32_t *lvl0, *lvl1, *wide, *out;
+  void carve(kgv_carve& c) {
+    lvl0 = c.take<uint32_t>(n * 96); lvl1 = c.take<uint32_t>((n + 1) / 2 * 96); wide = c.take<uint32_t>((n + 1) / 2 * 192); out = c.take<uint32_t>(128);
+  }
+};
+// the two trees of kgv_mu_reserve / kgv_mu_reduce, the denominator's first
+struct MuTrees {
+  MuTree den, num;
+  void carve(kgv_carve& c) { den.carve(c); num.carve(c); }
+};
 
 int kgv_mu_reserve(kgv_ctx* ctx, size_t n_den, size_t n_num, uint32_t** e_den, uint32_t** e_num) {
-  size_t need = tree_bytes(n_den) + tree_bytes(n_num);
-  int rc = kgv_reserve(ctx, &ctx->d_mu, &ctx->d_mu_cap, need);
+  MuTrees t{{n_den}, {n_num}};
+  int rc = kgv_reserve_carved(ctx, &ctx->d_mu, &ctx->d_mu_cap, [&](kgv_carve& c) { t.carve(c); });
   if (rc) return rc;
-  *e_den = tree_mem(ctx->d_mu, n_den).lvl0;
-  *e_num = tree_mem(ctx->d_mu + tree_bytes(n_den), n_num).lvl0;
+  *e_den = t.den.lvl0;
+  *e_num = t.num.lvl0;
   return KGV_OK;
 }
 
-static int reduce_one(kgv_ctx* ctx, uint8_t* base, size_t n, cudaStream_t st) {
-  MuTreeMem m = tree_mem(base, n);
+static int reduce_one(kgv_ctx* ctx, const MuTree& m, cudaStream_t st) {
+  const size_t n = m.n;
   uint32_t* cur = m.lvl0;
   uint32_t* nxt = m.lvl1;
   size_t k = n;
@@ -115,7 +117,7 @@ static int reduce_one(kgv_ctx* ctx, uint8_t* base, size_t n, cudaStream_t st) {
     uint32_t* t = cur; cur = nxt; nxt = t;
     k = h;
   }
-  k_u3072_emit<<<1, 32, 0, st>>>(cur, 1, n == 0 ? 1 : 0, tree_out(base, n));
+  k_u3072_emit<<<1, 32, 0, st>>>(cur, 1, n == 0 ? 1 : 0, m.out);
   CK(cudaGetLastError());
   ctx->launches++;
   return KGV_OK;
@@ -123,18 +125,19 @@ static int reduce_one(kgv_ctx* ctx, uint8_t* base, size_t n, cudaStream_t st) {
 
 int kgv_mu_reduce(kgv_ctx* ctx, kgv_io& io, size_t n_den, size_t n_num, uint8_t* out_num384, uint8_t* out_den384) {
   cudaStream_t st = ctx->stream, sx = ctx->aux_stream;
-  uint8_t* b_den = ctx->d_mu;
-  uint8_t* b_num = ctx->d_mu + tree_bytes(n_den);
+  MuTrees t{{n_den}, {n_num}};
+  kgv_carve c{ctx->d_mu};  // the layout kgv_mu_reserve gave d_mu
+  t.carve(c);
   CK(cudaEventRecord(ctx->ev_fork, st));
   CK(cudaStreamWaitEvent(sx, ctx->ev_fork, 0));
-  int rc = reduce_one(ctx, b_den, n_den, st);
+  int rc = reduce_one(ctx, t.den, st);
   if (rc) return rc;
-  rc = reduce_one(ctx, b_num, n_num, sx);
+  rc = reduce_one(ctx, t.num, sx);
   if (rc) return rc;
   CK(cudaEventRecord(ctx->ev_join, sx));
   CK(cudaStreamWaitEvent(st, ctx->ev_join, 0));
-  if ((rc = io.copy_out(out_den384, tree_out(b_den, n_den), 384))) return rc;
-  if ((rc = io.copy_out(out_num384, tree_out(b_num, n_num), 384))) return rc;
+  if ((rc = io.copy_out(out_den384, t.den.out, 384))) return rc;
+  if ((rc = io.copy_out(out_num384, t.num.out, 384))) return rc;
   return io.finish();
 }
 
@@ -178,20 +181,20 @@ extern "C" int kgv_debug_u3072_level(kgv_ctx* ctx, int coop, const uint8_t* in38
   if (kgv_ptr_is_device(in384) || kgv_ptr_is_device(out384)) { ctx->err = "kgv_debug_u3072_level takes host pointers"; return KGV_ERR_ARG; }
   CK(cudaSetDevice(ctx->device));
   const size_t h = (n_in + 1) / 2;
-  const size_t o_out = al256(n_in * 384), o_wide = al256(o_out + h * 384);
-  int rc = kgv_reserve(ctx, &ctx->d_mu, &ctx->d_mu_cap, al256(o_wide + h * 768));
+  uint8_t *lvl, *out, *wide;
+  int rc = kgv_reserve_carved(ctx, &ctx->d_mu, &ctx->d_mu_cap,
+                              [&](kgv_carve& c) { lvl = c.take<uint8_t>(n_in * 384); out = c.take<uint8_t>(h * 384); wide = c.take<uint8_t>(h * 768); });
   if (rc) return rc;
-  uint8_t* M = ctx->d_mu;
   cudaStream_t st = ctx->stream;
   // contiguous values -> block-transposed level (limb block i of element e at (i * n_in + e) * 32 bytes) and back
   for (int i = 0; i < KGV_U3072_BLOCKS; i++)
-    CK(cudaMemcpy2DAsync(M + (size_t)i * n_in * 32, 32, in384 + 32 * i, 384, 32, n_in, cudaMemcpyHostToDevice, st));
-  if (coop) k_u3072_tree_level_coop<<<nblk(h, KGV_COOP_GROUPS), 128, 0, st>>>((const uint32_t*)M, n_in, (uint32_t*)(M + o_out));
-  else k_u3072_tree_level<<<nblk(h, 128), 128, 0, st>>>((const uint32_t*)M, n_in, (uint32_t*)(M + o_out), (uint32_t*)(M + o_wide));
+    CK(cudaMemcpy2DAsync(lvl + (size_t)i * n_in * 32, 32, in384 + 32 * i, 384, 32, n_in, cudaMemcpyHostToDevice, st));
+  if (coop) k_u3072_tree_level_coop<<<nblk(h, KGV_COOP_GROUPS), 128, 0, st>>>((const uint32_t*)lvl, n_in, (uint32_t*)out);
+  else k_u3072_tree_level<<<nblk(h, 128), 128, 0, st>>>((const uint32_t*)lvl, n_in, (uint32_t*)out, (uint32_t*)wide);
   CK(cudaGetLastError());
   ctx->launches++;
   for (int i = 0; i < KGV_U3072_BLOCKS; i++)
-    CK(cudaMemcpy2DAsync(out384 + 32 * i, 384, M + o_out + (size_t)i * h * 32, 32, 32, h, cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpy2DAsync(out384 + 32 * i, 384, out + (size_t)i * h * 32, 32, 32, h, cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
   return KGV_OK;
 }
@@ -277,10 +280,9 @@ extern "C" int kgv_muhash_finalize(kgv_ctx* ctx, const uint8_t* numerator384, co
   std::lock_guard<std::recursive_mutex> g(ctx->mu);
   if (!numerator384 || !denominator384 || !hash32) { ctx->err = "null argument"; return KGV_ERR_ARG; }
   CK(cudaSetDevice(ctx->device));
-  int rc = kgv_reserve(ctx, &ctx->d_mu, &ctx->d_mu_cap, 8192);
+  uint8_t *w, *o;
+  int rc = kgv_reserve_carved(ctx, &ctx->d_mu, &ctx->d_mu_cap, [&](kgv_carve& c) { w = c.take<uint8_t>(4096); o = c.take<uint8_t>(4096); });
   if (rc) return rc;
-  uint8_t* w = ctx->d_mu;
-  uint8_t* o = w + 4096;
   kgv_io io(ctx);
   const uint8_t* ins[2] = {numerator384, denominator384};  // each copied in from its own side
   for (int i = 0; i < 2; i++)
@@ -469,15 +471,14 @@ int kgv_mu_scan(kgv_ctx* ctx, uint32_t* vals, size_t pitch, size_t n, bool rev, 
   return KGV_OK;
 }
 
-// [P n] [S n] [out n] [tot chunks] [inverse scratch 3]
-size_t kgv_mu_finalize_scratch(size_t n) { return 3 * al256(n * 384) + al256((n + KGV_SCAN_CHUNK - 1) / KGV_SCAN_CHUNK * 384) + al256(3 * 384); }
-int kgv_mu_finalize_run(kgv_ctx* ctx, const uint32_t* dnum, const uint32_t* dden, size_t n, size_t pitch_words, uint8_t* scratch, uint32_t* dser,
-                        uint32_t* dhashes, cudaStream_t st) {
+void kgv_mu_finalize_work::carve(kgv_carve& c, size_t n) {
+  P = c.take<uint32_t>(n * 96); S = c.take<uint32_t>(n * 96); out = c.take<uint32_t>(n * 96);
+  tot = c.take<uint32_t>((n + KGV_SCAN_CHUNK - 1) / KGV_SCAN_CHUNK * 96); inv = c.take<uint32_t>(3 * 96);
+}
+int kgv_mu_finalize_run(kgv_ctx* ctx, const uint32_t* dnum, const uint32_t* dden, size_t n, size_t pitch_words, const kgv_mu_finalize_work& w,
+                        uint32_t* dser, uint32_t* dhashes, cudaStream_t st) {
   if (n == 0) return KGV_OK;
-  const size_t n_chunks = (n + KGV_SCAN_CHUNK - 1) / KGV_SCAN_CHUNK;
-  const size_t o_P = 0, o_S = al256(n * 384), o_out = o_S + al256(n * 384), o_tot = o_out + al256(n * 384), o_inv = o_tot + al256(n_chunks * 384);
-  uint32_t *P = (uint32_t*)(scratch + o_P), *S = (uint32_t*)(scratch + o_S), *out = (uint32_t*)(scratch + o_out), *tot = (uint32_t*)(scratch + o_tot),
-           *inv = (uint32_t*)(scratch + o_inv);
+  uint32_t *P = w.P, *S = w.S, *out = w.out, *tot = w.tot, *inv = w.inv;
   CK(cudaMemcpy2DAsync(P, 384, dden, pitch_words * 4, 384, n, cudaMemcpyDeviceToDevice, st));
   CK(cudaMemcpyAsync(S, P, n * 384, cudaMemcpyDeviceToDevice, st));
   int rc = kgv_mu_scan(ctx, P, 96, n, false, tot, st);
@@ -513,7 +514,8 @@ extern "C" int kgv_muhash_finalize_batch(kgv_ctx* ctx, const uint8_t* numerators
   }
   // a strided host array is one contiguous span (the pitch interleaves numerators and denominators of MuHash records)
   const size_t span = (n - 1) * pitch_bytes + 384;
-  int rc = kgv_reserve(ctx, &ctx->d_mu, &ctx->d_mu_cap, kgv_mu_finalize_scratch(n));
+  kgv_mu_finalize_work w;
+  int rc = kgv_reserve_carved(ctx, &ctx->d_mu, &ctx->d_mu_cap, [&](kgv_carve& c) { w.carve(c, n); });
   if (rc) return rc;
   const uint32_t *dnum, *dden;
   uint32_t *dh, *dser;
@@ -522,21 +524,21 @@ extern "C" int kgv_muhash_finalize_batch(kgv_ctx* ctx, const uint8_t* numerators
   io.out((uint32_t*)hashes32, n * 32, &dh);
   io.out((uint32_t*)serialized384, n * 384, &dser);
   if ((rc = io.stage())) return rc;
-  if ((rc = kgv_mu_finalize_run(ctx, dnum, dden, n, pitch_bytes / 4, ctx->d_mu, dser, dh, ctx->stream))) return rc;
+  if ((rc = kgv_mu_finalize_run(ctx, dnum, dden, n, pitch_bytes / 4, w, dser, dh, ctx->stream))) return rc;
   return io.finish();
 }
 
-size_t kgv_mu_prefix_scratch(size_t n) { return al256((n + KGV_SCAN_CHUNK - 1) / KGV_SCAN_CHUNK * 384); }
-int kgv_mu_prefix_combine_run(kgv_ctx* ctx, const uint32_t* dinit, uint32_t* v, size_t n, uint32_t* tot, cudaStream_t st) {
+void kgv_mu_prefix_work::carve(kgv_carve& c, size_t n) { tot = c.take<uint32_t>((n + KGV_SCAN_CHUNK - 1) / KGV_SCAN_CHUNK * 96); }
+int kgv_mu_prefix_combine_run(kgv_ctx* ctx, const uint32_t* dinit, uint32_t* v, size_t n, const kgv_mu_prefix_work& w, cudaStream_t st) {
   if (n == 0) return KGV_OK;
   if (dinit) {
     k_u3072_mul_first<<<1, 32, 0, st>>>(v, dinit, 2, 96);
     CK(cudaGetLastError());
     ctx->launches++;
   }
-  int rc = kgv_mu_scan(ctx, v, 192, n, false, tot, st);        // numerators
+  int rc = kgv_mu_scan(ctx, v, 192, n, false, w.tot, st);        // numerators
   if (rc) return rc;
-  rc = kgv_mu_scan(ctx, v + 96, 192, n, false, tot, st);   // denominators
+  rc = kgv_mu_scan(ctx, v + 96, 192, n, false, w.tot, st);   // denominators
   if (rc) return rc;
   k_u3072_canonicalize<<<nblk(2 * n, 128), 128, 0, st>>>(v, 96, 2 * n);
   CK(cudaGetLastError());
@@ -552,16 +554,16 @@ extern "C" int kgv_muhash_prefix_combine(kgv_ctx* ctx, const uint8_t* init768, u
   CK(cudaSetDevice(ctx->device));
   kgv_io io(ctx);
   if (io.is_device(values768) && ((uintptr_t)values768 & 15)) { ctx->err = "kgv_muhash_prefix_combine: device values768 must be 16-byte aligned"; return KGV_ERR_ARG; }  // scanned in place with 16-byte loads
-  const size_t o_init = kgv_mu_prefix_scratch(n);
-  int rc = kgv_reserve(ctx, &ctx->d_mu, &ctx->d_mu_cap, al256(o_init + 768));
+  kgv_mu_prefix_work w;
+  uint32_t* dinit;
+  int rc = kgv_reserve_carved(ctx, &ctx->d_mu, &ctx->d_mu_cap, [&](kgv_carve& c) { w.carve(c, n); dinit = c.take<uint32_t>(192); });
   if (rc) return rc;
-  uint8_t* M = ctx->d_mu;
   cudaStream_t st = ctx->stream;
   uint32_t* v;
   io.inout((uint32_t*)values768, n * 768, &v);
   if ((rc = io.stage())) return rc;
-  if (init768) CK(cudaMemcpyAsync(M + o_init, init768, 768, io.is_device(init768) ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, st));
-  rc = kgv_mu_prefix_combine_run(ctx, init768 ? (const uint32_t*)(M + o_init) : nullptr, v, n, (uint32_t*)M, st);
+  if (init768) CK(cudaMemcpyAsync(dinit, init768, 768, io.is_device(init768) ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, st));
+  rc = kgv_mu_prefix_combine_run(ctx, init768 ? dinit : nullptr, v, n, w, st);
   if (rc) return rc;
   return io.finish();
 }

@@ -613,48 +613,34 @@ extern "C" int kgv_replay_window(kgv_ctx* ctx, kgv_utxo_table* table, const kgv_
   const size_t nt = d.n_txs, ni = d.n_inputs, no = d.n_outputs;
   uint64_t wm_cap = 1024;
   while (wm_cap < 2 * nt) wm_cap <<= 1;
-  // window state
-  size_t o_ids = 0;
-  size_t o_wm = al256(o_ids + nt * 32);
-  size_t o_blk = al256(o_wm + wm_cap * 4);
-  size_t o_txb = al256(o_blk + n_blocks * sizeof(kgv_replay_block));
-  size_t o_itx = al256(o_txb + nt * 4);
-  size_t o_otx = al256(o_itx + ni * 4);
-  size_t o_ent = al256(o_otx + no * 4);
-  size_t o_pre = al256(o_ent + ni * sizeof(DevEntry));
-  size_t o_res = al256(o_pre + nt * sizeof(kgv_tx_result));
-  size_t o_acc = al256(o_res + nt * sizeof(kgv_tx_result));
-  size_t o_scr = al256(o_acc + nt);
-  size_t o_slp = al256(o_scr + ni * 72);
-  size_t o_rng = al256(o_slp + ni * sizeof(UtxoSlot*));
-  size_t o_cnt = al256(o_rng + n_blocks * sizeof(ReplayRange));
   // state of the walk
   uint64_t sm_cap = 1024;
   while (sm_cap < 2 * ni) sm_cap <<= 1;
   const uint32_t words_in = (uint32_t)((ni + 31) / 32), words_out = (uint32_t)((no + 31) / 32), words_tx = (uint32_t)((nt + 31) / 32);
-  size_t o_sib = al256(o_cnt + 64);
-  size_t o_src = al256(o_sib + nt);
-  size_t o_sfl = al256(o_src + ni * sizeof(ReplaySrc));
-  size_t o_inf = al256(o_sfl + nt * 4);
-  size_t o_fee = al256(o_inf + nt * sizeof(ReplayTxInfo));
-  size_t o_wst = al256(o_fee + nt * 8);
-  size_t o_wfl = al256(o_wst + nt);
-  size_t o_apv = al256(o_wfl + nt * 4);
-  size_t o_bm = al256(o_apv + nt * 8);
-  size_t o_smk = al256(o_bm + ((size_t)words_in + words_out + 2 * (size_t)words_tx) * 4);
-  size_t o_smv = al256(o_smk + sm_cap * 8);
-  size_t total = al256(o_smv + sm_cap * 4);
-  rc = kgv_reserve(ctx, &ctx->d_replay, &ctx->d_replay_cap, total);
+  const size_t bm_words = (size_t)words_in + words_out + 2 * (size_t)words_tx;
+  uint64_t *ids, *fee;
+  uint32_t *wm, *txb, *itx, *otx, *sfail, *wfl, *bm, *smv;
+  kgv_tx_result *pre, *res;
+  uint8_t *dacc, *scr, *sib, *wst;
+  unsigned long long *cnt, *apov, *smk;
+  kgv_replay_block* dblk;
+  DevEntry* dent;
+  UtxoSlot** slotp;
+  ReplayRange* ranges;
+  ReplaySrc* src;
+  ReplayTxInfo* info;
+  rc = kgv_reserve_carved(ctx, &ctx->d_replay, &ctx->d_replay_cap, [&](kgv_carve& c) {
+    // window state
+    ids = c.take<uint64_t>(nt * 4); wm = c.take<uint32_t>(wm_cap); dblk = c.take<kgv_replay_block>(n_blocks);
+    txb = c.take<uint32_t>(nt); itx = c.take<uint32_t>(ni); otx = c.take<uint32_t>(no); dent = c.take<DevEntry>(ni);
+    pre = c.take<kgv_tx_result>(nt); res = c.take<kgv_tx_result>(nt); dacc = c.take<uint8_t>(nt);
+    scr = c.take<uint8_t>(ni * 72); slotp = c.take<UtxoSlot*>(ni); ranges = c.take<ReplayRange>(n_blocks); cnt = c.take<unsigned long long>(8);
+    // state of the walk
+    sib = c.take<uint8_t>(nt); src = c.take<ReplaySrc>(ni); sfail = c.take<uint32_t>(nt); info = c.take<ReplayTxInfo>(nt);
+    fee = c.take<uint64_t>(nt); wst = c.take<uint8_t>(nt); wfl = c.take<uint32_t>(nt); apov = c.take<unsigned long long>(nt);
+    bm = c.take<uint32_t>(bm_words); smk = c.take<unsigned long long>(sm_cap); smv = c.take<uint32_t>(sm_cap);
+  });
   if (rc) return rc;
-  uint8_t* R = ctx->d_replay;
-  uint64_t* ids = (uint64_t*)(R + o_ids);
-  uint32_t* wm = (uint32_t*)(R + o_wm);
-  kgv_replay_block* dblk = (kgv_replay_block*)(R + o_blk);
-  uint32_t *txb = (uint32_t*)(R + o_txb), *itx = (uint32_t*)(R + o_itx), *otx = (uint32_t*)(R + o_otx);
-  DevEntry* dent = (DevEntry*)(R + o_ent);
-  kgv_tx_result *pre = (kgv_tx_result*)(R + o_pre), *res = (kgv_tx_result*)(R + o_res);
-  uint8_t* dacc = R + o_acc;
-  unsigned long long* cnt = (unsigned long long*)(R + o_cnt);
   cudaStream_t st = ctx->stream;
   if (stats) {
     for (cudaEvent_t& e : ctx->ev_time) if (!e) CK(cudaEventCreate(&e));
@@ -674,8 +660,8 @@ extern "C" int kgv_replay_window(kgv_ctx* ctx, kgv_utxo_table* table, const kgv_
   CK(cudaMemsetAsync(wm, 0, wm_cap * 4, st));
   CK(cudaMemsetAsync(cnt, 0, 64, st));
   if ((rc = kgv_tx_digests_run(ctx, d, nt, ids, false))) return rc;
-  CK(cudaMemsetAsync(R + o_sib, 0, nt, st));
-  k_wm_insert<<<nblk(nt, 128), 128, 0, st>>>(ids, (uint32_t)nt, wm, wm_cap - 1, R + o_sib);
+  CK(cudaMemsetAsync(sib, 0, nt, st));
+  k_wm_insert<<<nblk(nt, 128), 128, 0, st>>>(ids, (uint32_t)nt, wm, wm_cap - 1, sib);
   CK(cudaGetLastError());
   k_input_tx_index<<<nblk(nt, 128), 128, 0, st>>>(d.txs, (uint32_t)nt, itx);
   CK(cudaGetLastError());
@@ -683,16 +669,14 @@ extern "C" int kgv_replay_window(kgv_ctx* ctx, kgv_utxo_table* table, const kgv_
   CK(cudaGetLastError());
   k_replay_tx_block<<<(unsigned)n_blocks, 128, 0, st>>>(dblk, (uint32_t)n_blocks, txb);
   CK(cudaGetLastError());
-  k_replay_ranges<<<nblk(n_blocks, 128), 128, 0, st>>>(dblk, (uint32_t)n_blocks, d.txs, (ReplayRange*)(R + o_rng));
+  k_replay_ranges<<<nblk(n_blocks, 128), 128, 0, st>>>(dblk, (uint32_t)n_blocks, d.txs, ranges);
   CK(cudaGetLastError());
   ctx->launches += 5;
   // ---- pre-check of every script of the window
   BatchView v{d.txs, d.inputs, d.outputs, dent, d.bytes};
-  ReplaySrc* src = (ReplaySrc*)(R + o_src);
-  UtxoSlot** slotp = (UtxoSlot**)(R + o_slp);
   auto find_sources = [&]() -> int {
     if (!ni) return KGV_OK;
-    k_replay_sources<<<nblk(ni, 128), 128, 0, st>>>(view_of(table), v, ni, ids, wm, wm_cap - 1, txb, (const ReplayRange*)(R + o_rng), dent, slotp, src);
+    k_replay_sources<<<nblk(ni, 128), 128, 0, st>>>(view_of(table), v, ni, ids, wm, wm_cap - 1, txb, ranges, dent, slotp, src);
     CK(cudaGetLastError());
     ctx->launches++;
     return KGV_OK;
@@ -723,17 +707,6 @@ extern "C" int kgv_replay_window(kgv_ctx* ctx, kgv_utxo_table* table, const kgv_
   mark("script engine");
   if (stats) CK(cudaEventRecord(ctx->ev_time[1], st));
   // ---- the walk
-  const ReplayRange* ranges = (const ReplayRange*)(R + o_rng);
-  uint32_t* sfail = (uint32_t*)(R + o_sfl);
-  ReplayTxInfo* info = (ReplayTxInfo*)(R + o_inf);
-  uint64_t* fee = (uint64_t*)(R + o_fee);
-  uint8_t* wst = R + o_wst;
-  uint32_t* wfl = (uint32_t*)(R + o_wfl);
-  unsigned long long* apov = (unsigned long long*)(R + o_apv);
-  uint32_t* bm = (uint32_t*)(R + o_bm);
-  unsigned long long* smk = (unsigned long long*)(R + o_smk);
-  uint32_t* smv = (uint32_t*)(R + o_smv);
-  const size_t bm_words = (size_t)words_in + words_out + 2 * (size_t)words_tx;
   CK(cudaMemsetAsync(bm, 0, bm_words * 4, st));
   CK(cudaMemsetAsync(apov, 0, nt * 8, st));
   if (ni) {
@@ -746,7 +719,7 @@ extern "C" int kgv_replay_window(kgv_ctx* ctx, kgv_utxo_table* table, const kgv_
     ctx->launches += 2;
   }
   mark("slot map");
-  k_replay_static<<<nblk(nt, 128), 128, 0, st>>>(v, (uint32_t)nt, *prm, ranges, txb, pre, src, ids, wm, wm_cap - 1, R + o_sib, info, fee, sfail);
+  k_replay_static<<<nblk(nt, 128), 128, 0, st>>>(v, (uint32_t)nt, *prm, ranges, txb, pre, src, ids, wm, wm_cap - 1, sib, info, fee, sfail);
   CK(cudaGetLastError());
   ctx->launches++;
   mark("static rules");
@@ -770,7 +743,7 @@ extern "C" int kgv_replay_window(kgv_ctx* ctx, kgv_utxo_table* table, const kgv_
   ctx->launches++;
   const TableView tv = view_of(table);
   if (ni) {
-    k_replay_finish_inputs<<<nblk(ni, 128), 128, 0, st>>>(tv, v, ni, itx, dacc, slotp, src, apov, dent, R + o_scr);
+    k_replay_finish_inputs<<<nblk(ni, 128), 128, 0, st>>>(tv, v, ni, itx, dacc, slotp, src, apov, dent, scr);
     CK(cudaGetLastError());
     ctx->launches++;
   }
@@ -806,10 +779,10 @@ extern "C" int kgv_replay_window(kgv_ctx* ctx, kgv_utxo_table* table, const kgv_
   ctx->last_replay.valid = true;
   ctx->last_replay.txs = d.txs; ctx->last_replay.inputs = d.inputs; ctx->last_replay.outputs = d.outputs; ctx->last_replay.bytes = d.bytes;
   ctx->last_replay.nt = nt; ctx->last_replay.ni = ni; ctx->last_replay.no = no; ctx->last_replay.n_blocks = n_blocks;
-  ctx->last_replay.o_ids = o_ids; ctx->last_replay.o_itx = o_itx; ctx->last_replay.o_otx = o_otx; ctx->last_replay.o_ent = o_ent; ctx->last_replay.o_acc = o_acc;
-  ctx->last_replay.o_txb = o_txb; ctx->last_replay.o_rng = o_rng;
-  ctx->last_replay.o_src = o_src; ctx->last_replay.o_inf = o_inf; ctx->last_replay.o_apv = o_apv;
-  ctx->last_replay.o_blk = o_blk; ctx->last_replay.o_res = o_res;
+  ctx->last_replay.ids = ids; ctx->last_replay.itx = itx; ctx->last_replay.otx = otx; ctx->last_replay.ent = dent; ctx->last_replay.acc = dacc;
+  ctx->last_replay.txb = txb; ctx->last_replay.rng = ranges;
+  ctx->last_replay.src = src; ctx->last_replay.inf = info; ctx->last_replay.apv = apov;
+  ctx->last_replay.blk = dblk; ctx->last_replay.res = res;
   ctx->last_replay.table = table; ctx->last_replay.rehashes = kgv_chain_rehashes(table);
   ctx->last_replay.block_flags.resize(n_blocks); ctx->last_replay.block_n_txs.resize(n_blocks);
   for (size_t i = 0; i < n_blocks; i++) { ctx->last_replay.block_flags[i] = blocks[i].flags; ctx->last_replay.block_n_txs[i] = blocks[i].n_txs; }
@@ -879,36 +852,30 @@ __global__ void k_replay_group_ranges(const ReplayRange* __restrict__ ranges, co
   ilo[g] = i0; ihi[g] = any ? i1 : i0; olo[g] = o0; ohi[g] = any ? o1 : o0;
 }
 
-// scratch: [pov nt] [first nt] [ilo] [ihi] [olo] [ohi]
-size_t kgv_replay_muhash_scratch(kgv_ctx* ctx, size_t n_groups) { return al256(ctx->last_replay.nt * 8) + al256(ctx->last_replay.nt) + 4 * al256(n_groups * 4); }
-int kgv_replay_muhash_run(kgv_ctx* ctx, const uint32_t* dgf, size_t n_groups, uint8_t* scratch, uint32_t* vals, cudaStream_t st) {
+void kgv_replay_muhash_work::carve(kgv_carve& c, size_t nt, size_t n_groups) {
+  pov = c.take<uint64_t>(nt); first = c.take<uint8_t>(nt);
+  ilo = c.take<uint32_t>(n_groups); ihi = c.take<uint32_t>(n_groups); olo = c.take<uint32_t>(n_groups); ohi = c.take<uint32_t>(n_groups);
+}
+int kgv_replay_muhash_run(kgv_ctx* ctx, const uint32_t* dgf, size_t n_groups, const kgv_replay_muhash_work& w, uint32_t* vals, cudaStream_t st) {
   const auto& L = ctx->last_replay;
-  uint8_t* R = ctx->d_replay;
   const size_t nt = L.nt, ni = L.ni, no = L.no;
-  const size_t o_pov = 0, o_first = al256(nt * 8), o_ilo = o_first + al256(nt), o_ihi = o_ilo + al256(n_groups * 4), o_olo = o_ihi + al256(n_groups * 4),
-               o_ohi = o_olo + al256(n_groups * 4);
-  uint8_t* Wk = scratch;
   uint32_t *e_den = nullptr, *e_num = nullptr;
   int rc = kgv_mu_reserve(ctx, ni, no, &e_den, &e_num);
   if (rc) return rc;
-  const ReplayRange* ranges = (const ReplayRange*)(R + L.o_rng);
-  const uint32_t *itx = (const uint32_t*)(R + L.o_itx), *otx = (const uint32_t*)(R + L.o_otx), *txb = (const uint32_t*)(R + L.o_txb);
-  const uint8_t* acc = R + L.o_acc;
-  k_replay_tx_pov<<<nblk(nt, 256), 256, 0, st>>>(ranges, txb, (uint32_t)nt, (uint64_t*)(Wk + o_pov), Wk + o_first);
+  k_replay_tx_pov<<<nblk(nt, 256), 256, 0, st>>>(L.rng, L.txb, (uint32_t)nt, w.pov, w.first);
   CK(cudaGetLastError());
-  BatchView v{(const kgv_tx*)L.txs, (const kgv_input*)L.inputs, (const kgv_output*)L.outputs, (const DevEntry*)(R + L.o_ent), (const uint8_t*)L.bytes};
+  BatchView v{(const kgv_tx*)L.txs, (const kgv_input*)L.inputs, (const kgv_output*)L.outputs, L.ent, (const uint8_t*)L.bytes};
   if (ni + no) {
-    k_muhash_replay_elements<<<nblk(ni + no, 128), 128, 0, st>>>(v, ni, no, itx, otx, acc, (const uint64_t*)(R + L.o_ids), (const uint64_t*)(Wk + o_pov), Wk + o_first, e_den, e_num);
+    k_muhash_replay_elements<<<nblk(ni + no, 128), 128, 0, st>>>(v, ni, no, L.itx, L.otx, L.acc, L.ids, w.pov, w.first, e_den, e_num);
     CK(cudaGetLastError());
   }
-  k_replay_group_ranges<<<nblk(n_groups, 128), 128, 0, st>>>(ranges, dgf, (uint32_t)n_groups, (uint32_t*)(Wk + o_ilo), (uint32_t*)(Wk + o_ihi),
-                                                            (uint32_t*)(Wk + o_olo), (uint32_t*)(Wk + o_ohi));
+  k_replay_group_ranges<<<nblk(n_groups, 128), 128, 0, st>>>(L.rng, dgf, (uint32_t)n_groups, w.ilo, w.ihi, w.olo, w.ohi);
   CK(cudaGetLastError());
   ctx->launches += 3;
   // an input of an accepted transaction is always found (the context rules saw it), so accept[itx[j]] alone selects the denominators
-  rc = kgv_mu_range_products(ctx, e_num, no, acc, otx, (const uint32_t*)(Wk + o_olo), (const uint32_t*)(Wk + o_ohi), (uint32_t)n_groups, vals, 192, st);
+  rc = kgv_mu_range_products(ctx, e_num, no, L.acc, L.otx, w.olo, w.ohi, (uint32_t)n_groups, vals, 192, st);
   if (rc) return rc;
-  rc = kgv_mu_range_products(ctx, e_den, ni, acc, itx, (const uint32_t*)(Wk + o_ilo), (const uint32_t*)(Wk + o_ihi), (uint32_t)n_groups, vals + 96, 192, st);
+  rc = kgv_mu_range_products(ctx, e_den, ni, L.acc, L.itx, w.ilo, w.ihi, (uint32_t)n_groups, vals + 96, 192, st);
   if (rc) return rc;
   return kgv_mu_canonicalize(ctx, vals, 96, 2 * n_groups, st);
 }
@@ -928,13 +895,13 @@ extern "C" int kgv_replay_muhash(kgv_ctx* ctx, const uint32_t* group_first_block
   if (int rc = kgv_last_replay_read(ctx, acc, "kgv_replay_muhash")) return rc;
   cudaStream_t st = ctx->stream;
   // scratch (d_work is free between validation calls)
-  const size_t o_gf = 0, o_mu = al256((n_groups + 1) * 4), o_val = o_mu + kgv_replay_muhash_scratch(ctx, n_groups);
-  int rc = kgv_reserve(ctx, &ctx->d_work, &ctx->d_work_cap, al256(o_val + n_groups * 768));
+  uint32_t *dgf, *vals;
+  kgv_replay_muhash_work w;
+  int rc = kgv_reserve_carved(ctx, &ctx->d_work, &ctx->d_work_cap,
+                              [&](kgv_carve& c) { dgf = c.take<uint32_t>(n_groups + 1); w.carve(c, L.nt, n_groups); vals = c.take<uint32_t>(n_groups * 192); });
   if (rc) return rc;
-  uint8_t* Wk = ctx->d_work;
-  uint32_t* vals = (uint32_t*)(Wk + o_val);
-  CK(cudaMemcpyAsync(Wk + o_gf, group_first_block, (n_groups + 1) * 4, cudaMemcpyHostToDevice, st));
-  rc = kgv_replay_muhash_run(ctx, (const uint32_t*)(Wk + o_gf), n_groups, Wk + o_mu, vals, st);
+  CK(cudaMemcpyAsync(dgf, group_first_block, (n_groups + 1) * 4, cudaMemcpyHostToDevice, st));
+  rc = kgv_replay_muhash_run(ctx, dgf, n_groups, w, vals, st);
   if (rc) return rc;
   kgv_io io(ctx);
   if ((rc = io.copy_out(values768, vals, n_groups * 768))) return rc;
@@ -1135,16 +1102,21 @@ extern "C" int kgv_replay_diffs(kgv_ctx* ctx, const uint32_t* group_first_block,
   kgv_table_access acc(ctx);
   if (int rc = kgv_last_replay_read(ctx, acc, "kgv_replay_diffs")) return rc;
   cudaStream_t st = ctx->stream;
-  uint8_t* R = ctx->d_replay;
   const size_t nt = L.nt, ni = L.ni, no = L.no;
   // scratch (d_work is free between validation calls)
-  size_t o_ai = 0, o_bg = al256(nt * 4), o_sp = al256(o_bg + L.n_blocks * 4), o_gf = al256(o_sp + no * 4), o_gi = al256(o_gf + (n_groups + 1) * 4),
-         o_go = al256(o_gi + (n_groups + 1) * 4), o_rf = al256(o_go + (n_groups + 1) * 4), o_rl = al256(o_rf + ni * 4), o_af = al256(o_rl + ni * 4),
-         o_al = al256(o_af + no * 4), o_rs = al256(o_al + no * 4), o_rb = al256(o_rs + (ni + 1) * 8), o_as = al256(o_rb + (ni + 1) * 8),
-         o_ab = al256(o_as + (no + 1) * 8), o_rg = al256(o_ab + (no + 1) * 8), o_tot = al256(o_rg + n_groups * sizeof(kgv_diff_range));
-  int rc = kgv_reserve(ctx, &ctx->d_work, &ctx->d_work_cap, o_tot + 64);
+  DiffArgs a;
+  uint32_t* dgf;
+  kgv_diff_range* drg;
+  unsigned long long* dtot;
+  int rc = kgv_reserve_carved(ctx, &ctx->d_work, &ctx->d_work_cap, [&](kgv_carve& c) {
+    a.acc_inst = c.take<uint32_t>(nt); a.bgrp = c.take<uint32_t>(L.n_blocks); a.spg = c.take<uint32_t>(no);
+    dgf = c.take<uint32_t>(n_groups + 1); a.gi = c.take<uint32_t>(n_groups + 1); a.go = c.take<uint32_t>(n_groups + 1);
+    a.rflag = c.take<uint32_t>(ni); a.rlen = c.take<uint32_t>(ni); a.aflag = c.take<uint32_t>(no); a.alen = c.take<uint32_t>(no);
+    a.rs = c.take<unsigned long long>(ni + 1); a.rb = c.take<unsigned long long>(ni + 1);
+    a.as = c.take<unsigned long long>(no + 1); a.ab = c.take<unsigned long long>(no + 1);
+    drg = c.take<kgv_diff_range>(n_groups); dtot = c.take<unsigned long long>(8);
+  });
   if (rc) return rc;
-  uint8_t* Wk = ctx->d_work;
   // the diffs come back up to their sizes, known after the scan
   uint8_t *rk = nullptr, *ak = nullptr, *db = nullptr;
   kgv_utxo_entry *re = nullptr, *ae = nullptr;
@@ -1156,24 +1128,16 @@ extern "C" int kgv_replay_diffs(kgv_ctx* ctx, const uint32_t* group_first_block,
     io.out(bytes, bytes_cap, &db);
     if ((rc = io.stage())) return rc;
   }
-  DiffArgs a;
   a.txs = (const kgv_tx*)L.txs; a.inputs = (const kgv_input*)L.inputs; a.outputs = (const kgv_output*)L.outputs; a.bytes = (const uint8_t*)L.bytes;
-  a.dent = (const DevEntry*)(R + L.o_ent); a.ids = (const uint64_t*)(R + L.o_ids);
-  a.itx = (const uint32_t*)(R + L.o_itx); a.otx = (const uint32_t*)(R + L.o_otx); a.txb = (const uint32_t*)(R + L.o_txb);
-  a.ranges = (const ReplayRange*)(R + L.o_rng); a.accept = R + L.o_acc; a.src = (const ReplaySrc*)(R + L.o_src); a.info = (const ReplayTxInfo*)(R + L.o_inf);
-  a.acc_pov = (const unsigned long long*)(R + L.o_apv);
+  a.dent = L.ent; a.ids = L.ids; a.itx = L.itx; a.otx = L.otx; a.txb = L.txb;
+  a.ranges = L.rng; a.accept = L.acc; a.src = L.src; a.info = L.inf; a.acc_pov = L.apv;
   a.nt = (uint32_t)nt; a.ni = (uint32_t)ni; a.no = (uint32_t)no; a.n_blocks = (uint32_t)L.n_blocks;
-  a.acc_inst = (uint32_t*)(Wk + o_ai); a.bgrp = (uint32_t*)(Wk + o_bg); a.spg = (uint32_t*)(Wk + o_sp); a.gi = (uint32_t*)(Wk + o_gi); a.go = (uint32_t*)(Wk + o_go);
-  a.rflag = (uint32_t*)(Wk + o_rf); a.rlen = (uint32_t*)(Wk + o_rl); a.aflag = (uint32_t*)(Wk + o_af); a.alen = (uint32_t*)(Wk + o_al);
-  a.rs = (unsigned long long*)(Wk + o_rs); a.rb = (unsigned long long*)(Wk + o_rb); a.as = (unsigned long long*)(Wk + o_as); a.ab = (unsigned long long*)(Wk + o_ab);
-  kgv_diff_range* drg = (kgv_diff_range*)(Wk + o_rg);
-  unsigned long long* dtot = (unsigned long long*)(Wk + o_tot);
-  CK(cudaMemcpyAsync(Wk + o_gf, group_first_block, (n_groups + 1) * 4, cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync(dgf, group_first_block, (n_groups + 1) * 4, cudaMemcpyHostToDevice, st));
   CK(cudaMemsetAsync(a.acc_inst, 0xFF, nt * 4, st));
   if (no) CK(cudaMemsetAsync(a.spg, 0xFF, no * 4, st));
   k_diff_acc_inst<<<nblk(nt, 256), 256, 0, st>>>(a);
   CK(cudaGetLastError());
-  k_diff_groups<<<nblk(n_groups + 1, 128), 128, 0, st>>>(a, (const uint32_t*)(Wk + o_gf), (uint32_t)n_groups);
+  k_diff_groups<<<nblk(n_groups + 1, 128), 128, 0, st>>>(a, dgf, (uint32_t)n_groups);
   CK(cudaGetLastError());
   if (ni) { k_diff_spender_group<<<nblk(ni, 256), 256, 0, st>>>(a); CK(cudaGetLastError()); }
   if (ni + no) { k_diff_classify<<<nblk(ni + no, 256), 256, 0, st>>>(a); CK(cudaGetLastError()); }

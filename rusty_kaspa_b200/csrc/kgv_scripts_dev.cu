@@ -170,29 +170,32 @@ int kgv_script_engine_run(kgv_ctx* ctx, const BatchView& v, size_t n_txs, const 
   if (n_list > 0xFFFFFFFFull) { ctx->err = "kgv_check_scripts: too many transactions"; return KGV_ERR_ARG; }
   cudaStream_t st = ctx->stream;
   const uint32_t nl = (uint32_t)n_list;
-  // phase 1, in ctx->d_out: per listed tx its input count, work offset, first failing input and sub-hashes; flags
-  size_t o_cnt = 0, o_off = al256(o_cnt + n_list * 4), o_fail = al256(o_off + n_list * 4), o_reu = al256(o_fail + n_list * 4);
-  size_t o_flag = al256(o_reu + n_list * sizeof(SigHashReused)), o_list = al256(o_flag + 64);
-  size_t o_sel = al256(o_list + (dlist ? 0 : n_list * 4)), o_selo = al256(o_sel + (dlist ? 0 : n_txs * 4));
-  int rc = kgv_reserve(ctx, &ctx->d_out, &ctx->d_out_cap, al256(o_selo + (dlist ? 0 : n_txs * 4)));
+  // phase 1, in ctx->d_out: per listed tx its input count, work offset, first failing input and sub-hashes; flags; without dlist the
+  // selected list and its flags and offsets
+  const bool select = !dlist;
+  uint32_t *cnt, *off, *fail_at, *list, *sel, *selo;
+  SigHashReused* reu;
+  unsigned int* flags;  // [0] bad index, [1] overflow, [2..3] round totals, [4] work total, [6..7] its 64-bit sum, [8] the selection's total
+  int rc = kgv_reserve_carved(ctx, &ctx->d_out, &ctx->d_out_cap, [&](kgv_carve& c) {
+    cnt = c.take<uint32_t>(n_list); off = c.take<uint32_t>(n_list); fail_at = c.take<uint32_t>(n_list); reu = c.take<SigHashReused>(n_list);
+    flags = c.take<unsigned int>(16);
+    list = select ? c.take<uint32_t>(n_list) : nullptr; sel = select ? c.take<uint32_t>(n_txs) : nullptr; selo = select ? c.take<uint32_t>(n_txs) : nullptr;
+  });
   if (rc) return rc;
-  uint8_t* O = ctx->d_out;
-  if (!dlist) {
-    uint32_t *sel = (uint32_t*)(O + o_sel), *selo = (uint32_t*)(O + o_selo);
+  if (select) {
     k_se_select_flag<<<nblk(n_txs, 256), 256, 0, st>>>(dres, (uint32_t)n_txs, sel);
     CK(cudaGetLastError());
-    rc = kgv_scan_u32(ctx, sel, selo, nullptr, nullptr, n_txs, (uint32_t*)(O + o_flag + 32), st);
+    rc = kgv_scan_u32(ctx, sel, selo, nullptr, nullptr, n_txs, (uint32_t*)(flags + 8), st);
     if (rc) return rc;
-    k_se_select_scatter<<<nblk(n_txs, 256), 256, 0, st>>>(sel, selo, (uint32_t)n_txs, (uint32_t*)(O + o_list));
+    k_se_select_scatter<<<nblk(n_txs, 256), 256, 0, st>>>(sel, selo, (uint32_t)n_txs, list);
     CK(cudaGetLastError());
     ctx->launches += 3;
-    dlist = (const uint32_t*)(O + o_list);
+    dlist = list;
   }
-  unsigned int* flags = (unsigned int*)(O + o_flag);  // [0] bad index, [1] overflow, [2..3] round totals, [4] work total, [6..7] its 64-bit sum
   CK(cudaMemsetAsync(flags, 0, 64, st));
-  k_se_count<<<nblk(nl, 128), 128, 0, st>>>(v.txs, n_txs, dlist, nl, (uint32_t*)(O + o_cnt), (uint32_t*)(O + o_fail), flags, (unsigned long long*)(flags + 6));
+  k_se_count<<<nblk(nl, 128), 128, 0, st>>>(v.txs, n_txs, dlist, nl, cnt, fail_at, flags, (unsigned long long*)(flags + 6));
   CK(cudaGetLastError());
-  rc = kgv_scan_u32(ctx, (const uint32_t*)(O + o_cnt), (uint32_t*)(O + o_off), nullptr, nullptr, n_list, (uint32_t*)(flags + 4), st);
+  rc = kgv_scan_u32(ctx, cnt, off, nullptr, nullptr, n_list, (uint32_t*)(flags + 4), st);
   if (rc) return rc;
   ctx->launches += 1;
   unsigned int hf[8];
@@ -202,7 +205,6 @@ int kgv_script_engine_run(kgv_ctx* ctx, const BatchView& v, size_t n_txs, const 
   const uint64_t nw64 = (uint64_t)hf[6] | ((uint64_t)hf[7] << 32);
   if (nw64 > 0xFFFFFFFFull) { ctx->err = "kgv_check_scripts: the listed transactions have 2^32 or more inputs in all"; return KGV_ERR_ARG; }
   const size_t nw = (size_t)nw64;
-  const uint32_t* off = (const uint32_t*)(O + o_off);
   if (nw == 0) {
     k_se_finalize<<<nblk(nl, 128), 128, 0, st>>>(v, dlist, nl, off, nullptr, dres, patch);
     CK(cudaGetLastError());
@@ -210,20 +212,17 @@ int kgv_script_engine_run(kgv_ctx* ctx, const BatchView& v, size_t n_txs, const 
     return KGV_OK;
   }
   // phase 2, in ctx->d_scratch: per-work-item state and the slots
-  const size_t o_work = 0, o_st = al256(o_work + nw * sizeof(ScriptWork)), o_nlog = al256(o_st + nw), o_log = al256(o_nlog + nw);
-  const size_t o_req = al256(o_log + nw * SE_LOG_BYTES), o_cs = al256(o_req + nw * sizeof(ScriptReq)), o_ce = al256(o_cs + nw * 4);
-  const size_t o_os = al256(o_ce + nw * 4), o_oe = al256(o_os + nw * 4), o_slot = al256(o_oe + nw * 4);
   const uint32_t n_slots = (uint32_t)std::min(nw, kSlotBytes / sizeof(ScriptSlot));
-  rc = kgv_reserve(ctx, &ctx->d_scratch, &ctx->d_scratch_cap, o_slot + (size_t)n_slots * sizeof(ScriptSlot));
+  ScriptWork* work;
+  uint8_t *status, *nlog, *logs;
+  ScriptReq* req;
+  uint32_t *cs, *ce, *os, *oe;
+  ScriptSlot* slots;
+  rc = kgv_reserve_carved(ctx, &ctx->d_scratch, &ctx->d_scratch_cap, [&](kgv_carve& c) {
+    work = c.take<ScriptWork>(nw); status = c.take<uint8_t>(nw); nlog = c.take<uint8_t>(nw); logs = c.take<uint8_t>(nw * SE_LOG_BYTES); req = c.take<ScriptReq>(nw);
+    cs = c.take<uint32_t>(nw); ce = c.take<uint32_t>(nw); os = c.take<uint32_t>(nw); oe = c.take<uint32_t>(nw); slots = c.take<ScriptSlot>(n_slots);
+  });
   if (rc) return rc;
-  uint8_t* S = ctx->d_scratch;
-  uint32_t* fail_at = (uint32_t*)(O + o_fail);
-  SigHashReused* reu = (SigHashReused*)(O + o_reu);
-  ScriptWork* work = (ScriptWork*)(S + o_work);
-  uint8_t *status = S + o_st, *nlog = S + o_nlog, *logs = S + o_log;
-  ScriptReq* req = (ScriptReq*)(S + o_req);
-  uint32_t *cs = (uint32_t*)(S + o_cs), *ce = (uint32_t*)(S + o_ce), *os = (uint32_t*)(S + o_os), *oe = (uint32_t*)(S + o_oe);
-  ScriptSlot* slots = (ScriptSlot*)(S + o_slot);
   CK(cudaMemsetAsync(logs, 0, nw * SE_LOG_BYTES, st));
   k_se_expand<<<nblk(nl, 128), 128, 0, st>>>(v.txs, dlist, nl, off, work, status, nlog);
   CK(cudaGetLastError());
@@ -246,31 +245,28 @@ int kgv_script_engine_run(kgv_ctx* ctx, const BatchView& v, size_t n_txs, const 
     const size_t ns = h[1], ne = h[2];
     if (ns + ne == 0) break;
     if (round >= 256) { ctx->err = "script engine: an input asked for more than 255 signature checks (internal error)"; return KGV_ERR_LIMIT; }
-    struct Kind { size_t n, pk, sig, msg, ref, st, dig, idx, nm; } kind[2];
-    size_t tot = 0;
-    for (int e = 0; e < 2; e++) {
-      Kind& k = kind[e];
-      k.n = e ? ne : ns;
-      k.pk = tot; k.sig = al256(k.pk + k.n * (e ? 33 : 32)); k.msg = al256(k.sig + k.n * 64); k.ref = al256(k.msg + k.n * 32);
-      k.st = al256(k.ref + k.n * 4); k.dig = al256(k.st + k.n + 64); k.idx = al256(k.dig + (sc ? k.n * 32 : 0)); k.nm = al256(k.idx + (sc ? k.n * 4 : 0));
-      tot = al256(k.nm + 64);
-    }
-    rc = kgv_reserve(ctx, &ctx->d_in, &ctx->d_in_cap, tot);
+    struct Kind { size_t n; uint8_t *pk, *sig, *msg, *st, *dig; uint32_t *ref, *idx, *nm; } kind[2] = {{ns}, {ne}};
+    rc = kgv_reserve_carved(ctx, &ctx->d_in, &ctx->d_in_cap, [&](kgv_carve& c) {
+      for (int e = 0; e < 2; e++) {
+        Kind& k = kind[e];
+        k.pk = c.take<uint8_t>(k.n * (e ? 33 : 32)); k.sig = c.take<uint8_t>(k.n * 64); k.msg = c.take<uint8_t>(k.n * 32); k.ref = c.take<uint32_t>(k.n);
+        k.st = c.take<uint8_t>(k.n, 64);
+        k.dig = c.take<uint8_t>(sc ? k.n * 32 : 0); k.idx = c.take<uint32_t>(sc ? k.n : 0); k.nm = c.take<uint32_t>(16);
+      }
+    });
     if (rc) return rc;
-    uint8_t* I = ctx->d_in;
-    k_se_emit<<<nblk(nw, 128), 128, 0, st>>>(cs, ce, os, oe, (uint32_t)nw, req, I + kind[0].pk, I + kind[0].sig, (uint32_t*)(I + kind[0].ref), I + kind[1].pk,
-                                             I + kind[1].sig, (uint32_t*)(I + kind[1].ref));
+    k_se_emit<<<nblk(nw, 128), 128, 0, st>>>(cs, ce, os, oe, (uint32_t)nw, req, kind[0].pk, kind[0].sig, kind[0].ref, kind[1].pk, kind[1].sig, kind[1].ref);
     CK(cudaGetLastError());
     ctx->launches++;
     for (int e = 0; e < 2; e++) {
       const Kind& k = kind[e];
       if (!k.n) continue;
-      k_se_msgs<<<nblk(k.n, 128), 128, 0, st>>>(v, work, req, reu, (const uint32_t*)(I + k.ref), (uint32_t)k.n, e == 1, (uint32_t*)(I + k.msg));
+      k_se_msgs<<<nblk(k.n, 128), 128, 0, st>>>(v, work, req, reu, k.ref, (uint32_t)k.n, e == 1, (uint32_t*)k.msg);
       CK(cudaGetLastError());
       ctx->launches++;
-      rc = kgv_verify_items(ctx, sc, I + k.pk, I + k.msg, I + k.sig, k.n, e == 1, I + k.st, I + k.dig, (uint32_t*)(I + k.idx), (uint32_t*)(I + k.nm), st);
+      rc = kgv_verify_items(ctx, sc, k.pk, k.msg, k.sig, k.n, e == 1, k.st, k.dig, k.idx, k.nm, st);
       if (rc) return rc;
-      k_se_append<<<nblk(k.n, 128), 128, 0, st>>>((const uint32_t*)(I + k.ref), I + k.st, (uint32_t)k.n, nlog, logs);
+      k_se_append<<<nblk(k.n, 128), 128, 0, st>>>(k.ref, k.st, (uint32_t)k.n, nlog, logs);
       CK(cudaGetLastError());
       ctx->launches++;
     }
@@ -324,12 +320,10 @@ extern "C" int kgv_check_scripts(kgv_ctx* ctx, const kgv_tx_batch* batch, const 
   int rc = kgv_batch_to_device(ctx, batch, &d, true);
   if (rc) return rc;
   const size_t ni = d.n_inputs;
-  size_t o_ent = 0, o_res = al256(ni * sizeof(DevEntry));
-  rc = kgv_reserve(ctx, &ctx->d_work, &ctx->d_work_cap, al256(o_res + n * sizeof(kgv_tx_result)));
+  DevEntry* dent;
+  kgv_tx_result* dres;
+  rc = kgv_reserve_carved(ctx, &ctx->d_work, &ctx->d_work_cap, [&](kgv_carve& c) { dent = c.take<DevEntry>(ni); dres = c.take<kgv_tx_result>(n); });
   if (rc) return rc;
-  uint8_t* W = ctx->d_work;
-  DevEntry* dent = (DevEntry*)(W + o_ent);
-  kgv_tx_result* dres = (kgv_tx_result*)(W + o_res);
   cudaStream_t st = ctx->stream;
   const uint32_t* dlist;
   io.in(tx_indices, n * 4, &dlist);

@@ -871,22 +871,16 @@ int kgv_verify_items(kgv_ctx* ctx, kgv_sigcache* sc, const uint8_t* pk, const ui
 int kgv_scripts_phase(kgv_ctx* ctx, const BatchView& v, size_t nt, size_t ni, const uint32_t* itx, kgv_tx_result* dres, uint64_t* n_items_out) {
   if (n_items_out) *n_items_out = 0;
   if (ni == 0) return KGV_OK;
-  size_t o_plan = 0;
-  size_t o_cs = al256(o_plan + ni * sizeof(InputPlan));
-  size_t o_ce = al256(o_cs + ni * 4);
-  size_t o_os = al256(o_ce + ni * 4);
-  size_t o_oe = al256(o_os + ni * 4);
-  size_t o_tot = al256(o_oe + ni * 4);
-  size_t o_err = al256(o_tot + 64);
-  size_t o_reu = al256(o_err + ni);
-  size_t total = al256(o_reu + nt * sizeof(SigHashReused));
-  int rc = kgv_reserve(ctx, &ctx->d_scratch, &ctx->d_scratch_cap, total);
+  InputPlan* plans;
+  uint32_t *cs, *ce, *os, *oe, *tot;
+  uint8_t* ierr;
+  SigHashReused* reu;
+  int rc = kgv_reserve_carved(ctx, &ctx->d_scratch, &ctx->d_scratch_cap, [&](kgv_carve& c) {
+    plans = c.take<InputPlan>(ni);
+    cs = c.take<uint32_t>(ni); ce = c.take<uint32_t>(ni); os = c.take<uint32_t>(ni); oe = c.take<uint32_t>(ni); tot = c.take<uint32_t>(16);
+    ierr = c.take<uint8_t>(ni); reu = c.take<SigHashReused>(nt);
+  });
   if (rc) return rc;
-  uint8_t* S = ctx->d_scratch;
-  InputPlan* plans = (InputPlan*)(S + o_plan);
-  uint32_t *cs = (uint32_t*)(S + o_cs), *ce = (uint32_t*)(S + o_ce), *os = (uint32_t*)(S + o_os), *oe = (uint32_t*)(S + o_oe), *tot = (uint32_t*)(S + o_tot);
-  uint8_t* ierr = S + o_err;
-  SigHashReused* reu = (SigHashReused*)(S + o_reu);
   cudaStream_t st = ctx->stream;
   k_plan<<<nblk(ni, 128), 128, 0, st>>>(v, ni, itx, dres, plans, cs, ce);
   CK(cudaGetLastError());
@@ -909,27 +903,29 @@ int kgv_scripts_phase(kgv_ctx* ctx, const BatchView& v, size_t nt, size_t ni, co
   // item arrays of the two kinds ([0] Schnorr, [1] ECDSA) in d_in: pk, sig, msg, refs, status (padded to nr * per), and with the signature
   // cache the digests, the miss list and the miss count
   struct ItemKind {
-    size_t n, per, lo, hi;                       // items, range length per rank, this rank's range [lo, hi)
-    size_t pk, sig, msg, ref, st, dig, idx, nm;  // offsets in d_in
+    size_t n, per, lo, hi;  // items, range length per rank, this rank's range [lo, hi)
+    uint8_t *pk, *sig, *msg, *st, *dig;  // the item arrays in d_in
+    ItemRef* ref;
+    uint32_t *idx, *nm;
   } kind[2];
-  size_t total2 = 0;
   for (int e = 0; e < 2; e++) {
     ItemKind& k = kind[e];
     k.n = e ? ne : ns;
     k.per = nr > 1 ? al256((k.n + nr - 1) / nr) : k.n;
     k.lo = std::min(rk * k.per, k.n);
     k.hi = std::min((rk + 1) * k.per, k.n);
-    k.pk = total2; k.sig = al256(k.pk + k.n * (e ? 33 : 32)); k.msg = al256(k.sig + k.n * 64); k.ref = al256(k.msg + k.n * 32);
-    k.st = al256(k.ref + k.n * sizeof(ItemRef)); k.dig = al256(k.st + nr * k.per + 64);
-    k.idx = al256(k.dig + (sc ? k.n * 32 : 0)); k.nm = al256(k.idx + (sc ? k.n * 4 : 0));
-    total2 = al256(k.nm + 64);
   }
-  rc = kgv_reserve(ctx, &ctx->d_in, &ctx->d_in_cap, total2);
+  rc = kgv_reserve_carved(ctx, &ctx->d_in, &ctx->d_in_cap, [&](kgv_carve& c) {
+    for (int e = 0; e < 2; e++) {
+      ItemKind& k = kind[e];
+      k.pk = c.take<uint8_t>(k.n * (e ? 33 : 32)); k.sig = c.take<uint8_t>(k.n * 64); k.msg = c.take<uint8_t>(k.n * 32); k.ref = c.take<ItemRef>(k.n);
+      k.st = c.take<uint8_t>(nr * k.per, 64);
+      k.dig = c.take<uint8_t>(sc ? k.n * 32 : 0); k.idx = c.take<uint32_t>(sc ? k.n : 0); k.nm = c.take<uint32_t>(16);
+    }
+  });
   if (rc) return rc;
-  uint8_t* I = ctx->d_in;
   if (ns + ne) {
-    k_emit_items<<<nblk(ni, 128), 128, 0, st>>>(v, ni, plans, os, oe, I + kind[0].pk, I + kind[0].sig, (ItemRef*)(I + kind[0].ref), I + kind[1].pk,
-                                                I + kind[1].sig, (ItemRef*)(I + kind[1].ref));
+    k_emit_items<<<nblk(ni, 128), 128, 0, st>>>(v, ni, plans, os, oe, kind[0].pk, kind[0].sig, kind[0].ref, kind[1].pk, kind[1].sig, kind[1].ref);
     CK(cudaGetLastError());
     k_sighash_reused_v<<<nblk(nt, 128), 128, 0, st>>>(v, (uint32_t)nt, dres, reu);
     CK(cudaGetLastError());
@@ -941,13 +937,12 @@ int kgv_scripts_phase(kgv_ctx* ctx, const BatchView& v, size_t nt, size_t ni, co
     const ItemKind& k = kind[ecdsa];
     if (k.hi <= k.lo) return KGV_OK;
     const size_t m = k.hi - k.lo;
-    k_item_msgs<<<nblk(m, 128), 128, 0, s>>>(v, reu, itx, plans, (const ItemRef*)(I + k.ref) + k.lo, m, ecdsa, (uint32_t*)(I + k.msg) + 8 * k.lo);
+    k_item_msgs<<<nblk(m, 128), 128, 0, s>>>(v, reu, itx, plans, k.ref + k.lo, m, ecdsa, (uint32_t*)k.msg + 8 * k.lo);
     CK(cudaGetLastError());
     ctx->launches++;
     STAGE(ecdsa ? "msgs ecdsa" : "msgs schnorr");
     // (with the cache there is one rank: lo = 0, m = n)
-    return kgv_verify_items(ctx, sc, I + k.pk + (ecdsa ? 33 : 32) * k.lo, I + k.msg + 32 * k.lo, I + k.sig + 64 * k.lo, m, ecdsa, I + k.st + k.lo, I + k.dig,
-                            (uint32_t*)(I + k.idx), (uint32_t*)(I + k.nm), s);
+    return kgv_verify_items(ctx, sc, k.pk + (ecdsa ? 33 : 32) * k.lo, k.msg + 32 * k.lo, k.sig + 64 * k.lo, m, ecdsa, k.st + k.lo, k.dig, k.idx, k.nm, s);
   };
   if (ns && ne) CK(cudaEventRecord(ctx->ev_fork, st));  // fork point: everything both item kinds depend on is queued
   if (ns) {
@@ -971,10 +966,10 @@ int kgv_scripts_phase(kgv_ctx* ctx, const BatchView& v, size_t nt, size_t ni, co
   }
   if (nr > 1) {
     for (const ItemKind& k : kind)
-      if (k.n) { rc = kgv_comm_exchange_slices(ctx, ctx->shard_comm, I + k.st, k.per); if (rc) return rc; }
+      if (k.n) { rc = kgv_comm_exchange_slices(ctx, ctx->shard_comm, k.st, k.per); if (rc) return rc; }
     STAGE("verdict exchange");
   }
-  k_resolve<<<nblk(ni, 128), 128, 0, st>>>(v, ni, itx, dres, plans, I + kind[0].st, I + kind[1].st, ierr);
+  k_resolve<<<nblk(ni, 128), 128, 0, st>>>(v, ni, itx, dres, plans, kind[0].st, kind[1].st, ierr);
   CK(cudaGetLastError());
   STAGE("resolve");
   k_tx_finalize<<<nblk(nt, 128), 128, 0, st>>>(v, (uint32_t)nt, ierr, dres);
@@ -1024,16 +1019,14 @@ static int validate_core(kgv_ctx* ctx, kgv_utxo_table* table, const kgv_tx_batch
   int rc = kgv_batch_to_device(ctx, batch, &d, table == nullptr);
   if (rc) return rc;
   const size_t nt = d.n_txs, ni = d.n_inputs;
-  size_t o_ent = 0;
-  size_t o_itx = al256(o_ent + ni * sizeof(DevEntry));
-  size_t o_res = al256(o_itx + ni * 4);
-  size_t o_cnt = al256(o_res + nt * sizeof(kgv_tx_result));
-  rc = kgv_reserve(ctx, &ctx->d_work, &ctx->d_work_cap, o_cnt + 8);
+  DevEntry* dent;
+  uint32_t* itx;
+  kgv_tx_result* dres;
+  unsigned long long* cnt;
+  rc = kgv_reserve_carved(ctx, &ctx->d_work, &ctx->d_work_cap, [&](kgv_carve& c) {
+    dent = c.take<DevEntry>(ni); itx = c.take<uint32_t>(ni); dres = c.take<kgv_tx_result>(nt); cnt = c.take<unsigned long long>(1);
+  });
   if (rc) return rc;
-  uint8_t* S = ctx->d_work;
-  DevEntry* dent = (DevEntry*)(S + o_ent);
-  uint32_t* itx = (uint32_t*)(S + o_itx);
-  kgv_tx_result* dres = (kgv_tx_result*)(S + o_res);
   cudaStream_t st = ctx->stream;
 
   if (ni) {
@@ -1051,7 +1044,7 @@ static int validate_core(kgv_ctx* ctx, kgv_utxo_table* table, const kgv_tx_batch
   ctx->launches++;
   STAGE("tx_context");
   if (flags != KGV_FLAGS_SKIP_SCRIPT_CHECKS && ni) {
-    rc = table ? scripts_with_engine(ctx, (unsigned long long*)(S + o_cnt), d, v, itx, dres) : kgv_scripts_phase(ctx, v, nt, ni, itx, dres, nullptr);
+    rc = table ? scripts_with_engine(ctx, cnt, d, v, itx, dres) : kgv_scripts_phase(ctx, v, nt, ni, itx, dres, nullptr);
     if (rc) return rc;
   }
   kgv_io io(ctx);
@@ -1117,22 +1110,22 @@ static int mempool_core(kgv_ctx* ctx, kgv_utxo_table* t, const kgv_tx_batch* bat
   // d_work: populated entries, input -> tx, verdicts, masses, script lengths and their offsets,
   // counters [script bytes (64-bit), zero divisors, the scan's 32-bit total, the relay-fee overflow flag of the standardness policy, the
   // script engine's count]
-  size_t o_ent = 0;
-  size_t o_itx = al256(o_ent + ni * sizeof(DevEntry));
-  size_t o_res = al256(o_itx + ni * 4);
-  size_t o_mass = al256(o_res + nt * sizeof(kgv_tx_result));
-  size_t o_len = al256(o_mass + nt * 8);
-  size_t o_off = al256(o_len + ni * 4);
-  size_t o_cnt = al256(o_off + ni * 4);
   // with iso: its verdicts, max(compute, transient) per tx, the masses (for the policy when the caller takes none), the large-transaction list
   const kgv_mempool_policy* pol = iso ? iso->policy : nullptr;
   uint64_t* detail = iso ? iso->detail : nullptr;
   const bool own_masses = iso && !iso->masses && pol;
-  size_t o_iso = al256(o_cnt + 40);
-  size_t o_nc = al256(o_iso + (iso ? nt * sizeof(kgv_tx_result) : 0));
-  size_t o_ism = al256(o_nc + (iso ? nt * 8 : 0));
-  size_t o_lst = al256(o_ism + (own_masses ? nt * sizeof(kgv_tx_masses) : 0));
-  rc = kgv_reserve(ctx, &ctx->d_work, &ctx->d_work_cap, iso ? al256(o_lst + (nt + 1) * 4) : al256(o_cnt + 40));
+  DevEntry* dent;
+  uint32_t *itx, *len, *off, *lst;
+  kgv_tx_result *dres, *gate;
+  uint64_t *dmass, *dnc;
+  unsigned long long* cnt;
+  kgv_tx_masses* own;
+  rc = kgv_reserve_carved(ctx, &ctx->d_work, &ctx->d_work_cap, [&](kgv_carve& c) {
+    dent = c.take<DevEntry>(ni); itx = c.take<uint32_t>(ni); dres = c.take<kgv_tx_result>(nt); dmass = c.take<uint64_t>(nt);
+    len = c.take<uint32_t>(ni); off = c.take<uint32_t>(ni); cnt = c.take<unsigned long long>(5);
+    gate = iso ? c.take<kgv_tx_result>(nt) : nullptr; dnc = iso ? c.take<uint64_t>(nt) : nullptr;
+    own = own_masses ? c.take<kgv_tx_masses>(nt) : nullptr; lst = iso ? c.take<uint32_t>(nt + 1) : nullptr;
+  });
   if (rc) return rc;
   // the entries' scripts come back up to their size, known after the context rules
   const kgv_mempool_tx_args* dargs;
@@ -1146,21 +1139,11 @@ static int mempool_core(kgv_ctx* ctx, kgv_utxo_table* t, const kgv_tx_batch* bat
   io.out(ni ? entries_out : nullptr, ni * sizeof(kgv_utxo_entry), &de);
   io.out(ni && entries_out && scripts_cap ? scripts_out : nullptr, scripts_cap, &ds);
   if ((rc = io.stage())) return rc;
-  uint8_t* S = ctx->d_work;
-  DevEntry* dent = (DevEntry*)(S + o_ent);
-  uint32_t *itx = (uint32_t*)(S + o_itx), *len = (uint32_t*)(S + o_len), *off = (uint32_t*)(S + o_off);
-  unsigned long long* cnt = (unsigned long long*)(S + o_cnt);
-  kgv_tx_result* dres = (kgv_tx_result*)(S + o_res);
-  uint64_t* dmass = (uint64_t*)(S + o_mass);
   cudaStream_t st = ctx->stream;
   CK(cudaMemsetAsync(cnt, 0, 32, st));
-  kgv_tx_result* gate = nullptr;
-  uint64_t* dnc = nullptr;
   if (iso) {
-    gate = (kgv_tx_result*)(S + o_iso);
-    dnc = (uint64_t*)(S + o_nc);
-    if (own_masses) dism = (kgv_tx_masses*)(S + o_ism);
-    rc = kgv_isolation_run(ctx, d, *iso->rules, virtual_daa_score, iso->past_median_time, true, gate, dism, dnc, (uint32_t*)(S + o_lst), st);
+    if (own_masses) dism = own;
+    rc = kgv_isolation_run(ctx, d, *iso->rules, virtual_daa_score, iso->past_median_time, true, gate, dism, dnc, lst, st);
     if (rc) return rc;
     STAGE("isolation");
     if (pol) {
@@ -1265,24 +1248,25 @@ extern "C" int kgv_utxo_apply_accepted(kgv_ctx* ctx, kgv_utxo_table* t, const kg
   rc = kgv_batch_to_device(ctx, batch, &d, false);
   if (rc) return rc;
   size_t nt = d.n_txs, ni = d.n_inputs, no = d.n_outputs;
-  size_t o_itx = 0, o_otx = al256(ni * 4), o_ids = al256(o_otx + no * 4);
-  rc = kgv_reserve(ctx, &ctx->d_scratch, &ctx->d_scratch_cap, al256(o_ids + nt * 32));
+  uint32_t *itx, *otx;
+  uint64_t* ids;
+  rc = kgv_reserve_carved(ctx, &ctx->d_scratch, &ctx->d_scratch_cap,
+                          [&](kgv_carve& c) { itx = c.take<uint32_t>(ni); otx = c.take<uint32_t>(no); ids = c.take<uint64_t>(nt * 4); });
   if (rc) return rc;
-  uint8_t* S = ctx->d_scratch;
   kgv_io io(ctx);
   const uint8_t* dacc;
   io.in(accept, nt, &dacc);
   if ((rc = io.stage())) return rc;
   BatchView v{d.txs, d.inputs, d.outputs, nullptr, d.bytes};
   cudaStream_t st = ctx->stream;
-  if ((rc = kgv_tx_digests_run(ctx, d, nt, (uint64_t*)(S + o_ids), false))) return rc;
-  k_input_tx_index<<<nblk(nt, 128), 128, 0, st>>>(d.txs, (uint32_t)nt, (uint32_t*)(S + o_itx));
+  if ((rc = kgv_tx_digests_run(ctx, d, nt, ids, false))) return rc;
+  k_input_tx_index<<<nblk(nt, 128), 128, 0, st>>>(d.txs, (uint32_t)nt, itx);
   CK(cudaGetLastError());
-  k_output_tx_index<<<nblk(nt, 128), 128, 0, st>>>(d.txs, (uint32_t)nt, (uint32_t*)(S + o_otx));
+  k_output_tx_index<<<nblk(nt, 128), 128, 0, st>>>(d.txs, (uint32_t)nt, otx);
   CK(cudaGetLastError());
   ctx->launches += 2;
-  if (ni) { k_apply_erase<<<nblk(ni, 128), 128, 0, st>>>(view_of(t), d.txs, d.inputs, ni, (const uint32_t*)(S + o_itx), dacc); CK(cudaGetLastError()); ctx->launches++; }
-  if (no) { k_apply_insert<<<nblk(no, 128), 128, 0, st>>>(view_of(t), v, no, (const uint32_t*)(S + o_otx), dacc, (const uint64_t*)(S + o_ids), pov_daa_score); CK(cudaGetLastError()); ctx->launches++; }
+  if (ni) { k_apply_erase<<<nblk(ni, 128), 128, 0, st>>>(view_of(t), d.txs, d.inputs, ni, itx, dacc); CK(cudaGetLastError()); ctx->launches++; }
+  if (no) { k_apply_insert<<<nblk(no, 128), 128, 0, st>>>(view_of(t), v, no, otx, dacc, ids, pov_daa_score); CK(cudaGetLastError()); ctx->launches++; }
   if (!io.is_device(accept)) CK(cudaStreamSynchronize(st));  // a host-pointer call returns with the table updated
   return KGV_OK;
 }
@@ -1312,15 +1296,17 @@ extern "C" int kgv_muhash_txs(kgv_ctx* ctx, kgv_utxo_table* table, const kgv_tx_
   int rc = kgv_mu_reserve(ctx, ni, no, &e_den, &e_num);
   if (rc) return rc;
   if (nt) {
-    size_t o_ent = 0, o_itx = al256(o_ent + ni * sizeof(DevEntry)), o_otx = al256(o_itx + ni * 4), o_ids = al256(o_otx + no * 4);
-    rc = kgv_reserve(ctx, &ctx->d_scratch, &ctx->d_scratch_cap, al256(o_ids + nt * 32));
+    DevEntry* dent;
+    uint32_t *itx, *otx;
+    uint64_t* ids;
+    rc = kgv_reserve_carved(ctx, &ctx->d_scratch, &ctx->d_scratch_cap, [&](kgv_carve& c) {
+      dent = c.take<DevEntry>(ni); itx = c.take<uint32_t>(ni); otx = c.take<uint32_t>(no); ids = c.take<uint64_t>(nt * 4);
+    });
     if (rc) return rc;
-    uint8_t* S = ctx->d_scratch;
     cudaStream_t st = ctx->stream;
     const uint8_t* dacc;
     io.in(accept, nt, &dacc);
     if ((rc = io.stage())) return rc;
-    DevEntry* dent = (DevEntry*)(S + o_ent);
     if (ni) {
       if (table) k_populate<<<nblk(ni, 128), 128, 0, st>>>(view_of(table), d.inputs, ni, dent);
       else k_entries_from_batch<<<nblk(ni, 128), 128, 0, st>>>(d.entries, d.bytes, ni, dent);
@@ -1328,14 +1314,13 @@ extern "C" int kgv_muhash_txs(kgv_ctx* ctx, kgv_utxo_table* table, const kgv_tx_
       ctx->launches++;
     }
     BatchView v{d.txs, d.inputs, d.outputs, dent, d.bytes};
-    if ((rc = kgv_tx_digests_run(ctx, d, nt, (uint64_t*)(S + o_ids), false))) return rc;
-    k_input_tx_index<<<nblk(nt, 128), 128, 0, st>>>(d.txs, (uint32_t)nt, (uint32_t*)(S + o_itx));
+    if ((rc = kgv_tx_digests_run(ctx, d, nt, ids, false))) return rc;
+    k_input_tx_index<<<nblk(nt, 128), 128, 0, st>>>(d.txs, (uint32_t)nt, itx);
     CK(cudaGetLastError());
-    k_output_tx_index<<<nblk(nt, 128), 128, 0, st>>>(d.txs, (uint32_t)nt, (uint32_t*)(S + o_otx));
+    k_output_tx_index<<<nblk(nt, 128), 128, 0, st>>>(d.txs, (uint32_t)nt, otx);
     CK(cudaGetLastError());
     if (ni + no) {
-      k_muhash_tx_elements<<<nblk(ni + no, 128), 128, 0, st>>>(v, ni, no, (const uint32_t*)(S + o_itx), (const uint32_t*)(S + o_otx), dacc,
-                                                               (const uint64_t*)(S + o_ids), pov_daa_score, e_den, e_num);
+      k_muhash_tx_elements<<<nblk(ni + no, 128), 128, 0, st>>>(v, ni, no, itx, otx, dacc, ids, pov_daa_score, e_den, e_num);
       CK(cudaGetLastError());
     }
     ctx->launches += 3;
